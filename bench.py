@@ -2,7 +2,7 @@
 """bench.py -- end-to-end frames/s of the per-frame ADAS path (YOLOv8l + UFLDv2-CULane-ResNet34 + ByteTrack) on
 synthetic 1280x720 frames, one process per GPU.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--batch 8] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--batch 8] [--impl b200|reference] [--dump-outputs DIR]
 
 A "step" = one batch of `--batch` consecutive frames of one stream through the whole hot path:
     frames -> [letterbox + YOLOv8l + DFL decode + candidate select + reference NMS]  (adas_yolo_detect)
@@ -15,6 +15,8 @@ A "step" = one batch of `--batch` consecutive frames of one stream through the w
 nets with the same seeded weights; onnxruntime is not installed, so ORT-CPU is substituted by torch-CPU) on a
 bounded sample.  Multi-GPU (torchrun): every rank runs its own stream (weak scaling); the only collective is an
 NCCL all_gather of the fixed-size detection records per step.
+`--dump-outputs DIR` writes what the timed path returned for the last batch of its last timed step as DIR/<name>.npy
+(float32 / float64): inputs and weights are seeded, so two builds run with the same arguments can be compared array by array.
 """
 import argparse
 import json
@@ -73,7 +75,7 @@ def build_plans(seed: int = 0):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md clocks line).  One nvidia-smi process
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region.  One nvidia-smi process
     logs every 25 ms for the whole run (its start-up takes longer than a short timed region); each line carries nvidia-smi's own
     timestamp and `window(t0, t1)` keeps the samples taken between the two wall-clock marks of a timed region."""
     Q = ("timestamp,index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
@@ -133,7 +135,7 @@ class ClockSampler:
 
 
 # ------------------------------------------------------------------------------------------------------------
-# the B200 arm
+# the device arm
 # ------------------------------------------------------------------------------------------------------------
 def run_b200(args):
     import torch
@@ -171,7 +173,7 @@ def run_b200(args):
     pipe = AdasPipeline(plans["yolov8"][0], plans["ufldv2"][0], device=local, batch=B, box_score=BOX_SCORE, box_nms_iou=NMS_IOU, max_det=MAX_DET,
                         sets=args.sets, depth=args.depth)
 
-    # one stream per rank; frames differ per step (pool larger than L2: 24 batches x 22 MB = 530 MB >> 126 MB)
+    # one stream per rank; frames differ per step (pool larger than L2: 24 batches x 22 MB = 530 MB >> the H100's 50 MB)
     pool_batches = max(6, min(24, 192 // B))
     stream = synth_stream(1000 + rank, B * 4)
     host_pool = torch.empty((pool_batches, B, FRAME_H, FRAME_W, 3), dtype=torch.uint8).pin_memory()
@@ -183,7 +185,7 @@ def run_b200(args):
     # BASELINE configs[4] "NCCL gather of boxes": EVERY batch's detection / track records ([B, 300, 7] fp32, 67 KB) are all-gathered
     # across the ranks inside the timed region: one library call per step (adas_comm_all_gather) stages the block, uploads it and runs
     # ncclAllGather on the library's private stream with its own communicator -- no torch.distributed and no host synchronisation in
-    # the loop (round 1 exchanged once per run of steps because the Python-issued per-step collective cost 0.5 ms per step).
+    # the loop (a Python-issued per-step collective would add interpreter / host-sync time to every step).
     multi = world > 1 and os.environ.get("ADAS_B200_NO_GATHER") != "1"
     comm = None
     rec = np.zeros((B, MAX_DET, 7), np.float32) if multi else None
@@ -205,8 +207,11 @@ def run_b200(args):
             os.dup2(saved_fd2, 1)
             os.close(saved_fd2)
     gather_n = [0]
+    last = [None]                   # the latest batch result the timed path returned (--dump-outputs)
 
     def gather(r):
+        if r is not None:
+            last[0] = r
         if not multi or r is None:
             return
         gather_n[0] += 1
@@ -295,38 +300,29 @@ def run_b200(args):
     ms_dev, launches, clocks = timed(True)
     ms_e2e, _, clocks_e2e = timed(False)
     sampler.close()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(last[0], args.dump_outputs)
 
     result = None
     if rank == 0:
         fps = world * B * K / (ms_dev / 1e3)
         fps_e2e = world * B * K / (ms_e2e / 1e3)
-        # roofline of the dominant kernel (conv_gemm_v3_kernel / conv_chain_v3_kernel): all GEMM launches of one step back to back on the engine stream
+        # roofline of the dominant kernel (conv_gemm_v3_kernel): all GEMM launches of one step back to back on the engine stream
         peaks = {}
         try:
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = float(peaks.get("bf16_tflops", 1590.0))
+        peak = float(peaks.get("bf16_tflops", 989.0))      # H100 SXM data sheet, dense FP16/BF16 at 700 W
         ms_y, n_y = pipe.yolo.time_ops(B, 1 << 1, 5)
         ms_u, n_u = pipe.ufld.time_ops(B, 1 << 1, 5)
         ms_all_y, _ = pipe.yolo.time_ops(B, 0xFFFFFFFF, 5)
         ms_all_u, _ = pipe.ufld.time_ops(B, 0xFFFFFFFF, 5)
-        # FLOPs of the launches that are timed here: the stem convs run in stem_conv.cu (warp MMA), not in the tcgen05 GEMM launches
+        # FLOPs of the launches that are timed here: the stem convs run in stem_conv.cu (warp MMA), not in the wgmma GEMM launches
         gf_y = (plans["yolov8"][2].flops_per_img - plans["yolov8"][2].stem_flops_per_img) / 1e9
         gf_u = (plans["ufldv2"][2].flops_per_img - plans["ufldv2"][2].stem_flops_per_img) / 1e9
         gflop_step = (gf_y + gf_u) * B
         achieved = gflop_step / (ms_y + ms_u)          # GFLOP / ms == TFLOP/s
-        # DRAM bytes per GEMM launch: measured by ncu over whole steps of THIS command (bench.py --profile-steps, caches not flushed
-        # between launches); tools/traffic_report.py turns the capture into the JSON read here.  null if the capture is absent.
-        traffic, traffic_detail = None, None
-        try:
-            tj = json.load(open(os.path.join(ROOT, "profiles", "r02_bench_traffic.json")))
-            if tj.get("batch") == B:
-                traffic = tj.get("dram_bytes_per_launch")
-                traffic_detail = {k: tj.get(k) for k in ("gemm_dram_bytes_per_step", "algorithmic_bytes_per_step", "algorithmic_bytes_per_launch",
-                                                         "dram_over_algorithmic", "all_kernels_dram_bytes_per_step", "gemm_launches_per_step", "source", "command")}
-        except Exception:
-            pass
         result = {
             "metric": "end-to-end frames/sec (YOLOv8l+UFLDv2+ByteTrack) 1280x720", "value": round(fps, 2), "unit": "frames/s",
             "n_gpus": world, "steps": K, "warmup": Wm, "ms_per_step": round(ms_dev / K, 4), "higher_is_better": True, "scaling": "weak",
@@ -335,7 +331,7 @@ def run_b200(args):
                                    f"batch {B} frames per step (BASELINE configs[3]; configs[4] when n_gpus=8)",
                        "global_batch": world * B, "parallelism": f"dp{world} (one stream per GPU; the detection/track records of EVERY batch are NCCL all-gathered per step, inside the timed region, by the library's own communicator on a private stream)",
                        "weights": "seeded synthetic (He-normal, BN folded), fp16 operands, fp32 accumulate",
-                       "l2": f"inputs rotate through a {pool_batches}-batch pool ({pool_batches * B * FRAME_H * FRAME_W * 3 / 1e6:.0f} MB > 126 MB L2)"},
+                       "l2": f"inputs rotate through a {pool_batches}-batch pool ({pool_batches * B * FRAME_H * FRAME_W * 3 / 1e6:.0f} MB > 50 MB L2)"},
             "e2e": {"value": round(fps_e2e, 2), "unit": "frames/s", "h2d_bytes_per_step": B * FRAME_H * FRAME_W * 3,
                     "d2h_bytes_per_step": int(B * (MAX_DET * (16 + 4 + 4 + 4) + 8) + B * (4 * 81 * 2 * 4 + 16 + 4)),
                     "ms_per_step": round(ms_e2e / K, 4),
@@ -348,9 +344,9 @@ def run_b200(args):
             "tracks_alive": len(pipe.tracker.tracked_stracks),
             "gather": ({"per_step": True, "nccl_ranks": comm.info()[0], "all_gathers": comm.info()[1], "bytes_per_rank_per_step": int(rec.nbytes)} if comm is not None else None),
             "clocks": clocks, "clocks_e2e": clocks_e2e,
-            "roofline": {"bound": "tensor", "kernel": "conv_gemm_v3_kernel (tcgen05 implicit-GEMM conv/FC, persistent, warp-specialised, staged TMA-store epilogue)", "achieved": round(achieved, 1), "peak": peak,
-                         "unit": "TFLOP/s", "frac": round(achieved / peak, 4), "traffic": traffic, "traffic_detail": traffic_detail,
-                         "peak_source": "MEASURED_PEAKS.json bf16_tflops (burst; GEMM launches timed alone, of measured)" if peaks else "fallback 1590 (of fallback)",
+            "roofline": {"bound": "tensor", "kernel": "conv_gemm_v3_kernel (wgmma implicit-GEMM conv/FC, persistent, warp-specialised, TMA operands)", "achieved": round(achieved, 1), "peak": peak,
+                         "unit": "TFLOP/s", "frac": round(achieved / peak, 4),
+                         "peak_source": "MEASURED_PEAKS.json bf16_tflops (burst; GEMM launches timed alone, of measured)" if peaks else "H100 SXM data sheet, dense FP16 (of data sheet)",
                          "launches_per_step": n_y + n_u, "avg_launch_us": round(1e3 * (ms_y + ms_u) / (n_y + n_u), 2),
                          "algorithmic_gflop_per_step": round(gflop_step, 1),
                          "gemm_ms_per_step": round(ms_y + ms_u, 4), "all_plan_kernels_ms_per_step": round(ms_all_y + ms_all_u, 4)},
@@ -377,6 +373,36 @@ def run_b200(args):
         dist.barrier()
         dist.destroy_process_group()
     return result
+
+
+def dump_outputs(r, out_dir: str) -> None:
+    """The arrays a caller of AdasPipeline.step_pipelined received for the last batch: detections and lane points (entries past
+    each frame's / lane's count are zeroed: the library leaves them unwritten) and every frame's track records, one row per track
+    with its frame index first.  Integers are stored as float64 (exact), so every file is float32 or float64."""
+    os.makedirs(out_dir, exist_ok=True)
+    counts = np.asarray(r.counts)
+    det = np.arange(r.boxes.shape[1])[None, :] < counts[:, None]
+    npts = np.asarray(r.lane_npts)
+    on_lane = np.arange(r.lane_pts.shape[2])[None, None, :] < npts[..., None]
+    rows = []
+    for f, tr in enumerate(r.tracks or []):
+        for t in tr:
+            rows.append([f, t["track_id"], t["state"], t["is_activated"], t["class_id"], t["start_frame"], t["frame_id"], t["tracklet_len"],
+                         t["score"], *t["tlwh"], *t["det_tlbr"]])
+    arrays = {
+        "det_boxes_xywh": np.where(det[..., None], r.boxes, 0).astype(np.float32),
+        "det_scores": np.where(det, r.scores, 0).astype(np.float32),
+        "det_class_ids": np.where(det, r.class_ids, -1).astype(np.float64),
+        "det_counts": counts.astype(np.float64),
+        "det_n_candidates": np.asarray(r.n_candidates).astype(np.float64),
+        "lane_points": np.where(on_lane[..., None], r.lane_pts, 0).astype(np.float64),
+        "lane_npts": npts.astype(np.float64),
+        "lane_status": np.asarray(r.lane_status).astype(np.float64),
+        # frame, track_id, state, is_activated, class_id, start_frame, frame_id, tracklet_len, score, tlwh[4], det_tlbr[4]
+        "tracks": np.asarray(rows, np.float64).reshape(-1, 17),
+    }
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 # ------------------------------------------------------------------------------------------------------------
@@ -497,6 +523,8 @@ def main():
     ap.add_argument("--depth", type=int, default=3, help="batches queued ahead of the tracker")
     ap.add_argument("--cpu-frames", type=int, default=8, help="frames in the cpu_baseline sample (0 disables)")
     ap.add_argument("--ref-frames", type=int, default=2, help="frames per step of the --impl reference arm")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed batch's detections, lane points and track records to DIR/<name>.npy")
     ap.add_argument("--watchdog", type=int, default=int(os.environ.get("ADAS_B200_WATCHDOG", "1500")),
                     help="seconds after which a stuck run dumps every thread's stack to stderr and exits non-zero (0 disables)")
     args = ap.parse_args()

@@ -1,5 +1,5 @@
 /*
- * adas_b200.h -- C ABI of libadas_b200.so: the B200-native (sm_100a) replacement for the
+ * adas_b200.h -- C ABI of libadas_b200.so: the H100-native (sm_90a) replacement for the
  * ONNXRuntime / TensorRT dispatch behind the reference's coreEngine.py, plus the fused
  * per-frame post-processing (YOLO decode + NMS, UFLDv2 row/col-anchor decode, ByteTrack
  * IoU cost + linear assignment).
@@ -48,7 +48,7 @@ int64_t     adas_launch_count(void);
  * replaces: TensorRTEngine.__init__ / OnnxEngine.__init__ (coreEngine.py:122-142,161-170):
  * deserialize a plan file (.b200w, produced by the packer), allocate device buffers for
  * batches up to max_batch, create the stream.  `device` replaces the hard-coded
- * cuda.Device(0) (coreEngine.py:47).  conv_impl: 0 = tcgen05 implicit-GEMM (product path),
+ * cuda.Device(0) (coreEngine.py:47).  conv_impl: 0 = wgmma implicit-GEMM (product path),
  * 1 = plain SIMT CUDA-core kernel (validation path for tests; same plan, same buffers). */
 int adas_engine_create(const char* plan_path, int device, int max_batch, int conv_impl,
                        adas_engine** out);

@@ -1,5 +1,5 @@
 """GPU: single-kernel parity through the C ABI (test hooks write/read plan buffers).
-conv_impl 0 = tcgen05 implicit GEMM (product), 1 = SIMT validation kernel.  Reference = torch fp32 conv on the
+conv_impl 0 = wgmma implicit GEMM (product), 1 = SIMT validation kernel.  Reference = torch fp32 conv on the
 fp16-rounded operands (so the only difference is accumulation order): tolerance 2e-3 relative to the output scale."""
 import os
 
@@ -17,7 +17,7 @@ pytestmark = pytest.mark.gpu
 
 def _run_conv(tmp_path, impl, B, cin, cout, H, W, k, s, act, residual=None, out_f32=False, pad=None, seed=0, im_c=None, tile=None,
               out_slice=None):
-    """tile = (BN, MT) forces the tile shape of the tcgen05 kernel; out_slice = (C_total, coff) writes the result into a channel
+    """tile = (BN, MT) forces the tile shape of the wgmma kernel; out_slice = (C_total, coff) writes the result into a channel
     slice of a wider (concat) buffer whose other channels must stay untouched."""
     if pad is None and k == 1:
         pad = 0
@@ -101,24 +101,24 @@ def test_conv_parity(tmp_path, impl, case):
 
 
 TILE_CASES = [
-    # (B cin cout H W k s act residual) , (BN, MT)   -- tcgen05 kernel only: every epilogue / accumulator / operand-fetch mode
-    ((2, 256, 256, 40, 40, 3, 1, 1, "post"), (256, 1)),     # plain 9 taps, staged stores, 4 chunks
-    ((2, 256, 256, 40, 40, 3, 1, 1, None), (256, 2)),       # one 512-column accumulator set
-    ((2, 256, 256, 40, 40, 3, 1, 1, "post"), (128, 2)),     # slab, two sub-tiles, two accumulator stages
-    ((2, 128, 128, 80, 80, 3, 1, 1, None), (128, 1)),       # slab, many tiles per CTA (accumulator / staging ping-pong)
-    ((2, 128, 128, 48, 80, 3, 1, 2, "pre"), (128, 4)),      # four sub-tiles, one accumulator stage, residual before ReLU
+    # (B cin cout H W k s act residual) , (BN, MT)   -- wgmma kernel only: every epilogue / accumulator / operand-fetch mode
+    ((2, 256, 256, 40, 40, 3, 1, 1, "post"), (256, 1)),     # 9 taps, BN = two 128-column wgmmas
+    ((2, 256, 256, 40, 40, 3, 1, 1, None), (256, 2)),       # taller than the registers hold: runs as (256, 1)
+    ((2, 256, 256, 40, 40, 3, 1, 1, "post"), (128, 2)),     # two sub-tiles
+    ((2, 128, 128, 80, 80, 3, 1, 1, None), (128, 1)),       # many tiles per CTA (operand ring carried across tiles)
+    ((2, 128, 128, 48, 80, 3, 1, 2, "pre"), (128, 4)),      # runs as (128, 2); residual before ReLU
     ((2, 256, 256, 20, 20, 3, 1, 1, None), (64, 3)),        # 64-wide tiles, three sub-tiles
     ((1, 256, 320, 40, 40, 3, 1, 1, None), (128, 1)),       # N = 320: last N tile half outside the tensor (TMA clips it)
     ((1, 256, 320, 40, 40, 3, 1, 1, None), (192, 1)),       # 192-wide tiles
-    ((1, 256, 320, 40, 40, 3, 1, 1, None), (160, 1)),       # direct-store epilogue (BN not a multiple of 64)
-    ((2, 256, 512, 40, 40, 3, 2, 1, None), (256, 1)),       # stride 2, 4-D TMA store of output patches
+    ((1, 256, 320, 40, 40, 3, 1, 1, None), (160, 1)),       # BN not a multiple of 64 (128 + 32 column wgmmas)
+    ((2, 256, 512, 40, 40, 3, 2, 1, None), (256, 1)),       # stride 2, output patches
     ((2, 256, 512, 40, 40, 3, 2, 1, None), (128, 2)),       # stride 2 with two patches per CTA tile
     ((3, 128, 256, 80, 80, 3, 2, 1, None), (128, 3)),       # stride 2, three patches, patch count not a multiple of MT
     ((1, 64, 64, 160, 96, 3, 2, 2, "pre"), (64, 2)),        # stride 2 with residual, 48-wide output rows (clipped patches)
     ((2, 1024, 512, 40, 40, 1, 1, 1, None), (256, 2)),      # 1x1, long K, 256x256 tiles
     ((2, 320, 128, 80, 80, 1, 1, 1, None), (128, 3)),       # 1x1, K = 320 (five k-blocks)
     ((1, 192, 64, 17, 23, 1, 1, 1, None), (64, 1)),         # K tail, ragged M
-    ((2, 64, 80, 20, 20, 1, 1, 0, None), (80, 1)),          # fp16 N = 80 through the direct path
+    ((2, 64, 80, 20, 20, 1, 1, 0, None), (80, 1)),          # fp16 N = 80 (64 + 16 column wgmmas)
 ]
 
 

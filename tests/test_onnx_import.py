@@ -196,7 +196,7 @@ def test_checkpoint_conversion_matches_seeded_plan(tmp_path):
 
 
 def test_engine_accepts_onnx_path_and_fails_loudly_without_a_device(tmp_path, monkeypatch):
-    """`B200Engine("model.onnx")` converts and caches the plan, then hands it to the C ABI; with no sm_100 device here the library
+    """`B200Engine("model.onnx")` converts and caches the plan, then hands it to the C ABI; on a machine without an sm_90 device the library
     must raise (there is no CPU fallback on the product path)."""
     if torch.cuda.is_available():
         pytest.skip("needs a machine without a GPU")

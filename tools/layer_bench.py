@@ -29,5 +29,5 @@ for name, B, cin, cout, H, W, k in LAYERS:
     eng = _capi.Engine(path, 0, max_batch=B)
     ms, n = eng.time_ops(B, 1 << 1, 20)
     macs = B * (H + 2) * (W + 2) * cout * cin * k * k
-    print(f"dbg={os.environ.get('ADAS_B200_DBG','0'):>2} bn={os.environ.get('ADAS_B200_BN','-')} mt={os.environ.get('ADAS_B200_MT','-')} {name:28s} {ms*1e3:8.1f} us  {2*macs/ms/1e9:7.1f} TFLOP/s(incl halo)", flush=True)
+    print(f"bn={os.environ.get('ADAS_B200_BN','-')} mt={os.environ.get('ADAS_B200_MT','-')} {name:28s} {ms*1e3:8.1f} us  {2*macs/ms/1e9:7.1f} TFLOP/s(incl halo)", flush=True)
     eng.close()

@@ -3,7 +3,7 @@ Prints the probability / box error the device path will show, the candidates per
 of the threshold.  Test infrastructure (uses oracle/):  python tools/synth_operating_point.py yolov8 l 45,-9 40,-8.2
 """
 import sys, os
-sys.path.insert(0,'/root/repo'); sys.path.insert(0,'/root/repo/tests')
+R = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, R); sys.path.insert(0, os.path.join(R, 'tests'))
 import numpy as np, torch
 torch.set_num_threads(8)
 import adas_b200

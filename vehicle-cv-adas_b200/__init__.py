@@ -1,4 +1,4 @@
-"""adas_b200 -- B200-native (sm_100a) per-frame ADAS inference path with the reference's
+"""adas_b200 -- H100-native (sm_90a) per-frame ADAS inference path with the reference's
 Python API surface (YoloDetector / UltrafastLaneDetectorV2 / BYTETracker, coreEngine protocol).
 
 Host code is Python; all arithmetic on the hot path runs in hand-written CUDA kernels inside

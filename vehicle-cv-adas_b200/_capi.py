@@ -1,6 +1,6 @@
 """_capi.py -- ctypes binding of libadas_b200.so (the C ABI declared in include/adas_b200.h).
 
-The product path has no CPU fallback: if the shared library is missing or there is no sm_100
+The product path has no CPU fallback: if the shared library is missing or there is no sm_90
 device, the calls raise.  Errors returned by the library become Python `Exception`s, mirroring
 the reference's error style (coreEngine.py:12-14,20,26).
 """
@@ -35,7 +35,7 @@ def lib() -> C.CDLL:
         if not os.path.isfile(LIB_PATH):
             raise Exception(
                 f"libadas_b200.so not built ({LIB_PATH}); run `python -c 'import __graft_entry__ as g; g.build()'`. "
-                "There is no CPU fallback for the B200 path.")
+                "There is no CPU fallback for the H100 path.")
         _lib = C.CDLL(LIB_PATH)
         _lib.adas_last_error.restype = C.c_char_p
         _lib.adas_launch_count.restype = C.c_int64

@@ -2,7 +2,7 @@
 
 Counterpart of the reference's conversion scripts: `convertOnnxToTensorRT.py` (ONNX -> .trt engine written next to the model)
 and `TrafficLaneDetector/convertPytorchToONNX.py:77-87` (UFLD `.pth` checkpoint -> ONNX: `torch.load(...)['model']`, the
-`module.` prefix of DataParallel checkpoints stripped).  Here both sources go straight to the plan the sm_100a engine loads:
+`module.` prefix of DataParallel checkpoints stripped).  Here both sources go straight to the plan the sm_90a engine loads:
 
     python -m adas_b200.convert yolov8l.onnx                       # architecture recognised from the graph
     python -m adas_b200.convert culane_res34.pth --kind ufldv2 --backbone 34

@@ -16,14 +16,14 @@ from . import _capi
 
 
 class EngineBase(abc.ABC):
-    """Supports B200 plans and ONNX model files (the reference supports Onnx/TensorRT, coreEngine.py:12-14)."""
+    """Supports .b200w plans and ONNX model files (the reference supports Onnx/TensorRT, coreEngine.py:12-14)."""
 
     SUFFIXES = (".b200w", ".onnx")
 
     def __init__(self, model_path):
         if not os.path.isfile(model_path):
             raise Exception("The model path [%s] can't not found!" % model_path)
-        assert model_path.endswith(self.SUFFIXES), "B200 Parameters must be a .b200w or .onnx file."
+        assert model_path.endswith(self.SUFFIXES), "Parameters must be a .b200w or .onnx file."
         self._framework_type = None
 
     @property
@@ -52,7 +52,7 @@ class EngineBase(abc.ABC):
 
 
 class B200Engine(EngineBase):
-    """Drop-in for TensorRTEngine / OnnxEngine: same methods, sm_100a kernels underneath.
+    """Drop-in for TensorRTEngine / OnnxEngine: same methods, sm_90a kernels underneath.
 
     device    replaces the hard-coded cuda.Device(0) of coreEngine.py:47 (defaults to LOCAL_RANK or 0)
     max_batch the reference is batch-1; batched calls are an extension (per-frame results are identical)
@@ -69,7 +69,7 @@ class B200Engine(EngineBase):
             plan_path = plan_from_onnx(plan_path)        # parsed and packed once, cached next to the temp dir (ADAS_B200_PLAN_CACHE)
         self.plan_path = plan_path
         self.handle = _capi.Engine(plan_path, device=device, max_batch=max_batch, conv_impl=conv_impl)
-        self.providers = "B200ExecutionProvider(sm_100a)"
+        self.providers = "B200ExecutionProvider(sm_90a)"
         self.framework_type = "b200"
         self.engine_dtype = np.float32          # the input binding is fp32 NCHW; arithmetic is fp16 x fp16 -> fp32
         self.device = device

@@ -2,8 +2,8 @@
 //
 // (No reference counterpart: the reference is single-GPU, SURVEY 8e.  BASELINE configs[4] asks for an NCCL gather of boxes.)
 // Frames / streams are independent, so nothing is exchanged on the data path; what consumers of configs[4] need is every rank's
-// fixed-size record block per batch.  Round 1 issued torch.distributed.all_gather from Python once per run of steps because a
-// per-step collective cost 0.5 ms of interpreter / host-sync time.  Here each step is ONE library call that returns immediately:
+// fixed-size record block per batch.  A per-step torch.distributed.all_gather from Python would cost interpreter / host-sync
+// time every step.  Here each step is ONE library call that returns immediately:
 // the caller's records are staged into a pinned ring slot, copied to the device and all-gathered (ncclAllGather) on a private
 // side stream with its own communicator (ncclCommInitRank) -- nothing on the detectors' streams waits for it.
 // NCCL is bound at run time (dlopen of the libnccl.so.2 the process already loaded through torch, else the system one), so the

@@ -1,4 +1,4 @@
-// common.h -- shared declarations for libadas_b200 (sm_100a only).
+// common.h -- shared declarations for libadas_b200 (sm_90a: H100).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -67,13 +67,11 @@ struct GemmParams {
     int out_ld;     // row stride of out, elements
     int res_ld;     // row stride of res, elements; NEGATIVE = add the residual before the activation (ResNet)
     int mask_H, mask_W;  // > 0: only rows in the interior of the padded (H+2)x(W+2) grid are stored
-    int dbg;        // debug switches (ADAS_B200_DBG), 0 in production
     int mt_hint;    // number of 128-row sub-tiles per CTA tile (1..4; they share each weight tile), 0 = auto
     // stride-2 convs (3x3 pad 1, or 1x1) read the input through a 4-D TMA map with traversal stride 2: an M tile is a
     // bw x bh patch of output pixels of one image; s2_* describe the output grid and the input's padded height
     int s2, s2_bw, s2_bh, s2_tw, s2_th, s2_Ho, s2_Wo, s2_Hp_in;
     int transposed; // 1: out[n * out_ld + row] (swap-AB FC: rows = features, cols = batch), bias per row
-    int chain;      // 1: this layer runs inside a chain launch (gemm_chain.cu): three staging buffers whatever its residual
     const float* bias;   // [N] ([M] when transposed) or nullptr
     const __half* res;   // residual, same row indexing as out, or nullptr
     void* out;
@@ -85,8 +83,6 @@ struct GemmParams {
 int  gemm_simt_launch(const GemmParams& p, cudaStream_t st);
 int  make_tmap_4d_s2(CUtensorMap* tm, const void* base, uint64_t C, uint64_t Wp, uint64_t Hp, uint64_t B, uint64_t ld_elems,
                      uint32_t box_w_src, uint32_t box_h_src);
-int  make_tmap_4d(CUtensorMap* tm, const void* base, uint64_t C, uint64_t W, uint64_t H, uint64_t B, uint64_t ld_elems, uint64_t Wp, uint64_t Hp,
-                  uint32_t box_c, uint32_t box_w, uint32_t box_h);
 // v3 kernel (gemm_v3.cu): the product path
 int  gemm_v3_prepare(const GemmParams& p, const void* a_base, uint64_t a_inner, uint64_t a_rows, uint64_t a_stride_bytes,
                      const void* b_base, uint64_t b_inner, uint64_t b_rows, uint64_t b_stride_bytes, void** opaque);
@@ -94,16 +90,8 @@ int  gemm_v3_prepare_s2(const GemmParams& p, const void* a_base, uint64_t a_C, u
                         const void* b_base, uint64_t b_inner, uint64_t b_rows, uint64_t b_stride_bytes, void** opaque);
 int  gemm_v3_run(void* opaque, cudaStream_t st);
 void gemm_v3_free(void* opaque);
-int  gemm_v3_grid(const void* opaque);
 void gemm_v3_describe(const void* opaque, char* out, int cap);
-void gemm_v3_tile_of(const void* opaque, int* BN, int* MT);
-bool gemm_v3_is_staged(const void* opaque);
 int  gemm_v3_candidates(const GemmParams& base, int max_out, int* BN_out, int* mt_out);
-// chain of same-shape layers in one launch (gemm_chain.cu); layer_opaques are gemm_v3_prepare results with GemmParams::chain = 1
-int  gemm_chain_prepare(void* const* layer_opaques, int n_layers, void** out);
-int  gemm_chain_run(void* opaque, cudaStream_t st);
-void gemm_chain_free(void* opaque);
-void gemm_chain_describe(const void* opaque, char* out, int cap);
 int  make_tmap_2d(CUtensorMap* tm, const void* base, uint64_t inner, uint64_t rows, uint64_t row_stride_bytes,
                   uint32_t box_inner, uint32_t box_rows);
 

@@ -1,5 +1,5 @@
 // elementwise.cu -- HBM-bound glue kernels on the padded-NHWC fp16 layout (16-byte vector accesses,
-// one thread per 8 channels, grids sized in waves of the 148 SMs by the launch helpers).
+// one thread per 8 channels, grids sized in waves of the 132 SMs of an H100 by the launch helpers).
 // These are the non-GEMM graph nodes that ONNXRuntime/TensorRT execute inside the opaque model
 // behind coreEngine.py:150-157/184-186: strided-conv patch gather (feeds the GEMM), MaxPool
 // (SPPF 5x5 s1, ResNet 3x3 s2), nearest Upsample x2 (+Concat by writing a channel slice),
@@ -79,7 +79,7 @@ int launch_im2col(const __half* in, int in_ld, int in_coff, int B, int H, int W,
     if (Cin % 8 == 0 && in_ld % 8 == 0 && in_coff % 8 == 0 && Kpad % 8 == 0) {
         const long long total8 = (long long)B * Ho * Wo * kh * kw * (Cin / 8);
         int blocks8 = grid_for(total8, 256);
-        if (blocks8 > 148 * 16) blocks8 = 148 * 16;
+        if (blocks8 > 132 * 16) blocks8 = 132 * 16;
         im2col8_kernel<<<blocks8, 256, 0, st>>>(in, in_ld, in_coff, B, H, W, Cin, kh, kw, stride, pad, Ho, Wo, out, Kpad);
         count_launch();
         ADAS_CUDA(cudaGetLastError());
@@ -87,7 +87,7 @@ int launch_im2col(const __half* in, int in_ld, int in_coff, int B, int H, int W,
     }
     const long long total = (long long)B * Ho * Wo * kh * kw * (Cin / 4);
     int blocks = grid_for(total, 256);
-    if (blocks > 148 * 32) blocks = 148 * 32;
+    if (blocks > 132 * 32) blocks = 132 * 32;
     im2col_kernel<<<blocks, 256, 0, st>>>(in, in_ld, in_coff, B, H, W, Cin, kh, kw, stride, pad, Ho, Wo, out, Kpad);
     count_launch();
     ADAS_CUDA(cudaGetLastError());
@@ -141,7 +141,7 @@ int launch_maxpool(const __half* in, int in_ld, int B, int H, int W, int C, int 
     ADAS_CHECK(C % 8 == 0 && in_ld % 8 == 0 && out_ld % 8 == 0, "maxpool: channel alignment");
     const long long total = (long long)B * Ho * Wo * (C / 8);
     int blocks = grid_for(total, 256);
-    if (blocks > 148 * 32) blocks = 148 * 32;
+    if (blocks > 132 * 32) blocks = 132 * 32;
     maxpool_kernel<<<blocks, 256, 0, st>>>(in, in_ld, B, H, W, C, k, s, p, out, out_ld, Ho, Wo);
     count_launch();
     ADAS_CUDA(cudaGetLastError());
@@ -171,7 +171,7 @@ int launch_upsample2x(const __half* in, int in_ld, int B, int H, int W, int C, _
     ADAS_CHECK(C % 8 == 0 && in_ld % 8 == 0 && out_ld % 8 == 0, "upsample: channel alignment");
     const long long total = (long long)B * 4 * H * W * (C / 8);
     int blocks = grid_for(total, 256);
-    if (blocks > 148 * 32) blocks = 148 * 32;
+    if (blocks > 132 * 32) blocks = 132 * 32;
     upsample2x_kernel<<<blocks, 256, 0, st>>>(in, in_ld, B, H, W, C, out, out_ld);
     count_launch();
     ADAS_CUDA(cudaGetLastError());
@@ -246,7 +246,7 @@ __global__ void nchw_to_padded_kernel(const float* __restrict__ in, int B, int C
 int launch_nchw_to_padded(const float* in, int B, int C, int H, int W, __half* out, int out_ld, cudaStream_t st) {
     const long long total = (long long)B * H * W;
     int blocks = grid_for(total, 256);
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     nchw_to_padded_kernel<<<blocks, 256, 0, st>>>(in, B, C, H, W, out, out_ld);
     count_launch();
     ADAS_CUDA(cudaGetLastError());
@@ -284,7 +284,7 @@ __global__ void stempack_kernel(const __half* __restrict__ img, int B, int H, in
 int launch_stempack(const __half* img, int B, int H, int W, __half* q, cudaStream_t st) {
     const long long total = (long long)B * (H / 2 + 1) * (W / 2) * 8;
     int blocks = grid_for(total, 256);
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     stempack_kernel<<<blocks, 256, 0, st>>>(img, B, H, W, q);
     count_launch();
     ADAS_CUDA(cudaGetLastError());
@@ -302,7 +302,7 @@ namespace adas {
 // ---- fully connected layer at small batch: weight-streaming kernel ------------------------------------------------------------
 // Replaces the first Linear of the UFLDv2 head (exportLib/ultrafastLaneV2/model_culane.py:35-37, `cls` Sequential) at the batch
 // sizes the pipeline uses: out[b][n] = act(bias[n] + sum_k x[b][k] * W[n][k]).  At batch <= 32 the layer is a stream of the
-// weight matrix (FC1: 2048 x 4992 fp16 = 20 MB, L2-resident): the swap-AB tensor-core GEMM had 8 CTAs for it (47.8 us, 0.43 TB/s).
+// weight matrix (FC1: 2048 x 4992 fp16 = 20 MB, L2-resident): the swap-AB tensor-core GEMM has 8 CTAs for it.
 // One CTA owns FC_F output features and 8 batch rows; its 8 warps split K, lanes stride over 16-byte chunks (8 independent weight
 // loads per lane per step), fp32 accumulation, fixed-order reduction (xor-shuffle over lanes, then warps in ascending order).  Every (b, n) value is computed by the same instruction sequence whatever the batch size (batch rows are independent
 // accumulators), so per-frame results do not depend on the batch.

@@ -3,7 +3,7 @@
 // Replaces the engine layer of the reference (coreEngine.py): TensorRTBase.__init__/_allocate_buffers (:41-88),
 // TensorRTBase.inference (:93-118), TensorRTEngine/OnnxEngine shape queries (:144-148,178-182) and
 // engine_inference (:150-157,184-186).  One handle = one device + one private stream; every activation
-// tensor of the network owns its own HBM buffer (180 GB: no reuse planning, zero halos stay zero forever).
+// tensor of the network owns its own HBM buffer (no reuse planning, zero halos stay zero forever).
 #include "common.h"
 #include "plan.h"
 #include "../../include/adas_b200.h"
@@ -45,7 +45,7 @@ struct Program {   // launch list for one batch size
     std::vector<std::string> step_desc;   // human-readable shape / tile choice per step (adas_engine_step_desc)
     cudaGraphExec_t graph = nullptr;
     int runs = 0;
-    int n_launch() const { int n = 0; for (uint32_t t : step_type) n += (t != 31); return n; }   // steps folded into a chain launch do not launch
+    int n_launch() const { return (int)step_type.size(); }
 };
 
 }  // namespace adas
@@ -57,10 +57,6 @@ struct adas_engine {
     int max_batch = 1;
     int conv_impl = 0;
     bool use_graph = true;
-    int use_chain = 0;            // ADAS_B200_CHAIN: 0 (default) = one launch per layer; 2 = chain a run where the chain launch (gemm_chain.cu) timed
-                                  // faster than its per-layer launches when the program was built; 1 = chain every eligible run.  Off by default:
-                                  // one bench process in ~6 hung on the device with chains enabled (never with ADAS_B200_CHAIN=0, 16 runs) --
-                                  // root cause not found, see DESIGN.md section 4.2
     bool autotune = true;         // ADAS_B200_AUTOTUNE=0: modelled tile choice only
     cudaStream_t stream = nullptr;
     PlanHeader hdr;
@@ -124,118 +120,7 @@ static const void* tensor_ptr(const adas_engine* e, int idx) {
     return static_cast<const uint8_t*>(e->d_blob) + e->tensors[idx].offset;
 }
 
-// one v3 GEMM step as the chain builder sees it (gemm_chain.cu)
-struct GemmRec {
-    size_t step;                       // index into Program::steps
-    GemmParams g;                      // with the tile shape that was finally chosen
-    int a_buf, a_coff, out_buf, out_coff, res_buf, res_coff;
-    bool eligible;
-    std::function<int(const GemmParams&, void**)> prep;
-};
-
-static bool chain_edge_ok(const GemmRec& a, const GemmRec& b) {
-    if (!a.eligible || !b.eligible || b.step != a.step + 1) return false;
-    const GemmParams &x = a.g, &y = b.g;
-    if (x.M != y.M || x.N != y.N || x.Kc != y.Kc || x.ntaps != y.ntaps || x.act != y.act || x.Wp != y.Wp || x.mask_H != y.mask_H || x.mask_W != y.mask_W) return false;
-    if (b.a_buf != a.out_buf || b.a_coff != a.out_coff || y.Kc != x.N) return false;        // b reads exactly what a wrote
-    if (b.res_buf >= 0 && !(b.res_buf == a.a_buf && b.res_coff == a.a_coff)) return false;     // residual = the previous layer's input
-    return true;
-}
-
-static int build_chains(adas_engine* e, Program* prog, std::vector<GemmRec>& recs) {
-    if (!e->use_chain) return 0;
-    size_t i = 0;
-    while (i < recs.size()) {
-        size_t j = i;
-        while (j + 1 < recs.size() && chain_edge_ok(recs[j], recs[j + 1])) {
-            // no layer may write a view an earlier layer of the chain still reads
-            bool clash = false;
-            const GemmRec& w = recs[j + 1];
-            for (size_t k = i; k <= j && !clash; ++k) {
-                const GemmRec& r = recs[k];
-                auto overlap = [&](int buf, int coff, int C) { return buf == w.out_buf && coff < w.out_coff + w.g.N && w.out_coff < coff + C; };
-                clash = overlap(r.a_buf, r.a_coff, r.g.Kc) || (r.res_buf >= 0 && overlap(r.res_buf, r.res_coff, r.g.N));
-            }
-            if (clash) break;
-            ++j;
-        }
-        if (j > i) {
-            static const bool chain_log = getenv("ADAS_B200_CHAIN_LOG") != nullptr;
-            // tile shapes worth trying for the chain: the ones the member layers chose for themselves
-            std::vector<std::pair<int, int>> shapes;
-            for (size_t k = i; k <= j; ++k) {
-                const std::pair<int, int> sh(recs[k].g.BN, recs[k].g.mt_hint);
-                if (std::find(shapes.begin(), shapes.end(), sh) == shapes.end()) shapes.push_back(sh);
-            }
-            const bool timed = e->use_chain == 2 && e->autotune;
-            if (!timed) shapes.resize(1);
-            cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-            float best_ms = 1e30f;
-            if (timed) {
-                // the alternative: the per-layer launches as they stand, back to back
-                ADAS_CUDA(cudaEventCreate(&ev0)); ADAS_CUDA(cudaEventCreate(&ev1));
-                int rc = 0;
-                for (int r = 0; r < 5 && !rc; ++r) {
-                    if (r == 1) cudaEventRecord(ev0, e->stream);
-                    for (size_t k = i; k <= j && !rc; ++k) rc = prog->steps[recs[k].step](e->stream);
-                }
-                cudaEventRecord(ev1, e->stream);
-                if (rc || cudaEventSynchronize(ev1) != cudaSuccess) { cudaEventDestroy(ev0); cudaEventDestroy(ev1); ADAS_CHECK(false, "chain timing: per-layer launches failed (%s)", g_err); }
-                cudaEventElapsedTime(&best_ms, ev0, ev1);
-                if (chain_log) fprintf(stderr, "[chain] steps %zu..%zu per-layer launches: %.1f us\n", recs[i].step, recs[j].step, best_ms * 250.0);
-            }
-            void* best_chain = nullptr;
-            for (const auto& sh : shapes) {
-                std::vector<void*> layers;
-                bool ok = true;
-                for (size_t k = i; k <= j && ok; ++k) {
-                    GemmParams gc = recs[k].g;
-                    gc.BN = sh.first; gc.mt_hint = sh.second; gc.chain = 1;
-                    void* op = nullptr;
-                    if (recs[k].prep(gc, &op)) ok = false; else layers.push_back(op);
-                }
-                void* chain = nullptr;
-                if (ok && gemm_chain_prepare(layers.data(), (int)layers.size(), &chain)) ok = false;
-                for (void* op : layers) gemm_v3_free(op);                    // the chain keeps its own copies of the tensor maps
-                if (!ok) {
-                    if (chain_log) fprintf(stderr, "[chain] steps %zu..%zu BN=%d MT=%d not chainable: %s\n", recs[i].step, recs[j].step, sh.first, sh.second, g_err);
-                    continue;
-                }
-                if (!timed) { best_chain = chain; break; }
-                int rc = 0;
-                for (int r = 0; r < 5 && !rc; ++r) {
-                    if (r == 1) cudaEventRecord(ev0, e->stream);
-                    rc = gemm_chain_run(chain, e->stream);
-                }
-                cudaEventRecord(ev1, e->stream);
-                float ms = 1e30f;
-                if (!rc && cudaEventSynchronize(ev1) == cudaSuccess) cudaEventElapsedTime(&ms, ev0, ev1);
-                if (chain_log) fprintf(stderr, "[chain] steps %zu..%zu one launch BN=%d MT=%d: %.1f us\n", recs[i].step, recs[j].step, sh.first, sh.second, ms * 250.0);
-                if (ms < best_ms * 0.98f) { best_ms = ms; if (best_chain) gemm_chain_free(best_chain); best_chain = chain; }
-                else gemm_chain_free(chain);
-            }
-            if (ev0) { cudaEventDestroy(ev0); cudaEventDestroy(ev1); }
-            if (best_chain) {
-                std::shared_ptr<void> keep(best_chain, gemm_chain_free);
-                char d[256];
-                gemm_chain_describe(best_chain, d, sizeof(d));
-                prog->step_desc.resize(prog->steps.size());
-                prog->step_desc[recs[i].step] = d;
-                prog->steps[recs[i].step] = [keep](cudaStream_t st) { return gemm_chain_run(keep.get(), st); };
-                for (size_t k = i + 1; k <= j; ++k) {
-                    prog->steps[recs[k].step] = [](cudaStream_t) { return 0; };   // folded into the chain launch above
-                    prog->step_type[recs[k].step] = 31;
-                    prog->step_desc[recs[k].step] = "(in the chain above)";
-                }
-            }
-        }
-        i = j + 1;
-    }
-    return 0;
-}
-
 static int build_program(adas_engine* e, int batch, Program* prog) {
-    std::vector<GemmRec> recs;
     for (size_t oi = 0; oi < e->ops.size(); ++oi) {
         const PlanOp& op = e->ops[oi];
         const int32_t* p = op.p;
@@ -295,7 +180,7 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
                         g.s2_tw = (Wo + best_bw - 1) / best_bw; g.s2_th = (Ho + best_bh - 1) / best_bh;
                         g.s2_Ho = Ho; g.s2_Wo = Wo; g.s2_Hp_in = (int)ab.H + 2;
                         if (e->conv_impl == 1) g.M = batch * (int)ob.rows_per_img;        // SIMT kernel walks output rows
-                        else g.M = batch * g.s2_tw * g.s2_th * 128;                         // tcgen05 kernel walks patches
+                        else g.M = batch * g.s2_tw * g.s2_th * 128;                         // wgmma kernel walks patches
                         if (p[15] <= 0) BN = N <= 256 ? (N + 15) / 16 * 16 : (N % 256 == 0 ? 256 : 128);
                     }
                 } else {
@@ -314,10 +199,10 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
                     g.out_ld = (int)(ob.rows_per_img * ob.C);
                 }
                 if (p[17] > 0) g.mt_hint = p[17];       // plan-forced sub-tile count (test hook of plan.py)
-                // Fully connected layers whose weight matrix stays in L2 (FC1 of the UFLD head: 20 MB) run as a weight stream on the CUDA
-                // cores: the swap-AB tensor-core GEMM has only N/256 CTAs for them (profiles/r02_optable_ufld_b8: 47.8 us = 0.43 TB/s).
+                // Fully connected layers whose weight matrix stays in L2 (FC1 of the UFLD head: 20 MB; up to half of the H100's 50 MB) run
+                // as a weight stream on the CUDA cores: the swap-AB tensor-core GEMM has only N/256 CTAs for them.
                 static const bool fc_stream_on = !(getenv("ADAS_B200_FC_STREAM") && getenv("ADAS_B200_FC_STREAM")[0] == '0');
-                if (transposed && e->conv_impl == 0 && fc_stream_on && ntaps == 1 && (size_t)N * Kc * 2 <= ((size_t)48 << 20) && Kc % 8 == 0 && ab.C % 8 == 0) {
+                if (transposed && e->conv_impl == 0 && fc_stream_on && ntaps == 1 && (size_t)N * Kc * 2 <= ((size_t)25 << 20) && Kc % 8 == 0 && ab.C % 8 == 0) {
                     const float* bias_p = static_cast<const float*>(tensor_ptr(e, bias_t));
                     void* out_p = static_cast<uint8_t*>(e->dbufs[out_buf].ptr) + (size_t)out_coff * elem_size(ob.dtype);
                     const int x_ld = (int)(ab.rows_per_img * ab.C), o_ld = (int)(ob.rows_per_img * ob.C), of32 = ob.dtype == 1 ? 1 : 0;
@@ -387,17 +272,6 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
                         gemm_v3_describe(opaque, d, sizeof(d));
                         prog->step_desc.resize(prog->step_type.size());
                         prog->step_desc.back() = d;
-                    }
-                    {
-                        GemmRec rec;
-                        rec.step = prog->steps.size();
-                        rec.g = g;
-                        gemm_v3_tile_of(opaque, &rec.g.BN, &rec.g.mt_hint);
-                        rec.a_buf = a_buf; rec.a_coff = a_coff; rec.out_buf = out_buf; rec.out_coff = out_coff; rec.res_buf = res_buf; rec.res_coff = res_coff;
-                        rec.eligible = !s2 && !transposed && ob.dtype == 0 && masked && (ntaps == 1 || ntaps == 9) && N % 64 == 0 && rec.g.BN % 64 == 0 &&
-                                       gemm_v3_is_staged(opaque);
-                        rec.prep = prep;
-                        recs.push_back(rec);
                     }
                     prog->steps.push_back([keep](cudaStream_t st) { return gemm_v3_run(keep.get(), st); });
                 } else {
@@ -484,7 +358,7 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
         }
     }
     prog->step_desc.resize(prog->steps.size());
-    return build_chains(e, prog, recs);
+    return 0;
 }
 
 // run the network for `batch` images already staged in buffer 0 (fp16 padded NHWC image)
@@ -759,8 +633,6 @@ int adas_engine_create(const char* plan_path, int device, int max_batch, int con
     e->device = device; e->max_batch = max_batch; e->conv_impl = conv_impl;
     const char* ng = getenv("ADAS_B200_NO_GRAPH");
     e->use_graph = !(ng && ng[0] == '1');
-    const char* ch = getenv("ADAS_B200_CHAIN");
-    e->use_chain = !ch ? 0 : ch[0] == '0' ? 0 : ch[0] == '1' ? 1 : 2;
     const char* at = getenv("ADAS_B200_AUTOTUNE");
     e->autotune = !(at && at[0] == '0');
     bool ok = fread(&e->hdr, sizeof(PlanHeader), 1, f) == 1 && memcmp(e->hdr.magic, kPlanMagic, 8) == 0 && e->hdr.version == kPlanVersion;
@@ -787,7 +659,7 @@ int adas_engine_create(const char* plan_path, int device, int max_batch, int con
     ADAS_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     ADAS_CUDA(cudaGetDeviceProperties(&prop, device));
-    ADAS_CHECK(prop.major == 10, "device %d is sm_%d%d; libadas_b200 is built for sm_100a only", device, prop.major, prop.minor);
+    ADAS_CHECK(prop.major == 9 && prop.minor == 0, "device %d is sm_%d%d; libadas_b200 is built for sm_90a (H100) only", device, prop.major, prop.minor);
     ADAS_CUDA(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
     ADAS_CUDA(cudaMalloc(&e->d_blob, blob.size() + 256));
     ADAS_CUDA(cudaMemcpy(e->d_blob, blob.data(), blob.size(), cudaMemcpyHostToDevice));
@@ -1408,7 +1280,7 @@ int adas_engine_time_ops(adas_engine* e, int batch, unsigned type_mask, int iter
         for (int r = 0; r < reps; ++r) {
             n = 0;
             for (size_t i = 0; i < pg.steps.size(); ++i)
-                if (pg.step_type[i] != 31 && (type_mask & (1u << pg.step_type[i]))) { if (pg.steps[i](e->stream)) return 1; ++n; }
+                if (type_mask & (1u << pg.step_type[i])) { if (pg.steps[i](e->stream)) return 1; ++n; }
         }
     }
     ADAS_CUDA(cudaEventRecord(b, e->stream));

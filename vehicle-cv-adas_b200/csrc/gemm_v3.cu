@@ -1,6 +1,5 @@
 // gemm_v3.cu -- the product GEMM / implicit-GEMM conv kernel: fused conv(+folded BN)+bias+SiLU/ReLU(+residual) and the FC layers as a
-// persistent, warp-specialised tcgen05 kernel (fp16 x fp16 -> fp32 in TMEM) with TMA-staged operands and a shared-memory staged,
-// TMA-stored epilogue.
+// persistent, warp-specialised Hopper kernel (wgmma, fp16 x fp16 -> fp32 in registers) with TMA-staged operands.
 //
 // Replaces: the opaque conv stacks ONNXRuntime/TensorRT execute behind coreEngine.py:150-157 (TensorRTEngine.engine_inference) /
 // :184-186 (OnnxEngine.engine_inference).
@@ -8,20 +7,15 @@
 // Tile: BM = 128 output rows (pixels of the padded NHWC grid) x MT sub-tiles x BN output channels x BK = 64 channels per k-block.
 // A 3x3 stride-1 conv runs 9 taps x (Cin/64) k-blocks, each A tile being the SAME 2-D activation matrix loaded at row offset
 // m0 + dy*(W+2) + dx (the zero halo of the padded layout supplies the conv padding, TMA's out-of-bounds zero fill covers the matrix
-// ends); "slab" mode loads one 136-row slab per (dy, k-block) and points the three dx MMAs at row offsets 0/1/2 inside it;
-// stride-2 convs read 4-D boxes with traversal stride 2.  K order is (dy, k-block, dx) in every mode and for every tile shape, so
-// results are bit-identical whatever tile is chosen and whatever the batch size.
+// ends); every tap's tile is its own TMA box, so each wgmma operand starts on a 1024-byte swizzle boundary.  Stride-2 convs read
+// 4-D boxes with traversal stride 2.  K order is (dy, k-block, dx) for every tile shape, so results are bit-identical whatever tile
+// is chosen and whatever the batch size.
 //
-// Warp roles (576 threads): warp 0 = TMA producer (one elected lane), warp 1 = TMEM allocator + MMA issuer (warp-uniform loop, one
-// elected lane issues), warps 2..17 = epilogue (four per TMEM lane quarter, 16-column batches).  Persistent: grid = min(tiles, SMs),
-// two TMEM accumulator stages so the epilogue of tile i overlaps the main loop of tile i+1.
-//
-// Epilogue: tcgen05.ld -> +bias -> activation -> (+residual) -> fp16 -> 128-row x 64-column staging tile in shared memory (128-byte
-// swizzle, conflict-free 16-byte st.shared) -> ONE cp.async.bulk.tensor store per chunk (SASS: UTMASTG) through a 2-D map (dense
-// outputs) or a 4-D interior map (padded feature maps: halo rows are never written and stay zero).  The residual tile arrives by TMA
-// load into the same staging buffers two chunks ahead.  Output-row / halo-mask arithmetic runs BEFORE the accumulator wait
-// (multiply-shift divisors); the TMEM stage is released right after the last tcgen05.ld of a tile.  fp32 / transposed (FC swap-AB) /
-// BN % 64 != 0 outputs use direct per-lane stores.
+// Warp roles (384 threads): warpgroup 0 = TMA producer (one elected thread; the group gives its registers up with setmaxnreg),
+// warpgroups 1 and 2 = consumers: each issues the wgmmas of 64 rows of every sub-tile (m64nBNk16, BN split into instructions of
+// 128/64/32/16 columns) and runs the epilogue of those rows straight from its accumulator registers: +bias -> activation ->
+// (+residual) -> fp16/fp32 stores of interior rows (the zero halo of padded outputs is never written).  Persistent: grid =
+// min(tiles, SMs); the producer runs ahead into the next tile while the consumers finish the epilogue of the current one.
 //
 // Function attributes and the SM count are per device (a process may hold engines on several GPUs).
 #include "common.h"
@@ -34,80 +28,49 @@
 
 namespace adas {
 
-template <bool kTmaStore>
+template <int BN>
 __global__ void __launch_bounds__(V3_THREADS, 1)
-conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmC,
-                    const __grid_constant__ CUtensorMap tmR, const GemmV3 g) {
+conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmV3 g) {
+    constexpr int MTX = V3_ACC_COLS / BN >= 4 ? 4 : V3_ACC_COLS / BN >= 1 ? V3_ACC_COLS / BN : 1;   // sub-tiles held in registers
     extern __shared__ uint8_t smem_raw[];
     __shared__ __align__(8) uint64_t full_bar[8];
     __shared__ __align__(8) uint64_t empty_bar[8];
-    __shared__ __align__(8) uint64_t tfull_bar[2];
-    __shared__ __align__(8) uint64_t tempty_bar[2];
-    __shared__ __align__(8) uint64_t res_bar[V3_STG_BUFS];      // residual tile of a chunk has landed in its staging buffer
-    __shared__ uint32_t tmem_holder;
-    __shared__ __align__(16) float s_bias[2][256];
 
     const GemmParams& p = g.p;
     const int warp_idx = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     const int stages = g.stages;
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const int taps_per_step = g.slab ? 3 : 1;
     const int BMT = BM * g.MT;
-    const int mt_cols = g.sub_cols;
-    const int acc_stride = g.MT * g.sub_cols;
-    const bool acc2 = g.acc_stages == 2;
 
-    if (warp_idx == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmB)) : "memory");
-        if (kTmaStore) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmC)) : "memory");
-        if (kTmaStore && g.res_tma) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmR)) : "memory");
-        for (int s = 0; s < V3_STG_BUFS; ++s) mbar_init(smem_u32(&res_bar[s]), 1);
         for (int s = 0; s < stages; ++s) {
             mbar_init(smem_u32(&full_bar[s]), 1);
-            mbar_init(smem_u32(&empty_bar[s]), 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(smem_u32(&tfull_bar[s]), 1);
-            mbar_init(smem_u32(&tempty_bar[s]), V3_EPI_WARPS);      // one arrive per epilogue warp
+            mbar_init(smem_u32(&empty_bar[s]), 4 * V3_CONSUMERS);     // one arrive per consumer warp
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     }
-    if (warp_idx == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_holder)), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = tmem_holder;
-    // ---- TMA producer pieces (warp 0, lane 0) ----
-    const uint32_t a_bytes = p.s2 ? (uint32_t)(p.s2_bw * p.s2_bh * BK * 2) : (uint32_t)(g.slab ? V3_SLAB_BYTES : A_STAGE_BYTES);
-    const uint32_t tx_bytes = (uint32_t)g.MT * a_bytes + (uint32_t)(taps_per_step * p.BN * BK * 2);
-    const int n_grp = g.slab ? 3 : p.ntaps;              // outer tap groups (slab: dy)
-    const bool dx_inner = (!g.slab && p.ntaps == 9);      // plain 9-tap order is (dy, k-block, dx) too
-    const int o_cnt = dx_inner ? 3 : n_grp;              // outer loop: dy (9-tap plain) or tap group
-    const int i_cnt = dx_inner ? 3 : 1;                  // inner loop: dx (9-tap plain)
+    // ---- TMA producer pieces (thread 0) ----
+    const uint32_t a_bytes = p.s2 ? (uint32_t)(p.s2_bw * p.s2_bh * BK * 2) : (uint32_t)A_STAGE_BYTES;
+    const uint32_t tx_bytes = (uint32_t)g.MT * a_bytes + (uint32_t)(BN * BK * 2);
+    const bool dx_inner = p.ntaps == 9;                   // 9-tap order is (dy, k-block, dx)
+    const int o_cnt = dx_inner ? 3 : p.ntaps;            // outer loop: dy (9 taps) or tap
+    const int i_cnt = dx_inner ? 3 : 1;                  // inner loop: dx (9 taps)
     const int per_img = p.s2_tw * p.s2_th;
-    // weight (B operand) tiles of one pipeline step
+    // weight (B operand) tile of one pipeline step
     auto load_b = [&](int grp, int kc, int n0, uint32_t stage, uint32_t fb) {
         const uint32_t b_dst = smem_base + stage * g.stage_bytes + g.MT * g.a_sub_bytes;
-        if (g.slab) {
-            for (int dx = 0; dx < 3; ++dx) tma_load_2d(b_dst + dx * g.b_bytes, &tmB, (grp * 3 + dx) * p.Kc + kc * BK, n0, fb);
-        } else {
-            tma_load_2d(b_dst, &tmB, grp * p.Kc + kc * BK, n0, fb);
-        }
+        tma_load_2d(b_dst, &tmB, grp * p.Kc + kc * BK, n0, fb);
     };
     // activation (A operand) tiles of one pipeline step
     auto load_a = [&](int grp, int kc, int m_t, uint32_t stage, uint32_t fb) {
         const uint32_t a_dst = smem_base + stage * g.stage_bytes;
         const int m0 = m_t * BMT;
-        if (g.slab) {
-            const int r0 = m0 + (grp - 1) * p.Wp - 1;
-            for (int mt = 0; mt < g.MT; ++mt) tma_load_2d(a_dst + mt * g.a_sub_bytes, &tmA, kc * BK, r0 + mt * BM, fb);
-        } else if (p.s2) {
+        if (p.s2) {
             // stride-2 conv: sub-tile = bw x bh output pixels of image b; input pixel of tap (dy,dx) is (2*yo+dy, 2*xo+dx)
             // in padded coordinates, fetched by one 4-D TMA box with traversal stride 2 in x and y
             const int dy = p.ntaps == 9 ? grp / 3 : 1, dx = p.ntaps == 9 ? grp % 3 : 1;
@@ -128,12 +91,11 @@ conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     // Programmatic dependent launch: everything above overlapped the tail of the previous kernel in the stream; its results may
     // only be touched after `griddepcontrol.wait`.  Weights do not depend on the previous kernel: the producer arms the first
     // pipeline stages and fetches their weight tiles BEFORE the wait, so only the activation tiles see the dependency.
-    const bool run = !(p.dbg & 64);
     int pre = 0;                                          // pipeline steps whose weight tiles were fetched ahead of the wait
-    if (warp_idx == 0 && lane == 0 && run && g.pdl && g.prefetch_w && !(p.dbg & 32) && (int)blockIdx.x < g.total_tiles) {
+    if (threadIdx.x == 0 && g.pdl && g.prefetch_w && (int)blockIdx.x < g.total_tiles) {
         const int steps_tile = o_cnt * p.kpt * i_cnt;
         pre = steps_tile < stages ? steps_tile : stages;
-        const int n0 = ((int)blockIdx.x % g.n_tiles) * p.BN;
+        const int n0 = ((int)blockIdx.x % g.n_tiles) * BN;
         for (int j = 0; j < pre; ++j) {
             const int in = j % i_cnt, kc = (j / i_cnt) % p.kpt, o = j / (i_cnt * p.kpt);
             const uint32_t fb = smem_u32(&full_bar[j]);
@@ -146,17 +108,15 @@ conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     }
 
-    if (!run) {
-        // DEBUG: launch skeleton only
-    } else if (warp_idx == 0) {
-        if (lane == 0) {
+    if (warp_idx < 4) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+        if (threadIdx.x == 0) {
             // ================= TMA producer =================
             uint32_t s = 0, ph = 0;
             int step = 0;                                        // steps issued by this CTA (only compared against `pre`)
             for (int w = blockIdx.x; w < g.total_tiles; w += gridDim.x) {
-                if (p.dbg & 32) break;                           // DEBUG: no loads at all
                 const int n_t = w % g.n_tiles, m_t = w / g.n_tiles;
-                const int n0 = n_t * p.BN;
+                const int n0 = n_t * BN;
                 for (int o = 0; o < o_cnt; ++o) {
                     for (int kc = 0; kc < p.kpt; ++kc) {
                         for (int in = 0; in < i_cnt; ++in) {
@@ -177,114 +137,63 @@ conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                 }
             }
         }
-    } else if (warp_idx == 1) {
-        // ================= MMA issuer =================
-        // The WHOLE warp walks the loop and waits on the barriers; one elected lane issues tcgen05.mma / commit (warp-uniform
-        // control flow keeps descriptors in uniform registers).
-        const uint32_t idesc = (1u << 4) | ((uint32_t)(p.BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-        const uint64_t desc_hi = ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-        const uint32_t a_step = (uint32_t)g.a_sub_bytes >> 4, b_step = (uint32_t)g.b_bytes >> 4;
-        const int n_dx = taps_per_step, n_mt = g.MT;
-        const int ksteps = (g.slab ? 3 : p.ntaps) * p.kpt;
-        const bool skip_mma = (p.dbg & 2) != 0, no_wait = (p.dbg & 32) != 0;
-        uint32_t s = 0, ph = 0, tile_it = 0;
-        for (int w = blockIdx.x; w < g.total_tiles; w += gridDim.x, ++tile_it) {
-            const int as = acc2 ? (int)(tile_it & 1) : 0;
-            mbar_wait(smem_u32(&tempty_bar[as]), ((acc2 ? (tile_it >> 1) : tile_it) & 1u) ^ 1u);     // epilogue drained this accumulator stage
-            tcgen05_fence_after();
-            const uint32_t d_base = tmem_base + (uint32_t)(as * acc_stride);
-            for (int ks = 0; ks < ksteps; ++ks) {
-                if (!no_wait) mbar_wait(smem_u32(&full_bar[s]), ph);
-                tcgen05_fence_after();
-                const uint32_t a_lo = ((smem_base + s * g.stage_bytes) & 0x3FFFFu) >> 4;      // 16-byte units
-                const uint32_t b_lo = a_lo + (uint32_t)n_mt * a_step;
-                if (elect_one()) {
-                    if (!skip_mma) {
-                        for (int dx = 0; dx < n_dx; ++dx) {
-                            for (int mt = 0; mt < n_mt; ++mt) {
-                                const uint32_t a_sub = a_lo + (uint32_t)mt * a_step + (g.slab ? (uint32_t)dx * 8u : 0u);   // +dx rows of 128 B
-                                const uint32_t b_sub = b_lo + (uint32_t)dx * b_step;
-                                const uint32_t d = d_base + (uint32_t)(mt * mt_cols);
+    } else {
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+        // ================= consumers (MMA + epilogue) =================
+        const int cw = (warp_idx - 4) >> 2;                 // consumer warpgroup: rows cw*64 .. cw*64+63 of every sub-tile
+        const int wq = warp_idx & 3;                        // warp of the group: 16 of those rows
+        const int ksteps = p.ntaps * p.kpt;
+        const size_t res_ld = (size_t)(p.res_ld < 0 ? -p.res_ld : p.res_ld);
+        float acc[MTX][BN / 2];
 #pragma unroll
-                                for (int k = 0; k < BK / 16; ++k) {
-                                    const uint64_t ad = desc_hi | (uint64_t)(a_sub + 2u * k);
-                                    const uint64_t bd = desc_hi | (uint64_t)(b_sub + 2u * k);
-                                    umma_f16(d, ad, bd, idesc, (uint32_t)((ks | dx | k) != 0));
-                                }
-                            }
-                        }
+        for (int mt = 0; mt < MTX; ++mt)
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) acc[mt][i] = 0.f;
+        uint32_t s = 0, ph = 0;
+        for (int w = blockIdx.x; w < g.total_tiles; w += gridDim.x) {
+            uint32_t prev = 0;
+            for (int ks = 0; ks < ksteps; ++ks) {
+                mbar_wait(smem_u32(&full_bar[s]), ph);
+                const uint32_t a_base = smem_base + s * g.stage_bytes + (uint32_t)cw * (64u * 128u);
+                const uint64_t bdesc = make_smem_desc(smem_base + s * g.stage_bytes + g.MT * g.a_sub_bytes);
+#pragma unroll
+                for (int mt = 0; mt < MTX; ++mt)
+#pragma unroll
+                    for (int i = 0; i < BN / 2; ++i) reg_fence(acc[mt][i]);
+                wgmma_fence();
+#pragma unroll
+                for (int mt = 0; mt < MTX; ++mt) {
+                    if (mt < g.MT) {
+                        const uint64_t adesc = make_smem_desc(a_base + (uint32_t)(mt * g.a_sub_bytes));
+#pragma unroll
+                        for (int k = 0; k < BK / 16; ++k)
+                            WgmmaCols<0, BN>::run(acc[mt], adesc + 2u * k, bdesc + 2u * k, (uint32_t)((ks | k) != 0));
                     }
-                    umma_commit(smem_u32(&empty_bar[s]));
                 }
-                __syncwarp();
+                wgmma_commit();
+                wgmma_wait<1>();                            // the wgmmas of the previous step are done: its stage can be refilled
+                if (ks > 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
+                prev = s;
                 if (++s == (uint32_t)stages) { s = 0; ph ^= 1u; }
             }
-            if (elect_one()) umma_commit(smem_u32(&tfull_bar[as]));
-            __syncwarp();
-        }
-    } else {
-        // ================= epilogue (16 warps) =================
-        // Warp (q, part): TMEM lane quarter q = warp_idx % 4 (rows q*32 .. q*32+31 of a sub-tile), `part` = which 16-column
-        // slice of a 64-column chunk.  Staged path: every chunk of a sub-tile is assembled in a swizzled staging buffer and
-        // leaves through one TMA store issued by thread `et == 0`.
-        const int ew = warp_idx - 2;
-        const int q = warp_idx & 3;
-        const int part = ew >> 2;
-        const int et = threadIdx.x - 64;
-        const int r = q * 32 + lane;                        // this thread's row inside a sub-tile
-        const bool issuer = (et == 0);
-        const uint32_t stg_base = smem_base + (uint32_t)g.stg_off;
-        const int n_chunks = kTmaStore ? (p.BN >> 6) : ((p.BN + 63) >> 6);
-        const size_t res_ld = (size_t)(p.res_ld < 0 ? -p.res_ld : p.res_ld);
-        const int per_img = p.s2_tw * p.s2_th;
-        const int act = (p.dbg & 8) ? 0 : p.act;
-        uint32_t tile_it = 0, chunk_it = 0;
-        // Residual through the staging buffers (staged path): chunk j lives in buffer j % 3 -- its residual tile is fetched by TMA two
-        // chunks ahead (the issuer walks a prefetch cursor over (tile, sub-tile, chunk), across tile boundaries), every thread adds the
-        // 32 bytes it is about to overwrite, and the finished chunk leaves through the TMA store.  Buffer reuse: R(j+2) targets the
-        // buffer store S(j-1) read; the issuer waits for S(j-1) (`wait_group.read 1` right after committing S(j)) before issuing it.
-        const bool res_tma = kTmaStore && g.res_tma;
-        const bool stg3 = g.stg_bufs == V3_STG_BUFS;        // always with a residual; otherwise whenever the third buffer costs no pipeline stage
-        auto buf_of = [&](uint32_t j) -> uint32_t { return stg3 ? j % V3_STG_BUFS : (j & 1u); };
-        int pf_w = blockIdx.x, pf_mt = 0, pf_cc = 0;
-        uint32_t pf_j = 0;
-        auto issue_res = [&]() {
-            if (pf_w >= g.total_tiles) return;
-            const int n_t2 = pf_w % g.n_tiles, m_t2 = pf_w / g.n_tiles;
-            const uint32_t bar = smem_u32(&res_bar[pf_j % V3_STG_BUFS]);
-            const uint32_t dst = stg_base + (pf_j % V3_STG_BUFS) * (uint32_t)V3_STG_BYTES;
-            if (p.s2) {
-                const int pi = m_t2 * g.MT + pf_mt;
-                const int b = fast_div(pi, g.fd_per_img);
-                const int rem = pi - b * per_img;
-                const int ty = fast_div(rem, g.fd_tw), tx = rem - ty * p.s2_tw;
-                mbar_expect_tx(bar, (uint32_t)(p.s2_bw * p.s2_bh * 128));
-                tma_load_4d(dst, &tmR, n_t2 * p.BN + pf_cc * 64, tx * p.s2_bw, ty * p.s2_bh, b, bar);     // out-of-range patches read zeros
-            } else {
-                mbar_expect_tx(bar, (uint32_t)V3_STG_BYTES);
-                tma_load_2d(dst, &tmR, n_t2 * p.BN + pf_cc * 64, m_t2 * BMT + pf_mt * BM, bar);
-            }
-            ++pf_j;
-            if (++pf_cc == n_chunks) { pf_cc = 0; if (++pf_mt == g.MT) { pf_mt = 0; pf_w += gridDim.x; } }
-        };
-        if (res_tma && issuer && !(p.dbg & 16)) { issue_res(); issue_res(); }
-        __syncwarp();
-        for (int w = blockIdx.x; w < g.total_tiles; w += gridDim.x, ++tile_it) {
-            const int as = acc2 ? (int)(tile_it & 1) : 0;
-            const int bs = (int)(tile_it & 1);
-            const int n_t = w % g.n_tiles, m_t = w / g.n_tiles;
-            const int n0 = n_t * p.BN;
-            const int m0 = m_t * BMT;
-            if (!p.transposed) {
-                for (int j = et; j < p.BN; j += 32 * V3_EPI_WARPS) s_bias[bs][j] = (p.bias != nullptr && (n0 + j) < p.N) ? __ldg(p.bias + n0 + j) : 0.f;
-            }
-            // output row of every sub-tile and its halo mask, computed while the main loop is still running
-            int row_of[4];
-            uint32_t okmask = 0;
+            wgmma_wait<0>();
 #pragma unroll
-            for (int mt = 0; mt < 4; ++mt) {
-                row_of[mt] = 0;
-                if (mt < g.MT) {
+            for (int mt = 0; mt < MTX; ++mt)
+#pragma unroll
+                for (int i = 0; i < BN / 2; ++i) reg_fence(acc[mt][i]);
+            if (lane == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
+
+            // ---- epilogue: thread holds rows r0 and r0 + 8 of each sub-tile, columns 8j + 2(lane%4) + {0,1} ----
+            const int n_t = w % g.n_tiles, m_t = w / g.n_tiles;
+            const int n0 = n_t * BN;
+            const int m0 = m_t * BMT;
+            const int c0 = 2 * (lane & 3);
+#pragma unroll
+            for (int mt = 0; mt < MTX; ++mt) {
+                if (mt >= g.MT) break;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int r = cw * 64 + wq * 16 + (lane >> 2) + 8 * h;      // row inside the sub-tile
                     int row = m0 + mt * BM + r;
                     bool ok = row < p.M;
                     if (p.s2) {
@@ -303,188 +212,59 @@ conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                         const int xx = pp - yy * Wp;
                         ok = (yy >= 1) && (yy <= p.mask_H) && (xx >= 1) && (xx <= p.mask_W);
                     }
-                    row_of[mt] = row;
-                    okmask |= ok ? (1u << mt) : 0u;
-                }
-            }
-            asm volatile("bar.sync 1, 512;" ::: "memory");          // bias slice staged
-            mbar_wait(smem_u32(&tfull_bar[as]), (acc2 ? (tile_it >> 1) : tile_it) & 1u);
-            tcgen05_fence_after();
-            for (int mt = 0; mt < g.MT; ++mt) {
-                const int row = mt == 0 ? row_of[0] : mt == 1 ? row_of[1] : mt == 2 ? row_of[2] : row_of[3];
-                const bool row_ok = (okmask >> mt) & 1u;
-                const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * acc_stride + mt * mt_cols);
-                float row_bias = 0.f;
-                if (p.transposed && p.bias != nullptr && row < p.M) row_bias = p.bias[row];
-                for (int cc = 0; cc < n_chunks; ++cc) {
-                    if (p.dbg & 16) break;
-                    const int c = cc * 64 + part * 16;                 // first tile column of this warp's slice
-                    const bool last_ld = (mt == g.MT - 1) && (cc == n_chunks - 1);
-                    const bool have = c < p.BN;                         // legacy path: BN need not be a multiple of 64
-                    uint32_t v[16];
-                    if (have) tmem_ld16(taddr + (uint32_t)c, v);
-                    const int n = n0 + c;
-                    const int ncols = have ? min(16, p.N - n) : 0;      // valid columns (multiple of 8 when not transposed; may be <= 0)
-                    uint4 rr[2];
-                    const bool has_res = (p.res != nullptr) && row_ok && !p.transposed && ncols > 0;
-                    if (res_tma) {
-                        // the residual tile of this chunk sits in the staging buffer the output will overwrite (same swizzled slots)
-                        mbar_wait(smem_u32(&res_bar[chunk_it % V3_STG_BUFS]), (chunk_it / V3_STG_BUFS) & 1u);
-                        const uint32_t rs = stg_base + (chunk_it % V3_STG_BUFS) * (uint32_t)V3_STG_BYTES + (uint32_t)r * 128u;
-                        const uint32_t sw = (uint32_t)(r & 7);
-                        asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(rr[0].x), "=r"(rr[0].y), "=r"(rr[0].z), "=r"(rr[0].w)
-                                     : "r"(rs + ((((uint32_t)(2 * part)) ^ sw) << 4)));
-                        asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(rr[1].x), "=r"(rr[1].y), "=r"(rr[1].z), "=r"(rr[1].w)
-                                     : "r"(rs + ((((uint32_t)(2 * part + 1)) ^ sw) << 4)));
-                    } else if (has_res) {
-                        const __half* rp = p.res + (size_t)row * res_ld + n;
+                    if (!ok) continue;
+                    if (p.transposed) {
+                        // swap-AB FC: rows are output features, columns are batch entries
+                        const float row_bias = p.bias != nullptr ? __ldg(p.bias + row) : 0.f;
 #pragma unroll
-                        for (int k = 0; k < 2; ++k)
-                            if (k * 8 < ncols) rr[k] = *reinterpret_cast<const uint4*>(rp + k * 8);
-                    }
-                    if (have) tmem_ld_wait();
-                    if (last_ld) {
-                        // every tcgen05.ld of this warp for this tile has completed: the accumulator stage can be refilled
-                        tcgen05_fence_before();
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive(smem_u32(&tempty_bar[as]));
-                    }
-                    float f[16];
-                    if (!p.transposed) {
-                        const float4* sb4 = reinterpret_cast<const float4*>(&s_bias[bs][c & 255]);
+                        for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            const float4 b4 = sb4[j];
-                            f[4 * j] = __uint_as_float(v[4 * j]) + b4.x; f[4 * j + 1] = __uint_as_float(v[4 * j + 1]) + b4.y;
-                            f[4 * j + 2] = __uint_as_float(v[4 * j + 2]) + b4.z; f[4 * j + 3] = __uint_as_float(v[4 * j + 3]) + b4.w;
-                        }
-                        if (has_res && p.res_ld < 0) {
-#pragma unroll
-                            for (int k = 0; k < 2; ++k)
-                                if (k * 8 < ncols) {
-                                    const __half2* h = reinterpret_cast<const __half2*>(&rr[k]);
-#pragma unroll
-                                    for (int j = 0; j < 4; ++j) { float2 tt = __half22float2(h[j]); f[k * 8 + 2 * j] += tt.x; f[k * 8 + 2 * j + 1] += tt.y; }
-                                }
-                        }
-                        if (act == 1) {
-                            if (p.dbg & 128) {                      // DEBUG: four-value SiLU of the round-1 kernel (numerics A/B)
-#pragma unroll
-                                for (int j = 0; j < 16; j += 4) silu4(f[j], f[j + 1], f[j + 2], f[j + 3]);
-                            } else {
-#pragma unroll
-                                for (int j = 0; j < 16; j += 2) silu2(f[j], f[j + 1]);
-                            }
-                        } else if (act == 2) {
-#pragma unroll
-                            for (int j = 0; j < 16; ++j) f[j] = fmaxf(f[j], 0.f);
-                        }
-                        if (has_res && p.res_ld > 0) {
-#pragma unroll
-                            for (int k = 0; k < 2; ++k)
-                                if (k * 8 < ncols) {
-                                    const __half2* h = reinterpret_cast<const __half2*>(&rr[k]);
-#pragma unroll
-                                    for (int j = 0; j < 4; ++j) { float2 tt = __half22float2(h[j]); f[k * 8 + 2 * j] += tt.x; f[k * 8 + 2 * j + 1] += tt.y; }
-                                }
-                        }
-                    }
-                    if constexpr (kTmaStore) {
-                        // ---- staged path: swizzled 16-byte stores into the staging tile, one TMA store per chunk ----
-                        uint32_t o[8];
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const __half2 h = __floats2half2_rn(f[2 * j], f[2 * j + 1]);
-                            o[j] = row_ok ? *reinterpret_cast<const uint32_t*>(&h) : 0u;      // halo / out-of-range rows are written as zeros
-                        }
-                        const uint32_t stg = stg_base + buf_of(chunk_it) * (uint32_t)V3_STG_BYTES + (uint32_t)r * 128u;
-                        const uint32_t sw = (uint32_t)(r & 7);
-                        st_shared_v4(stg + ((((uint32_t)(2 * part)) ^ sw) << 4), o[0], o[1], o[2], o[3]);
-                        st_shared_v4(stg + ((((uint32_t)(2 * part + 1)) ^ sw) << 4), o[4], o[5], o[6], o[7]);
-                        fence_async_smem();                 // generic-proxy writes -> visible to the TMA (async proxy)
-                        if (issuer) { if (stg3) bulk_wait_read1(); else bulk_wait_read0(); }        // see the protocol below
-                        __syncwarp();
-                        asm volatile("bar.sync 1, 512;" ::: "memory");
-                        // Protocol (3 buffers): chunk i fills buffer i % 3.  The issuer waits for all stores but the most recent
-                        // one before it arrives at barrier(i); after barrier(i) every thread therefore knows stores <= i-2 are done, and the
-                        // next write, into buffer (i+1) % 3 (last read by store i-2), is safe.  (2 buffers, no residual): the issuer waits for
-                        // ALL earlier stores, so after barrier(i) stores <= i-1 are done and buffer (i+1) & 1 may be rewritten.
-                        if (issuer && !(p.dbg & 4)) {
-                            const uint32_t src = stg_base + buf_of(chunk_it) * (uint32_t)V3_STG_BYTES;
-                            if (p.s2) {
-                                const int pi = m_t * g.MT + mt;
-                                if (pi < g.n_patches) {
-                                    const int b = pi / per_img;
-                                    const int rem = pi - b * per_img;
-                                    const int ty = rem / p.s2_tw, tx = rem - ty * p.s2_tw;
-                                    tma_store_4d(&tmC, src, n0 + cc * 64, tx * p.s2_bw, ty * p.s2_bh, b);
-                                }
-                            } else if (n0 + cc * 64 < p.N && m0 + mt * BM < p.M) {
-                                tma_store_2d(&tmC, src, n0 + cc * 64, m0 + mt * BM);
-                            }
-                            bulk_commit();
-                        }
-                        if (res_tma && issuer) {
-                            bulk_wait_read1();              // store (i-1) has left buffer (i+2) % 3 ...
-                            issue_res();                    // ... which now receives the residual tile of chunk i+2
-                        }
-                        __syncwarp();
-                        ++chunk_it;
-                    } else {
-                        // ---- direct path: fp32 heads, transposed FC outputs, tile widths that are not a multiple of 64 ----
-                        if (!p.transposed) {
-                            if (row_ok && ncols > 0 && !(p.dbg & 4)) {
-                                if (p.out_f32) {
-                                    float* op = reinterpret_cast<float*>(p.out) + (size_t)row * (size_t)p.out_ld + n;
-#pragma unroll
-                                    for (int k = 0; k < 4; ++k)
-                                        if (k * 4 < ncols) *reinterpret_cast<float4*>(op + k * 4) = make_float4(f[4 * k], f[4 * k + 1], f[4 * k + 2], f[4 * k + 3]);
-                                } else {
-                                    __half* op = reinterpret_cast<__half*>(p.out) + (size_t)row * (size_t)p.out_ld + n;
-                                    uint32_t o[8];
-#pragma unroll
-                                    for (int j = 0; j < 8; ++j) {
-                                        const __half2 h = __floats2half2_rn(f[2 * j], f[2 * j + 1]);
-                                        o[j] = *reinterpret_cast<const uint32_t*>(&h);
-                                    }
-                                    *reinterpret_cast<uint4*>(op) = make_uint4(o[0], o[1], o[2], o[3]);
-                                    if (ncols > 8) *reinterpret_cast<uint4*>(op + 8) = make_uint4(o[4], o[5], o[6], o[7]);
-                                }
-                            }
-                        } else if (row_ok && have) {
-                            // swap-AB FC: rows are output features, columns are batch entries
-#pragma unroll
-                            for (int j = 0; j < 16; ++j) {
-                                const int col = n + j;
+                            for (int e = 0; e < 2; ++e) {
+                                const int col = n0 + 8 * j + c0 + e;
                                 if (col < p.N) {
-                                    const float x = act_apply(__uint_as_float(v[j]) + row_bias, p.act);
+                                    const float x = act_apply(acc[mt][4 * j + 2 * h + e] + row_bias, p.act);
                                     if (p.out_f32) reinterpret_cast<float*>(p.out)[(size_t)col * (size_t)p.out_ld + row] = x;
                                     else reinterpret_cast<__half*>(p.out)[(size_t)col * (size_t)p.out_ld + row] = __float2half_rn(x);
                                 }
                             }
                         }
+                        continue;
+                    }
+                    const __half* rp = p.res != nullptr ? p.res + (size_t)row * res_ld : nullptr;
+#pragma unroll
+                    for (int j = 0; j < BN / 8; ++j) {
+                        const int n = n0 + 8 * j + c0;
+                        if (n0 + 8 * j >= p.N) break;                  // N % 8 == 0: an 8-column group is all in or all out
+                        float x0 = acc[mt][4 * j + 2 * h], x1 = acc[mt][4 * j + 2 * h + 1];
+                        if (p.bias != nullptr) { x0 += __ldg(p.bias + n); x1 += __ldg(p.bias + n + 1); }
+                        float2 rv = make_float2(0.f, 0.f);
+                        if (rp != nullptr) rv = __half22float2(*reinterpret_cast<const __half2*>(rp + n));
+                        if (p.res_ld < 0) { x0 += rv.x; x1 += rv.y; }
+                        if (p.act == 1) silu2(x0, x1);
+                        else if (p.act == 2) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+                        if (p.res_ld > 0) { x0 += rv.x; x1 += rv.y; }
+                        if (p.out_f32) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + (size_t)row * (size_t)p.out_ld + n) = make_float2(x0, x1);
+                        else *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.out) + (size_t)row * (size_t)p.out_ld + n) = __floats2half2_rn(x0, x1);
                     }
                 }
             }
-            if (p.dbg & 16) {
-                // DEBUG (no epilogue): the accumulator stage still has to be handed back
-                tcgen05_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(smem_u32(&tempty_bar[as]));
-            }
         }
-        if (kTmaStore && issuer) bulk_wait_all();       // all output tiles have left shared memory and are performed
-    }
-
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp_idx == 1) {
-        __syncwarp();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
     }
 }
 
 // ---- host side ---------------------------------------------------------------------------------------------------------
+// BN is a template parameter (the accumulator array and the wgmma widths are static): every multiple of 16 up to 256.
+#define V3_FOR_EACH_BN(X) X(16) X(32) X(48) X(64) X(80) X(96) X(112) X(128) X(144) X(160) X(176) X(192) X(208) X(224) X(240) X(256)
+
+static const void* v3_kernel(int BN) {
+    switch (BN) {
+#define V3_CASE(b) case b: return reinterpret_cast<const void*>(&conv_gemm_v3_kernel<b>);
+        V3_FOR_EACH_BN(V3_CASE)
+#undef V3_CASE
+        default: return nullptr;
+    }
+}
+
 struct V3Device { bool attr_set = false; int num_sms = 0; };
 static std::mutex g_v3_mu;
 static V3Device g_v3_dev[64];
@@ -497,8 +277,7 @@ static int v3_device_state(int* num_sms) {
     V3Device& d = g_v3_dev[dev];
     if (!d.attr_set) {
         // function attributes are per device: set them once for every device an engine runs on
-        ADAS_CUDA(cudaFuncSetAttribute(conv_gemm_v3_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, V3_DYN_SMEM_MAX));
-        ADAS_CUDA(cudaFuncSetAttribute(conv_gemm_v3_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, V3_DYN_SMEM_MAX));
+        for (int bn = 16; bn <= 256; bn += 16) ADAS_CUDA(cudaFuncSetAttribute(v3_kernel(bn), cudaFuncAttributeMaxDynamicSharedMemorySize, V3_DYN_SMEM_MAX));
         ADAS_CUDA(cudaDeviceGetAttribute(&d.num_sms, cudaDevAttrMultiProcessorCount, dev));
         d.attr_set = true;
     }
@@ -529,45 +308,26 @@ static int env_int(const char* name, int dflt) {
 
 int gemm_v3_config(const GemmParams& p_in, GemmV3* g) {
     GemmParams p = p_in;
-    static const int force_bn = env_int("ADAS_B200_BN", 0), force_mt = env_int("ADAS_B200_MT", 0), dbg = env_int("ADAS_B200_DBG", 0);
-    static const int no_tma_st = env_int("ADAS_B200_NO_TMA_STORE", 0), no_slab = env_int("ADAS_B200_NOSLAB", 0);
+    static const int force_bn = env_int("ADAS_B200_BN", 0), force_mt = env_int("ADAS_B200_MT", 0);
     if (force_bn >= 16 && force_bn <= 256 && force_bn % 16 == 0 && force_bn <= ((p.N + 15) / 16) * 16 && !p.transposed) p.BN = force_bn;   // test hook
+    if (p.BN % 16 != 0 || p.BN < 16 || p.BN > 256) return 1;
     g->p = p;
-    g->p.dbg = dbg;
-    g->sub_cols = p.BN <= 32 ? 32 : p.BN <= 64 ? 64 : p.BN <= 128 ? 128 : 256;
     g->MT = p.mt_hint >= 1 ? p.mt_hint : ((p.BN <= 128) ? 2 : 1);
-    if (force_mt >= 1 && force_mt <= 4 && force_mt * g->sub_cols <= 512) g->MT = force_mt;     // test hook: exercise every sub-tile count
-    if (g->MT > 4 || g->MT * g->sub_cols > 512) return 1;
-    g->acc_stages = (2 * g->MT * g->sub_cols <= 512) ? 2 : 1;
-    g->tma_st = (!no_tma_st && !p.out_f32 && !p.transposed && p.BN % 64 == 0 && p.N >= 64 && p.N % 8 == 0 && p.out_ld % 8 == 0 &&
-                 (reinterpret_cast<uintptr_t>(p.out) & 15u) == 0) ? 1 : 0;
+    if (force_mt >= 1 && force_mt <= 4) g->MT = force_mt;     // test hook: exercise every sub-tile count
+    if (g->MT > 4) return 1;
+    // the accumulators of a CTA tile live in registers (MT * BN / 2 per consumer thread): a taller tile than fits runs as the
+    // tallest one that does -- results do not depend on the tile shape
+    const int mt_max = V3_ACC_COLS / p.BN < 4 ? V3_ACC_COLS / p.BN : 4;
+    if (g->MT > mt_max) g->MT = mt_max;
     const int b_bytes = ((p.BN * BK * 2) + 1023) & ~1023;
     g->b_bytes = b_bytes;
-    static const int no_res_tma = env_int("ADAS_B200_NO_RES_TMA", 0);
-    g->res_tma = (g->tma_st && p.res != nullptr && !no_res_tma && (reinterpret_cast<uintptr_t>(p.res) & 15u) == 0 &&
-                  (p.res_ld < 0 ? -p.res_ld : p.res_ld) % 8 == 0) ? 1 : 0;
-    // staging buffers: three with a residual (its prefetch protocol needs them) and in chain launches; otherwise three only where the
-    // third one does not cost an operand pipeline stage (decided below), else two
-    static const int force_stg2 = env_int("ADAS_B200_STG2", 0);
-    g->stg_bufs = (g->res_tma || p.chain) ? V3_STG_BUFS : 2;
-    int budget = V3_DYN_SMEM_MAX - 1024 - (g->tma_st ? g->stg_bufs * V3_STG_BYTES : 0);
-    g->slab = 0;
-    if (p.ntaps == 9 && !p.s2 && !no_slab) {
-        const int slab_stage = g->MT * V3_SLAB_BYTES + 3 * b_bytes;
-        if (2 * slab_stage <= budget) g->slab = 1;
-    }
-    g->a_sub_bytes = g->slab ? V3_SLAB_BYTES : A_STAGE_BYTES;
-    g->stage_bytes = g->MT * g->a_sub_bytes + (g->slab ? 3 : 1) * b_bytes;
-    int stages = budget / g->stage_bytes;
+    g->a_sub_bytes = A_STAGE_BYTES;
+    g->stage_bytes = g->MT * g->a_sub_bytes + b_bytes;
+    int stages = (V3_DYN_SMEM_MAX - 1024) / g->stage_bytes;
     if (stages > 8) stages = 8;
     if (stages < 2) return 1;
-    if (g->tma_st && g->stg_bufs == 2 && !force_stg2) {
-        const int s3 = (budget - V3_STG_BYTES) / g->stage_bytes;
-        if ((s3 > 8 ? 8 : s3) == stages) g->stg_bufs = V3_STG_BUFS;
-    }
     g->stages = stages;
     g->p.stages = stages;
-    g->stg_off = stages * g->stage_bytes;          // stage_bytes is a multiple of 1024
     const int BMT = BM * g->MT;
     g->n_tiles = (p.N + p.BN - 1) / p.BN;
     g->m_tiles = (p.M + BMT - 1) / BMT;
@@ -584,7 +344,7 @@ int gemm_v3_config(const GemmParams& p_in, GemmV3* g) {
     return 0;
 }
 
-static int v3_smem_bytes(const GemmV3& g) { return g.stages * g.stage_bytes + (g.tma_st ? g.stg_bufs * V3_STG_BYTES : 0) + 1024; }
+static int v3_smem_bytes(const GemmV3& g) { return g.stages * g.stage_bytes + 1024; }
 
 int gemm_v3_launch(const GemmV3Launch& L, cudaStream_t st) {
     int num_sms = 0;
@@ -592,6 +352,8 @@ int gemm_v3_launch(const GemmV3Launch& L, cudaStream_t st) {
     static const int pdl = env_int("ADAS_B200_PDL", 1);
     GemmV3 gp = L.g;
     gp.pdl = pdl ? 1 : 0;
+    const void* fn = v3_kernel(gp.p.BN);
+    ADAS_CHECK(fn != nullptr, "gemm_v3: no kernel for BN %d", gp.p.BN);
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(gp.total_tiles < num_sms ? gp.total_tiles : num_sms, 1, 1);
     cfg.blockDim = dim3(V3_THREADS, 1, 1);
@@ -602,16 +364,19 @@ int gemm_v3_launch(const GemmV3Launch& L, cudaStream_t st) {
     attr1.val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = &attr1;
     cfg.numAttrs = pdl ? 1 : 0;
-    if (gp.tma_st) ADAS_CUDA(cudaLaunchKernelEx(&cfg, conv_gemm_v3_kernel<true>, L.tmA, L.tmB, L.tmC, L.tmR, gp));
-    else ADAS_CUDA(cudaLaunchKernelEx(&cfg, conv_gemm_v3_kernel<false>, L.tmA, L.tmB, L.tmC, L.tmR, gp));
+    CUtensorMap tmA = L.tmA, tmB = L.tmB;
+    void* args[] = {&tmA, &tmB, &gp};
+    ADAS_CUDA(cudaLaunchKernelExC(&cfg, fn, args));
     count_launch();
     return 0;
 }
 
-// Tile candidates ranked by a cost model (the engine times the best few on the device once per (op, batch)).  Measured on B200
-// (profiles/r02_probe1_*): L2 -> SM operand delivery sustains ~10 TB/s chip-wide (~36 B/clk/SM at 1.9 GHz), 128x64x16 MMAs run
-// at ~2/3 rate (A re-read from shared memory), a launch costs ~1.8 us of skeleton, and single-tile CTAs expose their epilogue.
+// Tile candidates ranked by a rough cost model (the engine times the best few on the device once per (op, batch)): operand bytes
+// delivered from L2 at ~32 B/clk/SM, wgmma time, an epilogue that does not overlap the main loop of the same CTA, waves of tiles
+// over the SMs and a fixed launch cost.
 int gemm_v3_candidates(const GemmParams& base, int max_out, int* BN_out, int* mt_out) {
+    int num_sms = 132;
+    if (v3_num_sms(&num_sms)) return 0;
     const int cand[] = {256, 192, 128, 64, 160, 96, 80, 48, 32, 16};
     struct C { double t; int BN, mt; } list[64];
     int n = 0;
@@ -632,16 +397,16 @@ int gemm_v3_candidates(const GemmParams& base, int max_out, int* BN_out, int* mt
             p.BN = BN; p.mt_hint = mt;
             GemmV3 g;
             if (gemm_v3_config(p, &g)) continue;
-            if (g.p.BN != BN || g.MT != mt) continue;            // forced by a test hook
+            if (g.p.BN != BN || g.MT != mt) continue;            // clamped, or forced by a test hook
             const double tiles = (double)g.total_tiles;
-            const double ksteps = (g.slab ? 3.0 : (double)ntaps) * kpt;
-            const double bytes = ksteps * (g.MT * (double)g.a_sub_bytes + (g.slab ? 3 : 1) * BN * 128.0);
-            const double rate = BN >= 128 ? 1.0 : BN >= 96 ? 0.85 : 0.66;         // small-N MMAs are bound by the A re-read
-            const double mma = (double)g.MT * ntaps * kpt * 2.0 * BN / rate;
+            const double ksteps = (double)ntaps * kpt;
+            const double bytes = ksteps * (g.MT * (double)g.a_sub_bytes + BN * 128.0);
+            const double rate = BN >= 64 ? 1.0 : 0.7;                              // narrow wgmmas are bound by the A re-read
+            const double mma = (double)g.MT * ntaps * kpt * 4.0 * BN / rate;
             const double epi = (double)g.MT * 128.0 * BN * 0.12;
-            const double per_tile = (g.acc_stages == 2 ? fmax(fmax(bytes / 36.0, mma), epi) : fmax(bytes / 36.0, mma) + 0.5 * epi) + 400.0;
-            const double waves = ceil(tiles / 148.0);
-            const double t = waves * per_tile + epi + 3500.0;
+            const double per_tile = fmax(bytes / 32.0, mma) + epi + 400.0;
+            const double waves = ceil(tiles / (double)num_sms);
+            const double t = waves * per_tile + 3500.0;
             if (n < 64) { list[n].t = t; list[n].BN = BN; list[n].mt = mt; ++n; }
         }
     }
@@ -652,8 +417,6 @@ int gemm_v3_candidates(const GemmParams& base, int max_out, int* BN_out, int* mt
     return n;
 }
 
-static int make_tmap_out(CUtensorMap* tm, const GemmV3& g, const void* base, int ld);
-
 int gemm_v3_prepare(const GemmParams& p, const void* a_base, uint64_t a_inner, uint64_t a_rows, uint64_t a_stride_bytes,
                     const void* b_base, uint64_t b_inner, uint64_t b_rows, uint64_t b_stride_bytes, void** opaque) {
     ADAS_CHECK(p.BN % 16 == 0 && p.BN >= 16 && p.BN <= 256, "gemm_v3: bad BN %d", p.BN);
@@ -661,15 +424,11 @@ int gemm_v3_prepare(const GemmParams& p, const void* a_base, uint64_t a_inner, u
     ADAS_CHECK(!p.s2, "gemm_v3_prepare: stride-2 ops go through gemm_v3_prepare_s2");
     GemmV3Launch* L = new GemmV3Launch();
     if (gemm_v3_config(p, &L->g)) { delete L; ADAS_CHECK(false, "gemm_v3: tile does not fit (BN %d, mt %d)", p.BN, p.mt_hint); }
-    const uint32_t a_box_rows = L->g.slab ? V3_SLAB_ROWS : BM;
-    if (make_tmap_2d(&L->tmA, a_base, a_inner, a_rows, a_stride_bytes, 64, a_box_rows) ||
+    if (make_tmap_2d(&L->tmA, a_base, a_inner, a_rows, a_stride_bytes, 64, BM) ||
         make_tmap_2d(&L->tmB, b_base, b_inner, b_rows, b_stride_bytes, 64, (uint32_t)L->g.p.BN)) {
         delete L;
         return 1;
     }
-    L->tmC = L->tmA; L->tmR = L->tmA;
-    if (L->g.tma_st && make_tmap_out(&L->tmC, L->g, L->g.p.out, L->g.p.out_ld)) { delete L; return 1; }
-    if (L->g.res_tma && make_tmap_out(&L->tmR, L->g, L->g.p.res, L->g.p.res_ld < 0 ? -L->g.p.res_ld : L->g.p.res_ld)) { delete L; return 1; }
     *opaque = L;
     return 0;
 }
@@ -684,42 +443,17 @@ int gemm_v3_prepare_s2(const GemmParams& p, const void* a_base, uint64_t a_C, ui
         delete L;
         return 1;
     }
-    L->tmC = L->tmA; L->tmR = L->tmA;
-    if (L->g.tma_st && make_tmap_out(&L->tmC, L->g, L->g.p.out, L->g.p.out_ld)) { delete L; return 1; }
-    if (L->g.res_tma && make_tmap_out(&L->tmR, L->g, L->g.p.res, L->g.p.res_ld < 0 ? -L->g.p.res_ld : L->g.p.res_ld)) { delete L; return 1; }
     *opaque = L;
     return 0;
 }
 
-// Output tensor map of the staged epilogue.  Stride-1 / dense ops: the [M, N] slice of the output matrix, box 64 columns x 128
-// rows.  Stride-2 ops: the INTERIOR of the padded output grid as a 4-D tensor [N, Wo, Ho, B], box 64 x bw x bh x 1, so partial
-// patches at the right / bottom edge are clipped by the TMA unit and the halo is never touched.
-static int make_tmap_out(CUtensorMap* tm, const GemmV3& g, const void* base_ptr, int ld) {
-    const GemmParams& p = g.p;
-    if (!p.s2) return make_tmap_2d(tm, base_ptr, (uint64_t)p.N, (uint64_t)p.M, (uint64_t)ld * 2, 64, BM);
-    const uint64_t Wpo = (uint64_t)p.s2_Wo + 2, Hpo = (uint64_t)p.s2_Ho + 2;
-    const __half* base = reinterpret_cast<const __half*>(base_ptr) + (Wpo + 1) * (uint64_t)ld;
-    const uint64_t B = (uint64_t)(g.n_patches / (p.s2_tw * p.s2_th));
-    return make_tmap_4d(tm, base, (uint64_t)p.N, (uint64_t)p.s2_Wo, (uint64_t)p.s2_Ho, B, (uint64_t)ld, Wpo, Hpo, 64, (uint32_t)p.s2_bw,
-                        (uint32_t)p.s2_bh);
-}
-
 int gemm_v3_run(void* opaque, cudaStream_t st) { return gemm_v3_launch(*static_cast<GemmV3Launch*>(opaque), st); }
 void gemm_v3_free(void* opaque) { delete static_cast<GemmV3Launch*>(opaque); }
-int gemm_v3_grid(const void* opaque) {
-    const int n = static_cast<const GemmV3Launch*>(opaque)->g.total_tiles;
-    return n < 148 ? n : 148;
-}
-void gemm_v3_tile_of(const void* opaque, int* BN, int* MT) {
-    const GemmV3& g = static_cast<const GemmV3Launch*>(opaque)->g;
-    *BN = g.p.BN; *MT = g.MT;
-}
-bool gemm_v3_is_staged(const void* opaque) { return static_cast<const GemmV3Launch*>(opaque)->g.tma_st != 0; }
 void gemm_v3_describe(const void* opaque, char* out, int cap) {
     const GemmV3& g = static_cast<const GemmV3Launch*>(opaque)->g;
-    snprintf(out, (size_t)cap, "M=%d N=%d K=%d taps=%d act=%d res=%d f32=%d s2=%d tr=%d | v3 BN=%d MT=%d slab=%d stages=%d acc=%d tiles=%d tma_st=%d res_tma=%d stg=%d", g.p.M,
+    snprintf(out, (size_t)cap, "M=%d N=%d K=%d taps=%d act=%d res=%d f32=%d s2=%d tr=%d | v3 BN=%d MT=%d stages=%d tiles=%d", g.p.M,
              g.p.N, g.p.Kc * g.p.ntaps, g.p.ntaps, g.p.act, g.p.res ? (g.p.res_ld < 0 ? -1 : 1) : 0, g.p.out_f32, g.p.s2, g.p.transposed, g.p.BN, g.MT,
-             g.slab, g.stages, g.acc_stages, g.total_tiles, g.tma_st, g.res_tma, g.tma_st ? g.stg_bufs : 0);
+             g.stages, g.total_tiles);
 }
 
 }  // namespace adas

@@ -1,31 +1,20 @@
-// gemm_v3.h -- tile configuration / launch record of the product GEMM kernel, shared by gemm_v3.cu (one layer per launch) and
-// gemm_chain.cu (a chain of same-shape layers per launch).
+// gemm_v3.h -- tile configuration / launch record of the product GEMM kernel (gemm_v3.cu).
 #pragma once
 #include "common.h"
 #include "tc_common.cuh"
 
 namespace adas {
 
-static constexpr int V3_EPI_WARPS = 16;
-static constexpr int V3_THREADS = 64 + 32 * V3_EPI_WARPS;     // 576
-static constexpr int V3_SLAB_ROWS = 136;
-static constexpr int V3_SLAB_BYTES = V3_SLAB_ROWS * BK * 2;   // 17408
-static constexpr int V3_STG_BYTES = BM * 64 * 2;              // one staging buffer: 128 rows x 64 fp16 columns
-static constexpr int V3_STG_BUFS = 3;                          // rotating staging buffers (residual in -> output out)
-static constexpr int V3_DYN_SMEM_MAX = 227 * 1024 - 3072;
+static constexpr int V3_CONSUMERS = 2;                         // consumer warpgroups: rows 0..63 / 64..127 of every 128-row sub-tile
+static constexpr int V3_THREADS = 128 * (1 + V3_CONSUMERS);     // 384: one producer warpgroup (one TMA thread) + the consumers
+static constexpr int V3_ACC_COLS = 256;                         // MT * BN <= 256: MT * BN / 2 fp32 accumulator registers per thread
+static constexpr int V3_DYN_SMEM_MAX = 227 * 1024 - 1024;
 
 struct GemmV3 {
     GemmParams p;
     int MT;            // 1..4 sub-tiles of 128 rows (stride-2: output patches) per CTA tile; they share every weight tile
-    int sub_cols;      // TMEM columns per sub-tile accumulator
-    int acc_stages;    // 2 when two accumulator sets fit in 512 TMEM columns
-    int slab;          // 3x3 stride-1: one 136-row activation slab per (dy, k-block) feeds the three dx taps
     int a_sub_bytes, b_bytes, stage_bytes, stages;
     int n_tiles, m_tiles, total_tiles;
-    int tma_st;        // staged TMA-store epilogue (fp16, not transposed, BN % 64 == 0)
-    int stg_bufs;      // staging buffers of that epilogue: 3 (one store may still be reading while the next chunk is written) or 2
-    int res_tma;       // staged epilogue only: the residual tile of every chunk is fetched by TMA into the staging buffer
-    int stg_off;       // byte offset of the two staging buffers behind the operand ring
     int pdl;
     int prefetch_w;    // fetch the first stages' weight tiles before griddepcontrol.wait
     int n_patches;     // stride-2: batch * s2_tw * s2_th
@@ -33,7 +22,7 @@ struct GemmV3 {
 };
 
 struct GemmV3Launch {
-    CUtensorMap tmA, tmB, tmC, tmR;
+    CUtensorMap tmA, tmB;
     GemmV3 g;
 };
 

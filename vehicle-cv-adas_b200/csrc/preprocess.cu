@@ -168,7 +168,7 @@ int launch_yolo_pre(const uint8_t* frames, int B, const LetterboxGeom& g, __half
     if (get_resize_tab(g.src_w, g.src_h, g.new_w, g.new_h, &t)) return 1;
     const long long total = (long long)B * g.in_h * g.in_w;
     int blocks = (int)((total + 255) / 256);
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     yolo_pre_kernel<<<blocks, 256, 0, st>>>(frames, B, g, t, img_padded, img_ld, blob_nchw);
     count_launch();
     ADAS_CUDA(cudaGetLastError());
@@ -214,7 +214,7 @@ int launch_ufld_pre(const uint8_t* frames, int B, int H, int W, int in_h, int in
     ADAS_CHECK(resize_h >= in_h, "ufld_pre: resized height %d smaller than network height %d", resize_h, in_h);
     const long long total = (long long)B * in_h * in_w;
     int blocks = (int)((total + 255) / 256);
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     ufld_pre_kernel<<<blocks, 256, 0, st>>>(frames, B, H, W, in_h, in_w, resize_h - in_h, t, lut, img_padded, img_ld,
                                             blob_nchw);
     count_launch();

@@ -4,8 +4,8 @@
 // (R, G, B, 0) per pixel, so the k pixels one output needs from one input row are k*4 CONTIGUOUS halves.  The reduction index is laid
 // out as  K = k rows x KR,  KR = round_up(4k, 16):  element [dy][dx*4 + c]  (zero weights in the padding), which makes every
 // 16-wide k-step of a warp-level mma.m16n8k16 a run of consecutive bytes of one image row -- no gather, no patch matrix in memory.
-// The stem has 3 input channels: tcgen05's 64-channel k-blocks would be > 50 % zeros (the round-1 route ran it at 54 TFLOP/s behind
-// a 58 us im2col pass), and the layer is bound by writing its 64-channel output anyway.
+// The stem has 3 input channels: the GEMM kernel's 64-channel k-blocks would be > 50 % zeros behind an im2col pass, and the layer
+// is bound by writing its 64-channel output anyway.
 //
 // One warp owns 16 consecutive output pixels of one output row (the M of m16n8k16) and all Cout channels (NT n-tiles of 8):
 //   k-slot permutation: a thread of the warp MMA holds k-slots {2t, 2t+1, 2t+8, 2t+9} of a 16-wide step.  Mapping those four slots to
@@ -142,7 +142,7 @@ int launch_stem_conv_s2(const __half* img, int B, int H, int W, const __half* wq
     const int smem = Cout * p.w_ld * 2 + STEM_WARPS * 16 * STEM_STG_LD * 2;
     ADAS_CHECK(smem <= 48 * 1024, "stem_conv: %d bytes of shared memory", smem);
     int blocks = (p.total_tiles + STEM_WARPS - 1) / STEM_WARPS;
-    int n_sms = 148;
+    int n_sms = 132;
     if (v3_num_sms(&n_sms)) return 1;
     const int cap = n_sms * 3;                      // resident blocks only: the weight copy is per block, a warp walks ~20 tiles
     if (blocks > cap) blocks = cap;

@@ -1,4 +1,4 @@
-// tc_common.cuh -- device helpers shared by the tcgen05 GEMM kernels (mbarrier, TMA, UMMA descriptors, TMEM loads).
+// tc_common.cuh -- device helpers of the Hopper GEMM kernel (mbarrier, TMA, wgmma descriptors and instructions, epilogue math).
 #pragma once
 #include "common.h"
 
@@ -7,7 +7,6 @@ namespace adas {
 static constexpr int BM = 128;
 static constexpr int BK = 64;                       // fp16 elements per k-block = 128 bytes = one swizzle row
 static constexpr int A_STAGE_BYTES = BM * BK * 2;   // 16 KiB
-static constexpr int NUM_THREADS = 192;
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -33,6 +32,9 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     while (!mbar_try_wait(bar, parity)) {
     }
 }
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
 __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const CUtensorMap* tm, int c0, int c1, uint32_t bar) {
     asm volatile(
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
@@ -45,85 +47,71 @@ __device__ __forceinline__ void tma_load_4d(uint32_t smem_dst, const CUtensorMap
         ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar)
         : "memory");
 }
-__device__ __forceinline__ void tma_load_2d_mc(uint32_t smem_dst, const CUtensorMap* tm, int c0, int c1, uint32_t bar, uint16_t mask) {
-    // multicast: the box lands at the same shared-memory offset (and signals the same barrier offset) in every CTA of `mask`
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%2, %3}], [%4], %5;"
-        ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(c0), "r"(c1), "r"(bar), "h"(mask)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit_mc(uint32_t bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask) : "memory");
-}
-// ---- cta_group::2 (CTA pair) variants: one MMA spans both SMs of the pair (M = 256), each CTA stages its own 128 rows of
-// A and HALF of the weight tile; only the leader CTA (cluster rank 0) issues MMAs and commits.
-__device__ __forceinline__ uint32_t mapa_rank(uint32_t local_addr, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(rank));
-    return r;
-}
-__device__ __forceinline__ void tma_load_2d_pair(uint32_t smem_dst, const CUtensorMap* tm, int c0, int c1, uint32_t leader_bar) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-        ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(c0), "r"(c1), "r"(leader_bar)
-        : "memory");
-}
-__device__ __forceinline__ void umma_f16_pair(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit_pair(uint32_t bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
 
-// K-major, 128B-swizzled operand tile: rows of 128 bytes, 8-row groups 1024 bytes apart.
+// ---- wgmma (sm_90a warpgroup MMA, fp16 x fp16 -> fp32 in registers) ------------------------------------------------------
+// Shared-memory matrix descriptor of a K-major, 128B-swizzled operand tile as TMA writes it: rows of 128 bytes, 8-row groups
+// 1024 bytes apart.  The tile must start on a 1024-byte boundary (base offset 0); a k-step of 16 elements advances the start by 32 bytes.
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);   // start address, 16-byte units
     d |= (uint64_t)1 << 16;                         // leading byte offset (unused for swizzled K-major)
     d |= (uint64_t)(1024 >> 4) << 32;               // stride byte offset: 8 rows * 128 B
-    d |= (uint64_t)1 << 46;                         // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;                         // layout: SWIZZLE_128B
+    d |= (uint64_t)1 << 62;                         // layout: SWIZZLE_128B
     return d;
 }
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across a wgmma.wait_group
+__device__ __forceinline__ void reg_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, both operands K-major in shared memory; acc = 0 overwrites D.
+template <int N>
+__device__ __forceinline__ void wgmma_n(float* d, uint64_t ad, uint64_t bd, uint32_t acc);
+template <> __device__ __forceinline__ void wgmma_n<16>(float* d, uint64_t ad, uint64_t bd, uint32_t acc) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(ad), "l"(bd), "r"(acc));
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
+template <> __device__ __forceinline__ void wgmma_n<32>(float* d, uint64_t ad, uint64_t bd, uint32_t acc) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr));
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(ad), "l"(bd), "r"(acc));
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+template <> __device__ __forceinline__ void wgmma_n<64>(float* d, uint64_t ad, uint64_t bd, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(ad), "l"(bd), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma_n<128>(float* d, uint64_t ad, uint64_t bd, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(ad), "l"(bd), "r"(acc));
+}
+
+// A tile of width BN issued as instructions of 128 / 64 / 32 / 16 columns (each reads the A operand once more; at N >= 32 per
+// instruction the tensor cores, not shared-memory bandwidth, bound the rate).  OFF = first column of this piece.
+template <int OFF, int REM>
+struct WgmmaCols {
+    static __device__ __forceinline__ void run(float* d, uint64_t ad, uint64_t bd, uint32_t acc) {
+        constexpr int W = REM >= 128 ? 128 : REM >= 64 ? 64 : REM >= 32 ? 32 : 16;
+        wgmma_n<W>(d + OFF / 2, ad, bd + (uint64_t)(OFF * 128 / 16), acc);   // B rows OFF.. start OFF * 128 bytes further
+        WgmmaCols<OFF + W, REM - W>::run(d, ad, bd, acc);
+    }
+};
+template <int OFF>
+struct WgmmaCols<OFF, 0> {
+    static __device__ __forceinline__ void run(float*, uint64_t, uint64_t, uint32_t) {}
+};
 
 __device__ __forceinline__ float act_apply(float x, int act) {
     if (act == 1) return __fdividef(x, 1.0f + __expf(-x));   // SiLU
@@ -131,32 +119,12 @@ __device__ __forceinline__ float act_apply(float x, int act) {
     return x;
 }
 
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-
 __device__ __forceinline__ float ex2_approx(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float rcp_approx(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-// SiLU of four values with ONE reciprocal: 1/(1+t_i) = (prod_{j != i} (1+t_j)) / prod_j (1+t_j).  The SFU (16 lanes / clk / SM)
-// bounds the epilogue math, so 5 SFU ops per 4 elements instead of 8.  The exponent argument is clamped at -20 (SiLU(-20) = -4e-8,
-// below half precision) so the product of four (1 + e^20) stays inside fp32; the error is a few fp32 ulps.
-__device__ __forceinline__ void silu4(float& x0, float& x1, float& x2, float& x3) {
-    const float L = -1.4426950408889634f;
-    const float a0 = 1.0f + ex2_approx(fmaxf(x0, -20.f) * L);
-    const float a1 = 1.0f + ex2_approx(fmaxf(x1, -20.f) * L);
-    const float a2 = 1.0f + ex2_approx(fmaxf(x2, -20.f) * L);
-    const float a3 = 1.0f + ex2_approx(fmaxf(x3, -20.f) * L);
-    const float p01 = a0 * a1, p23 = a2 * a3;
-    const float r = rcp_approx(p01 * p23);
-    const float r01 = r * p23, r23 = r * p01;
-    x0 *= r01 * a1; x1 *= r01 * a0; x2 *= r23 * a3; x3 *= r23 * a2;
-}
 
-
-// SiLU of two values with one reciprocal: 1/(1+t0) = (1+t1) / ((1+t0)(1+t1)).  Per element 1.5 SFU ops (ex2 + half a rcp) and 4.5
-// fp32 ops -- the 16-warp epilogue is bound by instruction issue (ncu, profiles/r02_*), and this form issues ~7 instructions per
-// element against ~10.5 for the four-value form.  Arguments are clamped at -40 so the product of two (1 + e^40) stays inside fp32
-// (SiLU(-40) = -1.7e-16 rounds to -0 in half precision either way).
+// SiLU of two values with one reciprocal: 1/(1+t0) = (1+t1) / ((1+t0)(1+t1)).  Per element 1.5 SFU ops (ex2 + half a rcp) instead
+// of 2.  Arguments are clamped at -40 so the product of two (1 + e^40) stays inside fp32 (SiLU(-40) = -1.7e-16 rounds to -0 in half
+// precision either way).
 __device__ __forceinline__ void silu2(float& x0, float& x1) {
     const float L = -1.4426950408889634f;
     const float a0 = 1.0f + ex2_approx(fmaxf(x0, -40.f) * L);
@@ -166,28 +134,10 @@ __device__ __forceinline__ void silu2(float& x0, float& x1) {
     x1 *= r * a0;
 }
 
-// n / d for 0 <= n < 2^31 without a hardware divide (the epilogue computes two quotients per thread and sub-tile).
+// n / d for 0 <= n < 2^31 without a hardware divide (the epilogue's row arithmetic).
 struct FastDiv {
     uint32_t mul, shr;
     int d;
 };
 __device__ __forceinline__ int fast_div(int n, const FastDiv& f) { return f.d == 1 ? n : (int)(__umulhi((uint32_t)n, f.mul) >> f.shr); }
-
-// ---- TMA stores (shared -> global), bulk async groups -----------------------------------------------------------------
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* tm, uint32_t smem_src, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-                 ::"l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_src), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* tm, uint32_t smem_src, int c0, int c1, int c2, int c3) {
-    asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-                 ::"l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
 }  // namespace adas

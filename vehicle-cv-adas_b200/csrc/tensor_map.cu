@@ -1,8 +1,8 @@
-// tensor_map.cu -- TMA descriptors for the conv / FC GEMM kernels (gemm_v3.cu, gemm_chain.cu) and the CUDA-core validation kernel the
-// tests compare the tcgen05 path against (conv_impl = 1; never the product path).
+// tensor_map.cu -- TMA descriptors for the conv / FC GEMM kernel (gemm_v3.cu) and the CUDA-core validation kernel the
+// tests compare the wgmma path against (conv_impl = 1; never the product path).
 //
 // Tensor maps: 2-D [rows, channels] views of padded-NHWC activations and of weight matrices (128-byte swizzle, out-of-bounds rows read
-// as zero), 4-D [C, W, H, B] views with traversal stride 2 for stride-2 convs, and 4-D interior views for the TMA-store epilogue.
+// as zero) and 4-D [C, W, H, B] views with traversal stride 2 for stride-2 convs.
 #include "common.h"
 #include "tc_common.cuh"
 #include <stdlib.h>
@@ -56,25 +56,6 @@ int make_tmap_4d_s2(CUtensorMap* tm, const void* base, uint64_t C, uint64_t Wp, 
     CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     ADAS_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(4-D, stride 2) failed: %d", (int)r);
-    return 0;
-}
-
-// plain 4-D tiled map over [C, W, H, B] (row pitch Wp pixels, image pitch Hp rows): used for TMA STORES of output patches into the
-// interior of a padded NHWC grid (the tensor extent is the interior, so the unit clips partial patches and never touches the halo)
-int make_tmap_4d(CUtensorMap* tm, const void* base, uint64_t C, uint64_t W, uint64_t H, uint64_t B, uint64_t ld_elems, uint64_t Wp, uint64_t Hp,
-                 uint32_t box_c, uint32_t box_w, uint32_t box_h) {
-    PFN_encodeTiled fn = get_encode_fn();
-    ADAS_CHECK(fn != nullptr, "cuTensorMapEncodeTiled entry point unavailable");
-    ADAS_CHECK((reinterpret_cast<uintptr_t>(base) & 15) == 0 && (ld_elems * 2) % 16 == 0, "TMA 4-D map alignment");
-    ADAS_CHECK(box_w <= 256 && box_h <= 256 && box_c * 2 <= 128, "TMA 4-D box too large (%u x %u x %u)", box_c, box_w, box_h);
-    cuuint64_t dims[4] = {C, W, H, B};
-    cuuint64_t strides[3] = {ld_elems * 2, Wp * ld_elems * 2, Hp * Wp * ld_elems * 2};
-    cuuint32_t box[4] = {box_c, box_w, box_h, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    ADAS_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(4-D) failed: %d (C=%llu W=%llu H=%llu B=%llu)", (int)r, (unsigned long long)C,
-               (unsigned long long)W, (unsigned long long)H, (unsigned long long)B);
     return 0;
 }
 

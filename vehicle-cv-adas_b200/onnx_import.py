@@ -1,8 +1,8 @@
-"""onnx_import.py -- ingest the reference's model files: `.onnx` -> packed sm_100a plan (`.b200w`).
+"""onnx_import.py -- ingest the reference's model files: `.onnx` -> packed sm_90a plan (`.b200w`).
 
 The reference hands `.onnx` / `.trt` files to ONNXRuntime / TensorRT (coreEngine.py:54-55,164-166); its models come from
 ultralytics / yolov5 exports (README.md:53-58) and from `TrafficLaneDetector/convertPytorchToONNX.py:60-87` (UFLD).  This module
-is the B200 replacement of that ingestion step (SURVEY 8f rank 2): it reads the ONNX protobuf directly (the `onnx` package is
+is the H100 replacement of that ingestion step (SURVEY 8f rank 2): it reads the ONNX protobuf directly (the `onnx` package is
 not a dependency -- the wire format is parsed here), recovers the convolution / linear / LayerNorm parameters, recognises the
 architecture (YOLOv8 / YOLOv5 / UFLDv2, scale, class count, input size) and drives the same `plan.build_*` builders that the
 state_dict path uses.  Nothing here runs the network: the graph is only a parameter container plus a shape oracle.

@@ -4,7 +4,7 @@ demo.py does, per frame and strictly in sequence: `objectDetector.DetectFrame` (
 -> `laneDetector.DetectFrame` (280) -> analytics/drawing.  Here one step takes a batch of consecutive frames of one
 stream:  a worker thread makes ONE library call (`adas_detect_pair`) that enqueues the object network and the lane network
 on their own CUDA streams before waiting for either -- the tail waves of one network's persistent conv kernels are
-back-filled by the other's (measured 3.96 vs 4.35 ms per 8-frame step; driving the two streams from two Python threads
+back-filled by the other's (driving the two streams from two Python threads
 instead was slower, the interpreter lock serialises the launches) -- while the host thread runs the ByteTrack updates of
 the PREVIOUS batch; consecutive batches alternate between two engine pairs so the device never waits for the host:
 the tracker is sequential in time per stream (SURVEY 8e), so it pipelines one batch behind the detectors.  Per-frame

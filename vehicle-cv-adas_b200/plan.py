@@ -3,7 +3,7 @@
 Replaces the reference's offline model tooling for this runtime (convertOnnxToTensorRT.py,
 onnxQuantization.py, TrafficLaneDetector/convertPytorchToONNX.py:50-96): instead of exporting to
 ONNX and building a TensorRT engine, the weights are BN-folded, cast to fp16, laid out K-major
-([Cout, kh, kw, Cin]) for the sm_100a implicit-GEMM kernel, and written next to the op list the
+([Cout, kh, kw, Cin]) for the sm_90a implicit-GEMM kernel, and written next to the op list the
 C++ runtime replays (csrc/plan.h documents the binary layout).
 
 Network graphs
@@ -195,7 +195,7 @@ class PlanBuilder:
         self.outputs: List[Tuple[int, int, int, int]] = []
         self.meta = [0] * 16
         self.flops_per_img = 0   # 2*MAC of the convs/FCs as mathematically defined (no padding waste)
-        self.stem_flops_per_img = 0   # the part of flops_per_img that runs in stem_conv.cu (mma.sync) rather than in the tcgen05 GEMM launches
+        self.stem_flops_per_img = 0   # the part of flops_per_img that runs in stem_conv.cu (mma.sync) rather than in the wgmma GEMM launches
         self.stem_direct = os.environ.get("ADAS_B200_STEMCONV", "1") != "0"
         self.strided_tma = os.environ.get("ADAS_B200_STRIDED_TMA", "1") != "0"
         # buffer 0: the network input image, padded NHWC with C=4 (R,G,B,0)
@@ -582,7 +582,7 @@ def build_ufldv2(weights: Weights, backbone: str = "34", cfg=UFLD_CULANE) -> Pla
     pb = PlanBuilder(MODEL_UFLDV1 if v1 else MODEL_UFLDV2, 3, in_h, in_w)
     W = weights
     w, b = W.conv_bn("model", 64, 3, 7, BN_EPS_TV, conv_key="conv1", bn_key="bn1")
-    # stem: "pack" = re-layout pass + a 4-tap tcgen05 GEMM (stem7x7s2), "direct" = stem_conv.cu straight from the image
+    # stem: "pack" = re-layout pass + a 4-tap wgmma GEMM (stem7x7s2), "direct" = stem_conv.cu straight from the image
     if os.environ.get("ADAS_B200_UFLD_STEM", UFLD_STEM_DEFAULT) == "pack":
         x = pb.stem7x7s2(pb.image, w, b, ACT_RELU)
     else:

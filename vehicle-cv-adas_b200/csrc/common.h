@@ -68,6 +68,7 @@ struct GemmParams {
     int res_ld;     // row stride of res, elements; NEGATIVE = add the residual before the activation (ResNet)
     int mask_H, mask_W;  // > 0: only rows in the interior of the padded (H+2)x(W+2) grid are stored
     int mt_hint;    // number of 128-row sub-tiles per CTA tile (1..4; they share each weight tile), 0 = auto
+    int no_slab;    // 1: 3x3 stride-1 convs load one activation tile per tap instead of one slab per (dy, k-block) (A/B hook)
     // stride-2 convs (3x3 pad 1, or 1x1) read the input through a 4-D TMA map with traversal stride 2: an M tile is a
     // bw x bh patch of output pixels of one image; s2_* describe the output grid and the input's padded height
     int s2, s2_bw, s2_bh, s2_tw, s2_th, s2_Ho, s2_Wo, s2_Hp_in;
@@ -91,7 +92,7 @@ int  gemm_v3_prepare_s2(const GemmParams& p, const void* a_base, uint64_t a_C, u
 int  gemm_v3_run(void* opaque, cudaStream_t st);
 void gemm_v3_free(void* opaque);
 void gemm_v3_describe(const void* opaque, char* out, int cap);
-int  gemm_v3_candidates(const GemmParams& base, int max_out, int* BN_out, int* mt_out);
+int  gemm_v3_candidates(const GemmParams& base, int max_out, int* BN_out, int* mt_out, int* no_slab_out);
 int  make_tmap_2d(CUtensorMap* tm, const void* base, uint64_t inner, uint64_t rows, uint64_t row_stride_bytes,
                   uint32_t box_inner, uint32_t box_rows);
 

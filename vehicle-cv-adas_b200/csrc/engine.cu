@@ -199,6 +199,7 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
                     g.out_ld = (int)(ob.rows_per_img * ob.C);
                 }
                 if (p[17] > 0) g.mt_hint = p[17];       // plan-forced sub-tile count (test hook of plan.py)
+                g.no_slab = p[18];                      // plan-forced per-tap operand loads (test hook of plan.py)
                 // Fully connected layers whose weight matrix stays in L2 (FC1 of the UFLD head: 20 MB; up to half of the H100's 50 MB) run
                 // as a weight stream on the CUDA cores: the swap-AB tensor-core GEMM has only N/256 CTAs for them.
                 static const bool fc_stream_on = !(getenv("ADAS_B200_FC_STREAM") && getenv("ADAS_B200_FC_STREAM")[0] == '0');
@@ -235,14 +236,14 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
                     if (!transposed && p[15] <= 0) {
                         // tile candidates ranked by the cost model; with autotuning the best few are timed on the device once per
                         // (op, batch).  Every candidate accumulates in the same K order, so the choice never changes results.
-                        int cBN[16], cMT[16];
-                        const int nc = gemm_v3_candidates(g, e->autotune ? 10 : 1, cBN, cMT);
+                        int cBN[16], cMT[16], cNS[16];
+                        const int nc = gemm_v3_candidates(g, e->autotune ? (ntaps == 9 && !s2 ? 16 : 10) : 1, cBN, cMT, cNS);
                         float best_ms = 1e30f;
                         cudaEvent_t ev0 = nullptr, ev1 = nullptr;
                         if (nc > 1) { ADAS_CUDA(cudaEventCreate(&ev0)); ADAS_CUDA(cudaEventCreate(&ev1)); }
                         for (int ci = 0; ci < nc; ++ci) {
                             GemmParams gc = g;
-                            gc.BN = cBN[ci]; gc.mt_hint = cMT[ci];
+                            gc.BN = cBN[ci]; gc.mt_hint = cMT[ci]; gc.no_slab = g.no_slab | cNS[ci];
                             void* cand = nullptr;
                             if (prep(gc, &cand)) continue;
                             if (nc == 1) { opaque = cand; break; }
@@ -256,8 +257,8 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
                             float ms = 1e30f;
                             if (!rc) cudaEventElapsedTime(&ms, ev0, ev1);
                             static const bool at_log = getenv("ADAS_B200_AT_LOG") != nullptr;
-                            if (at_log) fprintf(stderr, "[autotune] op %zu M=%d N=%d K=%d taps=%d s2=%d BN=%d mt=%d : %.1f us\n", oi, g.M, g.N, Kc * ntaps, ntaps, s2,
-                                                gc.BN, gc.mt_hint, rc ? -1.0 : ms * 1000.0 / 4.0);
+                            if (at_log) fprintf(stderr, "[autotune] op %zu M=%d N=%d K=%d taps=%d s2=%d BN=%d mt=%d no_slab=%d : %.1f us\n", oi, g.M, g.N, Kc * ntaps, ntaps, s2,
+                                                gc.BN, gc.mt_hint, gc.no_slab, rc ? -1.0 : ms * 1000.0 / 4.0);
                             if (!rc && ms < best_ms) { best_ms = ms; if (opaque) gemm_v3_free(opaque); opaque = cand; }
                             else gemm_v3_free(cand);
                         }
@@ -557,7 +558,7 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
                 ADAS_CHECK(tensor_ok(p[4], (uint64_t)N * Kc * ntaps * 2) && e->tensors[p[4]].dtype == 0, "plan %s: op %zu: weight tensor missing or too small", path, oi);
                 ADAS_CHECK(p[5] < 0 || (tensor_ok(p[5], (uint64_t)N * 4) && e->tensors[p[5]].dtype == 1), "plan %s: op %zu: bias tensor missing or too small", path, oi);
                 ADAS_CHECK(p[8] < 0 || (!transposed && view_ok(p[8], p[9], N) && e->bufs[p[8]].dtype == 0), "plan %s: op %zu: residual slice exceeds its buffer", path, oi);
-                ADAS_CHECK(p[15] >= 0 && p[15] <= 256 && p[17] >= 0 && p[17] <= 4, "plan %s: op %zu: bad forced tile shape", path, oi);
+                ADAS_CHECK(p[15] >= 0 && p[15] <= 256 && p[17] >= 0 && p[17] <= 4 && (p[18] == 0 || p[18] == 1), "plan %s: op %zu: bad forced tile shape", path, oi);
                 break;
             }
             case OP_IM2COL:

@@ -5,11 +5,14 @@
 // :184-186 (OnnxEngine.engine_inference).
 //
 // Tile: BM = 128 output rows (pixels of the padded NHWC grid) x MT sub-tiles x BN output channels x BK = 64 channels per k-block.
-// A 3x3 stride-1 conv runs 9 taps x (Cin/64) k-blocks, each A tile being the SAME 2-D activation matrix loaded at row offset
+// A 3x3 stride-1 conv runs 9 taps x (Cin/64) k-blocks, each A tile being the SAME 2-D activation matrix read at row offset
 // m0 + dy*(W+2) + dx (the zero halo of the padded layout supplies the conv padding, TMA's out-of-bounds zero fill covers the matrix
-// ends); every tap's tile is its own TMA box, so each wgmma operand starts on a 1024-byte swizzle boundary.  Stride-2 convs read
-// 4-D boxes with traversal stride 2.  K order is (dy, k-block, dx) for every tile shape, so results are bit-identical whatever tile
-// is chosen and whatever the batch size.
+// ends).  The three dx taps of one (dy, k-block) differ only by a one-row shift, so in slab mode one pipeline stage holds one
+// (dy, k-block): per sub-tile one TMA box of SLAB_ROWS = 136 rows, read by the dx taps from rows 0, 1 and 2 on, plus the three dx
+// weight tiles -- a third of the activation bytes of one box per tap.  Slab mode needs two such stages in shared memory (not
+// MT = 1 x BN = 256); autotune times every slab tile against the same tile with one activation box per tap.  Stride-2 convs read
+// 4-D boxes with traversal stride 2.  K order is (dy, k-block, dx) for every tile shape and both operand modes, so results are
+// bit-identical whatever tile is chosen and whatever the batch size.
 //
 // Warp roles (384 threads): warpgroup 0 = TMA producer (one elected thread; the group gives its registers up with setmaxnreg),
 // warpgroups 1 and 2 = consumers: each issues the wgmmas of 64 rows of every sub-tile (m64nBNk16, BN split into instructions of
@@ -55,16 +58,17 @@ conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     }
     __syncthreads();
     // ---- TMA producer pieces (thread 0) ----
-    const uint32_t a_bytes = p.s2 ? (uint32_t)(p.s2_bw * p.s2_bh * BK * 2) : (uint32_t)A_STAGE_BYTES;
-    const uint32_t tx_bytes = (uint32_t)g.MT * a_bytes + (uint32_t)(BN * BK * 2);
+    const int tps = g.slab ? 3 : 1;                       // taps per pipeline stage
+    const uint32_t a_bytes = p.s2 ? (uint32_t)(p.s2_bw * p.s2_bh * BK * 2) : (uint32_t)g.a_sub_bytes;
+    const uint32_t tx_bytes = (uint32_t)g.MT * a_bytes + (uint32_t)(tps * BN * BK * 2);
     const bool dx_inner = p.ntaps == 9;                   // 9-tap order is (dy, k-block, dx)
     const int o_cnt = dx_inner ? 3 : p.ntaps;            // outer loop: dy (9 taps) or tap
-    const int i_cnt = dx_inner ? 3 : 1;                  // inner loop: dx (9 taps)
+    const int i_cnt = dx_inner && !g.slab ? 3 : 1;       // inner loop: dx (9 taps, one tap per stage)
     const int per_img = p.s2_tw * p.s2_th;
-    // weight (B operand) tile of one pipeline step
+    // weight (B operand) tiles of one pipeline step: taps grp .. grp + tps - 1
     auto load_b = [&](int grp, int kc, int n0, uint32_t stage, uint32_t fb) {
         const uint32_t b_dst = smem_base + stage * g.stage_bytes + g.MT * g.a_sub_bytes;
-        tma_load_2d(b_dst, &tmB, grp * p.Kc + kc * BK, n0, fb);
+        for (int t = 0; t < tps; ++t) tma_load_2d(b_dst + t * g.b_bytes, &tmB, (grp + t) * p.Kc + kc * BK, n0, fb);
     };
     // activation (A operand) tiles of one pipeline step
     auto load_a = [&](int grp, int kc, int m_t, uint32_t stage, uint32_t fb) {
@@ -82,6 +86,7 @@ conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                 tma_load_4d(a_dst + mt * g.a_sub_bytes, &tmA, kc * BK, 2 * tx * p.s2_bw + dx, 2 * ty * p.s2_bh + dy, b, fb);
             }
         } else {
+            // slab mode: grp = 3 * dy, so the slab starts at the dx = 0 tap's first row; its box is SLAB_ROWS tall
             int shift = 0;
             if (p.ntaps == 9) shift = (grp / 3 - 1) * p.Wp + (grp % 3 - 1);
             else if (p.ntaps == 4) shift = (grp - 2) * p.Wp;          // stem: row pairs yo-1 .. yo+2 (plan.py stem7x7s2)
@@ -142,7 +147,7 @@ conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         // ================= consumers (MMA + epilogue) =================
         const int cw = (warp_idx - 4) >> 2;                 // consumer warpgroup: rows cw*64 .. cw*64+63 of every sub-tile
         const int wq = warp_idx & 3;                        // warp of the group: 16 of those rows
-        const int ksteps = p.ntaps * p.kpt;
+        const int nsteps = p.ntaps * p.kpt / tps;           // pipeline stages per tile
         const size_t res_ld = (size_t)(p.res_ld < 0 ? -p.res_ld : p.res_ld);
         float acc[MTX][BN / 2];
 #pragma unroll
@@ -152,22 +157,27 @@ conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         uint32_t s = 0, ph = 0;
         for (int w = blockIdx.x; w < g.total_tiles; w += gridDim.x) {
             uint32_t prev = 0;
-            for (int ks = 0; ks < ksteps; ++ks) {
+            for (int ks = 0; ks < nsteps; ++ks) {
                 mbar_wait(smem_u32(&full_bar[s]), ph);
                 const uint32_t a_base = smem_base + s * g.stage_bytes + (uint32_t)cw * (64u * 128u);
-                const uint64_t bdesc = make_smem_desc(smem_base + s * g.stage_bytes + g.MT * g.a_sub_bytes);
+                const uint32_t b_base = smem_base + s * g.stage_bytes + g.MT * g.a_sub_bytes;
 #pragma unroll
                 for (int mt = 0; mt < MTX; ++mt)
 #pragma unroll
                     for (int i = 0; i < BN / 2; ++i) reg_fence(acc[mt][i]);
                 wgmma_fence();
+                // slab mode: tap dx reads the slab from row dx on and its own weight tile.  Per sub-tile the K order stays
+                // (dy, k-block, dx, k16), the per-tap order, so both modes give the same bits.
+                for (int t = 0; t < tps; ++t) {
+                    const uint64_t bdesc = make_smem_desc(b_base + t * g.b_bytes);
 #pragma unroll
-                for (int mt = 0; mt < MTX; ++mt) {
-                    if (mt < g.MT) {
-                        const uint64_t adesc = make_smem_desc(a_base + (uint32_t)(mt * g.a_sub_bytes));
+                    for (int mt = 0; mt < MTX; ++mt) {
+                        if (mt < g.MT) {
+                            const uint64_t adesc = make_smem_desc(a_base + (uint32_t)(mt * g.a_sub_bytes + t * 128));
 #pragma unroll
-                        for (int k = 0; k < BK / 16; ++k)
-                            WgmmaCols<0, BN>::run(acc[mt], adesc + 2u * k, bdesc + 2u * k, (uint32_t)((ks | k) != 0));
+                            for (int k = 0; k < BK / 16; ++k)
+                                WgmmaCols<0, BN>::run(acc[mt], adesc + 2u * k, bdesc + 2u * k, (uint32_t)((ks | t | k) != 0));
+                        }
                     }
                 }
                 wgmma_commit();
@@ -321,8 +331,13 @@ int gemm_v3_config(const GemmParams& p_in, GemmV3* g) {
     if (g->MT > mt_max) g->MT = mt_max;
     const int b_bytes = ((p.BN * BK * 2) + 1023) & ~1023;
     g->b_bytes = b_bytes;
-    g->a_sub_bytes = A_STAGE_BYTES;
-    g->stage_bytes = g->MT * g->a_sub_bytes + b_bytes;
+    // 3x3 stride-1: the three dx taps of one (dy, k-block) read the same activation rows shifted by one, so one slab of
+    // SLAB_ROWS rows per sub-tile feeds all three -- when two such stages fit (not at MT = 1, BN = 256)
+    static const int no_slab_env = env_int("ADAS_B200_NOSLAB", 0);
+    const int slab_stage = g->MT * SLAB_BYTES + 3 * b_bytes;
+    g->slab = p.ntaps == 9 && !p.s2 && !p.no_slab && !no_slab_env && 2 * slab_stage <= V3_DYN_SMEM_MAX - 1024;
+    g->a_sub_bytes = g->slab ? SLAB_BYTES : A_STAGE_BYTES;
+    g->stage_bytes = g->slab ? slab_stage : g->MT * g->a_sub_bytes + b_bytes;
     int stages = (V3_DYN_SMEM_MAX - 1024) / g->stage_bytes;
     if (stages > 8) stages = 8;
     if (stages < 2) return 1;
@@ -373,12 +388,14 @@ int gemm_v3_launch(const GemmV3Launch& L, cudaStream_t st) {
 
 // Tile candidates ranked by a rough cost model (the engine times the best few on the device once per (op, batch)): operand bytes
 // delivered from L2 at ~32 B/clk/SM, wgmma time, an epilogue that does not overlap the main loop of the same CTA, waves of tiles
-// over the SMs and a fixed launch cost.
-int gemm_v3_candidates(const GemmParams& base, int max_out, int* BN_out, int* mt_out) {
+// over the SMs and a fixed launch cost.  A tile that can run in slab mode is handed out twice, slab first and then per tap
+// (no_slab_out = 1): two slab stages hold only one stage of look-ahead, which measures slower than per-tap loads on some H100
+// layers (80x80 N = 128, 40x40 N = 256), so the device timing decides.
+int gemm_v3_candidates(const GemmParams& base, int max_out, int* BN_out, int* mt_out, int* no_slab_out) {
     int num_sms = 132;
     if (v3_num_sms(&num_sms)) return 0;
     const int cand[] = {256, 192, 128, 64, 160, 96, 80, 48, 32, 16};
-    struct C { double t; int BN, mt; } list[64];
+    struct C { double t; int BN, mt, slab; } list[64];
     int n = 0;
     const int N = base.N, ntaps = base.ntaps;
     const int kpt = (base.Kc + 63) / 64;
@@ -399,22 +416,26 @@ int gemm_v3_candidates(const GemmParams& base, int max_out, int* BN_out, int* mt
             if (gemm_v3_config(p, &g)) continue;
             if (g.p.BN != BN || g.MT != mt) continue;            // clamped, or forced by a test hook
             const double tiles = (double)g.total_tiles;
-            const double ksteps = (double)ntaps * kpt;
-            const double bytes = ksteps * (g.MT * (double)g.a_sub_bytes + BN * 128.0);
+            const int tps = g.slab ? 3 : 1;                      // taps per pipeline stage
+            const double bytes = (double)ntaps * kpt / tps * (g.MT * (double)g.a_sub_bytes + tps * BN * 128.0);
             const double rate = BN >= 64 ? 1.0 : 0.7;                              // narrow wgmmas are bound by the A re-read
             const double mma = (double)g.MT * ntaps * kpt * 4.0 * BN / rate;
             const double epi = (double)g.MT * 128.0 * BN * 0.12;
             const double per_tile = fmax(bytes / 32.0, mma) + epi + 400.0;
             const double waves = ceil(tiles / (double)num_sms);
             const double t = waves * per_tile + 3500.0;
-            if (n < 64) { list[n].t = t; list[n].BN = BN; list[n].mt = mt; ++n; }
+            if (n < 64) { list[n].t = t; list[n].BN = BN; list[n].mt = mt; list[n].slab = g.slab; ++n; }
         }
     }
     for (int i = 1; i < n; ++i) { C c = list[i]; int j = i - 1; while (j >= 0 && list[j].t > c.t) { list[j + 1] = list[j]; --j; } list[j + 1] = c; }
-    if (n == 0) { list[0].BN = N <= 256 ? (N + 15) / 16 * 16 : 256; list[0].mt = 1; n = 1; }
-    if (n > max_out) n = max_out;
-    for (int i = 0; i < n; ++i) { BN_out[i] = list[i].BN; mt_out[i] = list[i].mt; }
-    return n;
+    if (n == 0) { list[0].BN = N <= 256 ? (N + 15) / 16 * 16 : 256; list[0].mt = 1; list[0].slab = 0; n = 1; }
+    int out = 0;
+    for (int i = 0; i < n && out < max_out; ++i) {
+        for (int ns = 0; ns <= list[i].slab && out < max_out; ++ns) {
+            BN_out[out] = list[i].BN; mt_out[out] = list[i].mt; no_slab_out[out] = ns; ++out;
+        }
+    }
+    return out;
 }
 
 int gemm_v3_prepare(const GemmParams& p, const void* a_base, uint64_t a_inner, uint64_t a_rows, uint64_t a_stride_bytes,
@@ -424,7 +445,7 @@ int gemm_v3_prepare(const GemmParams& p, const void* a_base, uint64_t a_inner, u
     ADAS_CHECK(!p.s2, "gemm_v3_prepare: stride-2 ops go through gemm_v3_prepare_s2");
     GemmV3Launch* L = new GemmV3Launch();
     if (gemm_v3_config(p, &L->g)) { delete L; ADAS_CHECK(false, "gemm_v3: tile does not fit (BN %d, mt %d)", p.BN, p.mt_hint); }
-    if (make_tmap_2d(&L->tmA, a_base, a_inner, a_rows, a_stride_bytes, 64, BM) ||
+    if (make_tmap_2d(&L->tmA, a_base, a_inner, a_rows, a_stride_bytes, 64, L->g.slab ? SLAB_ROWS : BM) ||
         make_tmap_2d(&L->tmB, b_base, b_inner, b_rows, b_stride_bytes, 64, (uint32_t)L->g.p.BN)) {
         delete L;
         return 1;
@@ -451,9 +472,9 @@ int gemm_v3_run(void* opaque, cudaStream_t st) { return gemm_v3_launch(*static_c
 void gemm_v3_free(void* opaque) { delete static_cast<GemmV3Launch*>(opaque); }
 void gemm_v3_describe(const void* opaque, char* out, int cap) {
     const GemmV3& g = static_cast<const GemmV3Launch*>(opaque)->g;
-    snprintf(out, (size_t)cap, "M=%d N=%d K=%d taps=%d act=%d res=%d f32=%d s2=%d tr=%d | v3 BN=%d MT=%d stages=%d tiles=%d", g.p.M,
+    snprintf(out, (size_t)cap, "M=%d N=%d K=%d taps=%d act=%d res=%d f32=%d s2=%d tr=%d | v3 BN=%d MT=%d slab=%d stages=%d tiles=%d", g.p.M,
              g.p.N, g.p.Kc * g.p.ntaps, g.p.ntaps, g.p.act, g.p.res ? (g.p.res_ld < 0 ? -1 : 1) : 0, g.p.out_f32, g.p.s2, g.p.transposed, g.p.BN, g.MT,
-             g.stages, g.total_tiles);
+             g.slab, g.stages, g.total_tiles);
 }
 
 }  // namespace adas

@@ -13,6 +13,7 @@ static constexpr int V3_DYN_SMEM_MAX = 227 * 1024 - 1024;
 struct GemmV3 {
     GemmParams p;
     int MT;            // 1..4 sub-tiles of 128 rows (stride-2: output patches) per CTA tile; they share every weight tile
+    int slab;          // 3x3 stride-1: a stage holds one (dy, k-block) -- MT slabs of SLAB_ROWS rows + the three dx weight tiles
     int a_sub_bytes, b_bytes, stage_bytes, stages;
     int n_tiles, m_tiles, total_tiles;
     int pdl;

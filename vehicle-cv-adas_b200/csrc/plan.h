@@ -43,8 +43,9 @@ struct PlanOutput {
 #pragma pack(pop)
 
 enum PlanOpType : uint32_t {
-    OP_GEMM = 1,       // p: a_buf a_coff Kc ntaps w_tensor bias_tensor N act res_buf res_coff res_pre_act out_buf out_coff masked transposed BN s2 MT
-                       //    (BN / MT > 0 force the tile shape: test hooks, 0 = cost model + autotune)
+    OP_GEMM = 1,       // p: a_buf a_coff Kc ntaps w_tensor bias_tensor N act res_buf res_coff res_pre_act out_buf out_coff masked transposed BN s2 MT no_slab
+                       //    (BN / MT > 0 force the tile shape, no_slab = 1 one activation tile per 3x3 tap: test hooks;
+                       //    0 = cost model + autotune)
     OP_IM2COL = 2,     // p: in_buf in_coff Cin kh kw stride pad out_buf
     OP_MAXPOOL = 3,    // p: in_buf in_coff C k s pad out_buf out_coff
     OP_UPSAMPLE2X = 4, // p: in_buf in_coff C out_buf out_coff

@@ -7,6 +7,8 @@ namespace adas {
 static constexpr int BM = 128;
 static constexpr int BK = 64;                       // fp16 elements per k-block = 128 bytes = one swizzle row
 static constexpr int A_STAGE_BYTES = BM * BK * 2;   // 16 KiB
+static constexpr int SLAB_ROWS = BM + 8;            // 3x3 stride-1 slab: BM rows + the 2 rows the dx = 1, 2 taps reach, to 8-row groups
+static constexpr int SLAB_BYTES = SLAB_ROWS * BK * 2;   // 17 KiB: consecutive slabs stay 1024-byte aligned
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -50,7 +52,10 @@ __device__ __forceinline__ void tma_load_4d(uint32_t smem_dst, const CUtensorMap
 
 // ---- wgmma (sm_90a warpgroup MMA, fp16 x fp16 -> fp32 in registers) ------------------------------------------------------
 // Shared-memory matrix descriptor of a K-major, 128B-swizzled operand tile as TMA writes it: rows of 128 bytes, 8-row groups
-// 1024 bytes apart.  The tile must start on a 1024-byte boundary (base offset 0); a k-step of 16 elements advances the start by 32 bytes.
+// 1024 bytes apart; a k-step of 16 elements advances the start by 32 bytes.  The start may also lie whole rows into a swizzle atom
+// (slab mode: dx = 1, 2 rows into a 1024-byte aligned box) with the base-offset field (bits 49-51) left at 0: the swizzle XOR follows
+// the absolute shared-memory address, as TMA's does.  Setting it to (addr >> 7) & 7 is not needed; with 0 the slab path is bit-identical
+// to one aligned box per tap (tests/test_gpu_slab.py).
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);   // start address, 16-byte units

@@ -229,8 +229,9 @@ class PlanBuilder:
 
     def conv(self, x: View, w: np.ndarray, b: Optional[np.ndarray], k: int, s: int, act: int, out: Optional[View] = None,
              res: Optional[View] = None, res_pre_act: bool = False, out_f32: bool = False, pad: Optional[int] = None,
-             tile: Optional[Tuple[int, int]] = None) -> View:
-        """w: folded [Cout, Cin_real, k, k] fp32.  x.C may exceed Cin_real (zero-padded image channel)."""
+             tile: Optional[Tuple[int, int]] = None, no_slab: bool = False) -> View:
+        """w: folded [Cout, Cin_real, k, k] fp32.  x.C may exceed Cin_real (zero-padded image channel).
+        no_slab (test hook): a 3x3 stride-1 conv loads one activation tile per tap instead of one slab per (dy, k-block)."""
         cout, cin_real = int(w.shape[0]), int(w.shape[1])
         pad = k // 2 if pad is None else pad
         Ho = (x.H + 2 * pad - k) // s + 1
@@ -278,7 +279,7 @@ class PlanBuilder:
         w_t = self.tensor(wk.astype(np.float16))
         bn, mt = tile if tile is not None else (0, 0)          # (BN, MT) forced by tests; 0 = cost model + autotune
         self._op(OP_GEMM, [a.buf, a.coff, Kc, ntaps, w_t, bias_t, n_store, act, res_buf, res_coff, 1 if res_pre_act else 0,
-                           out.buf, out.coff, 1, 0, bn, s2, mt])
+                           out.buf, out.coff, 1, 0, bn, s2, mt, 1 if no_slab else 0])
         return View(out.buf, out.coff, cout, Ho, Wo)
 
     def stem_conv(self, x: View, w: np.ndarray, b: Optional[np.ndarray], k: int, pad: int, act: int, out: View) -> View:

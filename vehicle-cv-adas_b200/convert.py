@@ -7,6 +7,7 @@ and `TrafficLaneDetector/convertPytorchToONNX.py:77-87` (UFLD `.pth` checkpoint 
     python -m adas_b200.convert yolov8l.onnx                       # architecture recognised from the graph
     python -m adas_b200.convert culane_res34.pth --kind ufldv2 --backbone 34
     python -m adas_b200.convert yolov5n.pt.state_dict.pth --kind yolov5 --scale n
+    python -m adas_b200.convert yolov7-tiny.state_dict.pth --kind yolov7 --scale tiny
 
 Checkpoints hold un-fused Conv/BatchNorm parameters under the upstream key names (the names `plan.build_*` ask for), so BatchNorm
 is folded here in float64 exactly as for the seeded weights.  Only the parameter dictionary is read: pickled model objects
@@ -49,6 +50,8 @@ def plan_from_state_dict(sd: Dict[str, np.ndarray], kind: str, scale: str = "l",
         return plan.build_yolov8(w, scale, nc=nc)
     if kind == "yolov5":
         return plan.build_yolov5(w, scale, nc=nc)
+    if kind == "yolov7":
+        return plan.build_yolov7(w, scale, nc=nc)
     if kind == "ufldv2":
         return plan.build_ufldv2(w, backbone)
     raise Exception(f"unsupported model kind {kind}")
@@ -63,7 +66,7 @@ def convert(path: str, out: Optional[str] = None, kind: Optional[str] = None, sc
         pb = build_plan(model, recognise(model))
     else:
         if kind is None:
-            raise Exception("--kind is required for checkpoint files (yolov8 | yolov5 | ufldv2)")
+            raise Exception("--kind is required for checkpoint files (yolov8 | yolov5 | yolov7 | ufldv2)")
         pb = plan_from_state_dict(load_checkpoint_state_dict(path), kind, scale, backbone, nc)
     pb.write(out)
     return out
@@ -73,8 +76,8 @@ def main(argv=None) -> int:
     ap = argparse.ArgumentParser(description="convert an .onnx model or a state_dict checkpoint to a .b200w plan")
     ap.add_argument("model")
     ap.add_argument("--out", default=None)
-    ap.add_argument("--kind", default=None, choices=["yolov8", "yolov5", "ufldv2"])
-    ap.add_argument("--scale", default="l", help="YOLO scale letter (checkpoints only; ONNX files are recognised)")
+    ap.add_argument("--kind", default=None, choices=["yolov8", "yolov5", "yolov7", "ufldv2"])
+    ap.add_argument("--scale", default="l", help="YOLO scale letter, or tiny | base for yolov7 (checkpoints only; ONNX files are recognised)")
     ap.add_argument("--backbone", default="34", choices=["18", "34"], help="UFLDv2 ResNet depth (checkpoints only)")
     ap.add_argument("--nc", type=int, default=80)
     a = ap.parse_args(argv)

@@ -62,7 +62,7 @@ struct GemmParams {
     int kpt;        // k-blocks (of 64) per tap = ceil(Kc/64)
     int BN;         // tile width (multiple of 16, <= 256)
     int stages;     // smem pipeline depth
-    int act;        // 0 none, 1 SiLU, 2 ReLU
+    int act;        // 0 none, 1 SiLU, 2 ReLU, 3 LeakyReLU(0.1)
     int out_f32;    // 0: fp16 out, 1: fp32 out
     int out_ld;     // row stride of out, elements
     int res_ld;     // row stride of res, elements; NEGATIVE = add the residual before the activation (ResNet)
@@ -114,10 +114,10 @@ int launch_lane_geom(const int32_t* pts, const int32_t* npts, const uint8_t* sta
                      int adjust, int bird_w, int bird_h, int32_t* area, int cap_area, int32_t* bird, ::adas_lane_geom* out, cudaStream_t st);
 // warp.cu: cv2.warpPerspective (INTER_LINEAR, constant black border) of device-resident BGR frames
 int launch_warp_perspective(const uint8_t* d_src, int B, int H, int W, const double* M_host, double* d_Minv, uint8_t* d_dst, int oh, int ow, cudaStream_t st);
-// stem_conv.cu: k x k stride-2 conv of the padded C=4 image (warp-level MMA, no patch matrix)
+// stem_conv.cu: k x k stride-1 or stride-2 conv of the padded C=4 image (warp-level MMA, no patch matrix)
 int stem_conv_supported(int Cout, int k, int pad);
-int launch_stem_conv_s2(const __half* img, int B, int H, int W, const __half* wq, const float* bias, int Cout, int k, int pad, int act,
-                        __half* out, int out_ld, int Ho, int Wo, cudaStream_t st);
+int launch_stem_conv(const __half* img, int B, int H, int W, const __half* wq, const float* bias, int Cout, int k, int pad, int stride, int act,
+                     __half* out, int out_ld, int Ho, int Wo, cudaStream_t st);
 int launch_zero_rows(__half* buf, int ld, int C, int row0, int nrows, cudaStream_t st);
 
 // ---- pre-processing (preprocess.cu) -----------------------------------------------------------
@@ -137,7 +137,7 @@ struct YoloLevel { const float* ptr; int ld; int H, W; int stride; int rows_per_
 int launch_yolov8_head_decode(const YoloLevel* lv /*3*/, int B, int nc, float* raw /*[B,4+nc,A]*/, int A,
                               cudaStream_t st);
 int launch_yolov5_head_decode(const YoloLevel* lv /*3*/, int B, int nc, float* raw /*[B,A,5+nc]*/, int A, int lite,
-                              cudaStream_t st);
+                              const float* anchors /*device [3][3][2], nullptr = YOLOv5 table*/, cudaStream_t st);
 int launch_yolov5_lite_post(float* raw /*[B,A,5+nc], in place*/, int B, int A, int nc, int in_h, int in_w, cudaStream_t st);
 struct YoloPostBufs {
     // device scratch, sized for max_batch

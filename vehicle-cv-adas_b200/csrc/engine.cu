@@ -7,6 +7,7 @@
 #include "common.h"
 #include "plan.h"
 #include "../../include/adas_b200.h"
+#include <math.h>
 #include <stdarg.h>
 #include <time.h>
 #include <stdlib.h>
@@ -326,7 +327,7 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
             case OP_STEMCONV: {
                 const PlanBuffer& ib = e->bufs[p[0]];
                 const PlanBuffer& ob = e->bufs[p[7]];
-                const int Cout = p[3], k = p[4], pad = p[5], act = p[6], out_coff = p[8];
+                const int Cout = p[3], k = p[4], pad = p[5], act = p[6], out_coff = p[8], stride = p[9] == 0 ? 2 : p[9];
                 ADAS_CHECK(ib.C == 4 && ib.dtype == 0 && ob.dtype == 0 && stem_conv_supported(Cout, k, pad) && out_coff % 8 == 0 && ob.C % 8 == 0, "op %zu: stem conv geometry", oi);
                 const __half* in = static_cast<const __half*>(e->dbufs[p[0]].ptr);
                 const __half* wq = static_cast<const __half*>(tensor_ptr(e, p[1]));
@@ -334,10 +335,10 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
                 __half* out = static_cast<__half*>(e->dbufs[p[7]].ptr) + out_coff;
                 const int H = (int)ib.H, W = (int)ib.W, Ho = (int)ob.H, Wo = (int)ob.W, out_ld = (int)ob.C;
                 char d[128];
-                snprintf(d, sizeof(d), "stem %dx%d s2 p%d 3->%d, %dx%d -> %dx%d, warp MMA from the image", k, k, pad, Cout, H, W, Ho, Wo);
+                snprintf(d, sizeof(d), "stem %dx%d s%d p%d 3->%d, %dx%d -> %dx%d, warp MMA from the image", k, k, stride, pad, Cout, H, W, Ho, Wo);
                 prog->step_desc.resize(prog->step_type.size());
                 prog->step_desc.back() = d;
-                prog->steps.push_back([=](cudaStream_t st) { return launch_stem_conv_s2(in, batch, H, W, wq, bias, Cout, k, pad, act, out, out_ld, Ho, Wo, st); });
+                prog->steps.push_back([=](cudaStream_t st) { return launch_stem_conv(in, batch, H, W, wq, bias, Cout, k, pad, stride, act, out, out_ld, Ho, Wo, st); });
                 break;
             }
             case OP_LAYERNORM: {
@@ -397,6 +398,12 @@ static int run_plan(adas_engine* e, int batch) {
     return 0;
 }
 
+// Anchor table of a YOLOv5-layout head: header meta[3] = 1 + index of an fp32 [3 levels x 3 anchors x 2] plan tensor, 0 = none (the
+// YOLOv5 table of yolo_post.cu; every plan written before the field existed has 0 there).
+static const float* yolo_anchors(const adas_engine* e) {
+    return e->hdr.meta[3] == 0 ? nullptr : static_cast<const float*>(tensor_ptr(e, (int)e->hdr.meta[3] - 1));
+}
+
 static int head_decode(adas_engine* e, int batch) {
     if (is_ufld(e->hdr.model_kind)) return 0;   // heads are the raw FC output buffer
     YoloLevel lv[3];
@@ -410,7 +417,7 @@ static int head_decode(adas_engine* e, int batch) {
     }
     const int nc = (int)e->hdr.meta[0], A = (int)e->hdr.meta[1];
     if (e->hdr.model_kind == ADAS_MODEL_YOLOV8) return launch_yolov8_head_decode(lv, batch, nc, e->d_raw, A, e->stream);
-    return launch_yolov5_head_decode(lv, batch, nc, e->d_raw, A, (int)e->hdr.meta[2], e->stream);
+    return launch_yolov5_head_decode(lv, batch, nc, e->d_raw, A, (int)e->hdr.meta[2], yolo_anchors(e), e->stream);
 }
 // YOLOV5_LITE plans (meta[2] != 0): the network output is the sigmoid-only head; the fused detect calls apply
 // YoloLiteParameters.lite_postprocess (yoloDetector.py:36-50) on the device before candidate selection.
@@ -559,6 +566,7 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
                 ADAS_CHECK(p[5] < 0 || (tensor_ok(p[5], (uint64_t)N * 4) && e->tensors[p[5]].dtype == 1), "plan %s: op %zu: bias tensor missing or too small", path, oi);
                 ADAS_CHECK(p[8] < 0 || (!transposed && view_ok(p[8], p[9], N) && e->bufs[p[8]].dtype == 0), "plan %s: op %zu: residual slice exceeds its buffer", path, oi);
                 ADAS_CHECK(p[15] >= 0 && p[15] <= 256 && p[17] >= 0 && p[17] <= 4 && (p[18] == 0 || p[18] == 1), "plan %s: op %zu: bad forced tile shape", path, oi);
+                ADAS_CHECK(p[7] >= 0 && p[7] <= 3, "plan %s: op %zu: unknown activation %d", path, oi, p[7]);
                 break;
             }
             case OP_IM2COL:
@@ -578,11 +586,12 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
                 ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[1]) && e->bufs[p[0]].H > 0 && e->bufs[p[1]].H > 0 && e->bufs[p[0]].C == 4 && e->bufs[p[1]].C == 64, "plan %s: op %zu: bad stem re-layout", path, oi);
                 break;
             case OP_STEMCONV: {
-                const int Cout = p[3], k = p[4];
-                ADAS_CHECK(buf_ok(p[0]) && e->bufs[p[0]].H > 0 && e->bufs[p[0]].C == 4 && Cout >= 8 && Cout <= 64 && k >= 3 && k <= 7 && p[5] >= 0 && p[5] <= 3 &&
+                const int Cout = p[3], k = p[4], s = p[9] == 0 ? 2 : p[9];          // p[9] = 0: stride 2 (plans without the field)
+                ADAS_CHECK(p[6] >= 0 && p[6] <= 3, "plan %s: op %zu: unknown activation %d", path, oi, p[6]);
+                ADAS_CHECK((s == 1 || s == 2) && buf_ok(p[0]) && e->bufs[p[0]].H > 0 && e->bufs[p[0]].C == 4 && Cout >= 8 && Cout <= 64 && k >= 3 && k <= 7 && p[5] >= 0 && p[5] <= 3 &&
                            view_ok(p[7], p[8], Cout) && e->bufs[p[7]].H > 0 && tensor_ok(p[1], (uint64_t)Cout * k * ((4 * k + 15) / 16 * 16) * 2) &&
                            (p[2] < 0 || tensor_ok(p[2], (uint64_t)Cout * 4)) &&
-                           e->bufs[p[7]].H == (e->bufs[p[0]].H + 2 * p[5] - k) / 2 + 1 && e->bufs[p[7]].W == (e->bufs[p[0]].W + 2 * p[5] - k) / 2 + 1,
+                           e->bufs[p[7]].H == (e->bufs[p[0]].H + 2 * p[5] - k) / s + 1 && e->bufs[p[7]].W == (e->bufs[p[0]].W + 2 * p[5] - k) / s + 1,
                            "plan %s: op %zu: bad stem conv", path, oi);
                 break;
             }
@@ -602,6 +611,10 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
         ADAS_CHECK(buf_ok((int)o.buffer) && (uint64_t)o.coff + o.C <= (uint64_t)e->bufs[o.buffer].C * (e->bufs[o.buffer].H > 0 ? 1u : e->bufs[o.buffer].rows_per_img) && o.C >= 1,
                    "plan %s: output %zu exceeds its buffer", path, i);
     }
+    // YOLO meta[3]: anchor table (yolo_anchors); its values are checked once the blob is read
+    ADAS_CHECK(is_ufld(h.model_kind) || h.meta[3] == 0 ||
+                   (h.model_kind == ADAS_MODEL_YOLOV5 && h.meta[2] == 0 && tensor_ok((int)h.meta[3] - 1, 18 * 4) && e->tensors[h.meta[3] - 1].dtype == 1),
+               "plan %s: anchor table (meta[3] = %u) is not an fp32 tensor of 3 x 3 x 2 values of a YOLOv5-layout head", path, h.meta[3]);
     if (h.n_outputs == 0) return 0;          // single-layer plans of the kernel tests: no network outputs, no head geometry
     if (h.model_kind == ADAS_MODEL_UFLDV2) {
         const uint64_t ngr = h.meta[0], ncr = h.meta[1], ngc = h.meta[2], ncc = h.meta[3], nl = h.meta[4];
@@ -653,6 +666,12 @@ int adas_engine_create(const char* plan_path, int device, int max_batch, int con
     ok = fread(blob.data(), 1, blob.size(), f) == blob.size();
     fclose(f);
     ADAS_CHECK(ok, "truncated plan blob in %s", plan_path);
+    if (!is_ufld(e->hdr.model_kind) && e->hdr.meta[3] != 0) {
+        float anc[18];
+        memcpy(anc, blob.data() + e->tensors[e->hdr.meta[3] - 1].offset, sizeof(anc));
+        for (int i = 0; i < 18; ++i)
+            ADAS_CHECK(isfinite(anc[i]) && anc[i] > 0.f, "plan %s: anchor %d of the head's table is %g (finite and positive required)", plan_path, i, (double)anc[i]);
+    }
 
     int ndev = 0;
     cudaError_t ce = cudaGetDeviceCount(&ndev);

@@ -198,6 +198,7 @@ conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
             const int n0 = n_t * BN;
             const int m0 = m_t * BMT;
             const int c0 = 2 * (lane & 3);
+            const float neg_slope = p.act == 3 ? 0.1f : 0.f;     // ReLU and LeakyReLU(0.1) share one instruction sequence
 #pragma unroll
             for (int mt = 0; mt < MTX; ++mt) {
                 if (mt >= g.MT) break;
@@ -251,7 +252,7 @@ conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                         if (rp != nullptr) rv = __half22float2(*reinterpret_cast<const __half2*>(rp + n));
                         if (p.res_ld < 0) { x0 += rv.x; x1 += rv.y; }
                         if (p.act == 1) silu2(x0, x1);
-                        else if (p.act == 2) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+                        else if (p.act >= 2) { x0 = relu_leaky(x0, neg_slope); x1 = relu_leaky(x1, neg_slope); }
                         if (p.res_ld > 0) { x0 += rv.x; x1 += rv.y; }
                         if (p.out_f32) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + (size_t)row * (size_t)p.out_ld + n) = make_float2(x0, x1);
                         else *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.out) + (size_t)row * (size_t)p.out_ld + n) = __floats2half2_rn(x0, x1);

@@ -17,7 +17,7 @@ struct PlanHeader {
     uint32_t model_kind;          // ADAS_MODEL_*
     uint32_t in_c, in_h, in_w;    // network input binding (NCHW semantic)
     uint32_t n_buffers, n_ops, n_tensors, n_outputs;
-    uint32_t meta[16];            // YOLO: [0]=nc [1]=n_anchors(total)   UFLD: [0]=ngr [1]=ncr [2]=ngc [3]=ncc [4]=nl [5]=total_dim
+    uint32_t meta[16];            // YOLO: [0]=nc [1]=n_anchors(total) [2]=lite [3]=1+anchor tensor (0: YOLOv5 table)   UFLD: [0]=ngr [1]=ncr [2]=ngc [3]=ncc [4]=nl [5]=total_dim
     uint64_t blob_offset, blob_bytes;
 };
 struct PlanBuffer {               // activation buffer: [batch * rows_per_img, C] elements
@@ -43,14 +43,16 @@ struct PlanOutput {
 #pragma pack(pop)
 
 enum PlanOpType : uint32_t {
-    OP_GEMM = 1,       // p: a_buf a_coff Kc ntaps w_tensor bias_tensor N act res_buf res_coff res_pre_act out_buf out_coff masked transposed BN s2 MT no_slab
+    OP_GEMM = 1,       // act: 0 none, 1 SiLU, 2 ReLU, 3 LeakyReLU(0.1)
+                       // p: a_buf a_coff Kc ntaps w_tensor bias_tensor N act res_buf res_coff res_pre_act out_buf out_coff masked transposed BN s2 MT no_slab
                        //    (BN / MT > 0 force the tile shape, no_slab = 1 one activation tile per 3x3 tap: test hooks;
                        //    0 = cost model + autotune)
     OP_IM2COL = 2,     // p: in_buf in_coff Cin kh kw stride pad out_buf
     OP_MAXPOOL = 3,    // p: in_buf in_coff C k s pad out_buf out_coff
     OP_UPSAMPLE2X = 4, // p: in_buf in_coff C out_buf out_coff
     OP_STEMPACK = 6,   // p: in_buf(image, C=4) out_buf : 7x7 stride-2 stem re-layout, see elementwise.cu stempack_kernel
-    OP_STEMCONV = 7,   // p: in_buf(image, C=4) w_tensor bias_tensor Cout k pad act out_buf out_coff : k x k stride-2 stem conv, stem_conv.cu
+    OP_STEMCONV = 7,   // p: in_buf(image, C=4) w_tensor bias_tensor Cout k pad act out_buf out_coff stride : k x k stem conv, stem_conv.cu
+                       //    (stride 1 or 2; 0 = 2)
                        //    (weights packed [Cout][k][round_up(4k,16)])
     OP_LAYERNORM = 5,  // p: in_buf d_len gamma_tensor beta_tensor out_buf d_norm ; f0 = eps (statistics over d_norm entries; the
                        //    other d_len - d_norm slab entries are structural zeros with gamma = beta = 0)

@@ -1,4 +1,4 @@
-// stem_conv.cu -- the first convolution of a network (k x k, stride 2, 3 input channels) read straight from the padded NHWC image.
+// stem_conv.cu -- the first convolution of a network (k x k, stride 1 or 2, 3 input channels) read straight from the padded NHWC image.
 //
 // Replaces, for the stem only, the patch-matrix route (im2col_kernel / stempack_kernel + a GEMM launch): the image has C = 4
 // (R, G, B, 0) per pixel, so the k pixels one output needs from one input row are k*4 CONTIGUOUS halves.  The reduction index is laid
@@ -18,7 +18,8 @@
 //   epilogue:    + bias -> activation -> fp16 -> per-warp staging in shared memory -> 16-byte coalesced stores of interior pixels.
 // Accumulation is fp32 in a fixed order, independent of the batch size and of the grid: frame k of a batch equals the batch-1 result.
 //
-// Reference: the conv stacks behind coreEngine.py:150-157 / 184-186 (first Conv of YOLOv8 [3x3 s2], YOLOv5 [6x6 s2 p2], ResNet [7x7 s2 p3]).
+// Reference: the conv stacks behind coreEngine.py:150-157 / 184-186 (first Conv of YOLOv8 [3x3 s2], YOLOv5 [6x6 s2 p2], ResNet [7x7 s2 p3],
+// YOLOv7 [3x3 s1 at full input resolution], YOLOv7-tiny [3x3 s2]).
 #include "common.h"
 #include "tc_common.cuh"
 #include "gemm_v3.h"
@@ -42,13 +43,13 @@ struct StemParams {
     __half* out;            // padded NHWC output (+ channel offset), row stride out_ld
     int B, Hp, Wp;          // padded input geometry (H + 2, W + 2)
     int Ho, Wo, out_ld;
-    int k, pad, KR, K;      // K = k * KR
+    int k, pad, stride, KR, K;   // K = k * KR
     int w_ld;               // shared-memory row stride of the weights (halves)
     int act, tiles_per_row, total_tiles;
 };
 
 template <int NT>
-__global__ void __launch_bounds__(STEM_THREADS) stem_conv_s2_kernel(const StemParams p) {
+__global__ void __launch_bounds__(STEM_THREADS) stem_conv_kernel(const StemParams p) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int w_ld = p.w_ld;                                          // halves
     __half* ws = reinterpret_cast<__half*>(smem);
@@ -74,10 +75,10 @@ __global__ void __launch_bounds__(STEM_THREADS) stem_conv_s2_kernel(const StemPa
         float acc[NT][4];
 #pragma unroll
         for (int j = 0; j < NT; ++j) { acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f; }
-        // padded input coordinates of tap (dy = 0, dx = 0) for output pixel (y, x): row 2y + 1 - pad, column 2x + 1 - pad
-        const int col_g = 2 * (x0 + g) + 1 - p.pad, col_g8 = col_g + 16;
+        // padded input coordinates of tap (dy = 0, dx = 0) for output pixel (y, x): row s*y + 1 - pad, column s*x + 1 - pad
+        const int col_g = p.stride * (x0 + g) + 1 - p.pad, col_g8 = col_g + 8 * p.stride;
         for (int dy = 0; dy < p.k; ++dy) {
-            const int row = 2 * y + 1 - p.pad + dy;
+            const int row = p.stride * y + 1 - p.pad + dy;
             const bool row_ok = row >= 0 && row < p.Hp;
             const size_t row_base = ((size_t)b * p.Hp + (row_ok ? row : 0)) * p.Wp;
             for (int ks = 0; ks < ksteps_row; ++ks) {
@@ -124,15 +125,16 @@ int stem_conv_supported(int Cout, int k, int pad) {
     return (Cout == 16 || Cout == 32 || Cout == 48 || Cout == 64) && k >= 3 && k <= 7 && pad >= 0 && pad <= 3;
 }
 
-int launch_stem_conv_s2(const __half* img, int B, int H, int W, const __half* wq, const float* bias, int Cout, int k, int pad, int act,
-                        __half* out, int out_ld, int Ho, int Wo, cudaStream_t st) {
+int launch_stem_conv(const __half* img, int B, int H, int W, const __half* wq, const float* bias, int Cout, int k, int pad, int stride, int act,
+                     __half* out, int out_ld, int Ho, int Wo, cudaStream_t st) {
     ADAS_CHECK(stem_conv_supported(Cout, k, pad), "stem_conv: unsupported shape Cout=%d k=%d pad=%d", Cout, k, pad);
-    ADAS_CHECK(Ho == (H + 2 * pad - k) / 2 + 1 && Wo == (W + 2 * pad - k) / 2 + 1 && out_ld % 8 == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0,
-               "stem_conv: output geometry %dx%d (ld %d) does not match a %dx%d stride-2 conv of %dx%d", Ho, Wo, out_ld, k, k, H, W);
+    ADAS_CHECK(stride == 1 || stride == 2, "stem_conv: stride %d (1 or 2)", stride);
+    ADAS_CHECK(Ho == (H + 2 * pad - k) / stride + 1 && Wo == (W + 2 * pad - k) / stride + 1 && out_ld % 8 == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0,
+               "stem_conv: output geometry %dx%d (ld %d) does not match a %dx%d stride-%d conv of %dx%d", Ho, Wo, out_ld, k, k, stride, H, W);
     StemParams p;
     p.img = img; p.wq = wq; p.bias = bias; p.out = out;
     p.B = B; p.Hp = H + 2; p.Wp = W + 2; p.Ho = Ho; p.Wo = Wo; p.out_ld = out_ld;
-    p.k = k; p.pad = pad; p.KR = (4 * k + 15) / 16 * 16; p.K = k * p.KR; p.act = act;
+    p.k = k; p.pad = pad; p.stride = stride; p.KR = (4 * k + 15) / 16 * 16; p.K = k * p.KR; p.act = act;
     p.tiles_per_row = (Wo + 15) / 16;
     p.total_tiles = B * Ho * p.tiles_per_row;
     // weight row stride = 16 (mod 64) halves: the 8-byte fragment loads of a half-warp (4 rows x 4 lanes) then cover all 32 banks once;
@@ -147,10 +149,10 @@ int launch_stem_conv_s2(const __half* img, int B, int H, int W, const __half* wq
     const int cap = n_sms * 3;                      // resident blocks only: the weight copy is per block, a warp walks ~20 tiles
     if (blocks > cap) blocks = cap;
     switch (Cout / 8) {
-        case 2: stem_conv_s2_kernel<2><<<blocks, STEM_THREADS, smem, st>>>(p); break;
-        case 4: stem_conv_s2_kernel<4><<<blocks, STEM_THREADS, smem, st>>>(p); break;
-        case 6: stem_conv_s2_kernel<6><<<blocks, STEM_THREADS, smem, st>>>(p); break;
-        default: stem_conv_s2_kernel<8><<<blocks, STEM_THREADS, smem, st>>>(p); break;
+        case 2: stem_conv_kernel<2><<<blocks, STEM_THREADS, smem, st>>>(p); break;
+        case 4: stem_conv_kernel<4><<<blocks, STEM_THREADS, smem, st>>>(p); break;
+        case 6: stem_conv_kernel<6><<<blocks, STEM_THREADS, smem, st>>>(p); break;
+        default: stem_conv_kernel<8><<<blocks, STEM_THREADS, smem, st>>>(p); break;
     }
     count_launch();
     ADAS_CUDA(cudaGetLastError());

@@ -118,9 +118,14 @@ struct WgmmaCols<OFF, 0> {
     static __device__ __forceinline__ void run(float*, uint64_t, uint64_t, uint32_t) {}
 };
 
+// max(x, x * s) for 0 <= s < 1: ReLU at s = 0, torch.nn.LeakyReLU(s) otherwise (x if x >= 0 else x * s), in the same three
+// instructions, so the unrolled GEMM epilogues carry one code path for both.  The + 0 turns the -0 that ReLU would give for x < 0
+// (x * 0 = -0) into +0, the bits fmaxf(x, 0) gives.
+__device__ __forceinline__ float relu_leaky(float x, float s) { return fmaxf(x, x * s) + 0.0f; }
+
 __device__ __forceinline__ float act_apply(float x, int act) {
     if (act == 1) return __fdividef(x, 1.0f + __expf(-x));   // SiLU
-    if (act == 2) return fmaxf(x, 0.0f);                     // ReLU
+    if (act >= 2) return relu_leaky(x, act == 3 ? 0.1f : 0.0f);   // ReLU, LeakyReLU(0.1)
     return x;
 }
 

@@ -63,10 +63,12 @@ int launch_yolov8_head_decode(const YoloLevel* lv, int B, int nc, float* raw, in
 
 // YOLOv5 Detect: per level fp32 [rows, ld>=3*(5+nc)], channel = anchor*(5+nc) + k.
 // raw[b][idx][5+nc], idx = level offset + anchor*H*W + y*W + x  (yoloDetector.py:45-48 ordering).
+// Anchor (w, h) pairs [level][anchor]: the plan's own table (YOLOv7) or, without one, the YOLOv5 table below.
 __constant__ float c_v5_anchors[18] = {10, 13, 16, 30, 33, 23, 30, 61, 62, 45, 59, 119, 116, 90, 156, 198, 373, 326};
 
 // lite != 0: the head of a YOLOv5-lite export -- sigmoid only, grid/anchor decode left to lite_postprocess (yoloDetector.py:36-50).
-__global__ void yolov5_decode_kernel(YoloLevel l0, YoloLevel l1, YoloLevel l2, int B, int nc, float* __restrict__ raw, int A, int lite) {
+__global__ void yolov5_decode_kernel(YoloLevel l0, YoloLevel l1, YoloLevel l2, int B, int nc, float* __restrict__ raw, int A, int lite,
+                                     const float* __restrict__ anchors) {
     const long long total = (long long)B * A;
     const int no = 5 + nc;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -88,17 +90,19 @@ __global__ void yolov5_decode_kernel(YoloLevel l0, YoloLevel l1, YoloLevel l2, i
         else {
             o[0] = (sx * 2.f - 0.5f + (float)x) * st;
             o[1] = (sy * 2.f - 0.5f + (float)y) * st;
-            o[2] = (sw * 2.f) * (sw * 2.f) * c_v5_anchors[li * 6 + an * 2];
-            o[3] = (sh * 2.f) * (sh * 2.f) * c_v5_anchors[li * 6 + an * 2 + 1];
+            const float aw = anchors ? anchors[li * 6 + an * 2] : c_v5_anchors[li * 6 + an * 2];
+            const float ah = anchors ? anchors[li * 6 + an * 2 + 1] : c_v5_anchors[li * 6 + an * 2 + 1];
+            o[2] = (sw * 2.f) * (sw * 2.f) * aw;
+            o[3] = (sh * 2.f) * (sh * 2.f) * ah;
         }
         for (int k = 4; k < no; ++k) o[k] = 1.f / (1.f + expf(-p[k]));
     }
 }
 
-int launch_yolov5_head_decode(const YoloLevel* lv, int B, int nc, float* raw, int A, int lite, cudaStream_t st) {
+int launch_yolov5_head_decode(const YoloLevel* lv, int B, int nc, float* raw, int A, int lite, const float* anchors, cudaStream_t st) {
     const long long total = (long long)B * A;
     int blocks = (int)((total + 127) / 128);
-    yolov5_decode_kernel<<<blocks, 128, 0, st>>>(lv[0], lv[1], lv[2], B, nc, raw, A, lite);
+    yolov5_decode_kernel<<<blocks, 128, 0, st>>>(lv[0], lv[1], lv[2], B, nc, raw, A, lite, anchors);
     count_launch();
     ADAS_CUDA(cudaGetLastError());
     return 0;

@@ -4,7 +4,7 @@ The reference hands `.onnx` / `.trt` files to ONNXRuntime / TensorRT (coreEngine
 ultralytics / yolov5 exports (README.md:53-58) and from `TrafficLaneDetector/convertPytorchToONNX.py:60-87` (UFLD).  This module
 is the H100 replacement of that ingestion step (SURVEY 8f rank 2): it reads the ONNX protobuf directly (the `onnx` package is
 not a dependency -- the wire format is parsed here), recovers the convolution / linear / LayerNorm parameters, recognises the
-architecture (YOLOv8 / YOLOv5 / UFLDv2, scale, class count, input size) and drives the same `plan.build_*` builders that the
+architecture (YOLOv8 / YOLOv5 / YOLOv7 / UFLDv2, scale, class count, input size) and drives the same `plan.build_*` builders that the
 state_dict path uses.  Nothing here runs the network: the graph is only a parameter container plus a shape oracle.
 
 How parameters are matched to layers:
@@ -329,11 +329,13 @@ def _is_module_name(name: str) -> bool:
 # ---------------------------------------------------------------------------------------------------------------
 @dataclass
 class ModelSpec:
-    kind: str                 # "yolov8" | "yolov5" | "ufldv2"
-    scale: str                # YOLO scale letter or ResNet depth ("18" / "34")
+    kind: str                 # "yolov8" | "yolov5" | "yolov7" | "ufldv2"
+    scale: str                # YOLO scale letter ("tiny" / "base" for YOLOv7) or ResNet depth ("18" / "34")
     nc: int = 80
     in_h: int = 640
     in_w: int = 640
+    act: Optional[str] = None            # YOLOv7: "silu" | "leaky"
+    anchors: Optional[Tuple[float, ...]] = None     # YOLOv7: 18 anchor sizes in pixels when the file carries them
 
 
 _V8_WIDTH = {16: "n", 32: "s", 48: "m", 64: "l", 80: "x"}
@@ -354,6 +356,8 @@ def recognise(model: OnnxModel) -> ModelSpec:
         if depth is None:
             raise Exception(f"UFLD backbone with {n3} 3x3 convolutions is not supported (ResNet-18/34 only)")
         return ModelSpec("ufldv2", depth, 0, in_h or 320, in_w or 1600)
+    if _is_yolov7(model, w):
+        return _recognise_yolov7(model, w, in_h, in_w)
     cout0, k0 = first.shape[0], first.shape[2]
     if cout0 not in _V8_WIDTH:
         raise Exception(f"unrecognised YOLO width: first convolution has {cout0} output channels")
@@ -379,6 +383,51 @@ def recognise(model: OnnxModel) -> ModelSpec:
     raise Exception(f"unrecognised first convolution {first.shape}")
 
 
+_V7_SUPPORTED = "YOLOv7 and YOLOv7-tiny (P5, 3 detection levels; the X / W6 / E6 / D6 / E6E variants are not supported)"
+
+
+def _is_yolov7(model: OnnxModel, w: OnnxWeights) -> bool:
+    """YOLOv7 family: RepConv / IDetect names where they survive, else the 2x2 stride-2 max pool of its MP blocks (YOLOv5 / v8 pool
+    5x5 only) or the ReOrg space-to-depth stem of the P6 models (first convolution on 12 channels)."""
+    if any("rbr_reparam" in n or "rbr_dense" in n or n.endswith(".implicit") for n in model.initializers):
+        return True
+    if any(n.op_type == "MaxPool" and list(n.attrs.get("kernel_shape", [])) == [2, 2] for n in model.nodes):
+        return True
+    return w.convs[0][1].shape[1] == 12
+
+
+def _recognise_yolov7(model: OnnxModel, w: OnnxWeights, in_h: int, in_w: int) -> ModelSpec:
+    first = w.convs[0][1]
+    stem = next(n for n in model.nodes if n.op_type == "Conv" and n.inputs[1] == w.convs[0][0])
+    stride0 = list(stem.attrs.get("strides", [1, 1]))[0]
+    heads = [(name, cw) for name, cw, _ in w.convs if re.fullmatch(r"model\.\d+\.m\.\d+\.weight", name)]
+    if not heads:                               # names lost: the detection convs are the trailing 1x1 convs with 3 * (nc + 5) outputs
+        tail = w.convs[::-1]
+        no = tail[0][1].shape[0]
+        n = 0
+        while n < len(tail) and tail[n][1].shape[0] == no and tail[n][1].shape[2:] == (1, 1):
+            n += 1
+        heads = [(name, cw) for name, cw, _ in tail[:n][::-1]]
+    no = heads[-1][1].shape[0]
+    if first.shape != (32, 3, 3, 3) or stride0 not in (1, 2) or len(heads) != 3 or no % 3 != 0 or (in_h and in_h > 1024):
+        raise Exception(f"YOLOv7-family file outside the supported models: first convolution {tuple(first.shape)} stride {stride0}, "
+                        f"{len(heads)} detection levels, input {in_h}x{in_w}; supported: {_V7_SUPPORTED}")
+    scale = "base" if stride0 == 1 else "tiny"
+    named = re.fullmatch(r"model\.(\d+)\.m\.\d+\.weight", heads[-1][0])
+    if named and int(named.group(1)) != {"base": 105, "tiny": 77}[scale]:
+        raise Exception(f"YOLOv7 head at layer {named.group(1)} does not match the {scale} graph; supported: {_V7_SUPPORTED}")
+    act = "leaky" if any(n.op_type == "LeakyRelu" for n in model.nodes) else "silu"
+    anchors = None
+    grids = [v for k, v in model.initializers.items() if k.endswith("anchor_grid") and v.size == 18]
+    if not grids:                               # constant-folded exports: one [1, 3, 1, 1, 2] anchor tensor per level, in graph order
+        per_level = [v for k, v in model.initializers.items() if tuple(v.shape) == (1, 3, 1, 1, 2) and v.dtype.kind == "f"]
+        if len(per_level) == 3:
+            grids = [np.concatenate([g.reshape(6) for g in per_level])]
+    if grids:
+        anchors = tuple(float(v) for v in np.asarray(grids[0], np.float32).reshape(18))
+    return ModelSpec("yolov7", scale, no // 3 - 5, in_h or 640, in_w or 640, act, anchors)
+
+
 def build_plan(model: OnnxModel, spec: Optional[ModelSpec] = None) -> "plan.PlanBuilder":
     spec = spec or recognise(model)
     w = OnnxWeights(model)
@@ -386,6 +435,8 @@ def build_plan(model: OnnxModel, spec: Optional[ModelSpec] = None) -> "plan.Plan
         return plan.build_yolov8(w, spec.scale, nc=spec.nc, in_h=spec.in_h, in_w=spec.in_w)
     if spec.kind == "yolov5":
         return plan.build_yolov5(w, spec.scale, nc=spec.nc, in_h=spec.in_h, in_w=spec.in_w)
+    if spec.kind == "yolov7":
+        return plan.build_yolov7(w, spec.scale, nc=spec.nc, in_h=spec.in_h, in_w=spec.in_w, act=spec.act, anchors=spec.anchors)
     if spec.kind == "ufldv2":
         # the dataset follows from the input binding (ModelConfig: CULane 320x1600, TuSimple 320x800); the engine rejects any other
         cfg = dict(plan.UFLD_TUSIMPLE if (spec.in_h, spec.in_w) == (320, 800) else plan.UFLD_CULANE)

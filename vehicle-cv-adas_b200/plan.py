@@ -7,10 +7,10 @@ ONNX and building a TensorRT engine, the weights are BN-folded, cast to fp16, la
 C++ runtime replays (csrc/plan.h documents the binary layout).
 
 Network graphs
-  * YOLOv8 (ultralytics 8.1 `yolov8.yaml`, README.md:56 of the reference) and YOLOv5 v6.2
-    (`yolov5{n,s,...}.yaml`, README.md:53): not shipped by the reference; restated from the public
-    architecture (SURVEY.md Appendix A), state_dict keys follow the upstream naming so real
-    checkpoints can be packed.
+  * YOLOv8 (ultralytics 8.1 `yolov8.yaml`, README.md:56 of the reference), YOLOv5 v6.2
+    (`yolov5{n,s,...}.yaml`, README.md:53) and YOLOv7 / YOLOv7-tiny (`cfg/training/yolov7{,-tiny}.yaml`):
+    not shipped by the reference; restated from the public architecture (SURVEY.md Appendix A),
+    state_dict keys follow the upstream naming so real checkpoints can be packed.
   * UFLDv2: TrafficLaneDetector/ufldDetector/exportLib/ultrafastLaneV2/model_culane.py:7-63 and
     backbone.py:14-58 (torchvision ResNet18/34 trunk -> 1x1 pool conv -> LayerNorm -> MLP).
 
@@ -32,7 +32,7 @@ import numpy as np
 
 MODEL_YOLOV8, MODEL_YOLOV5, MODEL_UFLDV2, MODEL_UFLDV1 = 0, 1, 2, 4      # 3 = ADAS_MODEL_YOLOV5_LITE (post-processing kind only)
 OP_GEMM, OP_IM2COL, OP_MAXPOOL, OP_UPSAMPLE2X, OP_LAYERNORM, OP_STEMPACK, OP_STEMCONV = 1, 2, 3, 4, 5, 6, 7
-ACT_NONE, ACT_SILU, ACT_RELU = 0, 1, 2
+ACT_NONE, ACT_SILU, ACT_RELU, ACT_LEAKY = 0, 1, 2, 3          # ACT_LEAKY: LeakyReLU(0.1)
 PLAN_VERSION = 1
 
 
@@ -81,7 +81,9 @@ class Weights:
         r = self._rng(name)
         for pat, val in self.profile.get("fill", ()):       # e.g. detection-head biases that set the score operating point
             if re.fullmatch(pat, name):
-                a = np.full(shape, val, np.float32)
+                a = np.full(shape, val[1] if isinstance(val, tuple) else val, np.float32)
+                if isinstance(val, tuple):                  # (xywh, objectness + classes) of each of the 3 anchors of a YOLOv5-layout head
+                    a.reshape(3, -1)[:, :4] = val[0]
                 self.state_dict[name] = a
                 return a
         if kind == "conv":
@@ -110,6 +112,10 @@ class Weights:
             a = r.uniform(0.9, 1.1, shape).astype(np.float32)
         elif kind == "ln_beta":
             a = (r.standard_normal(shape) * 0.02).astype(np.float32)
+        elif kind == "implicit_a":          # YOLOv7 ImplicitA: nn.init.normal_(mean=0, std=0.02)
+            a = (r.standard_normal(shape) * 0.02).astype(np.float32)
+        elif kind == "implicit_m":          # YOLOv7 ImplicitM: nn.init.normal_(mean=1, std=0.02)
+            a = (1.0 + r.standard_normal(shape) * 0.02).astype(np.float32)
         else:
             raise ValueError(kind)
         self.state_dict[name] = a
@@ -120,6 +126,10 @@ class Weights:
 
     # folded conv+BN: returns (w [Cout,Cin,kh,kw] fp32, b [Cout] fp32)
     def conv_bn(self, prefix: str, cout: int, cin: int, k: int, eps: float, conv_key="conv", bn_key="bn", res_branch=False):
+        wf, bf = self._conv_bn64(prefix, cout, cin, k, eps, conv_key, bn_key, res_branch)
+        return wf.astype(np.float32), bf.astype(np.float32)
+
+    def _conv_bn64(self, prefix: str, cout: int, cin: int, k: int, eps: float, conv_key="conv", bn_key="bn", res_branch=False):
         w = self.get(f"{prefix}.{conv_key}.weight" if conv_key else f"{prefix}.weight", (cout, cin, k, k), "conv")
         bn = f"{prefix}.{bn_key}"
         g = self.get(f"{bn}.weight", (cout,), "bn_gamma_res" if res_branch else "bn_gamma")
@@ -129,9 +139,35 @@ class Weights:
         if not self.real and f"{bn}.num_batches_tracked" not in self.state_dict:
             self.state_dict[f"{bn}.num_batches_tracked"] = np.zeros((), dtype=np.int64)
         scale = (g.astype(np.float64) / np.sqrt(v.astype(np.float64) + eps))
-        wf = (w.astype(np.float64) * scale[:, None, None, None]).astype(np.float32)
-        bf = (b.astype(np.float64) - m.astype(np.float64) * scale).astype(np.float32)
-        return wf, bf
+        return w.astype(np.float64) * scale[:, None, None, None], b.astype(np.float64) - m.astype(np.float64) * scale
+
+    def repconv(self, prefix: str, cout: int, cin: int, eps: float):
+        """YOLOv7 RepConv (3x3, no identity branch: c1 != c2 in every P5 head) as one folded 3x3 conv: BN-folded rbr_dense + BN-folded
+        rbr_1x1 on the centre tap, summed in fp64.  A checkpoint that was re-parameterised upstream carries `rbr_reparam` instead."""
+        if f"{prefix}.rbr_reparam.weight" in self.state_dict or (self.real and f"{prefix}.rbr_dense.0.weight" not in self.state_dict):
+            return self.conv_bias(f"{prefix}.rbr_reparam", cout, cin, 3)
+        assert cin != cout and f"{prefix}.rbr_identity.running_var" not in self.state_dict, f"{prefix}: RepConv with an identity branch"
+        wd, bd = self._conv_bn64(f"{prefix}.rbr_dense", cout, cin, 3, eps, conv_key="0", bn_key="1")
+        w1, b1 = self._conv_bn64(f"{prefix}.rbr_1x1", cout, cin, 1, eps, conv_key="0", bn_key="1")
+        wd[:, :, 1, 1] += w1[:, :, 0, 0]
+        return wd.astype(np.float32), (bd + b1).astype(np.float32)
+
+    def implicit_head(self, prefix: str, li: int, no: int, cin: int):
+        """YOLOv7 IDetect level li: im * (m(x + ia)) folded into the 1x1 conv, w' = im * w, b' = im * (b + w @ ia) in fp64.  Files
+        fused upstream (IDetect.fuse) carry the folded m.li conv and no implicit tensors."""
+        w, b = self.conv_bias(f"{prefix}.m.{li}", no, cin, 1)
+        ka, km = f"{prefix}.ia.{li}.implicit", f"{prefix}.im.{li}.implicit"
+        if self.real and ka not in self.state_dict:
+            return w, b
+        ia = self.get(ka, (1, cin, 1, 1), "implicit_a").astype(np.float64).reshape(cin)
+        im = self.get(km, (1, no, 1, 1), "implicit_m").astype(np.float64).reshape(no)
+        w64 = w.astype(np.float64)
+        return (w64 * im[:, None, None, None]).astype(np.float32), (im * (b.astype(np.float64) + w64[:, :, 0, 0] @ ia)).astype(np.float32)
+
+    def anchor_grid(self, prefix: str) -> Optional[np.ndarray]:
+        """Anchors in input pixels from an upstream Detect / IDetect `anchor_grid` buffer ([3, 1, 3, 1, 1, 2]), when the source has one."""
+        a = self.state_dict.get(f"{prefix}.anchor_grid")
+        return None if a is None or a.size != 18 else np.asarray(a, np.float32).reshape(18)
 
     def conv_bias(self, prefix: str, cout: int, cin: int, k: int):
         w = self.get(f"{prefix}.weight", (cout, cin, k, k), "conv")
@@ -156,6 +192,12 @@ SYNTH_PROFILES = {
     # lane existence: random heads give P(valid) = 0.5 per anchor, i.e. no lane passes the "more than half / a quarter of the anchors
     # valid" test and nothing downstream of the decode is exercised; +1.0 on the "valid" logits makes ~88 % of the anchors valid
     "ufldv2": {"ufld_exist_bias": 1.0},
+    # YOLOv7 base (model.105, SiLU) and tiny (model.77, LeakyReLU).  The tiny net's activations are not damped layer by layer as with
+    # SiLU: its fp16 noise at the head is ~50x larger, so its head gain is 0.3, its objectness / class biases (-0.2) set the operating
+    # point and its box biases sit at -3, where the xywh sigmoids are flat (box noise 0.4 px -> 0.01 px).  CPU fp16 emulation on
+    # 4 frames: base 6.1e-4 / 0.10 px / ~280 candidates per frame, tiny 5.9e-4 / 0.01 px / ~100 candidates per frame.
+    "yolov7": {"gains": [(r"model\.105\.m\.\d\.weight", 16.0), (r"model\.77\.m\.\d\.weight", 0.3)],
+               "fill": [(r"model\.105\.m\.\d\.bias", -3.0), (r"model\.77\.m\.\d\.bias", (-3.0, -0.2))]},
 }
 
 
@@ -247,9 +289,9 @@ class PlanBuilder:
         if out is None:
             out = self.new_padded(Ho, Wo, n_store, f32=out_f32)
         assert out.H == Ho and out.W == Wo, (out, Ho, Wo)
-        if (self.stem_direct and x.buf == self.image.buf and x.C == 4 and s == 2 and 3 <= k <= 7 and cout in (16, 32, 48, 64) and res is None
+        if (self.stem_direct and x.buf == self.image.buf and x.C == 4 and s in (1, 2) and 3 <= k <= 7 and cout in (16, 32, 48, 64) and res is None
                 and not out_f32 and tile is None and out.coff % 8 == 0):
-            return self.stem_conv(x, w, b, k, pad, act, out)
+            return self.stem_conv(x, w, b, k, s, pad, act, out)
         wk = np.transpose(w, (0, 2, 3, 1)).reshape(cout, k * k * cin)   # [Cout, kh, kw, Cin]
         if n_store != cout:
             wk = np.concatenate([wk, np.zeros((n_store - cout, wk.shape[1]), np.float32)], 0)
@@ -282,8 +324,8 @@ class PlanBuilder:
                            out.buf, out.coff, 1, 0, bn, s2, mt, 1 if no_slab else 0])
         return View(out.buf, out.coff, cout, Ho, Wo)
 
-    def stem_conv(self, x: View, w: np.ndarray, b: Optional[np.ndarray], k: int, pad: int, act: int, out: View) -> View:
-        """k x k stride-2 conv of the C=4 image by stem_conv.cu (no patch matrix): weights packed [Cout][k][KR], KR = round_up(4k, 16),
+    def stem_conv(self, x: View, w: np.ndarray, b: Optional[np.ndarray], k: int, s: int, pad: int, act: int, out: View) -> View:
+        """k x k stride-1 or stride-2 conv of the C=4 image by stem_conv.cu (no patch matrix): weights packed [Cout][k][KR], KR = round_up(4k, 16),
         element [dy][dx*4 + c] -- one 16-wide k-step of the warp MMA is a run of consecutive bytes of one image row.
         `w` arrives zero-padded to 4 input channels."""
         cout = int(w.shape[0])
@@ -293,7 +335,7 @@ class PlanBuilder:
         w_t = self.tensor(wq.astype(np.float16))
         bias_t = self.tensor(b.astype(np.float32)) if b is not None else -1
         self.stem_flops_per_img += 2 * out.H * out.W * cout * 3 * k * k
-        self._op(OP_STEMCONV, [x.buf, w_t, bias_t, cout, k, pad, act, out.buf, out.coff])
+        self._op(OP_STEMCONV, [x.buf, w_t, bias_t, cout, k, pad, act, out.buf, out.coff, 0 if s == 2 else s])   # 0 = stride 2
         return View(out.buf, out.coff, cout, out.H, out.W)
 
     def stem7x7s2(self, x: View, w: np.ndarray, b: np.ndarray, act: int) -> View:
@@ -549,6 +591,171 @@ def build_yolov5(weights: Weights, scale: str = "n", nc: int = 80, in_h: int = 6
     pb.meta[0], pb.meta[1] = nc, A
     pb.meta[2] = 1 if lite else 0
     return pb
+
+
+# ---------------------------------------------------------------------------------------------
+# YOLOv7 / YOLOv7-tiny (cfg/training/yolov7.yaml, yolov7-tiny.yaml; P5 models only)
+# ---------------------------------------------------------------------------------------------
+YOLOV5_ANCHORS = ((10, 13, 16, 30, 33, 23), (30, 61, 62, 45, 59, 119), (116, 90, 156, 198, 373, 326))
+YOLOV7_ANCHORS = ((12, 16, 19, 36, 40, 28), (36, 75, 76, 55, 72, 146), (142, 110, 192, 243, 459, 401))
+YOLOV7_ACTS = {"silu": ACT_SILU, "leaky": ACT_LEAKY}
+
+
+def build_yolov7(weights: Weights, scale: str = "tiny", nc: int = 80, in_h: int = 640, in_w: int = 640, act: Optional[str] = None,
+                 anchors=None) -> PlanBuilder:
+    """YOLOv7 ("base", SiLU) or YOLOv7-tiny ("tiny", LeakyReLU(0.1); act="silu" gives the tiny-SiLU variant).  The head decodes like
+    YOLOv5's ([B, 25200, 5 + nc], MODEL_YOLOV5 kind) with the anchor table carried by the plan (header meta[3]).
+    RepConv (base head) and IDetect's implicit layers are folded here in fp64; an ELAN's two 1x1 convolutions on the same input run
+    as one GEMM writing the last two slices of its concat."""
+    assert scale in ("tiny", "base"), f"YOLOv7 scale {scale!r}: 'tiny' or 'base' (the X / W6 / E6 / D6 / E6E variants are not supported)"
+    act_id = YOLOV7_ACTS[act or ("leaky" if scale == "tiny" else "silu")]
+    pb = PlanBuilder(MODEL_YOLOV5, 3, in_h, in_w)
+    W = weights
+    eps = BN_EPS_YOLO
+
+    def cbs(x: View, name: str, cout: int, k: int, s: int = 1, out: Optional[View] = None, cin: Optional[int] = None) -> View:
+        w, b = W.conv_bn(name, cout, cin if cin is not None else x.C, k, eps)
+        return pb.conv(x, w, b, k, s, act_id, out=out)
+
+    def elan(x: View, i: int, c: int, c3: int, n3: int, cout: int, out: Optional[View] = None, keep=None) -> View:
+        """a = model.i, b = model.i+1 (1x1 on x), n3 chained 3x3 convs from b (model.i+2 ..), concat model.i+2+n3 of the kept 3x3
+        outputs in reverse order, then b, a; then the 1x1 model.i+3+n3.  `keep`: 0-based 3x3 positions in the concat (default all)."""
+        keep = list(range(n3)) if keep is None else list(keep)
+        cat = pb.new_padded(x.H, x.W, len(keep) * c3 + 2 * c)
+        wa, ba = W.conv_bn(f"model.{i}", c, x.C, 1, eps)
+        wb, bb = W.conv_bn(f"model.{i + 1}", c, x.C, 1, eps)
+        ab = pb.conv(x, np.concatenate([wb, wa], 0), np.concatenate([bb, ba]), 1, 1, act_id, out=pb.sub(cat, len(keep) * c3, 2 * c))
+        t = pb.sub(ab, 0, c)
+        for j in range(n3):
+            slot = keep[::-1].index(j) if j in keep else None
+            t = cbs(t, f"model.{i + 2 + j}", c3, 3, out=pb.sub(cat, slot * c3, c3) if slot is not None else None)
+        return cbs(cat, f"model.{i + 3 + n3}", cout, 1, out=out)
+
+    def mp_block(x: View, i: int, c: int, out: View) -> View:
+        """model.i MaxPool 2x2 s2; model.i+1 = 1x1 of the pool, model.i+2 = 1x1 of x, model.i+3 = 3x3 s2 of model.i+2;
+        out = [model.i+3, model.i+1, ...] (channel slices 0 and 1 of `out`)."""
+        p = pb.maxpool(x, 2, 2, 0)
+        cbs(p, f"model.{i + 1}", c, 1, out=pb.sub(out, c, c))
+        t = cbs(x, f"model.{i + 2}", c, 1)
+        cbs(t, f"model.{i + 3}", c, 3, 2, out=pb.sub(out, 0, c))
+        return out
+
+    def pools(x: View, cat: View, slots: List[int]) -> None:
+        """max pools 5, 9, 13 (stride 1, "same" padding) of x into the channel slots of `cat`: 9 and 13 as chained 5x5 pools (exact for
+        max pooling whose padding never wins; the pool op takes k <= 7)."""
+        y = x
+        for sl in slots:
+            y = pb.maxpool(y, 5, 1, 2, out=pb.sub(cat, sl * x.C, x.C))
+
+    H, Wd = in_h, in_w
+    if scale == "base":
+        x = cbs(pb.image, "model.0", 32, 3, 1, cin=3)
+        x = cbs(x, "model.1", 64, 3, 2)
+        x = cbs(x, "model.2", 64, 3, 1)
+        x = cbs(x, "model.3", 128, 3, 2)
+        bk = (1, 3)                                          # backbone ELAN: cat[3x3 #4, 3x3 #2, b, a]
+        x = elan(x, 4, 64, 64, 4, 256, keep=bk)                                          # -> 11
+        x = elan(mp_block(x, 12, 128, pb.new_padded(H // 8, Wd // 8, 256)), 17, 128, 128, 4, 512, keep=bk)          # 16, -> 24
+        p3 = x
+        x = elan(mp_block(x, 25, 256, pb.new_padded(H // 16, Wd // 16, 512)), 30, 256, 256, 4, 1024, keep=bk)       # 29, -> 37
+        p4 = x
+        x = elan(mp_block(x, 38, 512, pb.new_padded(H // 32, Wd // 32, 1024)), 43, 256, 256, 4, 1024, keep=bk)      # 42, -> 50
+        cat93 = pb.new_padded(H // 32, Wd // 32, 1024)       # [92, 90, 51]
+        cat80 = pb.new_padded(H // 16, Wd // 16, 512)        # [79, 77, 63]
+        cat55 = pb.new_padded(H // 16, Wd // 16, 512)        # [54, up(52)]
+        cat67 = pb.new_padded(H // 8, Wd // 8, 256)          # [66, up(64)]
+        # 51 SPPCSPC(1024, 512), c_ = 512
+        c_ = 512
+        cat7 = pb.new_padded(x.H, x.W, 2 * c_)               # cv7 input [y1, y2]
+        sp = pb.new_padded(x.H, x.W, 4 * c_)                 # cv5 input [x1, p5, p9, p13]
+        t = cbs(x, "model.51.cv1", c_, 1)
+        t = cbs(t, "model.51.cv3", c_, 3)
+        x1 = cbs(t, "model.51.cv4", c_, 1, out=pb.sub(sp, 0, c_))
+        pools(x1, sp, [1, 2, 3])
+        t = cbs(sp, "model.51.cv5", c_, 1)
+        cbs(t, "model.51.cv6", c_, 3, out=pb.sub(cat7, 0, c_))
+        cbs(x, "model.51.cv2", c_, 1, out=pb.sub(cat7, c_, c_))
+        h51 = cbs(cat7, "model.51.cv7", 512, 1, out=pb.sub(cat93, 512, 512))
+        t = cbs(h51, "model.52", 256, 1)
+        pb.upsample2x(t, pb.sub(cat55, 256, 256))
+        cbs(p4, "model.54", 256, 1, out=pb.sub(cat55, 0, 256))
+        h63 = elan(cat55, 56, 256, 128, 4, 256, out=pb.sub(cat80, 256, 256))
+        t = cbs(h63, "model.64", 128, 1)
+        pb.upsample2x(t, pb.sub(cat67, 128, 128))
+        cbs(p3, "model.66", 128, 1, out=pb.sub(cat67, 0, 128))
+        h75 = elan(cat67, 68, 128, 64, 4, 128)
+        h88 = elan(mp_block(h75, 76, 128, cat80), 81, 256, 128, 4, 256)
+        h101 = elan(mp_block(h88, 89, 256, cat93), 94, 512, 256, 4, 512)
+        feats, det = [], 105
+        for i, (f, c2) in enumerate(((h75, 256), (h88, 512), (h101, 1024))):
+            w, b = W.repconv(f"model.{102 + i}", c2, f.C, eps)
+            feats.append(pb.conv(f, w, b, 3, 1, act_id))
+    else:
+        x = cbs(pb.image, "model.0", 32, 3, 2, cin=3)
+        x = cbs(x, "model.1", 64, 3, 2)
+        x = elan(x, 2, 32, 32, 2, 64)                                                    # -> 7
+        x = elan(pb.maxpool(x, 2, 2, 0), 9, 64, 64, 2, 128)                              # 8, -> 14
+        p3 = x
+        x = elan(pb.maxpool(x, 2, 2, 0), 16, 128, 128, 2, 256)                           # 15, -> 21
+        p4 = x
+        x = elan(pb.maxpool(x, 2, 2, 0), 23, 256, 256, 2, 512)                           # 22, -> 28
+        cat67 = pb.new_padded(H // 32, Wd // 32, 512)        # [66, 37]
+        cat59 = pb.new_padded(H // 16, Wd // 16, 256)        # [58, 47]
+        cat36 = pb.new_padded(H // 32, Wd // 32, 512)        # [35, 29]
+        cat34 = pb.new_padded(H // 32, Wd // 32, 1024)       # [p13, p9, p5, 30]
+        cat41 = pb.new_padded(H // 16, Wd // 16, 256)        # [40, up(38)]
+        cat51 = pb.new_padded(H // 8, Wd // 8, 128)          # [50, up(48)]
+        cbs(x, "model.29", 256, 1, out=pb.sub(cat36, 256, 256))
+        h30 = cbs(x, "model.30", 256, 1, out=pb.sub(cat34, 768, 256))
+        pools(h30, cat34, [2, 1, 0])
+        cbs(cat34, "model.35", 256, 1, out=pb.sub(cat36, 0, 256))
+        h37 = cbs(cat36, "model.37", 256, 1, out=pb.sub(cat67, 256, 256))
+        t = cbs(h37, "model.38", 128, 1)
+        pb.upsample2x(t, pb.sub(cat41, 128, 128))
+        cbs(p4, "model.40", 128, 1, out=pb.sub(cat41, 0, 128))
+        h47 = elan(cat41, 42, 64, 64, 2, 128, out=pb.sub(cat59, 128, 128))
+        t = cbs(h47, "model.48", 64, 1)
+        pb.upsample2x(t, pb.sub(cat51, 64, 64))
+        cbs(p3, "model.50", 64, 1, out=pb.sub(cat51, 0, 64))
+        h57 = elan(cat51, 52, 32, 32, 2, 64)
+        cbs(h57, "model.58", 128, 3, 2, out=pb.sub(cat59, 0, 128))
+        h65 = elan(cat59, 60, 64, 64, 2, 128)
+        cbs(h65, "model.66", 256, 3, 2, out=pb.sub(cat67, 0, 256))
+        h73 = elan(cat67, 68, 128, 128, 2, 256)
+        feats = [cbs(f, f"model.{74 + i}", c2, 3) for i, (f, c2) in enumerate(((h57, 128), (h65, 256), (h73, 512)))]
+        det = 77
+    # IDetect: m[i](ia[i](x)) * im[i], folded into the 1x1 head convolutions
+    no = 3 * (nc + 5)
+    A = 0
+    for li, (feat, stride) in enumerate(zip(feats, (8, 16, 32))):
+        w, b = W.implicit_head(f"model.{det}", li, no, feat.C)
+        head = pb.new_padded(feat.H, feat.W, (no + 7) // 8 * 8, f32=True)
+        pb.conv(feat, w, b, 1, 1, ACT_NONE, out=head, out_f32=True)
+        pb.outputs.append((head.buf, 0, head.C, stride))
+        A += 3 * feat.H * feat.W
+    if anchors is None:
+        anchors = W.anchor_grid(f"model.{det}")
+    if anchors is None:
+        anchors = YOLOV7_ANCHORS if scale == "base" else YOLOV5_ANCHORS
+    anc = np.asarray(anchors, np.float32).reshape(18)
+    assert np.all(np.isfinite(anc)) and np.all(anc > 0), f"anchors must be finite and positive: {anc}"
+    pb.meta[0], pb.meta[1] = nc, A
+    pb.meta[3] = pb.tensor(anc) + 1                          # 1 + tensor index; 0 = the YOLOv5 table (plans without the field)
+    return pb
+
+
+def read_anchors(path: str) -> np.ndarray:
+    """Anchor table [3 levels, 3 anchors, 2] a YOLOv5-layout plan decodes with: its own (header meta[3]) or the YOLOv5 table."""
+    with open(path, "rb") as f:
+        raw = f.read()
+    h = struct.unpack_from("<8sII3I4I16IQQ", raw)
+    n_buf, n_ops, n_t, meta, blob = h[6], h[7], h[8], h[10:26], h[26]
+    if meta[3] == 0:
+        return np.asarray(YOLOV5_ANCHORS, np.float32).reshape(3, 3, 2)
+    rec = struct.calcsize("<8sII3I4I16IQQ") + n_buf * 24 + n_ops * 112 + (meta[3] - 1) * 24
+    off, nbytes, _, _ = struct.unpack_from("<QQII", raw, rec)
+    assert meta[3] <= n_t and nbytes >= 72
+    return np.frombuffer(raw, np.float32, 18, blob + off).reshape(3, 3, 2).copy()
 
 
 # ---------------------------------------------------------------------------------------------

@@ -35,7 +35,10 @@ enum { ADAS_MODEL_YOLOV8 = 0, ADAS_MODEL_YOLOV5 = 1, ADAS_MODEL_UFLDV2 = 2,
         * (ObjectDetector/yoloDetector.py:36-50, model_type == ObjectModelType.YOLOV5_LITE) runs on the device first.  A lite PLAN
         * is a YOLOV5 plan whose header meta[2] != 0 (adas_engine_meta). */
        ADAS_MODEL_YOLOV5_LITE = 3,
-       ADAS_MODEL_UFLDV1 = 4 };   /* UFLD v1 plans (ultrafastLaneDetector.py): one head tensor [griding_num + 1, rows, 4] */
+       ADAS_MODEL_UFLDV1 = 4,     /* UFLD v1 plans (ultrafastLaneDetector.py): one head tensor [griding_num + 1, rows, 4] */
+       /* YOLOv6 (anchor-free EffiDeHead, meta[2] = reg_max: 0 = raw l,t,r,b distances, 16 = 17-bin DFL).  Its output has the YOLOv5
+        * layout [anchors, 5 + nc] with column 4 = 1.0, so `conf = cls * obj` (yoloDetector.py:111-124) is the class probability. */
+       ADAS_MODEL_YOLOV6 = 5 };
 
 /* ---- errors ------------------------------------------------------------------------- */
 /* replaces: Python `raise Exception(...)` in coreEngine.py:12-14,20,26 */

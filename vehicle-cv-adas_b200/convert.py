@@ -8,6 +8,11 @@ and `TrafficLaneDetector/convertPytorchToONNX.py:77-87` (UFLD `.pth` checkpoint 
     python -m adas_b200.convert culane_res34.pth --kind ufldv2 --backbone 34
     python -m adas_b200.convert yolov5n.pt.state_dict.pth --kind yolov5 --scale n
     python -m adas_b200.convert yolov7-tiny.state_dict.pth --kind yolov7 --scale tiny
+    python -m adas_b200.convert yolov6s.state_dict.pth --kind yolov6 --scale s
+
+Upstream YOLOv6 checkpoints pickle the whole model; extract its parameters once, in the YOLOv6 repository:
+    torch.save(torch.load("yolov6s.pt", map_location="cpu", weights_only=False)["model"].float().state_dict(), "yolov6s.state_dict.pth")
+Training-form (rbr_dense / rbr_1x1 / rbr_identity + BatchNorm) and deployed (rbr_reparam, fused conv biases) keys are both accepted.
 
 Checkpoints hold un-fused Conv/BatchNorm parameters under the upstream key names (the names `plan.build_*` ask for), so BatchNorm
 is folded here in float64 exactly as for the seeded weights.  Only the parameter dictionary is read: pickled model objects
@@ -52,6 +57,8 @@ def plan_from_state_dict(sd: Dict[str, np.ndarray], kind: str, scale: str = "l",
         return plan.build_yolov5(w, scale, nc=nc)
     if kind == "yolov7":
         return plan.build_yolov7(w, scale, nc=nc)
+    if kind == "yolov6":
+        return plan.build_yolov6(w, scale, nc=nc)
     if kind == "ufldv2":
         return plan.build_ufldv2(w, backbone)
     raise Exception(f"unsupported model kind {kind}")
@@ -66,7 +73,7 @@ def convert(path: str, out: Optional[str] = None, kind: Optional[str] = None, sc
         pb = build_plan(model, recognise(model))
     else:
         if kind is None:
-            raise Exception("--kind is required for checkpoint files (yolov8 | yolov5 | yolov7 | ufldv2)")
+            raise Exception("--kind is required for checkpoint files (yolov8 | yolov5 | yolov7 | yolov6 | ufldv2)")
         pb = plan_from_state_dict(load_checkpoint_state_dict(path), kind, scale, backbone, nc)
     pb.write(out)
     return out
@@ -76,8 +83,8 @@ def main(argv=None) -> int:
     ap = argparse.ArgumentParser(description="convert an .onnx model or a state_dict checkpoint to a .b200w plan")
     ap.add_argument("model")
     ap.add_argument("--out", default=None)
-    ap.add_argument("--kind", default=None, choices=["yolov8", "yolov5", "yolov7", "ufldv2"])
-    ap.add_argument("--scale", default="l", help="YOLO scale letter, or tiny | base for yolov7 (checkpoints only; ONNX files are recognised)")
+    ap.add_argument("--kind", default=None, choices=["yolov8", "yolov5", "yolov7", "yolov6", "ufldv2"])
+    ap.add_argument("--scale", default="l", help="YOLO scale letter (n | s | m | l for yolov6), or tiny | base for yolov7 (checkpoints only; ONNX files are recognised)")
     ap.add_argument("--backbone", default="34", choices=["18", "34"], help="UFLDv2 ResNet depth (checkpoints only)")
     ap.add_argument("--nc", type=int, default=80)
     a = ap.parse_args(argv)

@@ -58,7 +58,7 @@ class B200Engine(EngineBase):
     max_batch the reference is batch-1; batched calls are an extension (per-frame results are identical)
     """
 
-    OUTPUT_NAMES = {0: ["output0"], 1: ["output0"], 2: ["loc_row", "loc_col", "exist_row", "exist_col"], 4: ["output0"]}
+    OUTPUT_NAMES = {0: ["output0"], 1: ["output0"], 2: ["loc_row", "loc_col", "exist_row", "exist_col"], 4: ["output0"], 5: ["output0"]}
 
     def __init__(self, plan_path, device=None, max_batch=1, conv_impl=0):
         EngineBase.__init__(self, plan_path)

@@ -73,6 +73,10 @@ struct GemmParams {
     // bw x bh patch of output pixels of one image; s2_* describe the output grid and the input's padded height
     int s2, s2_bw, s2_bh, s2_tw, s2_th, s2_Ho, s2_Wo, s2_Hp_in;
     int transposed; // 1: out[n * out_ld + row] (swap-AB FC: rows = features, cols = batch), bias per row
+    // 1: 2x2 stride-2 transposed conv (ConvTranspose2d k=2 s=2 p=0) as a 1x1 GEMM with N = 4 * Cout, columns (dy, dx, c): input pixel
+    // (y, x) stores column group (dy, dx) to pixel (2y + dy, 2x + dx) of the (2H+2) x (2W+2) padded output (masked rows only)
+    int up2;
+    float res_scale;     // out = act(acc + bias) + res_scale * res (1 for a plain residual add)
     const float* bias;   // [N] ([M] when transposed) or nullptr
     const __half* res;   // residual, same row indexing as out, or nullptr
     void* out;
@@ -139,6 +143,9 @@ int launch_yolov8_head_decode(const YoloLevel* lv /*3*/, int B, int nc, float* r
 int launch_yolov5_head_decode(const YoloLevel* lv /*3*/, int B, int nc, float* raw /*[B,A,5+nc]*/, int A, int lite,
                               const float* anchors /*device [3][3][2], nullptr = YOLOv5 table*/, cudaStream_t st);
 int launch_yolov5_lite_post(float* raw /*[B,A,5+nc], in place*/, int B, int A, int nc, int in_h, int in_w, cudaStream_t st);
+// YOLOv6 level columns: 4 * (reg_max + 1) box columns (stored as 8-column groups), the nc class logits from the next multiple of 8 on
+__host__ __device__ inline unsigned yolov6_cls_col(unsigned reg_max) { return (4u * (reg_max + 1u) + 7u) / 8u * 8u; }
+int launch_yolov6_head_decode(const YoloLevel* lv /*3*/, int B, int nc, int reg_max, float* raw /*[B,A,5+nc]*/, int A, cudaStream_t st);
 struct YoloPostBufs {
     // device scratch, sized for max_batch
     int32_t* flags;      // [B, A] candidate flag

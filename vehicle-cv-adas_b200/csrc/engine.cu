@@ -133,6 +133,7 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
                 const int transposed = p[14];
                 int BN = p[15];
                 const int s2 = p[16];
+                const int up2 = p[19];
                 const PlanBuffer& ab = e->bufs[a_buf];
                 const PlanBuffer& ob = e->bufs[out_buf];
                 ADAS_CHECK(ab.dtype == 0, "op %zu: GEMM input buffer must be fp16", oi);
@@ -162,7 +163,7 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
                     opB = wptr; b_inner = (uint64_t)Ktot; b_rows_u = (uint64_t)N; b_stride = (uint64_t)Ktot * 2;
                     g.A = aptr; g.a_ld = (int)ab.C; g.Wt = wptr; g.w_ld = Ktot;
                     g.out_ld = (int)ob.C;
-                    ADAS_CHECK(s2 || (int)ob.rows_per_img == (int)ab.rows_per_img, "op %zu: GEMM in/out row geometry differs", oi);
+                    ADAS_CHECK(s2 || up2 || (int)ob.rows_per_img == (int)ab.rows_per_img, "op %zu: GEMM in/out row geometry differs", oi);
                     if (s2) {
                         // output-pixel patch (bw x bh <= 128) that wastes the fewest rows of the 128-row MMA tile
                         const int Ho = (int)ob.H, Wo = (int)ob.W;
@@ -218,6 +219,8 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
                 g.Kc = Kc; g.ntaps = ntaps; g.Wp = (int)ab.W + 2; g.kpt = (Kc + 63) / 64; g.BN = BN;
                 g.act = act; g.out_f32 = ob.dtype == 1 ? 1 : 0;
                 g.transposed = transposed;
+                g.up2 = up2;
+                g.res_scale = op.f[0] == 0.f ? 1.f : op.f[0];     // f[0] = 0 (plans without the field): plain residual add
                 g.bias = static_cast<const float*>(tensor_ptr(e, bias_t));
                 if (res_buf >= 0) {
                     const PlanBuffer& rb = e->bufs[res_buf];
@@ -226,6 +229,7 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
                 }
                 g.out = static_cast<uint8_t*>(e->dbufs[out_buf].ptr) + (size_t)out_coff * elem_size(ob.dtype);
                 if (masked) { g.mask_H = (int)ob.H; g.mask_W = (int)ob.W; ADAS_CHECK(ob.H > 0, "op %zu: masked store into a dense buffer", oi); }
+                if (up2) { g.mask_H = (int)ab.H; g.mask_W = (int)ab.W; }     // the mask walks the INPUT grid; stores go to the 2H x 2W output
                 if (e->conv_impl == 0) {
                     // ---- product path: gemm_v3.cu ----
                     void* opaque = nullptr;
@@ -417,6 +421,7 @@ static int head_decode(adas_engine* e, int batch) {
     }
     const int nc = (int)e->hdr.meta[0], A = (int)e->hdr.meta[1];
     if (e->hdr.model_kind == ADAS_MODEL_YOLOV8) return launch_yolov8_head_decode(lv, batch, nc, e->d_raw, A, e->stream);
+    if (e->hdr.model_kind == ADAS_MODEL_YOLOV6) return launch_yolov6_head_decode(lv, batch, nc, (int)e->hdr.meta[2], e->d_raw, A, e->stream);
     return launch_yolov5_head_decode(lv, batch, nc, e->d_raw, A, (int)e->hdr.meta[2], yolo_anchors(e), e->stream);
 }
 // YOLOV5_LITE plans (meta[2] != 0): the network output is the sigmoid-only head; the fused detect calls apply
@@ -552,10 +557,19 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
         const int32_t* p = op.p;
         switch (op.type) {
             case OP_GEMM: {
-                const int Kc = p[2], ntaps = p[3], N = p[6], transposed = p[14];
+                const int Kc = p[2], ntaps = p[3], N = p[6], transposed = p[14], up2 = p[19];
                 ADAS_CHECK(Kc >= 8 && Kc <= (1 << 20) && N >= 1 && N <= (1 << 20) && (ntaps == 1 || ntaps == 4 || ntaps == 9), "plan %s: op %zu: bad GEMM shape", path, oi);
                 ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[11]) && p[1] >= 0 && p[12] >= 0, "plan %s: op %zu: GEMM buffer index out of range", path, oi);
-                if (!transposed) {
+                ADAS_CHECK(up2 == 0 || up2 == 1, "plan %s: op %zu: bad transposed-conv flag %d", path, oi, up2);
+                ADAS_CHECK(isfinite(op.f[0]), "plan %s: op %zu: residual scale is not finite", path, oi);
+                if (up2) {
+                    // 2x2 stride-2 transposed conv: a 1x1 GEMM with N = 4 * Cout (Cout % 8 == 0) from an H x W grid into a 2H x 2W one
+                    const PlanBuffer &ab = e->bufs[p[0]], &ob = e->bufs[p[11]];
+                    ADAS_CHECK(N % 32 == 0 && ntaps == 1 && !transposed && !p[16] && p[8] < 0 && (p[15] == 0 || p[15] == 64 || p[15] == 128 || p[15] == 256) && ab.H > 0 && ob.H == 2 * ab.H && ob.W == 2 * ab.W &&
+                                   view_ok(p[0], p[1], Kc) && view_ok(p[11], p[12], N / 4),
+                               "plan %s: op %zu: transposed conv needs Cout %% 8 == 0, a 2H x 2W output of its H x W input and BN 64 / 128 / 256 if forced (Cout %d, %ux%u -> %ux%u)",
+                               path, oi, N / 4, ab.H, ab.W, ob.H, ob.W);
+                } else if (!transposed) {
                     ADAS_CHECK(view_ok(p[0], p[1], Kc) && view_ok(p[11], p[12], N), "plan %s: op %zu: GEMM channel slice exceeds its buffer", path, oi);
                 } else {
                     const PlanBuffer &ab = e->bufs[p[0]], &ob = e->bufs[p[11]];
@@ -631,8 +645,22 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
         ADAS_CHECK((int)h.meta[0] == ds->G && (int)h.meta[1] == ds->R && h.meta[4] == 4 && h.meta[5] == (uint64_t)(ds->G + 1) * ds->R * 4 && h.in_h == 288 && h.in_w == 800,
                    "plan %s: head %ux%u at %ux%u is not the UFLD v1 %s geometry its header names", path, h.meta[0], h.meta[1], h.in_h, h.in_w, ds->name);
     } else {
-        ADAS_CHECK(h.model_kind == ADAS_MODEL_YOLOV8 || h.model_kind == ADAS_MODEL_YOLOV5, "plan %s: unknown model kind %u", path, h.model_kind);
+        ADAS_CHECK(h.model_kind == ADAS_MODEL_YOLOV8 || h.model_kind == ADAS_MODEL_YOLOV5 || h.model_kind == ADAS_MODEL_YOLOV6, "plan %s: unknown model kind %u", path, h.model_kind);
         ADAS_CHECK(h.meta[0] >= 1 && h.meta[0] <= 1024 && h.meta[1] >= 1 && h.meta[1] <= (1u << 22), "plan %s: bad class / anchor counts", path);
+        if (h.model_kind == ADAS_MODEL_YOLOV6) {
+            const uint32_t reg_max = h.meta[2];
+            ADAS_CHECK(reg_max == 0 || reg_max == 16, "plan %s: YOLOv6 reg_max %u (0: raw distances, 16: 17-bin DFL)", path, reg_max);
+            ADAS_CHECK(h.n_outputs == 3, "plan %s: a YOLOv6 head has 3 levels", path);
+            uint64_t A = 0;
+            for (size_t i = 0; i < e->outs.size(); ++i) {
+                const PlanOutput& o = e->outs[i];
+                const PlanBuffer& b = e->bufs[o.buffer];
+                ADAS_CHECK(b.dtype == 1 && b.H > 0 && o.C >= yolov6_cls_col(reg_max) + h.meta[0], "plan %s: YOLOv6 level %zu is %u columns wide; reg_max %u and %u classes need %u",
+                           path, i, o.C, reg_max, h.meta[0], yolov6_cls_col(reg_max) + h.meta[0]);
+                A += (uint64_t)b.H * b.W;
+            }
+            ADAS_CHECK(A == h.meta[1], "plan %s: YOLOv6 levels hold %llu anchors, the header %u", path, (unsigned long long)A, h.meta[1]);
+        }
     }
     return 0;
 }
@@ -776,7 +804,7 @@ int adas_engine_output_shape(const adas_engine* e, int idx, int64_t s[4], int* r
     const uint32_t* m = e->hdr.meta;
     s[0] = 1; s[1] = s[2] = s[3] = 0;
     if (e->hdr.model_kind == ADAS_MODEL_YOLOV8) { ADAS_CHECK(idx == 0, "bad output index"); s[1] = 4 + m[0]; s[2] = m[1]; *rank = 3; }
-    else if (e->hdr.model_kind == ADAS_MODEL_YOLOV5) { ADAS_CHECK(idx == 0, "bad output index"); s[1] = m[1]; s[2] = 5 + m[0]; *rank = 3; }
+    else if (e->hdr.model_kind == ADAS_MODEL_YOLOV5 || e->hdr.model_kind == ADAS_MODEL_YOLOV6) { ADAS_CHECK(idx == 0, "bad output index"); s[1] = m[1]; s[2] = 5 + m[0]; *rank = 3; }
     else if (e->hdr.model_kind == ADAS_MODEL_UFLDV1) { ADAS_CHECK(idx == 0, "bad output index"); s[1] = m[0] + 1; s[2] = m[1]; s[3] = m[4]; *rank = 4; }   // [griding_num + 1, rows, lanes]
     else {
         ADAS_CHECK(idx >= 0 && idx < 4, "bad output index");
@@ -889,7 +917,8 @@ int adas_yolo_postprocess(int device, const float* raw_host, int model_kind, int
                           int in_w, int src_h, int src_w, double box_score, double nms_iou, int max_det, float* boxes_xywh,
                           float* scores, int32_t* class_ids, int32_t* cand_index, int32_t* counts, int32_t* n_candidates) {
     ADAS_CUDA(cudaSetDevice(device));
-    ADAS_CHECK(model_kind == ADAS_MODEL_YOLOV8 || model_kind == ADAS_MODEL_YOLOV5 || model_kind == ADAS_MODEL_YOLOV5_LITE, "adas_yolo_postprocess: bad model kind %d", model_kind);
+    ADAS_CHECK(model_kind == ADAS_MODEL_YOLOV8 || model_kind == ADAS_MODEL_YOLOV5 || model_kind == ADAS_MODEL_YOLOV5_LITE || model_kind == ADAS_MODEL_YOLOV6,
+               "adas_yolo_postprocess: bad model kind %d", model_kind);
     const size_t per = model_kind == ADAS_MODEL_YOLOV8 ? (size_t)(4 + n_classes) * n_anchors : (size_t)n_anchors * (5 + n_classes);
     float* d_raw = nullptr;
     ADAS_CUDA(cudaMalloc(&d_raw, (size_t)batch * per * 4));

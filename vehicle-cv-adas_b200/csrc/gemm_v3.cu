@@ -31,7 +31,9 @@
 
 namespace adas {
 
-template <int BN>
+// UP2: the 2x2 transposed-conv store (GemmParams::up2).  A separate instantiation (BN 64 / 128 / 256 only): its address arithmetic in the
+// unrolled epilogue costs the other instantiations spill slots, so they are compiled without it.
+template <int BN, bool UP2>
 __global__ void __launch_bounds__(V3_THREADS, 1)
 conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmV3 g) {
     constexpr int MTX = V3_ACC_COLS / BN >= 4 ? 4 : V3_ACC_COLS / BN >= 1 ? V3_ACC_COLS / BN : 1;   // sub-tiles held in registers
@@ -241,6 +243,29 @@ conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                         }
                         continue;
                     }
+                    if constexpr (UP2) {
+                        // 2x2 stride-2 transposed conv (no residual): column n = (2 dy + dx) * Cout + c of input pixel (yy, xx) goes to
+                        // output pixel (2 yy - 1 + dy, 2 xx - 1 + dx) of the (2H+2) x (2W+2) grid.  Cout % 8 == 0, so an 8-column
+                        // group lies in one (dy, dx).
+                        const int bi = fast_div(row, g.fd_img);
+                        const int pp = row - bi * g.fd_img.d;
+                        const int yy = fast_div(pp, g.fd_wp), xx = pp - yy * (p.mask_W + 2);
+                        const int Wo2 = 2 * p.mask_W + 2, co = p.N >> 2;
+                        const int up_row = (bi * (2 * p.mask_H + 2) + 2 * yy - 1) * Wo2 + 2 * xx - 1;
+#pragma unroll
+                        for (int j = 0; j < BN / 8; ++j) {
+                            const int n = n0 + 8 * j + c0;
+                            if (n0 + 8 * j >= p.N) break;
+                            float x0 = acc[mt][4 * j + 2 * h], x1 = acc[mt][4 * j + 2 * h + 1];
+                            if (p.bias != nullptr) { x0 += __ldg(p.bias + n); x1 += __ldg(p.bias + n + 1); }
+                            x0 = act_apply(x0, p.act); x1 = act_apply(x1, p.act);
+                            const int q = (n >= co) + (n >= 2 * co) + (n >= 3 * co);
+                            const size_t o = (size_t)(up_row + (q >> 1) * Wo2 + (q & 1)) * (size_t)p.out_ld + (n - q * co);
+                            if (p.out_f32) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + o) = make_float2(x0, x1);
+                            else *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.out) + o) = __floats2half2_rn(x0, x1);
+                        }
+                        continue;
+                    }
                     const __half* rp = p.res != nullptr ? p.res + (size_t)row * res_ld : nullptr;
 #pragma unroll
                     for (int j = 0; j < BN / 8; ++j) {
@@ -253,7 +278,7 @@ conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                         if (p.res_ld < 0) { x0 += rv.x; x1 += rv.y; }
                         if (p.act == 1) silu2(x0, x1);
                         else if (p.act >= 2) { x0 = relu_leaky(x0, neg_slope); x1 = relu_leaky(x1, neg_slope); }
-                        if (p.res_ld > 0) { x0 += rv.x; x1 += rv.y; }
+                        if (p.res_ld > 0) { x0 += p.res_scale * rv.x; x1 += p.res_scale * rv.y; }   // scale 1: the bits of a plain add
                         if (p.out_f32) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + (size_t)row * (size_t)p.out_ld + n) = make_float2(x0, x1);
                         else *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.out) + (size_t)row * (size_t)p.out_ld + n) = __floats2half2_rn(x0, x1);
                     }
@@ -267,14 +292,23 @@ conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
 // BN is a template parameter (the accumulator array and the wgmma widths are static): every multiple of 16 up to 256.
 #define V3_FOR_EACH_BN(X) X(16) X(32) X(48) X(64) X(80) X(96) X(112) X(128) X(144) X(160) X(176) X(192) X(208) X(224) X(240) X(256)
 
-static const void* v3_kernel(int BN) {
+static const void* v3_kernel(int BN, bool up2 = false) {
+    if (up2) {
+        switch (BN) {
+            case 64: return reinterpret_cast<const void*>(&conv_gemm_v3_kernel<64, true>);
+            case 128: return reinterpret_cast<const void*>(&conv_gemm_v3_kernel<128, true>);
+            case 256: return reinterpret_cast<const void*>(&conv_gemm_v3_kernel<256, true>);
+            default: return nullptr;
+        }
+    }
     switch (BN) {
-#define V3_CASE(b) case b: return reinterpret_cast<const void*>(&conv_gemm_v3_kernel<b>);
+#define V3_CASE(b) case b: return reinterpret_cast<const void*>(&conv_gemm_v3_kernel<b, false>);
         V3_FOR_EACH_BN(V3_CASE)
 #undef V3_CASE
         default: return nullptr;
     }
 }
+static bool v3_up2_tile(int BN) { return BN == 64 || BN == 128 || BN == 256; }
 
 struct V3Device { bool attr_set = false; int num_sms = 0; };
 static std::mutex g_v3_mu;
@@ -289,6 +323,7 @@ static int v3_device_state(int* num_sms) {
     if (!d.attr_set) {
         // function attributes are per device: set them once for every device an engine runs on
         for (int bn = 16; bn <= 256; bn += 16) ADAS_CUDA(cudaFuncSetAttribute(v3_kernel(bn), cudaFuncAttributeMaxDynamicSharedMemorySize, V3_DYN_SMEM_MAX));
+        for (int bn = 64; bn <= 256; bn *= 2) ADAS_CUDA(cudaFuncSetAttribute(v3_kernel(bn, true), cudaFuncAttributeMaxDynamicSharedMemorySize, V3_DYN_SMEM_MAX));
         ADAS_CUDA(cudaDeviceGetAttribute(&d.num_sms, cudaDevAttrMultiProcessorCount, dev));
         d.attr_set = true;
     }
@@ -320,8 +355,9 @@ static int env_int(const char* name, int dflt) {
 int gemm_v3_config(const GemmParams& p_in, GemmV3* g) {
     GemmParams p = p_in;
     static const int force_bn = env_int("ADAS_B200_BN", 0), force_mt = env_int("ADAS_B200_MT", 0);
-    if (force_bn >= 16 && force_bn <= 256 && force_bn % 16 == 0 && force_bn <= ((p.N + 15) / 16) * 16 && !p.transposed) p.BN = force_bn;   // test hook
+    if (force_bn >= 16 && force_bn <= 256 && force_bn % 16 == 0 && force_bn <= ((p.N + 15) / 16) * 16 && !p.transposed && !p.up2) p.BN = force_bn;   // test hook
     if (p.BN % 16 != 0 || p.BN < 16 || p.BN > 256) return 1;
+    if (p.up2 && !v3_up2_tile(p.BN)) return 1;                 // the transposed-conv store is compiled for BN 64 / 128 / 256
     g->p = p;
     g->MT = p.mt_hint >= 1 ? p.mt_hint : ((p.BN <= 128) ? 2 : 1);
     if (force_mt >= 1 && force_mt <= 4) g->MT = force_mt;     // test hook: exercise every sub-tile count
@@ -368,8 +404,8 @@ int gemm_v3_launch(const GemmV3Launch& L, cudaStream_t st) {
     static const int pdl = env_int("ADAS_B200_PDL", 1);
     GemmV3 gp = L.g;
     gp.pdl = pdl ? 1 : 0;
-    const void* fn = v3_kernel(gp.p.BN);
-    ADAS_CHECK(fn != nullptr, "gemm_v3: no kernel for BN %d", gp.p.BN);
+    const void* fn = v3_kernel(gp.p.BN, gp.p.up2 != 0);
+    ADAS_CHECK(fn != nullptr, "gemm_v3: no kernel for BN %d%s", gp.p.BN, gp.p.up2 ? " with the transposed-conv store" : "");
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(gp.total_tiles < num_sms ? gp.total_tiles : num_sms, 1, 1);
     cfg.blockDim = dim3(V3_THREADS, 1, 1);
@@ -405,6 +441,7 @@ int gemm_v3_candidates(const GemmParams& base, int max_out, int* BN_out, int* mt
         if (BN > N) { if (BN - N >= 64 || (BN % 64 == 0 && BN - N >= 16 && N > 64)) continue; BN = (N + 15) / 16 * 16; }
         if (BN > 256) continue;
         if (BN < 64 && N >= 64) continue;                        // narrow tiles only ever win on narrow layers
+        if (base.up2 && !v3_up2_tile(BN)) continue;
         const int n_tiles = (N + BN - 1) / BN;
         if ((double)n_tiles * BN > 1.35 * N) continue;           // too much padded-N work
         bool dup = false;
@@ -430,6 +467,7 @@ int gemm_v3_candidates(const GemmParams& base, int max_out, int* BN_out, int* mt
     }
     for (int i = 1; i < n; ++i) { C c = list[i]; int j = i - 1; while (j >= 0 && list[j].t > c.t) { list[j + 1] = list[j]; --j; } list[j + 1] = c; }
     if (n == 0) { list[0].BN = N <= 256 ? (N + 15) / 16 * 16 : 256; list[0].mt = 1; list[0].slab = 0; n = 1; }
+    if (base.up2 && !v3_up2_tile(list[0].BN)) list[0].BN = N >= 256 ? 256 : N >= 128 ? 128 : 64;
     int out = 0;
     for (int i = 0; i < n && out < max_out; ++i) {
         for (int ns = 0; ns <= list[i].slab && out < max_out; ++ns) {
@@ -473,9 +511,9 @@ int gemm_v3_run(void* opaque, cudaStream_t st) { return gemm_v3_launch(*static_c
 void gemm_v3_free(void* opaque) { delete static_cast<GemmV3Launch*>(opaque); }
 void gemm_v3_describe(const void* opaque, char* out, int cap) {
     const GemmV3& g = static_cast<const GemmV3Launch*>(opaque)->g;
-    snprintf(out, (size_t)cap, "M=%d N=%d K=%d taps=%d act=%d res=%d f32=%d s2=%d tr=%d | v3 BN=%d MT=%d slab=%d stages=%d tiles=%d", g.p.M,
-             g.p.N, g.p.Kc * g.p.ntaps, g.p.ntaps, g.p.act, g.p.res ? (g.p.res_ld < 0 ? -1 : 1) : 0, g.p.out_f32, g.p.s2, g.p.transposed, g.p.BN, g.MT,
-             g.slab, g.stages, g.total_tiles);
+    snprintf(out, (size_t)cap, "M=%d N=%d K=%d taps=%d act=%d res=%d f32=%d s2=%d tr=%d up2=%d | v3 BN=%d MT=%d slab=%d stages=%d tiles=%d", g.p.M,
+             g.p.N, g.p.Kc * g.p.ntaps, g.p.ntaps, g.p.act, g.p.res ? (g.p.res_ld < 0 ? -1 : 1) : 0, g.p.out_f32, g.p.s2, g.p.transposed, g.p.up2,
+             g.p.BN, g.MT, g.slab, g.stages, g.total_tiles);
 }
 
 }  // namespace adas

@@ -17,7 +17,8 @@ struct PlanHeader {
     uint32_t model_kind;          // ADAS_MODEL_*
     uint32_t in_c, in_h, in_w;    // network input binding (NCHW semantic)
     uint32_t n_buffers, n_ops, n_tensors, n_outputs;
-    uint32_t meta[16];            // YOLO: [0]=nc [1]=n_anchors(total) [2]=lite [3]=1+anchor tensor (0: YOLOv5 table)   UFLD: [0]=ngr [1]=ncr [2]=ngc [3]=ncc [4]=nl [5]=total_dim
+    uint32_t meta[16];            // YOLO: [0]=nc [1]=n_anchors(total) [2]=lite (YOLOv6: reg_max) [3]=1+anchor tensor (0: YOLOv5 table)
+                                  // UFLD: [0]=ngr [1]=ncr [2]=ngc [3]=ncc [4]=nl [5]=total_dim
     uint64_t blob_offset, blob_bytes;
 };
 struct PlanBuffer {               // activation buffer: [batch * rows_per_img, C] elements
@@ -45,8 +46,12 @@ struct PlanOutput {
 enum PlanOpType : uint32_t {
     OP_GEMM = 1,       // act: 0 none, 1 SiLU, 2 ReLU, 3 LeakyReLU(0.1)
                        // p: a_buf a_coff Kc ntaps w_tensor bias_tensor N act res_buf res_coff res_pre_act out_buf out_coff masked transposed BN s2 MT no_slab
+                       //    up2
                        //    (BN / MT > 0 force the tile shape, no_slab = 1 one activation tile per 3x3 tap: test hooks;
                        //    0 = cost model + autotune)
+                       //    up2 = 1: 2x2 stride-2 transposed conv, N = 4 * Cout in (dy, dx, c) order stored to pixel (2y+dy, 2x+dx)
+                       //    of a 2H x 2W output (Cout % 8 == 0; out_coff / the output slice hold Cout channels)
+                       // f: res_scale (0 = 1): out = act(acc + bias) + res_scale * res
     OP_IM2COL = 2,     // p: in_buf in_coff Cin kh kw stride pad out_buf
     OP_MAXPOOL = 3,    // p: in_buf in_coff C k s pad out_buf out_coff
     OP_UPSAMPLE2X = 4, // p: in_buf in_coff C out_buf out_coff

@@ -66,6 +66,7 @@ __global__ void gemm_simt_kernel(const GemmParams p) {
     const int n = ng * 8;
     if (row >= p.M || n >= p.N) return;
     bool row_ok = true;
+    long out_row = row;
     if (p.mask_H > 0) {
         const int Wp = p.mask_W + 2;
         const int img = (p.mask_H + 2) * Wp;
@@ -73,6 +74,11 @@ __global__ void gemm_simt_kernel(const GemmParams p) {
         const int yy = pp / Wp;
         const int xx = pp - yy * Wp;
         row_ok = (yy >= 1) && (yy <= p.mask_H) && (xx >= 1) && (xx <= p.mask_W);
+        if (p.up2) {
+            // 2x2 stride-2 transposed conv: column group (dy, dx) of input pixel (yy, xx) -> output pixel (2yy - 1 + dy, 2xx - 1 + dx)
+            const int co = p.N / 4, q = n / co;
+            out_row = ((long)(row / img) * (2 * p.mask_H + 2) + 2 * yy - 1 + q / 2) * (2 * p.mask_W + 2) + 2 * xx - 1 + q % 2;
+        }
     }
     if (!row_ok) return;
     float acc[8];
@@ -105,8 +111,9 @@ __global__ void gemm_simt_kernel(const GemmParams p) {
         if (p.bias) x += p.transposed ? p.bias[row] : p.bias[n + j];
         if (p.res != nullptr && p.res_ld < 0) x += __half2float(p.res[(size_t)row * (size_t)(-p.res_ld) + n + j]);
         x = act_apply(x, p.act);
-        if (p.res != nullptr && p.res_ld > 0) x += __half2float(p.res[(size_t)row * (size_t)p.res_ld + n + j]);
-        const size_t o = p.transposed ? ((size_t)(n + j) * p.out_ld + row) : ((size_t)row * p.out_ld + n + j);
+        if (p.res != nullptr && p.res_ld > 0) x += p.res_scale * __half2float(p.res[(size_t)row * (size_t)p.res_ld + n + j]);
+        const size_t o = p.transposed ? ((size_t)(n + j) * p.out_ld + row)
+                                      : p.up2 ? ((size_t)out_row * p.out_ld + (n + j) % (p.N / 4)) : ((size_t)row * p.out_ld + n + j);
         if (p.out_f32) reinterpret_cast<float*>(p.out)[o] = x;
         else reinterpret_cast<__half*>(p.out)[o] = __float2half_rn(x);
     }

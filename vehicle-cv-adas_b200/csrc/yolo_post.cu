@@ -61,6 +61,56 @@ int launch_yolov8_head_decode(const YoloLevel* lv, int B, int nc, float* raw, in
     return 0;
 }
 
+// YOLOv6 EffiDeHead (anchor-free): per level fp32 [rows, ld] in padded-grid row order: cols 0 .. 4(R+1)-1 the box (side-major: l, t, r, b
+// x R+1 bins; R = reg_max), class logits from yolov6_cls_col(R).  R = 0: the four columns are the distances; R = 16: softmax over the 17
+// bins projected on 0..16 (the fixed proj_conv).  raw[b][a][5+nc], a = level offset + y*W + x: cx, cy, w, h (input pixels), 1.0, the class
+// sigmoids -- the YOLOv5 layout, so `conf = cls * obj` of the v5 post-processing is exactly the class probability.
+__global__ void yolov6_decode_kernel(YoloLevel l0, YoloLevel l1, YoloLevel l2, int B, int nc, int reg_max, float* __restrict__ raw, int A) {
+    const long long total = (long long)B * A;
+    const int nb = reg_max + 1, cc = (int)yolov6_cls_col((unsigned)reg_max);
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int b = (int)(i / A);
+        int a = (int)(i % A);
+        YoloLevel lv = l0;
+        if (a >= l0.H * l0.W) { a -= l0.H * l0.W; lv = l1; if (a >= l1.H * l1.W) { a -= l1.H * l1.W; lv = l2; } }
+        const int y = a / lv.W, x = a % lv.W;
+        const float* p = lv.ptr + ((size_t)b * lv.rows_per_img + (size_t)(y + 1) * (lv.W + 2) + (x + 1)) * lv.ld;
+        float d[4];
+#pragma unroll
+        for (int s = 0; s < 4; ++s) {
+            if (reg_max == 0) { d[s] = p[s]; continue; }
+            float m = p[s * nb];
+            for (int k = 1; k < nb; ++k) m = fmaxf(m, p[s * nb + k]);
+            float den = 0.f, num = 0.f;
+            for (int k = 0; k < nb; ++k) {
+                const float e = expf(p[s * nb + k] - m);
+                den += e;
+                num += e * (float)k;
+            }
+            d[s] = num / den;
+        }
+        const float ax = (float)x + 0.5f, ay = (float)y + 0.5f;
+        const float x1 = ax - d[0], y1 = ay - d[1], x2 = ax + d[2], y2 = ay + d[3];
+        const float st = (float)lv.stride;
+        float* o = raw + (size_t)i * (5 + nc);
+        o[0] = (x1 + x2) * 0.5f * st;
+        o[1] = (y1 + y2) * 0.5f * st;
+        o[2] = (x2 - x1) * st;
+        o[3] = (y2 - y1) * st;
+        o[4] = 1.f;
+        for (int c = 0; c < nc; ++c) o[5 + c] = 1.f / (1.f + expf(-p[cc + c]));
+    }
+}
+
+int launch_yolov6_head_decode(const YoloLevel* lv, int B, int nc, int reg_max, float* raw, int A, cudaStream_t st) {
+    const long long total = (long long)B * A;
+    int blocks = (int)((total + 127) / 128);
+    yolov6_decode_kernel<<<blocks, 128, 0, st>>>(lv[0], lv[1], lv[2], B, nc, reg_max, raw, A);
+    count_launch();
+    ADAS_CUDA(cudaGetLastError());
+    return 0;
+}
+
 // YOLOv5 Detect: per level fp32 [rows, ld>=3*(5+nc)], channel = anchor*(5+nc) + k.
 // raw[b][idx][5+nc], idx = level offset + anchor*H*W + y*W + x  (yoloDetector.py:45-48 ordering).
 // Anchor (w, h) pairs [level][anchor]: the plan's own table (YOLOv7) or, without one, the YOLOv5 table below.

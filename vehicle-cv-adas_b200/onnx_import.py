@@ -329,13 +329,15 @@ def _is_module_name(name: str) -> bool:
 # ---------------------------------------------------------------------------------------------------------------
 @dataclass
 class ModelSpec:
-    kind: str                 # "yolov8" | "yolov5" | "yolov7" | "ufldv2"
+    kind: str                 # "yolov8" | "yolov5" | "yolov7" | "yolov6" | "ufldv2"
     scale: str                # YOLO scale letter ("tiny" / "base" for YOLOv7) or ResNet depth ("18" / "34")
     nc: int = 80
     in_h: int = 640
     in_w: int = 640
     act: Optional[str] = None            # YOLOv7: "silu" | "leaky"
     anchors: Optional[Tuple[float, ...]] = None     # YOLOv7: 18 anchor sizes in pixels when the file carries them
+    reg_max: int = 0                     # YOLOv6: 0 (raw l, t, r, b) or 16 (17-bin DFL)
+    acts: Optional[Tuple[str, str, str]] = None     # YOLOv6: activations of the body / neck / head roles, read from the graph
 
 
 _V8_WIDTH = {16: "n", 32: "s", 48: "m", 64: "l", 80: "x"}
@@ -356,6 +358,8 @@ def recognise(model: OnnxModel) -> ModelSpec:
         if depth is None:
             raise Exception(f"UFLD backbone with {n3} 3x3 convolutions is not supported (ResNet-18/34 only)")
         return ModelSpec("ufldv2", depth, 0, in_h or 320, in_w or 1600)
+    if any(n.op_type == "ConvTranspose" for n in model.nodes):       # YOLOv6's BiFusion; v5 / v7 / v8 upsample with Resize
+        return _recognise_yolov6(model, w, in_h, in_w)
     if _is_yolov7(model, w):
         return _recognise_yolov7(model, w, in_h, in_w)
     cout0, k0 = first.shape[0], first.shape[2]
@@ -428,6 +432,81 @@ def _recognise_yolov7(model: OnnxModel, w: OnnxWeights, in_h: int, in_w: int) ->
     return ModelSpec("yolov7", scale, no // 3 - 5, in_h or 640, in_w or 640, act, anchors)
 
 
+_V6_SUPPORTED = "YOLOv6-N / S / M / L (release 0.4.0, P5, 3 detection levels; YOLOv6-Lite, the P6 models and the 2.x models are not supported)"
+_V6_WIDTH = {16: "n", 32: "s", 48: "m", 64: "l"}
+
+
+def conv_activations(model: OnnxModel) -> Dict[str, str]:
+    """weight name -> activation applied to that Conv's output: "relu" (Relu), "silu" (Sigmoid and a Mul of the conv output with it),
+    "sigmoid" (a Sigmoid alone) or "none"."""
+    users: Dict[str, List] = {}
+    for n in model.nodes:
+        for i in n.inputs:
+            users.setdefault(i, []).append(n)
+    acts = {}
+    for n in model.nodes:
+        if n.op_type != "Conv" or len(n.inputs) < 2 or not n.outputs:
+            continue
+        y = n.outputs[0]
+        us = users.get(y, [])
+        act = "none"
+        if any(u.op_type == "Relu" for u in us):
+            act = "relu"
+        else:
+            sig = [u for u in us if u.op_type == "Sigmoid"]
+            if sig:
+                act = "silu" if any(u.op_type == "Mul" and sig[0].outputs[0] in u.inputs for u in us) else "sigmoid"
+        acts[n.inputs[1]] = act
+    return acts
+
+
+def _v6_role(name: str) -> Optional[str]:
+    """activation role of a YOLOv6 conv by its module name (plan.build_yolov6): None for the prediction / DFL-projection convs."""
+    if re.match(r"detect\.(stems|cls_convs|reg_convs)\.", name):
+        return "head"
+    if name.startswith("detect."):
+        return None
+    if re.match(r"neck\.(reduce_layer\d|Bifusion\d|downsample\d)\.", name):
+        return "neck"
+    return "body"
+
+
+def _recognise_yolov6(model: OnnxModel, w: OnnxWeights, in_h: int, in_w: int) -> ModelSpec:
+    grouped = [n.inputs[1] for n in model.nodes if n.op_type == "Conv" and int(n.attrs.get("group", 1)) > 1]
+    if grouped:
+        raise Exception(f"YOLOv6 file with grouped / depthwise convolutions ({grouped[0]}: a YOLOv6-Lite model); supported: {_V6_SUPPORTED}")
+    named = {k for k in model.initializers if _is_module_name(k)}
+    cls = sorted((k for k in named if re.fullmatch(r"detect\.cls_preds\.\d+\.weight", k)), key=lambda k: int(k.split(".")[2]))
+    reg = sorted((k for k in named if re.fullmatch(r"detect\.reg_preds\.\d+\.weight", k)), key=lambda k: int(k.split(".")[2]))
+    if not cls or len(cls) != len(reg):
+        raise Exception("YOLOv6 file without its module names (detect.cls_preds.*): export the fused model with torch.onnx.export, which "
+                        f"keeps them; supported: {_V6_SUPPORTED}")
+    if len(cls) != 3 or (in_h and in_h > 1024) or (in_w and in_w > 1024):
+        raise Exception(f"YOLOv6 file with {len(cls)} detection levels at {in_h}x{in_w} (a P6 model?); supported: {_V6_SUPPORTED}")
+    cout0 = w.convs[0][1].shape[0]
+    if w.convs[0][1].shape[1:] != (3, 3, 3) or cout0 not in _V6_WIDTH:
+        raise Exception(f"YOLOv6 stem {tuple(w.convs[0][1].shape)} is not one of N / S / M / L; supported: {_V6_SUPPORTED}")
+    scale = _V6_WIDTH[cout0]
+    nc = int(model.initializers[cls[0]].shape[0])
+    nbox = int(model.initializers[reg[0]].shape[0])
+    if nbox not in (4, 68):
+        raise Exception(f"YOLOv6 box head with {nbox} outputs (4: raw distances, 68: 17-bin DFL); supported: {_V6_SUPPORTED}")
+    acts = conv_activations(model)
+    roles: Dict[str, str] = {}
+    for name, _, _ in w.convs:                          # graph order: each role's activation is its first conv's
+        role = _v6_role(name)
+        if role is None:
+            continue
+        a = acts.get(name, "none")
+        if a not in ("relu", "silu"):
+            raise Exception(f"YOLOv6 conv {name} has activation {a!r}; the {role} convolutions take ReLU or SiLU")
+        if roles.setdefault(role, a) != a:
+            raise Exception(f"YOLOv6 conv {name} has activation {a!r}, the other {role} convolutions {roles[role]!r}: "
+                            "a graph the packer cannot represent")
+    return ModelSpec("yolov6", scale, nc, in_h or 640, in_w or 640, reg_max=0 if nbox == 4 else 16,
+                     acts=(roles.get("body", "relu"), roles.get("neck", "relu"), roles.get("head", "silu")))
+
+
 def build_plan(model: OnnxModel, spec: Optional[ModelSpec] = None) -> "plan.PlanBuilder":
     spec = spec or recognise(model)
     w = OnnxWeights(model)
@@ -437,6 +516,10 @@ def build_plan(model: OnnxModel, spec: Optional[ModelSpec] = None) -> "plan.Plan
         return plan.build_yolov5(w, spec.scale, nc=spec.nc, in_h=spec.in_h, in_w=spec.in_w)
     if spec.kind == "yolov7":
         return plan.build_yolov7(w, spec.scale, nc=spec.nc, in_h=spec.in_h, in_w=spec.in_w, act=spec.act, anchors=spec.anchors)
+    if spec.kind == "yolov6":
+        body, neck, head = spec.acts or (None, "relu", "silu")
+        return plan.build_yolov6(w, spec.scale, nc=spec.nc, in_h=spec.in_h, in_w=spec.in_w, act_body=body, act_neck=neck, act_head=head,
+                                 reg_max=spec.reg_max)
     if spec.kind == "ufldv2":
         # the dataset follows from the input binding (ModelConfig: CULane 320x1600, TuSimple 320x800); the engine rejects any other
         cfg = dict(plan.UFLD_TUSIMPLE if (spec.in_h, spec.in_w) == (320, 800) else plan.UFLD_CULANE)

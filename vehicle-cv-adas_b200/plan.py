@@ -31,6 +31,7 @@ from typing import Dict, List, Optional, Tuple
 import numpy as np
 
 MODEL_YOLOV8, MODEL_YOLOV5, MODEL_UFLDV2, MODEL_UFLDV1 = 0, 1, 2, 4      # 3 = ADAS_MODEL_YOLOV5_LITE (post-processing kind only)
+MODEL_YOLOV6 = 5                                                         # anchor-free head, [B, 8400, 5 + nc] output; meta[2] = reg_max
 OP_GEMM, OP_IM2COL, OP_MAXPOOL, OP_UPSAMPLE2X, OP_LAYERNORM, OP_STEMPACK, OP_STEMCONV = 1, 2, 3, 4, 5, 6, 7
 ACT_NONE, ACT_SILU, ACT_RELU, ACT_LEAKY = 0, 1, 2, 3          # ACT_LEAKY: LeakyReLU(0.1)
 PLAN_VERSION = 1
@@ -116,6 +117,8 @@ class Weights:
             a = (r.standard_normal(shape) * 0.02).astype(np.float32)
         elif kind == "implicit_m":          # YOLOv7 ImplicitM: nn.init.normal_(mean=1, std=0.02)
             a = (1.0 + r.standard_normal(shape) * 0.02).astype(np.float32)
+        elif kind == "alpha":               # YOLOv6 BottleRep shortcut scale (initialised to 1, learned)
+            a = r.uniform(0.7, 1.3, shape).astype(np.float32)
         else:
             raise ValueError(kind)
         self.state_dict[name] = a
@@ -141,16 +144,34 @@ class Weights:
         scale = (g.astype(np.float64) / np.sqrt(v.astype(np.float64) + eps))
         return w.astype(np.float64) * scale[:, None, None, None], b.astype(np.float64) - m.astype(np.float64) * scale
 
-    def repconv(self, prefix: str, cout: int, cin: int, eps: float):
-        """YOLOv7 RepConv (3x3, no identity branch: c1 != c2 in every P5 head) as one folded 3x3 conv: BN-folded rbr_dense + BN-folded
-        rbr_1x1 on the centre tap, summed in fp64.  A checkpoint that was re-parameterised upstream carries `rbr_reparam` instead."""
-        if f"{prefix}.rbr_reparam.weight" in self.state_dict or (self.real and f"{prefix}.rbr_dense.0.weight" not in self.state_dict):
+    def repconv(self, prefix: str, cout: int, cin: int, eps: float, keys: Tuple[str, str] = ("0", "1"), identity: bool = False):
+        """RepVGG-style block (YOLOv7 RepConv, YOLOv6 RepVGGBlock) as one folded 3x3 conv, summed in fp64: BN-folded rbr_dense + BN-folded
+        rbr_1x1 on the centre tap (+ with `identity`, the rbr_identity BatchNorm as a scaled identity on the centre tap, cin == cout at
+        stride 1).  `keys` names the conv / BN inside each branch: ("0", "1") for YOLOv7's Sequential, ("conv", "bn") for YOLOv6.  A
+        checkpoint that was re-parameterised upstream carries `rbr_reparam` instead.  With `identity`, all three synthetic BNs are damped
+        like the last BN of a residual branch (a chain of undamped identity blocks grows its activations geometrically)."""
+        ck, bk = keys
+        if f"{prefix}.rbr_reparam.weight" in self.state_dict or (self.real and f"{prefix}.rbr_dense.{ck}.weight" not in self.state_dict):
             return self.conv_bias(f"{prefix}.rbr_reparam", cout, cin, 3)
-        assert cin != cout and f"{prefix}.rbr_identity.running_var" not in self.state_dict, f"{prefix}: RepConv with an identity branch"
-        wd, bd = self._conv_bn64(f"{prefix}.rbr_dense", cout, cin, 3, eps, conv_key="0", bn_key="1")
-        w1, b1 = self._conv_bn64(f"{prefix}.rbr_1x1", cout, cin, 1, eps, conv_key="0", bn_key="1")
+        if not identity:
+            assert f"{prefix}.rbr_identity.running_var" not in self.state_dict, f"{prefix}: RepConv with an identity branch"
+        wd, bd = self._conv_bn64(f"{prefix}.rbr_dense", cout, cin, 3, eps, conv_key=ck, bn_key=bk, res_branch=identity)
+        w1, b1 = self._conv_bn64(f"{prefix}.rbr_1x1", cout, cin, 1, eps, conv_key=ck, bn_key=bk, res_branch=identity)
         wd[:, :, 1, 1] += w1[:, :, 0, 0]
-        return wd.astype(np.float32), (bd + b1).astype(np.float32)
+        bd += b1
+        if identity:
+            assert cin == cout, f"{prefix}: identity branch needs cin == cout"
+            bn = f"{prefix}.rbr_identity"
+            g = self.get(f"{bn}.weight", (cout,), "bn_gamma_res").astype(np.float64)
+            be = self.get(f"{bn}.bias", (cout,), "bn_beta").astype(np.float64)
+            m = self.get(f"{bn}.running_mean", (cout,), "bn_mean").astype(np.float64)
+            v = self.get(f"{bn}.running_var", (cout,), "bn_var").astype(np.float64)
+            if not self.real and f"{bn}.num_batches_tracked" not in self.state_dict:
+                self.state_dict[f"{bn}.num_batches_tracked"] = np.zeros((), dtype=np.int64)
+            s = g / np.sqrt(v + eps)
+            wd[np.arange(cout), np.arange(cout), 1, 1] += s
+            bd += be - m * s
+        return wd.astype(np.float32), bd.astype(np.float32)
 
     def implicit_head(self, prefix: str, li: int, no: int, cin: int):
         """YOLOv7 IDetect level li: im * (m(x + ia)) folded into the 1x1 conv, w' = im * w, b' = im * (b + w @ ia) in fp64.  Files
@@ -198,6 +219,18 @@ SYNTH_PROFILES = {
     # 4 frames: base 6.1e-4 / 0.10 px / ~280 candidates per frame, tiny 5.9e-4 / 0.01 px / ~100 candidates per frame.
     "yolov7": {"gains": [(r"model\.105\.m\.\d\.weight", 16.0), (r"model\.77\.m\.\d\.weight", 0.3)],
                "fill": [(r"model\.105\.m\.\d\.bias", -3.0), (r"model\.77\.m\.\d\.bias", (-3.0, -0.2))]},
+    # YOLOv6 N/S/M/L: convs damped (0.85, and 0.6 on the BepC3 / SPPF / BiFusion 1x1 convs) so that the ReLU bodies of M do not grow
+    # their activations layer by layer; class logits widened (gain 12: at 16 the M device error is 1.04e-3); box biases of 2 grid cells
+    # keep the raw l, t, r, b distances of N/S positive (a constant bias cancels in the DFL softmax of M/L).  The class bias of each
+    # scale (`variants`) puts ~100 of the 8400 anchors per frame above box_score = 0.4, measured on the fp32 oracle over synthetic
+    # frames 0-3: the 100th-highest max-class logit sits 0.135 (N), 0.177 (S), 0.30 (M) above and 0.595 (L) below logit(0.4) at
+    # bias -3.  The per-anchor max-class logit spread is small (std 0.13-0.24), so the scores crowd the threshold.
+    "yolov6": {"conv_gain": 0.85,
+               "gains": [(r"(backbone|neck)\..*\.cv\d\.block\.conv\.weight", 0.6), (r"detect\.cls_preds\.\d\.weight", 12.0),
+                         (r"detect\.reg_preds\.\d\.weight", 1.0)],
+               "fill": [(r"detect\.reg_preds\.\d\.bias", 2.0)],
+               "variants": {sc: {"fill": [(r"detect\.cls_preds\.\d\.bias", -3.0 + d)]}
+                            for sc, d in (("n", -0.135), ("s", -0.177), ("m", -0.30), ("l", 0.595))}},
 }
 
 
@@ -211,8 +244,12 @@ SYNTH_PROFILES_WORKLOAD = {
 
 
 def synth_weights(kind: str, seed: int = 0, variant: Optional[str] = None, workload: bool = False) -> "Weights":
-    """Seeded synthetic weights (`variant` is accepted for call-site symmetry with the builders and ignored)."""
+    """Seeded synthetic weights.  A profile's `variants` entry (YOLOv6) adds per-variant `fill` rules ahead of the shared ones; other
+    kinds ignore `variant`."""
     prof = SYNTH_PROFILES_WORKLOAD.get(kind, SYNTH_PROFILES[kind]) if workload else SYNTH_PROFILES[kind]
+    extra = prof.get("variants", {}).get(variant)
+    if extra:
+        prof = {**prof, "fill": list(extra.get("fill", ())) + list(prof.get("fill", ()))}
     return Weights(None, seed=seed, profile=prof)
 
 
@@ -271,9 +308,11 @@ class PlanBuilder:
 
     def conv(self, x: View, w: np.ndarray, b: Optional[np.ndarray], k: int, s: int, act: int, out: Optional[View] = None,
              res: Optional[View] = None, res_pre_act: bool = False, out_f32: bool = False, pad: Optional[int] = None,
-             tile: Optional[Tuple[int, int]] = None, no_slab: bool = False) -> View:
+             tile: Optional[Tuple[int, int]] = None, no_slab: bool = False, res_scale: Optional[float] = None) -> View:
         """w: folded [Cout, Cin_real, k, k] fp32.  x.C may exceed Cin_real (zero-padded image channel).
+        res_scale: out = act(conv) + res_scale * res (YOLOv6 BottleRep's alpha); None = a plain residual add (op f[0] = 0).
         no_slab (test hook): a 3x3 stride-1 conv loads one activation tile per tap instead of one slab per (dy, k-block)."""
+        assert res_scale is None or (res is not None and not res_pre_act and math.isfinite(res_scale) and res_scale != 0.0), res_scale
         cout, cin_real = int(w.shape[0]), int(w.shape[1])
         pad = k // 2 if pad is None else pad
         Ho = (x.H + 2 * pad - k) // s + 1
@@ -321,8 +360,23 @@ class PlanBuilder:
         w_t = self.tensor(wk.astype(np.float16))
         bn, mt = tile if tile is not None else (0, 0)          # (BN, MT) forced by tests; 0 = cost model + autotune
         self._op(OP_GEMM, [a.buf, a.coff, Kc, ntaps, w_t, bias_t, n_store, act, res_buf, res_coff, 1 if res_pre_act else 0,
-                           out.buf, out.coff, 1, 0, bn, s2, mt, 1 if no_slab else 0])
+                           out.buf, out.coff, 1, 0, bn, s2, mt, 1 if no_slab else 0], [res_scale] if res_scale is not None else None)
         return View(out.buf, out.coff, cout, Ho, Wo)
+
+    def conv_transpose2x2(self, x: View, w: np.ndarray, b: Optional[np.ndarray], out: View, tile: Optional[Tuple[int, int]] = None) -> View:
+        """ConvTranspose2d(k=2, s=2, p=0), w [Cin, Cout, 2, 2] as upstream stores it.  The 2x2 windows do not overlap, so it is a 1x1 GEMM
+        with N = 4 * Cout, columns ordered (dy, dx, c); the epilogue stores column group (dy, dx) of input pixel (y, x) to output pixel
+        (2y + dy, 2x + dx) of `out` (a 2H x 2W view, possibly a concat slice).  The bias is replicated for the 4 groups."""
+        cin, cout = int(w.shape[0]), int(w.shape[1])
+        assert w.shape[2:] == (2, 2) and cout % 8 == 0 and x.C == cin and cin % 8 == 0, (w.shape, x.C)
+        assert out.H == 2 * x.H and out.W == 2 * x.W and out.C == cout, (out, x)
+        self.flops_per_img += 2 * x.H * x.W * cin * cout * 4
+        wk = np.transpose(w, (2, 3, 1, 0)).reshape(4 * cout, cin)             # [dy, dx, Cout, Cin]
+        bias_t = self.tensor(np.tile(b.astype(np.float32), 4)) if b is not None else -1
+        bn, mt = tile if tile is not None else (0, 0)
+        self._op(OP_GEMM, [x.buf, x.coff, cin, 1, self.tensor(wk.astype(np.float16)), bias_t, 4 * cout, ACT_NONE, -1, 0, 0,
+                           out.buf, out.coff, 1, 0, bn, 0, mt, 0, 1])
+        return View(out.buf, out.coff, cout, out.H, out.W)
 
     def stem_conv(self, x: View, w: np.ndarray, b: Optional[np.ndarray], k: int, s: int, pad: int, act: int, out: View) -> View:
         """k x k stride-1 or stride-2 conv of the C=4 image by stem_conv.cu (no patch matrix): weights packed [Cout][k][KR], KR = round_up(4k, 16),
@@ -756,6 +810,180 @@ def read_anchors(path: str) -> np.ndarray:
     off, nbytes, _, _ = struct.unpack_from("<QQII", raw, rec)
     assert meta[3] <= n_t and nbytes >= 72
     return np.frombuffer(raw, np.float32, 18, blob + off).reshape(3, 3, 2).copy()
+
+
+# ---------------------------------------------------------------------------------------------
+# YOLOv6 3.0 (meituan/YOLOv6 release 0.4.0, configs/yolov6{n,s,m,l}.py; P5 models only)
+# ---------------------------------------------------------------------------------------------
+YOLOV6_SCALES = {"n": (0.33, 0.25), "s": (0.33, 0.50), "m": (0.60, 0.75), "l": (1.0, 1.0)}     # depth, width
+YOLOV6_CSP_E = {"m": 2 / 3, "l": 1 / 2}
+YOLOV6_ACTS = {"relu": ACT_RELU, "silu": ACT_SILU}
+
+
+def yolov6_reg_max(scale: str) -> int:
+    """0 for N/S (the head regresses l, t, r, b directly), 16 for M/L (17-bin DFL)."""
+    return 16 if scale in ("m", "l") else 0
+
+
+def build_yolov6(weights: Weights, scale: str = "n", nc: int = 80, in_h: int = 640, in_w: int = 640, act_body: Optional[str] = None,
+                 act_neck: str = "relu", act_head: str = "silu", reg_max: Optional[int] = None) -> PlanBuilder:
+    """YOLOv6-N/S (EfficientRep + RepBiFPANNeck) or -M/L (CSPBepBackbone + CSPRepBiFPANNeck), EffiDeHead, under upstream module names
+    (`backbone.*`, `neck.*`, `detect.*`).  Output [B, 8400, 5 + nc] (MODEL_YOLOV6, header meta[2] = reg_max).
+
+    Activations by conv role (defaults as upstream builds them):
+      act_body  stem, backbone / neck blocks, the BepC3 1x1 convs and the SPPF convs: "relu" for N/S/M (RepVGG blocks), "silu" for L
+                (training_mode "conv_silu": Conv-BN-SiLU blocks, BepC3 / SPPF in their SiLU form)
+      act_neck  the neck's reduce layers, BiFusion cv1 / cv2 / cv3 / downsample and the PAN downsamples (ConvBNReLU upstream): "relu"
+      act_head  the head's stem, cls_conv and reg_conv (ConvBNSiLU upstream): "silu"
+    RepVGG blocks (3x3 + 1x1 + identity BN) are folded into one 3x3 conv here in fp64 (Weights.repconv); BottleRep's learned `alpha`
+    scales the shortcut in the GEMM epilogue; BiFusion's ConvTranspose2d(k=2, s=2) is a 1x1 GEMM storing 2x2 pixel groups.  Each level
+    of the head holds 4 * (reg_max + 1) box columns, then the class logits from the next multiple of 8 on (the anchor-aided `_ab`
+    branch of training checkpoints is not used at inference and is ignored)."""
+    assert scale in YOLOV6_SCALES, f"YOLOv6 scale {scale!r}: 'n', 's', 'm' or 'l' (Lite, P6 and the 2.x models are not supported)"
+    depth, width = YOLOV6_SCALES[scale]
+    ch = [int(math.ceil(c * width / 8) * 8) for c in (64, 128, 256, 512, 1024, 256, 128, 128, 256, 256, 512)]
+    rep = [max(round(n * depth), 1) if n > 1 else n for n in (1, 6, 12, 18, 6, 12, 12, 12, 12)]
+    csp = scale in YOLOV6_CSP_E
+    repvgg = scale != "l"                                  # L trains Conv-BN-SiLU blocks
+    a_body = YOLOV6_ACTS[act_body or ("silu" if scale == "l" else "relu")]
+    a_neck, a_head = YOLOV6_ACTS[act_neck], YOLOV6_ACTS[act_head]
+    reg_max = yolov6_reg_max(scale) if reg_max is None else reg_max
+    assert reg_max in (0, 16)
+    pb = PlanBuilder(MODEL_YOLOV6, 3, in_h, in_w)
+    W = weights
+    eps = BN_EPS_YOLO
+
+    def fused_or_bn(name: str, cout: int, cin: int, k: int, res_branch: bool = False):
+        """ConvModule (`name.conv` + `name.bn`) or its deployed form (`name.conv` with a bias)."""
+        if W.real and f"{name}.conv.bias" in W.state_dict and f"{name}.bn.weight" not in W.state_dict:
+            return W.conv_bias(f"{name}.conv", cout, cin, k)
+        return W.conv_bn(name, cout, cin, k, eps, res_branch=res_branch)
+
+    def cin_of(x: View) -> int:
+        return 3 if x.buf == pb.image.buf else x.C          # the image buffer carries a zero fourth channel
+
+    def cbr(x: View, name: str, cout: int, k: int, s: int, act: int, out: Optional[View] = None, **kw) -> View:
+        """ConvBNReLU / ConvBNSiLU: `name.block.conv`, `name.block.bn`."""
+        w, b = fused_or_bn(f"{name}.block", cout, cin_of(x), k, res_branch=kw.get("res") is not None)
+        return pb.conv(x, w, b, k, s, act, out=out, **kw)
+
+    def blk(x: View, name: str, cout: int, s: int = 1, out: Optional[View] = None, **kw) -> View:
+        """the body block: RepVGGBlock (folded) or, for L, ConvBNSiLU 3x3."""
+        if not repvgg:
+            return cbr(x, name, cout, 3, s, a_body, out=out, **kw)
+        cin = cin_of(x)
+        w, b = W.repconv(name, cout, cin, eps, keys=("conv", "bn"), identity=(cin == cout and s == 1))
+        return pb.conv(x, w, b, 3, s, a_body, out=out, **kw)
+
+    def rep_block(x: View, name: str, cout: int, n: int, out: Optional[View] = None) -> View:
+        """RepBlock of RepVGG blocks: conv1, then block.0 .. block.n-2."""
+        names = [f"{name}.conv1"] + [f"{name}.block.{i}" for i in range(n - 1)]
+        for i, nm in enumerate(names):
+            x = blk(x, nm, cout, out=out if i == len(names) - 1 else None)
+        return x
+
+    def bottle_rep(x: View, name: str, out: Optional[View] = None) -> View:
+        """BottleRep(c, c, weight=True): conv2(conv1(x)) + alpha * x."""
+        t = blk(x, f"{name}.conv1", x.C)
+        alpha = float(W.get(f"{name}.alpha", (1,), "alpha")[0])
+        if alpha == 0.0:                                    # op f[0] = 0 stands for a scale of 1: a zero alpha drops the shortcut
+            return blk(t, f"{name}.conv2", x.C, out=out)
+        return blk(t, f"{name}.conv2", x.C, out=out, res=x, res_scale=alpha)
+
+    def bepc3(x: View, name: str, cout: int, n: int, out: Optional[View] = None) -> View:
+        """BepC3: cv3(cat(m(cv1(x)), cv2(x))), m = RepBlock of n // 2 BottleReps (at least one)."""
+        c_ = int(cout * YOLOV6_CSP_E[scale])
+        cat = pb.new_padded(x.H, x.W, 2 * c_)
+        y = cbr(x, f"{name}.cv1", c_, 1, 1, a_body)
+        names = [f"{name}.m.conv1"] + [f"{name}.m.block.{i}" for i in range(max(n // 2, 1) - 1)]
+        for i, nm in enumerate(names):
+            y = bottle_rep(y, nm, out=pb.sub(cat, 0, c_) if i == len(names) - 1 else None)
+        cbr(x, f"{name}.cv2", c_, 1, 1, a_body, out=pb.sub(cat, c_, c_))
+        return cbr(cat, f"{name}.cv3", cout, 1, 1, a_body, out=out)
+
+    stage = (lambda x, name, c, n, out=None: bepc3(x, name, c, n, out)) if csp else rep_block
+
+    def sppf(x: View, name: str, out: Optional[View] = None) -> View:
+        """N/S: SimCSPSPPF (`.cspsppf`); M/L: SimSPPF / SPPF (`.sppf`).  The 5x5 pools are chained."""
+        c = x.C
+        if not csp:
+            c_ = c // 2
+            cat7 = pb.new_padded(x.H, x.W, 2 * c_)          # cv7 input [y0 = cv2(x), y3]
+            sp = pb.new_padded(x.H, x.W, 4 * c_)            # cv5 input [x1, m(x1), m(m(x1)), m(m(m(x1)))]
+            nm = f"{name}.cspsppf"
+            t = cbr(x, f"{nm}.cv1", c_, 1, 1, a_body)
+            t = cbr(t, f"{nm}.cv3", c_, 3, 1, a_body)
+            y = cbr(t, f"{nm}.cv4", c_, 1, 1, a_body, out=pb.sub(sp, 0, c_))
+            for i in range(3):
+                y = pb.maxpool(y, 5, 1, 2, out=pb.sub(sp, (i + 1) * c_, c_))
+            cbr(x, f"{nm}.cv2", c_, 1, 1, a_body, out=pb.sub(cat7, 0, c_))
+            t = cbr(sp, f"{nm}.cv5", c_, 1, 1, a_body)
+            cbr(t, f"{nm}.cv6", c_, 3, 1, a_body, out=pb.sub(cat7, c_, c_))
+            return cbr(cat7, f"{nm}.cv7", c, 1, 1, a_body, out=out)
+        c_ = c // 2
+        sp = pb.new_padded(x.H, x.W, 4 * c_)
+        nm = f"{name}.sppf"
+        y = cbr(x, f"{nm}.cv1", c_, 1, 1, a_body, out=pb.sub(sp, 0, c_))
+        for i in range(3):
+            y = pb.maxpool(y, 5, 1, 2, out=pb.sub(sp, (i + 1) * c_, c_))
+        return cbr(sp, f"{nm}.cv2", c, 1, 1, a_body, out=out)
+
+    def transpose(x: View, name: str, out: View) -> View:
+        c = x.C
+        w = W.get(f"{name}.upsample_transpose.weight", (c, c, 2, 2), "conv")
+        b = W.get(f"{name}.upsample_transpose.bias", (c,), "bias")
+        return pb.conv_transpose2x2(x, w, b, out)
+
+    def bifusion(x0: View, x1: View, x2: View, name: str, c: int) -> View:
+        """cv3(cat(Transpose(x0), cv1(x1), downsample(cv2(x2)))) at x1's resolution."""
+        cat = pb.new_padded(x1.H, x1.W, 3 * c)
+        transpose(x0, f"{name}.upsample", pb.sub(cat, 0, c))
+        cbr(x1, f"{name}.cv1", c, 1, 1, a_neck, out=pb.sub(cat, c, c))
+        t = cbr(x2, f"{name}.cv2", c, 1, 1, a_neck)
+        cbr(t, f"{name}.downsample", c, 3, 2, a_neck, out=pb.sub(cat, 2 * c, c))
+        return cbr(cat, f"{name}.cv3", c, 1, 1, a_neck)
+
+    H, Wd = in_h, in_w
+    # backbone (stem -> ERBlock_2 .. ERBlock_5); P2 feeds the neck (fuse_P2)
+    x = blk(pb.image, "backbone.stem", ch[0], 2)
+    feats = []
+    for i in range(1, 5):
+        x = blk(x, f"backbone.ERBlock_{i + 1}.0", ch[i], 2)
+        x = stage(x, f"backbone.ERBlock_{i + 1}.1", ch[i], rep[i])
+        feats.append(x)
+    p2, p3, p4, _ = feats
+    p5 = sppf(x, "backbone.ERBlock_5.2")
+    # neck (RepBiFPANNeck / CSPRepBiFPANNeck); PAN concats allocated up front, producers write their slices
+    cat_n4 = pb.new_padded(H // 32, Wd // 32, ch[9] + ch[5])      # [down_feat0, fpn_out0]
+    cat_n3 = pb.new_padded(H // 16, Wd // 16, ch[7] + ch[6])      # [down_feat1, fpn_out1]
+    fpn0 = cbr(p5, "neck.reduce_layer0", ch[5], 1, 1, a_neck, out=pb.sub(cat_n4, ch[9], ch[5]))
+    f_out0 = stage(bifusion(fpn0, p4, p3, "neck.Bifusion0", ch[5]), "neck.Rep_p4", ch[5], rep[5])
+    fpn1 = cbr(f_out0, "neck.reduce_layer1", ch[6], 1, 1, a_neck, out=pb.sub(cat_n3, ch[7], ch[6]))
+    pan2 = stage(bifusion(fpn1, p3, p2, "neck.Bifusion1", ch[6]), "neck.Rep_p3", ch[6], rep[6])
+    cbr(pan2, "neck.downsample2", ch[7], 3, 2, a_neck, out=pb.sub(cat_n3, 0, ch[7]))
+    pan1 = stage(cat_n3, "neck.Rep_n3", ch[8], rep[7])
+    cbr(pan1, "neck.downsample1", ch[9], 3, 2, a_neck, out=pb.sub(cat_n4, 0, ch[9]))
+    pan0 = stage(cat_n4, "neck.Rep_n4", ch[10], rep[8])
+    # EffiDeHead
+    nb = 4 * (reg_max + 1)
+    cls_col = (nb + 7) // 8 * 8
+    A = 0
+    for li, (feat, stride) in enumerate(((pan2, 8), (pan1, 16), (pan0, 32))):
+        c = feat.C
+        t = cbr(feat, f"detect.stems.{li}", c, 1, 1, a_head)
+        # cls_conv and reg_conv share their input: one GEMM with N = 2c, [cls | reg]
+        wc, bc = fused_or_bn(f"detect.cls_convs.{li}.block", c, c, 3)
+        wr, br = fused_or_bn(f"detect.reg_convs.{li}.block", c, c, 3)
+        t2 = pb.conv(t, np.concatenate([wc, wr], 0), np.concatenate([bc, br]), 3, 1, a_head)
+        head = pb.new_padded(feat.H, feat.W, cls_col + (nc + 7) // 8 * 8, f32=True)
+        wrp, brp = W.conv_bias(f"detect.reg_preds.{li}", nb, c, 1)
+        wcp, bcp = W.conv_bias(f"detect.cls_preds.{li}", nc, c, 1)
+        pb.conv(pb.sub(t2, c, c), wrp, brp, 1, 1, ACT_NONE, out=pb.sub(head, 0, cls_col), out_f32=True)
+        pb.conv(pb.sub(t2, 0, c), wcp, bcp, 1, 1, ACT_NONE, out=pb.sub(head, cls_col, (nc + 7) // 8 * 8), out_f32=True)
+        pb.outputs.append((head.buf, 0, head.C, stride))
+        A += feat.H * feat.W
+    pb.meta[0], pb.meta[1], pb.meta[2] = nc, A, reg_max
+    return pb
 
 
 # ---------------------------------------------------------------------------------------------

@@ -1,5 +1,6 @@
 """Per-layer table of a plan at real clocks: every launch replayed alone (CUDA events, L2-warm), GEMM shapes and tile choices.
-usage: python tools/op_table.py yolov8|ufldv2|yolov5|yolov7|yolov7-tiny|yolov6n|yolov6s|yolov6m|yolov6l [batch] [iters]   (env switches of the library apply)"""
+usage: python tools/op_table.py yolov8|ufldv2|yolov5|yolov7|yolov7-tiny|yolov7-w6|yolov7-e6|yolov7-d6|yolov7-e6e|yolov6n|yolov6s|yolov6m|yolov6l [batch] [iters]
+(the YOLOv7 P6 models run at 1280x1280)   (env switches of the library apply)"""
 import os, re, sys, tempfile
 R = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, R); sys.path.insert(0, os.path.join(R, "tests"))
 import adas_b200
@@ -7,7 +8,7 @@ from adas_b200 import _capi, plan
 from gpu_util import cached_plan
 kind = sys.argv[1]; B = int(sys.argv[2]) if len(sys.argv) > 2 else 8; iters = int(sys.argv[3]) if len(sys.argv) > 3 else 20
 if kind.startswith("yolov7"):        # built fresh: ADAS_B200_STEMCONV decides at pack time where the stem runs
-    pb = plan.build_yolov7(plan.synth_weights("yolov7", 0), "tiny" if kind == "yolov7-tiny" else "base")
+    pb = plan.build_yolov7(plan.synth_weights("yolov7", 0), {"yolov7": "base", "yolov7-tiny": "tiny"}.get(kind, kind[7:]))
     path = os.path.join(tempfile.mkdtemp(), kind + ".b200w")
     pb.write(path)
 elif kind.startswith("yolov6"):

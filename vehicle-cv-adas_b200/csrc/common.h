@@ -138,10 +138,11 @@ int launch_ufld_pre(const uint8_t* frames, int B, int H, int W, int in_h, int in
 
 // ---- YOLO post-processing (yolo_post.cu) --------------------------------------------------------
 struct YoloLevel { const float* ptr; int ld; int H, W; int stride; int rows_per_img; };
+static const int kYoloMaxLevels = 4;      // P6 heads (strides 8 / 16 / 32 / 64); every other head has 3 levels
 int launch_yolov8_head_decode(const YoloLevel* lv /*3*/, int B, int nc, float* raw /*[B,4+nc,A]*/, int A,
                               cudaStream_t st);
-int launch_yolov5_head_decode(const YoloLevel* lv /*3*/, int B, int nc, float* raw /*[B,A,5+nc]*/, int A, int lite,
-                              const float* anchors /*device [3][3][2], nullptr = YOLOv5 table*/, cudaStream_t st);
+int launch_yolov5_head_decode(const YoloLevel* lv /*n_levels*/, int n_levels /*3, or 4 with anchors*/, int B, int nc, float* raw /*[B,A,5+nc]*/,
+                              int A, int lite, const float* anchors /*device [n_levels][3][2], nullptr = YOLOv5 table*/, cudaStream_t st);
 int launch_yolov5_lite_post(float* raw /*[B,A,5+nc], in place*/, int B, int A, int nc, int in_h, int in_w, cudaStream_t st);
 // YOLOv6 level columns: 4 * (reg_max + 1) box columns (stored as 8-column groups), the nc class logits from the next multiple of 8 on
 __host__ __device__ inline unsigned yolov6_cls_col(unsigned reg_max) { return (4u * (reg_max + 1u) + 7u) / 8u * 8u; }

@@ -402,17 +402,21 @@ static int run_plan(adas_engine* e, int batch) {
     return 0;
 }
 
-// Anchor table of a YOLOv5-layout head: header meta[3] = 1 + index of an fp32 [3 levels x 3 anchors x 2] plan tensor, 0 = none (the
-// YOLOv5 table of yolo_post.cu; every plan written before the field existed has 0 there).
+// Anchor table of a YOLOv5-layout head: header meta[3] = 1 + index of an fp32 [L levels x 3 anchors x 2] plan tensor (L = n_outputs),
+// 0 = none (the YOLOv5 table of yolo_post.cu, 3 levels; every plan written before the field existed has 0 there).
 static const float* yolo_anchors(const adas_engine* e) {
     return e->hdr.meta[3] == 0 ? nullptr : static_cast<const float*>(tensor_ptr(e, (int)e->hdr.meta[3] - 1));
 }
 
+// A YOLOv5-layout (non-lite) head may have a fourth, stride-64 level (the P6 models); every other head has 3.
+static bool yolo_four_levels_ok(const PlanHeader& h) { return h.model_kind == ADAS_MODEL_YOLOV5 && h.meta[2] == 0; }
+
 static int head_decode(adas_engine* e, int batch) {
     if (is_ufld(e->hdr.model_kind)) return 0;   // heads are the raw FC output buffer
-    YoloLevel lv[3];
-    ADAS_CHECK(e->outs.size() == 3, "YOLO plan must declare 3 output levels");
-    for (int i = 0; i < 3; ++i) {
+    YoloLevel lv[kYoloMaxLevels];
+    const int nl = (int)e->outs.size();
+    ADAS_CHECK(nl == 3 || (nl == kYoloMaxLevels && yolo_four_levels_ok(e->hdr)), "YOLO plan must declare 3 output levels (4 for a YOLOv5-layout P6 head)");
+    for (int i = 0; i < nl; ++i) {
         const PlanOutput& o = e->outs[i];
         const PlanBuffer& b = e->bufs[o.buffer];
         lv[i].ptr = static_cast<const float*>(e->dbufs[o.buffer].ptr) + o.coff;
@@ -422,7 +426,7 @@ static int head_decode(adas_engine* e, int batch) {
     const int nc = (int)e->hdr.meta[0], A = (int)e->hdr.meta[1];
     if (e->hdr.model_kind == ADAS_MODEL_YOLOV8) return launch_yolov8_head_decode(lv, batch, nc, e->d_raw, A, e->stream);
     if (e->hdr.model_kind == ADAS_MODEL_YOLOV6) return launch_yolov6_head_decode(lv, batch, nc, (int)e->hdr.meta[2], e->d_raw, A, e->stream);
-    return launch_yolov5_head_decode(lv, batch, nc, e->d_raw, A, (int)e->hdr.meta[2], yolo_anchors(e), e->stream);
+    return launch_yolov5_head_decode(lv, nl, batch, nc, e->d_raw, A, (int)e->hdr.meta[2], yolo_anchors(e), e->stream);
 }
 // YOLOV5_LITE plans (meta[2] != 0): the network output is the sigmoid-only head; the fused detect calls apply
 // YoloLiteParameters.lite_postprocess (yoloDetector.py:36-50) on the device before candidate selection.
@@ -602,7 +606,7 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
             case OP_STEMCONV: {
                 const int Cout = p[3], k = p[4], s = p[9] == 0 ? 2 : p[9];          // p[9] = 0: stride 2 (plans without the field)
                 ADAS_CHECK(p[6] >= 0 && p[6] <= 3, "plan %s: op %zu: unknown activation %d", path, oi, p[6]);
-                ADAS_CHECK((s == 1 || s == 2) && buf_ok(p[0]) && e->bufs[p[0]].H > 0 && e->bufs[p[0]].C == 4 && Cout >= 8 && Cout <= 64 && k >= 3 && k <= 7 && p[5] >= 0 && p[5] <= 3 &&
+                ADAS_CHECK((s == 1 || s == 2) && buf_ok(p[0]) && e->bufs[p[0]].H > 0 && e->bufs[p[0]].C == 4 && stem_conv_supported(Cout, k, p[5]) &&
                            view_ok(p[7], p[8], Cout) && e->bufs[p[7]].H > 0 && tensor_ok(p[1], (uint64_t)Cout * k * ((4 * k + 15) / 16 * 16) * 2) &&
                            (p[2] < 0 || tensor_ok(p[2], (uint64_t)Cout * 4)) &&
                            e->bufs[p[7]].H == (e->bufs[p[0]].H + 2 * p[5] - k) / s + 1 && e->bufs[p[7]].W == (e->bufs[p[0]].W + 2 * p[5] - k) / s + 1,
@@ -625,10 +629,11 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
         ADAS_CHECK(buf_ok((int)o.buffer) && (uint64_t)o.coff + o.C <= (uint64_t)e->bufs[o.buffer].C * (e->bufs[o.buffer].H > 0 ? 1u : e->bufs[o.buffer].rows_per_img) && o.C >= 1,
                    "plan %s: output %zu exceeds its buffer", path, i);
     }
-    // YOLO meta[3]: anchor table (yolo_anchors); its values are checked once the blob is read
+    // YOLO meta[3]: anchor table (yolo_anchors), [n_outputs levels x 3 x 2]; its values are checked once the blob is read
     ADAS_CHECK(is_ufld(h.model_kind) || h.meta[3] == 0 ||
-                   (h.model_kind == ADAS_MODEL_YOLOV5 && h.meta[2] == 0 && tensor_ok((int)h.meta[3] - 1, 18 * 4) && e->tensors[h.meta[3] - 1].dtype == 1),
-               "plan %s: anchor table (meta[3] = %u) is not an fp32 tensor of 3 x 3 x 2 values of a YOLOv5-layout head", path, h.meta[3]);
+                   (h.model_kind == ADAS_MODEL_YOLOV5 && h.meta[2] == 0 && (h.n_outputs == 3 || h.n_outputs == 4) && tensor_ok((int)h.meta[3] - 1, 0) &&
+                    e->tensors[h.meta[3] - 1].bytes == (uint64_t)h.n_outputs * 6 * 4 && e->tensors[h.meta[3] - 1].dtype == 1),
+               "plan %s: anchor table (meta[3] = %u) is not an fp32 tensor of %u x 3 x 2 values of a YOLOv5-layout head", path, h.meta[3], h.n_outputs);
     if (h.n_outputs == 0) return 0;          // single-layer plans of the kernel tests: no network outputs, no head geometry
     if (h.model_kind == ADAS_MODEL_UFLDV2) {
         const uint64_t ngr = h.meta[0], ncr = h.meta[1], ngc = h.meta[2], ncc = h.meta[3], nl = h.meta[4];
@@ -660,6 +665,25 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
                 A += (uint64_t)b.H * b.W;
             }
             ADAS_CHECK(A == h.meta[1], "plan %s: YOLOv6 levels hold %llu anchors, the header %u", path, (unsigned long long)A, h.meta[1]);
+        } else if (h.model_kind == ADAS_MODEL_YOLOV8) {
+            ADAS_CHECK(h.n_outputs == 3, "plan %s: a YOLOv8 head has 3 levels, the plan declares %u", path, h.n_outputs);
+        } else {
+            // YOLOv5 layout: 3 levels (strides 8 / 16 / 32), or 4 (+ 64) for a non-lite head with its own anchor table (the YOLOv5 table
+            // has 3 levels); level i is the in / stride grid and holds 3 anchors per cell
+            const bool lite = h.meta[2] != 0;
+            ADAS_CHECK(h.n_outputs == 3 || (h.n_outputs == 4 && !lite), "plan %s: a YOLOv5-layout head has 3 levels (4 without the lite flag), the plan declares %u",
+                       path, h.n_outputs);
+            ADAS_CHECK(h.n_outputs == 3 || h.meta[3] != 0, "plan %s: a 4-level head needs its own anchor table (meta[3]); the YOLOv5 table has 3 levels", path);
+            uint64_t A = 0;
+            for (size_t i = 0; i < e->outs.size(); ++i) {
+                const PlanOutput& o = e->outs[i];
+                const PlanBuffer& b = e->bufs[o.buffer];
+                const uint32_t s = 8u << i;
+                ADAS_CHECK(o.stride == s && b.H > 0 && b.H == h.in_h / s && b.W == h.in_w / s, "plan %s: YOLO level %zu has stride %u and a %ux%u grid; "
+                           "stride %u of a %ux%u input needs %ux%u", path, i, o.stride, b.H, b.W, s, h.in_h, h.in_w, h.in_h / s, h.in_w / s);
+                A += 3ull * b.H * b.W;
+            }
+            ADAS_CHECK(A == h.meta[1], "plan %s: YOLOv5-layout levels hold %llu anchors, the header %u", path, (unsigned long long)A, h.meta[1]);
         }
     }
     return 0;
@@ -695,9 +719,10 @@ int adas_engine_create(const char* plan_path, int device, int max_batch, int con
     fclose(f);
     ADAS_CHECK(ok, "truncated plan blob in %s", plan_path);
     if (!is_ufld(e->hdr.model_kind) && e->hdr.meta[3] != 0) {
-        float anc[18];
-        memcpy(anc, blob.data() + e->tensors[e->hdr.meta[3] - 1].offset, sizeof(anc));
-        for (int i = 0; i < 18; ++i)
+        float anc[kYoloMaxLevels * 6];
+        const int n_anc = (int)e->hdr.n_outputs * 6;          // validated: 3 or 4 levels, tensor of exactly this size
+        memcpy(anc, blob.data() + e->tensors[e->hdr.meta[3] - 1].offset, n_anc * sizeof(float));
+        for (int i = 0; i < n_anc; ++i)
             ADAS_CHECK(isfinite(anc[i]) && anc[i] > 0.f, "plan %s: anchor %d of the head's table is %g (finite and positive required)", plan_path, i, (double)anc[i]);
     }
 

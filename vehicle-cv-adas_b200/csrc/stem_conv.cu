@@ -19,7 +19,8 @@
 // Accumulation is fp32 in a fixed order, independent of the batch size and of the grid: frame k of a batch equals the batch-1 result.
 //
 // Reference: the conv stacks behind coreEngine.py:150-157 / 184-186 (first Conv of YOLOv8 [3x3 s2], YOLOv5 [6x6 s2 p2], ResNet [7x7 s2 p3],
-// YOLOv7 [3x3 s1 at full input resolution], YOLOv7-tiny [3x3 s2]).
+// YOLOv7 [3x3 s1 at full input resolution], YOLOv7-tiny [3x3 s2], YOLOv7-W6 / E6 / E6E [ReOrg + 3x3 folded into 6x6 s2 p2, 64 / 80
+// channels; 96 for D6]).
 #include "common.h"
 #include "tc_common.cuh"
 #include "gemm_v3.h"
@@ -28,7 +29,8 @@ namespace adas {
 
 static constexpr int STEM_THREADS = 256;
 static constexpr int STEM_WARPS = STEM_THREADS / 32;
-static constexpr int STEM_STG_LD = 64 + 8;        // halves per staged pixel row (16-byte aligned, bank-shifted)
+// halves per staged pixel row (16-byte aligned, bank-shifted): 64 + 8 up to 64 channels, Cout + 8 for the 80 / 96-channel P6 stems
+__host__ __device__ constexpr int stem_stg_ld(int nt) { return nt <= 8 ? 64 + 8 : nt * 8 + 8; }
 
 __device__ __forceinline__ void mma_m16n8k16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
     asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
@@ -51,6 +53,7 @@ struct StemParams {
 template <int NT>
 __global__ void __launch_bounds__(STEM_THREADS) stem_conv_kernel(const StemParams p) {
     extern __shared__ __align__(16) uint8_t smem[];
+    constexpr int STEM_STG_LD = stem_stg_ld(NT);
     const int w_ld = p.w_ld;                                          // halves
     __half* ws = reinterpret_cast<__half*>(smem);
     __half* stg_all = ws + (size_t)NT * 8 * w_ld;
@@ -122,8 +125,12 @@ __global__ void __launch_bounds__(STEM_THREADS) stem_conv_kernel(const StemParam
 }
 
 int stem_conv_supported(int Cout, int k, int pad) {
-    return (Cout == 16 || Cout == 32 || Cout == 48 || Cout == 64) && k >= 3 && k <= 7 && pad >= 0 && pad <= 3;
+    return (Cout == 16 || Cout == 32 || Cout == 48 || Cout == 64 || Cout == 80 || Cout == 96) && k >= 3 && k <= 7 && pad >= 0 && pad <= 3;
 }
+
+// The 80 / 96-channel stems (YOLOv7-E6 / E6E / D6, ReOrg + 3x3 folded into a 6x6 stride-2 conv) stage more than 48 KB: the kernel opts
+// in on every launch (a host-side attribute, legal during graph capture).  k = 7 at 96 channels needs 77 KB.
+static constexpr int STEM_WIDE_SMEM = 96 * 1024;
 
 int launch_stem_conv(const __half* img, int B, int H, int W, const __half* wq, const float* bias, int Cout, int k, int pad, int stride, int act,
                      __half* out, int out_ld, int Ho, int Wo, cudaStream_t st) {
@@ -139,19 +146,37 @@ int launch_stem_conv(const __half* img, int B, int H, int W, const __half* wq, c
     p.total_tiles = B * Ho * p.tiles_per_row;
     // weight row stride = 16 (mod 64) halves: the 8-byte fragment loads of a half-warp (4 rows x 4 lanes) then cover all 32 banks once;
     // K + 8 (2-way conflicts) only where the conflict-free stride would not fit 48 KB
+    // (the 80 / 96-channel stems opt in to more than 48 KB and keep the conflict-free stride)
+    const int stg_bytes = STEM_WARPS * 16 * stem_stg_ld(Cout / 8) * 2;
+    const int smem_cap = Cout > 64 ? STEM_WIDE_SMEM : 48 * 1024;
     p.w_ld = p.K + ((16 - p.K % 64) + 64) % 64;
-    if (Cout * p.w_ld * 2 + STEM_WARPS * 16 * STEM_STG_LD * 2 > 48 * 1024) p.w_ld = p.K + 8;
-    const int smem = Cout * p.w_ld * 2 + STEM_WARPS * 16 * STEM_STG_LD * 2;
-    ADAS_CHECK(smem <= 48 * 1024, "stem_conv: %d bytes of shared memory", smem);
+    if (Cout * p.w_ld * 2 + stg_bytes > smem_cap) p.w_ld = p.K + 8;
+    const int smem = Cout * p.w_ld * 2 + stg_bytes;
+    ADAS_CHECK(smem <= smem_cap, "stem_conv: %d bytes of shared memory", smem);
     int blocks = (p.total_tiles + STEM_WARPS - 1) / STEM_WARPS;
     int n_sms = 132;
     if (v3_num_sms(&n_sms)) return 1;
-    const int cap = n_sms * 3;                      // resident blocks only: the weight copy is per block, a warp walks ~20 tiles
+    // resident blocks only (at most 3 per SM): the weight copy is per block, a warp walks ~20 tiles.  The 80 / 96-channel kernels hold
+    // fewer blocks per SM (96 channels: 92 registers, 2 blocks), so their cap comes from the occupancy of the kernel as launched.
+    int per_sm = 3;
+    auto wide = [&](auto kernel) -> int {
+        ADAS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, STEM_WIDE_SMEM));
+        int occ = 0;
+        ADAS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, STEM_THREADS, smem));
+        ADAS_CHECK(occ >= 1, "stem_conv: %d-channel kernel does not fit an SM (%d bytes of shared memory)", Cout, smem);
+        if (occ < per_sm) per_sm = occ;
+        return 0;
+    };
+    if (Cout == 80 && wide(stem_conv_kernel<10>)) return 1;
+    if (Cout == 96 && wide(stem_conv_kernel<12>)) return 1;
+    const int cap = n_sms * per_sm;
     if (blocks > cap) blocks = cap;
     switch (Cout / 8) {
         case 2: stem_conv_kernel<2><<<blocks, STEM_THREADS, smem, st>>>(p); break;
         case 4: stem_conv_kernel<4><<<blocks, STEM_THREADS, smem, st>>>(p); break;
         case 6: stem_conv_kernel<6><<<blocks, STEM_THREADS, smem, st>>>(p); break;
+        case 10: stem_conv_kernel<10><<<blocks, STEM_THREADS, smem, st>>>(p); break;
+        case 12: stem_conv_kernel<12><<<blocks, STEM_THREADS, smem, st>>>(p); break;
         default: stem_conv_kernel<8><<<blocks, STEM_THREADS, smem, st>>>(p); break;
     }
     count_launch();

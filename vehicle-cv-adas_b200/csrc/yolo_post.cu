@@ -113,20 +113,25 @@ int launch_yolov6_head_decode(const YoloLevel* lv, int B, int nc, int reg_max, f
 
 // YOLOv5 Detect: per level fp32 [rows, ld>=3*(5+nc)], channel = anchor*(5+nc) + k.
 // raw[b][idx][5+nc], idx = level offset + anchor*H*W + y*W + x  (yoloDetector.py:45-48 ordering).
-// Anchor (w, h) pairs [level][anchor]: the plan's own table (YOLOv7) or, without one, the YOLOv5 table below.
+// Anchor (w, h) pairs [level][anchor]: the plan's own table (YOLOv7; 3 or 4 levels) or, without one, the YOLOv5 table below (3 levels).
 __constant__ float c_v5_anchors[18] = {10, 13, 16, 30, 33, 23, 30, 61, 62, 45, 59, 119, 116, 90, 156, 198, 373, 326};
 
+// Up to four head levels by value (strides 8 / 16 / 32 / 64 of the P6 models), n of them in use.
+struct YoloLevels { YoloLevel l[kYoloMaxLevels]; int n; };
+
 // lite != 0: the head of a YOLOv5-lite export -- sigmoid only, grid/anchor decode left to lite_postprocess (yoloDetector.py:36-50).
-__global__ void yolov5_decode_kernel(YoloLevel l0, YoloLevel l1, YoloLevel l2, int B, int nc, float* __restrict__ raw, int A, int lite,
-                                     const float* __restrict__ anchors) {
+__global__ void yolov5_decode_kernel(const YoloLevels L, int B, int nc, float* __restrict__ raw, int A, int lite, const float* __restrict__ anchors) {
     const long long total = (long long)B * A;
     const int no = 5 + nc;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const int b = (int)(i / A);
         int a = (int)(i % A);
-        YoloLevel lv = l0;
+        YoloLevel lv = L.l[0];
         int li = 0;
-        if (a >= 3 * l0.H * l0.W) { a -= 3 * l0.H * l0.W; lv = l1; li = 1; if (a >= 3 * l1.H * l1.W) { a -= 3 * l1.H * l1.W; lv = l2; li = 2; } }
+        // level of row a: unrolled with constant indices so the levels stay in registers / parameter space
+#pragma unroll
+        for (int j = 1; j < kYoloMaxLevels; ++j)
+            if (j < L.n && a >= 3 * lv.H * lv.W) { a -= 3 * lv.H * lv.W; lv = L.l[j]; li = j; }
         const int hw = lv.H * lv.W;
         const int an = a / hw;
         const int r = a % hw;
@@ -149,10 +154,15 @@ __global__ void yolov5_decode_kernel(YoloLevel l0, YoloLevel l1, YoloLevel l2, i
     }
 }
 
-int launch_yolov5_head_decode(const YoloLevel* lv, int B, int nc, float* raw, int A, int lite, const float* anchors, cudaStream_t st) {
+int launch_yolov5_head_decode(const YoloLevel* lv, int n_levels, int B, int nc, float* raw, int A, int lite, const float* anchors, cudaStream_t st) {
+    ADAS_CHECK(n_levels == 3 || (n_levels == kYoloMaxLevels && !lite && anchors != nullptr),
+               "YOLOv5-layout decode: %d levels (3, or 4 with the plan's anchor table)", n_levels);
+    YoloLevels L;
+    for (int j = 0; j < kYoloMaxLevels; ++j) L.l[j] = lv[j < n_levels ? j : 0];
+    L.n = n_levels;
     const long long total = (long long)B * A;
     int blocks = (int)((total + 127) / 128);
-    yolov5_decode_kernel<<<blocks, 128, 0, st>>>(lv[0], lv[1], lv[2], B, nc, raw, A, lite, anchors);
+    yolov5_decode_kernel<<<blocks, 128, 0, st>>>(L, B, nc, raw, A, lite, anchors);
     count_launch();
     ADAS_CUDA(cudaGetLastError());
     return 0;

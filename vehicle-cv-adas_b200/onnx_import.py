@@ -387,7 +387,7 @@ def recognise(model: OnnxModel) -> ModelSpec:
     raise Exception(f"unrecognised first convolution {first.shape}")
 
 
-_V7_SUPPORTED = "YOLOv7 and YOLOv7-tiny (P5, 3 detection levels; the X / W6 / E6 / D6 / E6E variants are not supported)"
+_V7_SUPPORTED = "YOLOv7 and YOLOv7-tiny (P5, 3 detection levels), YOLOv7-W6 / E6 / D6 / E6E (P6, 4 levels; YOLOv7-X is not supported)"
 
 
 def _is_yolov7(model: OnnxModel, w: OnnxWeights) -> bool:
@@ -413,6 +413,8 @@ def _recognise_yolov7(model: OnnxModel, w: OnnxWeights, in_h: int, in_w: int) ->
             n += 1
         heads = [(name, cw) for name, cw, _ in tail[:n][::-1]]
     no = heads[-1][1].shape[0]
+    if first.shape[1] == 12:
+        return _recognise_yolov7_p6(model, w, stem, heads, in_h, in_w)
     if first.shape != (32, 3, 3, 3) or stride0 not in (1, 2) or len(heads) != 3 or no % 3 != 0 or (in_h and in_h > 1024):
         raise Exception(f"YOLOv7-family file outside the supported models: first convolution {tuple(first.shape)} stride {stride0}, "
                         f"{len(heads)} detection levels, input {in_h}x{in_w}; supported: {_V7_SUPPORTED}")
@@ -421,15 +423,79 @@ def _recognise_yolov7(model: OnnxModel, w: OnnxWeights, in_h: int, in_w: int) ->
     if named and int(named.group(1)) != {"base": 105, "tiny": 77}[scale]:
         raise Exception(f"YOLOv7 head at layer {named.group(1)} does not match the {scale} graph; supported: {_V7_SUPPORTED}")
     act = "leaky" if any(n.op_type == "LeakyRelu" for n in model.nodes) else "silu"
-    anchors = None
-    grids = [v for k, v in model.initializers.items() if k.endswith("anchor_grid") and v.size == 18]
-    if not grids:                               # constant-folded exports: one [1, 3, 1, 1, 2] anchor tensor per level, in graph order
+    return ModelSpec("yolov7", scale, no // 3 - 5, in_h or 640, in_w or 640, act, _v7_anchors(model, 3))
+
+
+def _v7_anchors(model: OnnxModel, levels: int) -> Optional[Tuple[float, ...]]:
+    """IDetect's `anchor_grid` ([levels, 1, 3, 1, 1, 2]) or, in constant-folded exports, one [1, 3, 1, 1, 2] tensor per level in graph order."""
+    grids = [v for k, v in model.initializers.items() if k.endswith("anchor_grid") and v.size == 6 * levels]
+    if not grids:
         per_level = [v for k, v in model.initializers.items() if tuple(v.shape) == (1, 3, 1, 1, 2) and v.dtype.kind == "f"]
-        if len(per_level) == 3:
+        if len(per_level) == levels:
             grids = [np.concatenate([g.reshape(6) for g in per_level])]
-    if grids:
-        anchors = tuple(float(v) for v in np.asarray(grids[0], np.float32).reshape(18))
-    return ModelSpec("yolov7", scale, no // 3 - 5, in_h or 640, in_w or 640, act, anchors)
+    return tuple(float(v) for v in np.asarray(grids[0], np.float32).reshape(6 * levels)) if grids else None
+
+
+def reorg_slices(model: OnnxModel, stem) -> Optional[List[Tuple[int, int]]]:
+    """(row, column) offsets of the four stride-2 slices of the image that the stem convolution's input concatenates, in concat order
+    (upstream ReOrg: x[..., ::2, ::2], x[..., 1::2, ::2], x[..., ::2, 1::2], x[..., 1::2, 1::2]); None if that input is not such a
+    Concat of Slice chains on the network input."""
+    image = model.inputs[0][0] if model.inputs else None
+    prod = {o: n for n in model.nodes for o in n.outputs}
+    cat = prod.get(stem.inputs[0])
+    if cat is None or cat.op_type != "Concat" or len(cat.inputs) != 4 or int(cat.attrs.get("axis", 1)) % 4 != 1:
+        return None
+    order = []
+    for t in cat.inputs:
+        off: Dict[int, int] = {}
+        while t != image:
+            n = prod.get(t)
+            if n is None or n.op_type != "Slice" or len(n.inputs) < 5 or any(i not in model.initializers for i in n.inputs[1:5]):
+                return None
+            starts, _, axes, steps = (np.asarray(model.initializers[i]).reshape(-1) for i in n.inputs[1:5])
+            for s, a, st in zip(starts, axes, steps):
+                a = int(a) % 4
+                if a not in (2, 3) or int(st) != 2 or a in off:
+                    return None
+                off[a] = int(s)
+            t = n.inputs[0]
+        if set(off) != {2, 3}:
+            return None
+        order.append((off[2], off[3]))
+    return order
+
+
+# convolutions of each P6 file (tells E6 from E6E when the module names are gone); stem width -> scales
+_P6_CONVS = {"w6": 107, "e6": 145, "d6": 167, "e6e": 244}
+_P6_STEM = {64: ("w6",), 80: ("e6", "e6e"), 96: ("d6",)}
+
+
+def _recognise_yolov7_p6(model: OnnxModel, w: OnnxWeights, stem, heads, in_h: int, in_w: int) -> ModelSpec:
+    """YOLOv7 P6 (W6 / E6 / D6 / E6E): a ReOrg stem (the image's four stride-2 slices, concatenated in upstream's order) feeding Conv(12, c, 3),
+    4 detection convs, an input that is a multiple of 64."""
+    first = w.convs[0][1]
+    cands = _P6_STEM.get(int(first.shape[0]), ()) if tuple(first.shape[1:]) == (12, 3, 3) else ()
+    if not cands:
+        raise Exception(f"YOLOv7 P6 stem {tuple(first.shape)}: 64 (W6), 80 (E6 / E6E) or 96 (D6) channels from a 12-channel ReOrg; supported: {_V7_SUPPORTED}")
+    order = reorg_slices(model, stem)
+    if order != [tuple(s) for s in plan.REORG_SLICES]:
+        raise Exception(f"YOLOv7 P6 stem input is not upstream's ReOrg of the image (slice offsets {order}, expected "
+                        f"{[tuple(s) for s in plan.REORG_SLICES]}); supported: {_V7_SUPPORTED}")
+    no = heads[-1][1].shape[0]
+    if len(heads) != 4 or no % 3 != 0:
+        raise Exception(f"YOLOv7 file with a ReOrg stem and {len(heads)} detection levels (a P6 model has 4); supported: {_V7_SUPPORTED}")
+    if (in_h and in_h % 64) or (in_w and in_w % 64):
+        raise Exception(f"YOLOv7 P6 file with a {in_h}x{in_w} input: a multiple of 64 (stride-64 head); supported: {_V7_SUPPORTED}")
+    named = re.fullmatch(r"model\.(\d+)\.m\.\d+\.weight", heads[-1][0])
+    if named:
+        scales = [s for s in cands if plan.YOLOV7_P6[s]["det"] == int(named.group(1))]
+    else:
+        scales = [s for s in cands if _P6_CONVS[s] == len(w.convs)]
+    if len(scales) != 1:
+        raise Exception(f"YOLOv7 P6 file with a {first.shape[0]}-channel stem and {len(w.convs)} convolutions"
+                        f"{f', head at layer {named.group(1)}' if named else ''} matches none of {', '.join(cands)}; supported: {_V7_SUPPORTED}")
+    act = "leaky" if any(n.op_type == "LeakyRelu" for n in model.nodes) else "silu"
+    return ModelSpec("yolov7", scales[0], no // 3 - 5, in_h or 1280, in_w or 1280, act, _v7_anchors(model, 4))
 
 
 _V6_SUPPORTED = "YOLOv6-N / S / M / L (release 0.4.0, P5, 3 detection levels; YOLOv6-Lite, the P6 models and the 2.x models are not supported)"

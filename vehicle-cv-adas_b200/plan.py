@@ -185,10 +185,10 @@ class Weights:
         w64 = w.astype(np.float64)
         return (w64 * im[:, None, None, None]).astype(np.float32), (im * (b.astype(np.float64) + w64[:, :, 0, 0] @ ia)).astype(np.float32)
 
-    def anchor_grid(self, prefix: str) -> Optional[np.ndarray]:
-        """Anchors in input pixels from an upstream Detect / IDetect `anchor_grid` buffer ([3, 1, 3, 1, 1, 2]), when the source has one."""
+    def anchor_grid(self, prefix: str, levels: int = 3) -> Optional[np.ndarray]:
+        """Anchors in input pixels from an upstream Detect / IDetect `anchor_grid` buffer ([levels, 1, 3, 1, 1, 2]), when the source has one."""
         a = self.state_dict.get(f"{prefix}.anchor_grid")
-        return None if a is None or a.size != 18 else np.asarray(a, np.float32).reshape(18)
+        return None if a is None or a.size != 6 * levels else np.asarray(a, np.float32).reshape(6 * levels)
 
     def conv_bias(self, prefix: str, cout: int, cin: int, k: int):
         w = self.get(f"{prefix}.weight", (cout, cin, k, k), "conv")
@@ -217,8 +217,14 @@ SYNTH_PROFILES = {
     # SiLU: its fp16 noise at the head is ~50x larger, so its head gain is 0.3, its objectness / class biases (-0.2) set the operating
     # point and its box biases sit at -3, where the xywh sigmoids are flat (box noise 0.4 px -> 0.01 px).  CPU fp16 emulation on
     # 4 frames: base 6.1e-4 / 0.10 px / ~280 candidates per frame, tiny 5.9e-4 / 0.01 px / ~100 candidates per frame.
-    "yolov7": {"gains": [(r"model\.105\.m\.\d\.weight", 16.0), (r"model\.77\.m\.\d\.weight", 0.3)],
-               "fill": [(r"model\.105\.m\.\d\.bias", -3.0), (r"model\.77\.m\.\d\.bias", (-3.0, -0.2))]},
+    # The P6 heads W6 (model.118), E6 (140) and D6 (162) take base's head gain.  W6's bias (-1.75) puts ~230 of the 102000 anchors
+    # of a letterboxed 1280x720 frame above box_score = 0.4 (fp32 oracle, frames 4 and 5; at -2.0 there are ~120 but half sit within 1e-3 of it).  E6E (261)
+    # runs every ELAN twice and sums the pair: at gain 16 its device error was 1.4e-3 / 0.99 px at 640, so its head gain is 6 and its box
+    # biases sit at -4, where the xywh sigmoids are flat.
+    "yolov7": {"gains": [(r"model\.105\.m\.\d\.weight", 16.0), (r"model\.77\.m\.\d\.weight", 0.3),
+                         (r"model\.(118|140|162)\.m\.\d\.weight", 16.0), (r"model\.261\.m\.\d\.weight", 6.0)],
+               "fill": [(r"model\.105\.m\.\d\.bias", -3.0), (r"model\.77\.m\.\d\.bias", (-3.0, -0.2)),
+                        (r"model\.118\.m\.\d\.bias", -1.75), (r"model\.(140|162)\.m\.\d\.bias", -3.0), (r"model\.261\.m\.\d\.bias", (-4.0, -3.0))]},
     # YOLOv6 N/S/M/L: convs damped (0.85, and 0.6 on the BepC3 / SPPF / BiFusion 1x1 convs) so that the ReLU bodies of M do not grow
     # their activations layer by layer; class logits widened (gain 12: at 16 the M device error is 1.04e-3); box biases of 2 grid cells
     # keep the raw l, t, r, b distances of N/S positive (a constant bias cancels in the DFL softmax of M/L).  The class bias of each
@@ -308,10 +314,13 @@ class PlanBuilder:
 
     def conv(self, x: View, w: np.ndarray, b: Optional[np.ndarray], k: int, s: int, act: int, out: Optional[View] = None,
              res: Optional[View] = None, res_pre_act: bool = False, out_f32: bool = False, pad: Optional[int] = None,
-             tile: Optional[Tuple[int, int]] = None, no_slab: bool = False, res_scale: Optional[float] = None) -> View:
+             tile: Optional[Tuple[int, int]] = None, no_slab: bool = False, res_scale: Optional[float] = None,
+             wide_stem: bool = False) -> View:
         """w: folded [Cout, Cin_real, k, k] fp32.  x.C may exceed Cin_real (zero-padded image channel).
         res_scale: out = act(conv) + res_scale * res (YOLOv6 BottleRep's alpha); None = a plain residual add (op f[0] = 0).
-        no_slab (test hook): a 3x3 stride-1 conv loads one activation tile per tap instead of one slab per (dy, k-block)."""
+        no_slab (test hook): a 3x3 stride-1 conv loads one activation tile per tap instead of one slab per (dy, k-block).
+        wide_stem: an 80 / 96-channel image conv also runs in stem_conv.cu (the YOLOv7 P6 stems); without it those widths keep the
+        im2col + GEMM route, so the 80-channel stems of YOLOv5x / YOLOv8x pack as before."""
         assert res_scale is None or (res is not None and not res_pre_act and math.isfinite(res_scale) and res_scale != 0.0), res_scale
         cout, cin_real = int(w.shape[0]), int(w.shape[1])
         pad = k // 2 if pad is None else pad
@@ -328,7 +337,8 @@ class PlanBuilder:
         if out is None:
             out = self.new_padded(Ho, Wo, n_store, f32=out_f32)
         assert out.H == Ho and out.W == Wo, (out, Ho, Wo)
-        if (self.stem_direct and x.buf == self.image.buf and x.C == 4 and s in (1, 2) and 3 <= k <= 7 and cout in (16, 32, 48, 64) and res is None
+        stem_couts = (16, 32, 48, 64, 80, 96) if wide_stem else (16, 32, 48, 64)
+        if (self.stem_direct and x.buf == self.image.buf and x.C == 4 and s in (1, 2) and 3 <= k <= 7 and cout in stem_couts and res is None
                 and not out_f32 and tile is None and out.coff % 8 == 0):
             return self.stem_conv(x, w, b, k, s, pad, act, out)
         wk = np.transpose(w, (0, 2, 3, 1)).reshape(cout, k * k * cin)   # [Cout, kh, kw, Cin]
@@ -652,28 +662,76 @@ def build_yolov5(weights: Weights, scale: str = "n", nc: int = 80, in_h: int = 6
 # ---------------------------------------------------------------------------------------------
 YOLOV5_ANCHORS = ((10, 13, 16, 30, 33, 23), (30, 61, 62, 45, 59, 119), (116, 90, 156, 198, 373, 326))
 YOLOV7_ANCHORS = ((12, 16, 19, 36, 40, 28), (36, 75, 76, 55, 72, 146), (142, 110, 192, 243, 459, 401))
+YOLOV7_P6_ANCHORS = ((19, 27, 44, 40, 38, 94), (96, 68, 86, 152, 180, 137), (140, 301, 303, 264, 238, 542), (436, 615, 739, 380, 925, 792))
 YOLOV7_ACTS = {"silu": ACT_SILU, "leaky": ACT_LEAKY}
+# P6 models (cfg/deploy/yolov7-{w6,e6,d6,e6e}.yaml): ReOrg + Conv(12, stem, 3, 1) stem; five stride-2 stages, each a down-sampling layer
+# (W6: Conv 3x3 s2, else DownC) to `cout` channels and an ELAN of width c with n3 chained 3x3 convs to `cout`; head output widths of the
+# P3 .. P6 levels (SPPCSPC's width is the P6 one); E6E runs every ELAN twice on the same input and sums the pair (Shortcut).
+# D6 as restated here (96-channel stem, 8-conv ELANs, E6's head widths) has 133.8 M parameters / 701.7 GFLOP against the published
+# 154.7 M / 806.8 G: some width of the upstream graph is not reproduced.  A D6 checkpoint whose shapes differ is refused by name and shape
+# (Weights.get), never packed wrongly.
+YOLOV7_P6 = {
+    "w6": dict(stem=64, downc=False, n3=4, stages=((128, 64), (256, 128), (512, 256), (768, 384), (1024, 512)), outs=(128, 256, 384, 512),
+               pair=False, det=118),
+    "e6": dict(stem=80, downc=True, n3=6, stages=((160, 64), (320, 128), (640, 256), (960, 384), (1280, 512)), outs=(160, 320, 480, 640),
+               pair=False, det=140),
+    "d6": dict(stem=96, downc=True, n3=8, stages=((192, 64), (384, 128), (768, 256), (1152, 384), (1536, 512)), outs=(192, 384, 576, 768),
+               pair=False, det=162),
+    "e6e": dict(stem=80, downc=True, n3=6, stages=((160, 64), (320, 128), (640, 256), (960, 384), (1280, 512)), outs=(160, 320, 480, 640),
+                pair=True, det=261),
+}
+# head ELAN widths (c, c3): top-down P5, P4, P3, then bottom-up P4, P5, P6
+YOLOV7_P6_HEAD = ((384, 192), (256, 128), (128, 64), (256, 128), (384, 192), (512, 256))
+YOLOV7_SCALES = ("tiny", "base") + tuple(YOLOV7_P6)
+# ReOrg's four strided slices in the order upstream concatenates them: (row, column) offsets of x[..., ::2, ::2], x[..., 1::2, ::2],
+# x[..., ::2, 1::2], x[..., 1::2, 1::2]
+REORG_SLICES = ((0, 0), (1, 0), (0, 1), (1, 1))
 
 
-def build_yolov7(weights: Weights, scale: str = "tiny", nc: int = 80, in_h: int = 640, in_w: int = 640, act: Optional[str] = None,
-                 anchors=None) -> PlanBuilder:
-    """YOLOv7 ("base", SiLU) or YOLOv7-tiny ("tiny", LeakyReLU(0.1); act="silu" gives the tiny-SiLU variant).  The head decodes like
-    YOLOv5's ([B, 25200, 5 + nc], MODEL_YOLOV5 kind) with the anchor table carried by the plan (header meta[3]).
+def reorg_stem_weights(w: np.ndarray) -> np.ndarray:
+    """Conv(12, c, 3, s=1, p=1) after ReOrg as one Conv(3, c, 6, s=2, p=2) on the image: w6[o, c, 2ky + dy, 2kx + dx] =
+    w[o, 3 * slice(dy, dx) + c, ky, kx].  A pure permutation (exact in any precision); ReOrg pixel -1 covers image rows / columns
+    -2 and -1, so the zero padding matches too."""
+    cout = w.shape[0]
+    assert w.shape[1:] == (12, 3, 3), w.shape
+    w6 = np.zeros((cout, 3, 6, 6), w.dtype)
+    for sl, (dy, dx) in enumerate(REORG_SLICES):
+        w6[:, :, dy::2, dx::2] = w[:, 3 * sl:3 * sl + 3]
+    return w6
+
+
+def yolov7_levels(scale: str) -> int:
+    return 4 if scale in YOLOV7_P6 else 3
+
+
+def build_yolov7(weights: Weights, scale: str = "tiny", nc: int = 80, in_h: Optional[int] = None, in_w: Optional[int] = None,
+                 act: Optional[str] = None, anchors=None) -> PlanBuilder:
+    """YOLOv7 ("base", SiLU), YOLOv7-tiny ("tiny", LeakyReLU(0.1); act="silu" gives the tiny-SiLU variant) or the P6 models "w6", "e6",
+    "d6", "e6e" (SiLU, 4 levels, 1280x1280 by default, inputs a multiple of 64).  The head decodes like YOLOv5's ([B, 25200, 5 + nc] at
+    640 for P5; [B, 102000, 5 + nc] at 1280 for P6; MODEL_YOLOV5 kind) with the anchor table carried by the plan (header meta[3]).
     RepConv (base head) and IDetect's implicit layers are folded here in fp64; an ELAN's two 1x1 convolutions on the same input run
-    as one GEMM writing the last two slices of its concat."""
-    assert scale in ("tiny", "base"), f"YOLOv7 scale {scale!r}: 'tiny' or 'base' (the X / W6 / E6 / D6 / E6E variants are not supported)"
+    as one GEMM writing the last two slices of its concat.  Training-form P6 checkpoints (IAuxDetect four layers after the deploy
+    IDetect, aux convs in between) pack from their main path: the deploy numbering is the same up to the head."""
+    assert scale in YOLOV7_SCALES, f"YOLOv7 scale {scale!r}: one of {', '.join(YOLOV7_SCALES)} (YOLOv7-X is not supported)"
+    p6 = YOLOV7_P6.get(scale)
+    in_h = in_h or (1280 if p6 else 640)
+    in_w = in_w or (1280 if p6 else 640)
+    if p6:
+        assert in_h % 64 == 0 and in_w % 64 == 0, f"YOLOv7-{scale.upper()} input {in_h}x{in_w}: a multiple of 64 (stride-64 head)"
     act_id = YOLOV7_ACTS[act or ("leaky" if scale == "tiny" else "silu")]
     pb = PlanBuilder(MODEL_YOLOV5, 3, in_h, in_w)
     W = weights
     eps = BN_EPS_YOLO
 
-    def cbs(x: View, name: str, cout: int, k: int, s: int = 1, out: Optional[View] = None, cin: Optional[int] = None) -> View:
+    def cbs(x: View, name: str, cout: int, k: int, s: int = 1, out: Optional[View] = None, cin: Optional[int] = None,
+            res: Optional[View] = None) -> View:
         w, b = W.conv_bn(name, cout, cin if cin is not None else x.C, k, eps)
-        return pb.conv(x, w, b, k, s, act_id, out=out)
+        return pb.conv(x, w, b, k, s, act_id, out=out, res=res)
 
-    def elan(x: View, i: int, c: int, c3: int, n3: int, cout: int, out: Optional[View] = None, keep=None) -> View:
+    def elan(x: View, i: int, c: int, c3: int, n3: int, cout: int, out: Optional[View] = None, keep=None, res: Optional[View] = None) -> View:
         """a = model.i, b = model.i+1 (1x1 on x), n3 chained 3x3 convs from b (model.i+2 ..), concat model.i+2+n3 of the kept 3x3
-        outputs in reverse order, then b, a; then the 1x1 model.i+3+n3.  `keep`: 0-based 3x3 positions in the concat (default all)."""
+        outputs in reverse order, then b, a; then the 1x1 model.i+3+n3 (+ `res` after its activation: E6E's Shortcut).  `keep`:
+        0-based 3x3 positions in the concat (default all)."""
         keep = list(range(n3)) if keep is None else list(keep)
         cat = pb.new_padded(x.H, x.W, len(keep) * c3 + 2 * c)
         wa, ba = W.conv_bn(f"model.{i}", c, x.C, 1, eps)
@@ -683,7 +741,7 @@ def build_yolov7(weights: Weights, scale: str = "tiny", nc: int = 80, in_h: int 
         for j in range(n3):
             slot = keep[::-1].index(j) if j in keep else None
             t = cbs(t, f"model.{i + 2 + j}", c3, 3, out=pb.sub(cat, slot * c3, c3) if slot is not None else None)
-        return cbs(cat, f"model.{i + 3 + n3}", cout, 1, out=out)
+        return cbs(cat, f"model.{i + 3 + n3}", cout, 1, out=out, res=res)
 
     def mp_block(x: View, i: int, c: int, out: View) -> View:
         """model.i MaxPool 2x2 s2; model.i+1 = 1x1 of the pool, model.i+2 = 1x1 of x, model.i+3 = 3x3 s2 of model.i+2;
@@ -701,8 +759,83 @@ def build_yolov7(weights: Weights, scale: str = "tiny", nc: int = 80, in_h: int 
         for sl in slots:
             y = pb.maxpool(y, 5, 1, 2, out=pb.sub(cat, sl * x.C, x.C))
 
+    def sppcspc(x: View, i: int, c_: int, out: View) -> View:
+        """model.i SPPCSPC(c_): cv7([cv6(cv5([x1, p5, p9, p13])), cv2(x)]), x1 = cv4(cv3(cv1(x)))."""
+        cat7 = pb.new_padded(x.H, x.W, 2 * c_)               # cv7 input [y1, y2]
+        sp = pb.new_padded(x.H, x.W, 4 * c_)                 # cv5 input [x1, p5, p9, p13]
+        t = cbs(x, f"model.{i}.cv1", c_, 1)
+        t = cbs(t, f"model.{i}.cv3", c_, 3)
+        x1 = cbs(t, f"model.{i}.cv4", c_, 1, out=pb.sub(sp, 0, c_))
+        pools(x1, sp, [1, 2, 3])
+        t = cbs(sp, f"model.{i}.cv5", c_, 1)
+        cbs(t, f"model.{i}.cv6", c_, 3, out=pb.sub(cat7, 0, c_))
+        cbs(x, f"model.{i}.cv2", c_, 1, out=pb.sub(cat7, c_, c_))
+        return cbs(cat7, f"model.{i}.cv7", c_, 1, out=out)
+
+    def down_c(x: View, i: int, cout: int, out: View) -> View:
+        """model.i DownC(cout): [cv2(cv1(x)) (3x3 s2), cv3(MaxPool 2x2 s2 (x))], cv1 keeping x's width."""
+        h = cout // 2
+        cbs(pb.maxpool(x, 2, 2, 0), f"model.{i}.cv3", h, 1, out=pb.sub(out, h, h))
+        t = cbs(x, f"model.{i}.cv1", x.C, 1)
+        cbs(t, f"model.{i}.cv2", h, 3, 2, out=pb.sub(out, 0, h))
+        return out
+
     H, Wd = in_h, in_w
-    if scale == "base":
+    det_levels = 3
+    if p6:
+        n3, pair = p6["n3"], p6["pair"]
+        n_elan = 4 + n3                                      # layers of one ELAN
+        blk = 2 * n_elan + 1 if pair else n_elan             # layers of an ELAN block (E6E: two ELANs + Shortcut)
+
+        def elan_block(x: View, i: int, c: int, c3: int, cout: int, out: Optional[View] = None, keep=None) -> View:
+            if not pair:
+                return elan(x, i, c, c3, n3, cout, out=out, keep=keep)
+            e1 = elan(x, i, c, c3, n3, cout, keep=keep)
+            return elan(x, i + n_elan, c, c3, n3, cout, out=out, keep=keep, res=e1)
+
+        def down(x: View, i: int, cout: int, out: Optional[View] = None) -> View:
+            out = out if out is not None else pb.new_padded(x.H // 2, x.W // 2, cout)
+            return down_c(x, i, cout, out) if p6["downc"] else cbs(x, f"model.{i}", cout, 3, 2, out=out)
+
+        # model.0 ReOrg + model.1 Conv(12, stem, 3, 1) = one 6x6 stride-2 conv of the image (stem_conv.cu)
+        w, b = W.conv_bn("model.1", p6["stem"], 12, 3, eps)
+        x = pb.conv(pb.image, reorg_stem_weights(w), b, 6, 2, act_id, pad=2, wide_stem=True)
+        bk = tuple(range(1, n3, 2))                          # backbone ELAN: cat[3x3 #n3, .., #4, #2, b, a]
+        i, stages = 2, []
+        for cout, c in p6["stages"]:
+            x = elan_block(down(x, i, cout), i + 1, c, c, cout, keep=bk)
+            i += 1 + blk
+            stages.append(x)
+        o3, o4, o5, o6 = p6["outs"]
+        cat_n6 = pb.new_padded(H // 64, Wd // 64, 2 * o6)    # [down(n5), sppcspc]
+        cat_n5 = pb.new_padded(H // 32, Wd // 32, 2 * o5)    # [down(n4), h5]
+        cat_n4 = pb.new_padded(H // 16, Wd // 16, 2 * o4)    # [down(n3), h4]
+        h = sppcspc(x, i, o6, pb.sub(cat_n6, o6, o6))
+        i += 1
+        # top-down: conv + upsample of the level above, route conv of the backbone level, ELAN (into the bottom-up concat's slice 1)
+        hd = p6.get("head", YOLOV7_P6_HEAD)
+        for src, (c, c3), cout, cat_n in ((stages[3], hd[0], o5, cat_n5), (stages[2], hd[1], o4, cat_n4), (stages[1], hd[2], o3, None)):
+            cat = pb.new_padded(src.H, src.W, 2 * cout)      # [route conv, up(conv)]
+            t = cbs(h, f"model.{i}", cout, 1)
+            pb.upsample2x(t, pb.sub(cat, cout, cout))
+            cbs(src, f"model.{i + 2}", cout, 1, out=pb.sub(cat, 0, cout))
+            i += 4
+            h = elan_block(cat, i, c, c3, cout, out=pb.sub(cat_n, cout, cout) if cat_n is not None else None)
+            i += blk
+        # bottom-up: down-sampling into slice 0 of the level's concat, ELAN
+        feats = [h]
+        for (c, c3), cout, cat_n in ((hd[3], o4, cat_n4), (hd[4], o5, cat_n5), (hd[5], o6, cat_n6)):
+            down(feats[-1], i, cout, out=pb.sub(cat_n, 0, cout))
+            i += 2
+            feats.append(elan_block(cat_n, i, c, c3, cout))
+            i += blk
+        feats = [cbs(f, f"model.{i + li}", 2 * f.C, 3) for li, f in enumerate(feats)]
+        det = i + 4
+        assert det == p6["det"], (scale, det)
+        det_levels = 4
+        if W.real and f"model.{det + 4}.m.0.weight" in W.state_dict and f"model.{det}.m.0.weight" not in W.state_dict:
+            det += 4                                         # training form: IAuxDetect after the four aux convs (not used here)
+    elif scale == "base":
         x = cbs(pb.image, "model.0", 32, 3, 1, cin=3)
         x = cbs(x, "model.1", 64, 3, 2)
         x = cbs(x, "model.2", 64, 3, 1)
@@ -718,18 +851,7 @@ def build_yolov7(weights: Weights, scale: str = "tiny", nc: int = 80, in_h: int 
         cat80 = pb.new_padded(H // 16, Wd // 16, 512)        # [79, 77, 63]
         cat55 = pb.new_padded(H // 16, Wd // 16, 512)        # [54, up(52)]
         cat67 = pb.new_padded(H // 8, Wd // 8, 256)          # [66, up(64)]
-        # 51 SPPCSPC(1024, 512), c_ = 512
-        c_ = 512
-        cat7 = pb.new_padded(x.H, x.W, 2 * c_)               # cv7 input [y1, y2]
-        sp = pb.new_padded(x.H, x.W, 4 * c_)                 # cv5 input [x1, p5, p9, p13]
-        t = cbs(x, "model.51.cv1", c_, 1)
-        t = cbs(t, "model.51.cv3", c_, 3)
-        x1 = cbs(t, "model.51.cv4", c_, 1, out=pb.sub(sp, 0, c_))
-        pools(x1, sp, [1, 2, 3])
-        t = cbs(sp, "model.51.cv5", c_, 1)
-        cbs(t, "model.51.cv6", c_, 3, out=pb.sub(cat7, 0, c_))
-        cbs(x, "model.51.cv2", c_, 1, out=pb.sub(cat7, c_, c_))
-        h51 = cbs(cat7, "model.51.cv7", 512, 1, out=pb.sub(cat93, 512, 512))
+        h51 = sppcspc(x, 51, 512, pb.sub(cat93, 512, 512))      # SPPCSPC(1024, 512)
         t = cbs(h51, "model.52", 256, 1)
         pb.upsample2x(t, pb.sub(cat55, 256, 256))
         cbs(p4, "model.54", 256, 1, out=pb.sub(cat55, 0, 256))
@@ -781,17 +903,17 @@ def build_yolov7(weights: Weights, scale: str = "tiny", nc: int = 80, in_h: int 
     # IDetect: m[i](ia[i](x)) * im[i], folded into the 1x1 head convolutions
     no = 3 * (nc + 5)
     A = 0
-    for li, (feat, stride) in enumerate(zip(feats, (8, 16, 32))):
+    for li, (feat, stride) in enumerate(zip(feats, (8, 16, 32, 64)[:det_levels])):
         w, b = W.implicit_head(f"model.{det}", li, no, feat.C)
         head = pb.new_padded(feat.H, feat.W, (no + 7) // 8 * 8, f32=True)
         pb.conv(feat, w, b, 1, 1, ACT_NONE, out=head, out_f32=True)
         pb.outputs.append((head.buf, 0, head.C, stride))
         A += 3 * feat.H * feat.W
     if anchors is None:
-        anchors = W.anchor_grid(f"model.{det}")
+        anchors = W.anchor_grid(f"model.{det}", det_levels)
     if anchors is None:
-        anchors = YOLOV7_ANCHORS if scale == "base" else YOLOV5_ANCHORS
-    anc = np.asarray(anchors, np.float32).reshape(18)
+        anchors = YOLOV7_P6_ANCHORS if p6 else YOLOV7_ANCHORS if scale == "base" else YOLOV5_ANCHORS
+    anc = np.asarray(anchors, np.float32).reshape(6 * det_levels)
     assert np.all(np.isfinite(anc)) and np.all(anc > 0), f"anchors must be finite and positive: {anc}"
     pb.meta[0], pb.meta[1] = nc, A
     pb.meta[3] = pb.tensor(anc) + 1                          # 1 + tensor index; 0 = the YOLOv5 table (plans without the field)
@@ -799,17 +921,18 @@ def build_yolov7(weights: Weights, scale: str = "tiny", nc: int = 80, in_h: int 
 
 
 def read_anchors(path: str) -> np.ndarray:
-    """Anchor table [3 levels, 3 anchors, 2] a YOLOv5-layout plan decodes with: its own (header meta[3]) or the YOLOv5 table."""
+    """Anchor table [L levels, 3 anchors, 2] a YOLOv5-layout plan decodes with: its own (header meta[3], L = its output count) or the
+    YOLOv5 table (L = 3)."""
     with open(path, "rb") as f:
         raw = f.read()
     h = struct.unpack_from("<8sII3I4I16IQQ", raw)
-    n_buf, n_ops, n_t, meta, blob = h[6], h[7], h[8], h[10:26], h[26]
+    n_buf, n_ops, n_t, n_out, meta, blob = h[6], h[7], h[8], h[9], h[10:26], h[26]
     if meta[3] == 0:
         return np.asarray(YOLOV5_ANCHORS, np.float32).reshape(3, 3, 2)
     rec = struct.calcsize("<8sII3I4I16IQQ") + n_buf * 24 + n_ops * 112 + (meta[3] - 1) * 24
     off, nbytes, _, _ = struct.unpack_from("<QQII", raw, rec)
-    assert meta[3] <= n_t and nbytes >= 72
-    return np.frombuffer(raw, np.float32, 18, blob + off).reshape(3, 3, 2).copy()
+    assert meta[3] <= n_t and nbytes == 24 * n_out
+    return np.frombuffer(raw, np.float32, 6 * n_out, blob + off).reshape(n_out, 3, 2).copy()
 
 
 # ---------------------------------------------------------------------------------------------

@@ -1,5 +1,5 @@
 """Per-layer table of a plan at real clocks: every launch replayed alone (CUDA events, L2-warm), GEMM shapes and tile choices.
-usage: python tools/op_table.py yolov8|ufldv2|yolov5|yolov7|yolov7-tiny|yolov7-w6|yolov7-e6|yolov7-d6|yolov7-e6e|yolov6n|yolov6s|yolov6m|yolov6l [batch] [iters]
+usage: python tools/op_table.py yolov8|ufldv2|yolov5|yolov7|yolov7-tiny|yolov7-w6|yolov7-e6|yolov7-d6|yolov7-e6e|yolov6n|yolov6s|yolov6m|yolov6l|yolov9-t|yolov9-s|yolov9-m|yolov9-c [batch] [iters]
 (the YOLOv7 P6 models run at 1280x1280)   (env switches of the library apply)"""
 import os, re, sys, tempfile
 R = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, R); sys.path.insert(0, os.path.join(R, "tests"))
@@ -15,13 +15,17 @@ elif kind.startswith("yolov6"):
     pb = plan.build_yolov6(plan.synth_weights("yolov6", 0, variant=kind[-1]), kind[-1])
     path = os.path.join(tempfile.mkdtemp(), kind + ".b200w")
     pb.write(path)
+elif kind.startswith("yolov9"):
+    pb = plan.build_yolov9(plan.synth_weights("yolov9", 0, variant=kind[-1]), kind[-1])
+    path = os.path.join(tempfile.mkdtemp(), kind + ".b200w")
+    pb.write(path)
 else:
     kw = {"yolov8": dict(scale="l"), "ufldv2": dict(backbone="34"), "yolov5": dict(scale="n")}[kind]
     path, sd, pb = cached_plan(kind, **kw)
 eng = _capi.Engine(path, 0, max_batch=B)
 eng.run(B)
 n = eng.num_steps(B)
-names = {1: "gemm", 2: "im2col", 3: "maxpool", 4: "upsample", 5: "layernorm", 6: "stempack", 7: "stemconv", 31: "(folded)"}
+names = {1: "gemm", 2: "im2col", 3: "maxpool", 4: "upsample", 5: "layernorm", 6: "stempack", 7: "stemconv", 8: "avgpool2", 31: "(folded)"}
 tot = 0.0; tot_g = 0.0; rows = []
 for i in range(n):
     ms, t, d = eng.time_step(B, i, iters)
@@ -39,5 +43,9 @@ flops = (pb.flops_per_img - pb.stem_flops_per_img) * B      # the stem conv is n
 print(f"TOTAL {kind} b{B}: sum of isolated launches {tot * 1e3:.1f} us (gemm {tot_g * 1e3:.1f} us) -> {flops / tot_g / 1e9:.1f} TFLOP/s algorithmic over GEMM time")
 ms_all, nl = eng.time_ops(B, 0xFFFFFFFF, 10)
 ms_g, ng = eng.time_ops(B, 1 << 1, 10)
-print(f"back-to-back: all {ms_all * 1e3:.1f} us ({nl} launches), gemm only {ms_g * 1e3:.1f} us ({ng}) -> {flops / ms_g / 1e9:.1f} TFLOP/s")
+print(f"back-to-back: all {ms_all * 1e3:.1f} us ({nl} launches), gemm only {ms_g * 1e3:.1f} us ({ng}) -> {flops / ms_g / 1e9:.1f} TFLOP/s, "
+      f"plan only {B / ms_all * 1e3:.0f} images/s")
+ms_ap = sum(r[0] for r in rows if r[2] == "avgpool2")
+ms_ic = sum(r[0] for r in rows if r[2] == "im2col" and pb.ops[r[1]][1][2] < 64)        # one launch per plan op; im2col p[2] = Cin
+print(f"share of the sum of isolated launches: avgpool2 {100 * ms_ap / tot:.1f} %, im2col of convs with < 64 input channels {100 * ms_ic / tot:.1f} %")
 eng.close()

@@ -105,6 +105,7 @@ int launch_im2col(const __half* in, int in_ld, int in_coff, int B, int H, int W,
                   int stride, int pad, int Ho, int Wo, __half* out, int Kpad, cudaStream_t st);
 int launch_maxpool(const __half* in, int in_ld, int B, int H, int W, int C, int k, int s, int p,
                    __half* out, int out_ld, int Ho, int Wo, cudaStream_t st);
+int launch_avgpool2(const __half* in, int in_ld, int B, int H, int W, int C, __half* out, int out_ld, int fill, cudaStream_t st);
 int launch_upsample2x(const __half* in, int in_ld, int B, int H, int W, int C, __half* out, int out_ld,
                       cudaStream_t st);
 int launch_layernorm(const __half* in, int in_ld, int rows, int d_len, int d_norm, const float* gamma,

@@ -148,6 +148,56 @@ int launch_maxpool(const __half* in, int in_ld, int B, int H, int W, int C, int 
     return 0;
 }
 
+// ---- 2x2 stride-1 average pool, written on the INPUT's H x W grid (YOLOv9 ADown / AConv) ----------------
+// out(y, x) = mean of in(y..y+1, x..x+1) for y < H-1, x < W-1 (fp32 sum, one rounding); row H-1 and column W-1 hold `fill`
+// (0 or -inf).  Upstream pools to an (H-1) x (W-1) map: with zeros there, a 3x3 stride-2 pad-1 conv of the H x W buffer equals
+// the same conv of that map, and with -inf a 3x3 stride-2 pad-1 max pool ignores them (H, W even).
+__global__ void avgpool2_kernel(const __half* __restrict__ in, int in_ld, int B, int H, int W, int C, __half* __restrict__ out, int out_ld,
+                                unsigned short fill_bits) {
+    const int c8 = C >> 3;
+    const long long total = (long long)B * H * W * c8;
+    const int Hp = H + 2, Wp = W + 2;
+    const __half2 f2 = __halves2half2(__ushort_as_half(fill_bits), __ushort_as_half(fill_bits));
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int cg = (int)(i % c8);
+        long long t = i / c8;
+        const int x = (int)(t % W); t /= W;
+        const int y = (int)(t % H);
+        const int b = (int)(t / H);
+        const size_t r = ((size_t)b * Hp + (y + 1)) * Wp + (x + 1);
+        uint4 o;
+        __half2* oh = reinterpret_cast<__half2*>(&o);
+        if (y == H - 1 || x == W - 1) {
+            oh[0] = f2; oh[1] = f2; oh[2] = f2; oh[3] = f2;
+        } else {
+            const __half* p = in + r * in_ld + cg * 8;
+            const uint4 a = *reinterpret_cast<const uint4*>(p);
+            const uint4 bb = *reinterpret_cast<const uint4*>(p + in_ld);
+            const uint4 c = *reinterpret_cast<const uint4*>(p + (size_t)Wp * in_ld);
+            const uint4 d = *reinterpret_cast<const uint4*>(p + (size_t)(Wp + 1) * in_ld);
+            const __half2 *ha = reinterpret_cast<const __half2*>(&a), *hb = reinterpret_cast<const __half2*>(&bb);
+            const __half2 *hc = reinterpret_cast<const __half2*>(&c), *hd = reinterpret_cast<const __half2*>(&d);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const float2 fa = __half22float2(ha[j]), fb = __half22float2(hb[j]), fc = __half22float2(hc[j]), fd = __half22float2(hd[j]);
+                oh[j] = __floats2half2_rn(((fa.x + fb.x) + (fc.x + fd.x)) * 0.25f, ((fa.y + fb.y) + (fc.y + fd.y)) * 0.25f);
+            }
+        }
+        *reinterpret_cast<uint4*>(out + r * out_ld + cg * 8) = o;
+    }
+}
+
+int launch_avgpool2(const __half* in, int in_ld, int B, int H, int W, int C, __half* out, int out_ld, int fill, cudaStream_t st) {
+    ADAS_CHECK(C % 8 == 0 && in_ld % 8 == 0 && out_ld % 8 == 0 && (fill == 0 || fill == 1), "avgpool2: channel alignment / fill");
+    const long long total = (long long)B * H * W * (C / 8);
+    int blocks = grid_for(total, 256);
+    if (blocks > 132 * 32) blocks = 132 * 32;
+    avgpool2_kernel<<<blocks, 256, 0, st>>>(in, in_ld, B, H, W, C, out, out_ld, fill ? (unsigned short)0xFC00 : (unsigned short)0);
+    count_launch();
+    ADAS_CUDA(cudaGetLastError());
+    return 0;
+}
+
 // ---- nearest upsample x2 into a channel slice of the consumer's concat buffer ---------------------
 __global__ void upsample2x_kernel(const __half* __restrict__ in, int in_ld, int B, int H, int W, int C,
                                   __half* __restrict__ out, int out_ld) {

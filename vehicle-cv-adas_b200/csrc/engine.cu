@@ -308,6 +308,15 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
                 prog->steps.push_back([=](cudaStream_t st) { return launch_maxpool(in, in_ld, batch, H, W, C, k, s, pad, out, out_ld, Ho, Wo, st); });
                 break;
             }
+            case OP_AVGPOOL2: {
+                const PlanBuffer& ib = e->bufs[p[0]];
+                const PlanBuffer& ob = e->bufs[p[3]];
+                const __half* in = static_cast<const __half*>(e->dbufs[p[0]].ptr) + p[1];
+                __half* out = static_cast<__half*>(e->dbufs[p[3]].ptr) + p[4];
+                const int in_ld = (int)ib.C, H = (int)ib.H, W = (int)ib.W, C = p[2], out_ld = (int)ob.C, fill = p[5];
+                prog->steps.push_back([=](cudaStream_t st) { return launch_avgpool2(in, in_ld, batch, H, W, C, out, out_ld, fill, st); });
+                break;
+            }
             case OP_UPSAMPLE2X: {
                 const PlanBuffer& ib = e->bufs[p[0]];
                 const PlanBuffer& ob = e->bufs[p[3]];
@@ -596,6 +605,19 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
                 ADAS_CHECK(view_ok(p[0], p[1], p[2]) && view_ok(p[6], p[7], p[2]) && e->bufs[p[0]].H > 0 && e->bufs[p[6]].H > 0 && p[3] >= 1 && p[3] <= 7 && p[4] >= 1 && p[4] <= 4 && p[5] >= 0 && p[5] <= 3,
                            "plan %s: op %zu: bad maxpool", path, oi);
                 break;
+            case OP_AVGPOOL2: {
+                ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[3]), "plan %s: op %zu: avgpool2 buffer index out of range", path, oi);
+                const PlanBuffer &ib = e->bufs[p[0]], &ob = e->bufs[p[3]];
+                ADAS_CHECK(ib.dtype == 0 && ob.dtype == 0, "plan %s: op %zu: avgpool2 buffers must be fp16", path, oi);
+                ADAS_CHECK(ib.H > 0 && ob.H == ib.H && ob.W == ib.W, "plan %s: op %zu: avgpool2 output must have its input's H x W (%ux%u -> %ux%u)", path, oi,
+                           ib.H, ib.W, ob.H, ob.W);
+                ADAS_CHECK(p[2] >= 8 && p[2] % 8 == 0 && p[1] % 8 == 0 && p[4] % 8 == 0 && ib.C % 8 == 0 && ob.C % 8 == 0,
+                           "plan %s: op %zu: avgpool2 channels and offsets must be multiples of 8", path, oi);
+                ADAS_CHECK(view_ok(p[0], p[1], p[2]) && view_ok(p[3], p[4], p[2]) && (p[0] != p[3] || p[4] >= p[1] + p[2] || p[1] >= p[4] + p[2]),
+                           "plan %s: op %zu: avgpool2 channel slice exceeds its buffer or overlaps its input", path, oi);
+                ADAS_CHECK(p[5] == 0 || p[5] == 1, "plan %s: op %zu: avgpool2 fill %d (0: zero, 1: -inf)", path, oi, p[5]);
+                break;
+            }
             case OP_UPSAMPLE2X:
                 ADAS_CHECK(view_ok(p[0], p[1], p[2]) && view_ok(p[3], p[4], p[2]) && e->bufs[p[0]].H > 0 && e->bufs[p[3]].H == 2 * e->bufs[p[0]].H && e->bufs[p[3]].W == 2 * e->bufs[p[0]].W,
                            "plan %s: op %zu: bad upsample", path, oi);

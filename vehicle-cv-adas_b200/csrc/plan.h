@@ -61,6 +61,8 @@ enum PlanOpType : uint32_t {
                        //    (weights packed [Cout][k][round_up(4k,16)])
     OP_LAYERNORM = 5,  // p: in_buf d_len gamma_tensor beta_tensor out_buf d_norm ; f0 = eps (statistics over d_norm entries; the
                        //    other d_len - d_norm slab entries are structural zeros with gamma = beta = 0)
+    OP_AVGPOOL2 = 8,   // p: in_buf in_coff C out_buf out_coff fill : 2x2 stride-1 mean into a buffer of the input's H x W geometry;
+                       //    row H-1 and column W-1 hold 0 (fill 0) or -inf (fill 1), see elementwise.cu avgpool2_kernel
 };
 
 }  // namespace adas

@@ -4,7 +4,7 @@ The reference hands `.onnx` / `.trt` files to ONNXRuntime / TensorRT (coreEngine
 ultralytics / yolov5 exports (README.md:53-58) and from `TrafficLaneDetector/convertPytorchToONNX.py:60-87` (UFLD).  This module
 is the H100 replacement of that ingestion step (SURVEY 8f rank 2): it reads the ONNX protobuf directly (the `onnx` package is
 not a dependency -- the wire format is parsed here), recovers the convolution / linear / LayerNorm parameters, recognises the
-architecture (YOLOv8 / YOLOv5 / YOLOv7 / UFLDv2, scale, class count, input size) and drives the same `plan.build_*` builders that the
+architecture (YOLOv8 / YOLOv5 / YOLOv6 / YOLOv7 / YOLOv9 / UFLDv2, scale, class count, input size) and drives the same `plan.build_*` builders that the
 state_dict path uses.  Nothing here runs the network: the graph is only a parameter container plus a shape oracle.
 
 How parameters are matched to layers:
@@ -318,6 +318,17 @@ class OnnxWeights(plan.Weights):
     def conv_bias(self, prefix: str, cout: int, cin: int, k: int):
         return self.conv_bn(prefix, cout, cin, k, 0.0, conv_key="", bn_key="__no_bn__")
 
+    def repconvn(self, prefix: str, cout: int, cin: int, eps: float):
+        """Fused (`conv.weight`) or named un-fused RepConvN as in plan.Weights; exporter-folded, its 3x3 and 1x1 branches are two
+        anonymous convolutions in graph order, summed here in fp64."""
+        if f"{prefix}.conv.weight" in self.state_dict or f"{prefix}.conv1.bn.running_var" in self.state_dict:
+            return super().repconvn(prefix, cout, cin, eps)
+        w3, b3 = self.conv_bn(f"{prefix}.conv1", cout, cin, 3, eps)
+        w1, b1 = self.conv_bn(f"{prefix}.conv2", cout, cin, 1, eps)
+        w = w3.astype(np.float64)
+        w[:, :, 1, 1] += w1[:, :, 0, 0]
+        return w.astype(np.float32), (b3.astype(np.float64) + b1).astype(np.float32)
+
 
 def _is_module_name(name: str) -> bool:
     """True for exporter-kept parameter names (`model.0.conv.weight`, `pool.weight`), False for `onnx::Conv_123` and friends."""
@@ -329,7 +340,7 @@ def _is_module_name(name: str) -> bool:
 # ---------------------------------------------------------------------------------------------------------------
 @dataclass
 class ModelSpec:
-    kind: str                 # "yolov8" | "yolov5" | "yolov7" | "yolov6" | "ufldv2"
+    kind: str                 # "yolov8" | "yolov5" | "yolov7" | "yolov6" | "yolov9" | "ufldv2"
     scale: str                # YOLO scale letter ("tiny" / "base" for YOLOv7) or ResNet depth ("18" / "34")
     nc: int = 80
     in_h: int = 640
@@ -358,6 +369,8 @@ def recognise(model: OnnxModel) -> ModelSpec:
         if depth is None:
             raise Exception(f"UFLD backbone with {n3} 3x3 convolutions is not supported (ResNet-18/34 only)")
         return ModelSpec("ufldv2", depth, 0, in_h or 320, in_w or 1600)
+    if _is_yolov9(model):                                            # ADown / AConv's 2x2 stride-1 average pool; no other family pools so
+        return _recognise_yolov9(model, w, in_h, in_w)
     if any(n.op_type == "ConvTranspose" for n in model.nodes):       # YOLOv6's BiFusion; v5 / v7 / v8 upsample with Resize
         return _recognise_yolov6(model, w, in_h, in_w)
     if _is_yolov7(model, w):
@@ -573,6 +586,58 @@ def _recognise_yolov6(model: OnnxModel, w: OnnxWeights, in_h: int, in_w: int) ->
                      acts=(roles.get("body", "relu"), roles.get("neck", "relu"), roles.get("head", "silu")))
 
 
+_V9_SUPPORTED = ("YOLOv9-T / S / M / C (WongKinYiu/yolov9 v0.1, the converted GELAN graphs with a DDetect head, exported with one output; "
+                 "YOLOv9-E / GELAN-E, files with the auxiliary branch, ultralytics' YOLOv9 and YOLOv10 are not supported)")
+_V9_STEM = {16: ("t",), 32: ("s", "m"), 64: ("c",)}
+_V9_DOWN3 = {128: "s", 240: "m"}            # layer 3 (AConv) width tells S from M
+
+
+def _is_yolov9(model: OnnxModel) -> bool:
+    return any(n.op_type == "AveragePool" and list(n.attrs.get("kernel_shape", [])) == [2, 2] and list(n.attrs.get("strides", [1, 1])) == [1, 1]
+               for n in model.nodes)
+
+
+def _recognise_yolov9(model: OnnxModel, w: OnnxWeights, in_h: int, in_w: int) -> ModelSpec:
+    """YOLOv9-T / S / M / C: the stem width gives the scale (32: S or M by layer 3's width), the head must have DDetect's grouped box
+    convolutions, and the convolution count must be the scale's (fused, or with RepConvN's two branches apart)."""
+    if len(model.outputs) != 1:
+        raise Exception(f"YOLOv9 file with {len(model.outputs)} outputs (an auxiliary-branch training file?); supported: {_V9_SUPPORTED}")
+    first = w.convs[0][1]
+    cands = _V9_STEM.get(int(first.shape[0]), ()) if tuple(first.shape[1:]) == (3, 3, 3) else ()
+    if not cands:
+        raise Exception(f"YOLOv9 stem {tuple(first.shape)}: 16 (T), 32 (S / M) or 64 (C) channels; supported: {_V9_SUPPORTED}")
+    grouped = [n for n in model.nodes if n.op_type == "Conv" and int(n.attrs.get("group", 1)) == 4]
+    if len(grouped) != 6:
+        raise Exception(f"YOLOv9 file with {len(grouped)} group-4 convolutions: a head without DDetect's grouped box convolutions "
+                        f"(6); supported: {_V9_SUPPORTED}")
+    if (in_h and in_h % 32) or (in_w and in_w % 32):
+        raise Exception(f"YOLOv9 file with a {in_h}x{in_w} input: a multiple of 32; supported: {_V9_SUPPORTED}")
+    scale = cands[0]
+    if len(cands) > 1:
+        named = model.initializers.get("model.3.cv1.conv.weight")
+        if named is not None:
+            width = int(named.shape[0])
+        else:                                                    # the conv reading the first 2x2 average pool (AConv's cv1)
+            pool = next(n for n in model.nodes if n.op_type == "AveragePool")
+            conv = next((n for n in model.nodes if n.op_type == "Conv" and n.inputs[0] == pool.outputs[0]), None)
+            width = int(model.initializers[conv.inputs[1]].shape[0]) if conv is not None and conv.inputs[1] in model.initializers else 0
+        if width not in _V9_DOWN3:
+            raise Exception(f"YOLOv9 file with a 32-channel stem and a {width}-channel layer 3 (128: S, 240: M); supported: {_V9_SUPPORTED}")
+        scale = _V9_DOWN3[width]
+    n = sum(1 for _, cw, _ in w.convs if tuple(cw.shape) != (1, 16, 1, 1))       # upstream's fixed DFL conv is not counted
+    fused = plan.yolov9_conv_count(scale)
+    if n not in (fused, fused + plan.yolov9_repconvn_count(scale)):
+        raise Exception(f"YOLOv9 file with {n} convolutions, YOLOv9-{scale.upper()} has {fused} ({fused + plan.yolov9_repconvn_count(scale)} with "
+                        f"RepConvN's branches apart); supported: {_V9_SUPPORTED}")
+    nc = None
+    for name, cw, _ in w.convs:
+        if re.fullmatch(r"model\.22\.cv3\.\d+\.2\.weight", name):      # DDetect.cv3[i][2]: Conv2d(c3, nc, 1)
+            nc = int(cw.shape[0])
+    if nc is None:                                               # names lost: the last 1x1 conv before the (optional) DFL conv
+        nc = int([cw.shape[0] for _, cw, _ in w.convs if cw.shape[2:] == (1, 1) and cw.shape[0] != 1][-1])
+    return ModelSpec("yolov9", scale, nc, in_h or 640, in_w or 640)
+
+
 def build_plan(model: OnnxModel, spec: Optional[ModelSpec] = None) -> "plan.PlanBuilder":
     spec = spec or recognise(model)
     w = OnnxWeights(model)
@@ -582,6 +647,8 @@ def build_plan(model: OnnxModel, spec: Optional[ModelSpec] = None) -> "plan.Plan
         return plan.build_yolov5(w, spec.scale, nc=spec.nc, in_h=spec.in_h, in_w=spec.in_w)
     if spec.kind == "yolov7":
         return plan.build_yolov7(w, spec.scale, nc=spec.nc, in_h=spec.in_h, in_w=spec.in_w, act=spec.act, anchors=spec.anchors)
+    if spec.kind == "yolov9":
+        return plan.build_yolov9(w, spec.scale, nc=spec.nc, in_h=spec.in_h, in_w=spec.in_w)
     if spec.kind == "yolov6":
         body, neck, head = spec.acts or (None, "relu", "silu")
         return plan.build_yolov6(w, spec.scale, nc=spec.nc, in_h=spec.in_h, in_w=spec.in_w, act_body=body, act_neck=neck, act_head=head,

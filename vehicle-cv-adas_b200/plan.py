@@ -33,6 +33,7 @@ import numpy as np
 MODEL_YOLOV8, MODEL_YOLOV5, MODEL_UFLDV2, MODEL_UFLDV1 = 0, 1, 2, 4      # 3 = ADAS_MODEL_YOLOV5_LITE (post-processing kind only)
 MODEL_YOLOV6 = 5                                                         # anchor-free head, [B, 8400, 5 + nc] output; meta[2] = reg_max
 OP_GEMM, OP_IM2COL, OP_MAXPOOL, OP_UPSAMPLE2X, OP_LAYERNORM, OP_STEMPACK, OP_STEMCONV = 1, 2, 3, 4, 5, 6, 7
+OP_AVGPOOL2 = 8
 ACT_NONE, ACT_SILU, ACT_RELU, ACT_LEAKY = 0, 1, 2, 3          # ACT_LEAKY: LeakyReLU(0.1)
 PLAN_VERSION = 1
 
@@ -173,6 +174,16 @@ class Weights:
             bd += be - m * s
         return wd.astype(np.float32), bd.astype(np.float32)
 
+    def repconvn(self, prefix: str, cout: int, cin: int, eps: float):
+        """YOLOv9 RepConvN (3x3 `conv1` + 1x1 `conv2`, each Conv2d + BatchNorm, no identity branch) as one folded 3x3 conv, summed in
+        fp64 with the 1x1 on the centre tap.  A file fused upstream carries `conv.weight` + `conv.bias` instead."""
+        if f"{prefix}.conv.weight" in self.state_dict:
+            return self.conv_bias(f"{prefix}.conv", cout, cin, 3)
+        w3, b3 = self._conv_bn64(f"{prefix}.conv1", cout, cin, 3, eps)
+        w1, b1 = self._conv_bn64(f"{prefix}.conv2", cout, cin, 1, eps)
+        w3[:, :, 1, 1] += w1[:, :, 0, 0]
+        return w3.astype(np.float32), (b3 + b1).astype(np.float32)
+
     def implicit_head(self, prefix: str, li: int, no: int, cin: int):
         """YOLOv7 IDetect level li: im * (m(x + ia)) folded into the 1x1 conv, w' = im * w, b' = im * (b + w @ ia) in fp64.  Files
         fused upstream (IDetect.fuse) carry the folded m.li conv and no implicit tensors."""
@@ -213,6 +224,13 @@ SYNTH_PROFILES = {
     # lane existence: random heads give P(valid) = 0.5 per anchor, i.e. no lane passes the "more than half / a quarter of the anchors
     # valid" test and nothing downstream of the decode is exercised; +1.0 on the "valid" logits makes ~88 % of the anchors valid
     "ufldv2": {"ufld_exist_bias": 1.0},
+    # YOLOv9 T/S/M/C: YOLOv8's head gains (CPU fp16 emulation: probability error 2-4e-4, box error 0.1 px on 8 frames); the class bias
+    # of each scale puts ~100 of the 8400 anchors per frame above box_score = 0.4 (fp32 oracle, synthetic frames 0-3: at bias -3.5 the
+    # 100th-highest max-class logit sits 0.53 (T), -0.31 (S), 0.04 (M), 0.05 (C) from logit(0.4); per-anchor spread 0.16-0.47).
+    "yolov9": {"gains": [(r"model\.22\.cv3\.\d\.2\.weight", 16.0), (r"model\.22\.cv2\.\d\.2\.weight", 25.0)],
+               "fill": [(r"model\.22\.cv3\.\d\.2\.bias", -3.5)],
+               "variants": {sc: {"fill": [(r"model\.22\.cv3\.\d\.2\.bias", -3.5 - d)]}
+                            for sc, d in (("t", 0.53), ("s", -0.31), ("m", 0.04), ("c", 0.05))}},
     # YOLOv7 base (model.105, SiLU) and tiny (model.77, LeakyReLU).  The tiny net's activations are not damped layer by layer as with
     # SiLU: its fp16 noise at the head is ~50x larger, so its head gain is 0.3, its objectness / class biases (-0.2) set the operating
     # point and its box biases sit at -3, where the xywh sigmoids are flat (box noise 0.4 px -> 0.01 px).  CPU fp16 emulation on
@@ -250,7 +268,7 @@ SYNTH_PROFILES_WORKLOAD = {
 
 
 def synth_weights(kind: str, seed: int = 0, variant: Optional[str] = None, workload: bool = False) -> "Weights":
-    """Seeded synthetic weights.  A profile's `variants` entry (YOLOv6) adds per-variant `fill` rules ahead of the shared ones; other
+    """Seeded synthetic weights.  A profile's `variants` entry (YOLOv6, YOLOv9) adds per-variant `fill` rules ahead of the shared ones; other
     kinds ignore `variant`."""
     prof = SYNTH_PROFILES_WORKLOAD.get(kind, SYNTH_PROFILES[kind]) if workload else SYNTH_PROFILES[kind]
     extra = prof.get("variants", {}).get(variant)
@@ -434,6 +452,16 @@ class PlanBuilder:
         self._op(OP_MAXPOOL, [x.buf, x.coff, x.C, k, s, p, out.buf, out.coff])
         return View(out.buf, out.coff, x.C, Ho, Wo)
 
+    def avgpool2(self, x: View, fill: int, out: Optional[View] = None) -> View:
+        """2x2 stride-1 average pool (upstream `avg_pool2d(x, 2, 1, 0)`, an (H-1) x (W-1) map) stored on x's H x W grid: row H-1 and
+        column W-1 hold 0 (fill 0: a following 3x3 stride-2 pad-1 conv sees upstream's zero padding there) or -inf (fill 1: a following
+        3x3 stride-2 pad-1 max pool ignores them)."""
+        if out is None:
+            out = self.new_padded(x.H, x.W, x.C)
+        assert out.H == x.H and out.W == x.W and x.C % 8 == 0 and x.coff % 8 == 0 and out.coff % 8 == 0 and fill in (0, 1)
+        self._op(OP_AVGPOOL2, [x.buf, x.coff, x.C, out.buf, out.coff, fill])
+        return View(out.buf, out.coff, x.C, x.H, x.W)
+
     def upsample2x(self, x: View, out: View) -> View:
         assert out.H == 2 * x.H and out.W == 2 * x.W and x.C % 8 == 0
         self._op(OP_UPSAMPLE2X, [x.buf, x.coff, x.C, out.buf, out.coff])
@@ -554,30 +582,52 @@ def build_yolov8(weights: Weights, scale: str = "l", nc: int = 80, in_h: int = 6
     h18 = c2f(cat17, "model.18", c4, rep(3), False)
     cbs(h18, "model.19", c4, 3, 2, out=pb.sub(cat20, 0, c4))
     h21 = c2f(cat20, "model.21", c5, rep(3), False)
-    # Detect
-    reg_max = 16
-    cb = max(16, c3 // 4, reg_max * 4)
-    cc = max(c3, min(nc, 100))
-    A = 0
-    for li, (feat, stride) in enumerate(((h15, 8), (h18, 16), (h21, 32))):
-        cin = feat.C
-        # first convs of the box and cls branches share their input: one GEMM with N = cb + cc
-        wb, bb = W.conv_bn(f"model.22.cv2.{li}.0", cb, cin, 3, BN_EPS_YOLO)
-        wc, bc = W.conv_bn(f"model.22.cv3.{li}.0", cc, cin, 3, BN_EPS_YOLO)
-        t0 = pb.conv(feat, np.concatenate([wb, wc], 0), np.concatenate([bb, bc]), 3, 1, ACT_SILU)
-        w1, b1 = W.conv_bn(f"model.22.cv2.{li}.1", cb, cb, 3, BN_EPS_YOLO)
-        tb = pb.conv(pb.sub(t0, 0, cb), w1, b1, 3, 1, ACT_SILU)
-        w2, b2 = W.conv_bn(f"model.22.cv3.{li}.1", cc, cc, 3, BN_EPS_YOLO)
-        tc = pb.conv(pb.sub(t0, cb, cc), w2, b2, 3, 1, ACT_SILU)
-        head = pb.new_padded(feat.H, feat.W, 4 * reg_max + (nc + 7) // 8 * 8, f32=True)
-        wbx, bbx = W.conv_bias(f"model.22.cv2.{li}.2", 4 * reg_max, cb, 1)
-        wcl, bcl = W.conv_bias(f"model.22.cv3.{li}.2", nc, cc, 1)
-        pb.conv(tb, wbx, bbx, 1, 1, ACT_NONE, out=pb.sub(head, 0, 4 * reg_max), out_f32=True)
-        pb.conv(tc, wcl, bcl, 1, 1, ACT_NONE, out=pb.sub(head, 4 * reg_max, (nc + 7) // 8 * 8), out_f32=True)
-        pb.outputs.append((head.buf, 0, head.C, stride))
-        A += feat.H * feat.W
+    A = v8_detect(pb, W, "model.22", (h15, h18, h21), nc)
     pb.meta[0], pb.meta[1] = nc, A
     return pb
+
+
+def grouped_to_dense(w: np.ndarray, groups: int) -> np.ndarray:
+    """Grouped conv weight [Cout, Cin / groups, k, k] as the equivalent dense [Cout, Cin, k, k] block-diagonal weight (exact)."""
+    if groups == 1:
+        return w
+    cout, cg = int(w.shape[0]), int(w.shape[1])
+    og = cout // groups
+    d = np.zeros((cout, cg * groups) + tuple(w.shape[2:]), w.dtype)
+    for g in range(groups):
+        d[g * og:(g + 1) * og, g * cg:(g + 1) * cg] = w[g * og:(g + 1) * og]
+    return d
+
+
+def v8_detect(pb: PlanBuilder, W: Weights, name: str, feats, nc: int, box_groups: int = 1, conv_bn=None) -> int:
+    """YOLOv8 Detect (and YOLOv9 DDetect: `box_groups` = 4 on the second and third box convs) on the P3 / P4 / P5 views; returns the
+    anchor count.  Grouped convs are packed as dense block-diagonal weights; flops_per_img counts their grouped MACs.  `conv_bn(name,
+    cout, cin, k)` replaces W.conv_bn for the Conv + BN layers (YOLOv9: upstream-fused files)."""
+    conv_bn = conv_bn or (lambda n, co, ci, k: W.conv_bn(n, co, ci, k, BN_EPS_YOLO))
+    reg_max = 16
+    cb = max(16, feats[0].C // 4, reg_max * 4)
+    cc = max(feats[0].C, min(nc, 100))
+    A = 0
+    for li, (feat, stride) in enumerate(zip(feats, (8, 16, 32))):
+        cin = feat.C
+        # first convs of the box and cls branches share their input: one GEMM with N = cb + cc
+        wb, bb = conv_bn(f"{name}.cv2.{li}.0", cb, cin, 3)
+        wc, bc = conv_bn(f"{name}.cv3.{li}.0", cc, cin, 3)
+        t0 = pb.conv(feat, np.concatenate([wb, wc], 0), np.concatenate([bb, bc]), 3, 1, ACT_SILU)
+        w1, b1 = conv_bn(f"{name}.cv2.{li}.1", cb, cb // box_groups, 3)
+        tb = pb.conv(pb.sub(t0, 0, cb), grouped_to_dense(w1, box_groups), b1, 3, 1, ACT_SILU)
+        w2, b2 = conv_bn(f"{name}.cv3.{li}.1", cc, cc, 3)
+        tc = pb.conv(pb.sub(t0, cb, cc), w2, b2, 3, 1, ACT_SILU)
+        head = pb.new_padded(feat.H, feat.W, 4 * reg_max + (nc + 7) // 8 * 8, f32=True)
+        wbx, bbx = W.conv_bias(f"{name}.cv2.{li}.2", 4 * reg_max, cb // box_groups, 1)
+        wcl, bcl = W.conv_bias(f"{name}.cv3.{li}.2", nc, cc, 1)
+        pb.conv(tb, grouped_to_dense(wbx, box_groups), bbx, 1, 1, ACT_NONE, out=pb.sub(head, 0, 4 * reg_max), out_f32=True)
+        pb.conv(tc, wcl, bcl, 1, 1, ACT_NONE, out=pb.sub(head, 4 * reg_max, (nc + 7) // 8 * 8), out_f32=True)
+        # the dense packing of the two grouped convs does (groups - 1) / groups of their counted MACs as zeros
+        pb.flops_per_img -= 2 * feat.H * feat.W * (cb * cb * 9 + 4 * reg_max * cb) * (box_groups - 1) // box_groups
+        pb.outputs.append((head.buf, 0, head.C, stride))
+        A += feat.H * feat.W
+    return A
 
 
 # ---------------------------------------------------------------------------------------------
@@ -1106,6 +1156,201 @@ def build_yolov6(weights: Weights, scale: str = "n", nc: int = 80, in_h: int = 6
         pb.outputs.append((head.buf, 0, head.C, stride))
         A += feat.H * feat.W
     pb.meta[0], pb.meta[1], pb.meta[2] = nc, A, reg_max
+    return pb
+
+
+# ---------------------------------------------------------------------------------------------
+# YOLOv9 (WongKinYiu/yolov9 release v0.1: the converted / GELAN yolov9-t, -s, -m, -c; P5 models only)
+# ---------------------------------------------------------------------------------------------
+# Per scale: stem convs (model.0, model.1); model.2 (ELAN1 (c2, c3, c4) for T / S, RepNCSPELAN4 (c2, c3, c4, n) for M / C); the down
+# block (AConv or ADown) and output widths of layers 3, 5, 7, 16, 19; RepNCSPELAN4 (c2, c3, c4, n) of layers 4, 6, 8, 12, 15, 18, 21;
+# SPPELAN (c2, c3) of layer 9.  The head is DDetect (model.22).  Not checked against any upstream file (none is available here): the
+# restatement reproduces the published parameter / FLOP counts (tests/test_yolov9_cpu.py).
+YOLOV9 = {
+    "t": dict(stem=(16, 32), l2=(32, 32, 16, None), down="aconv", downs=(64, 96, 128, 48, 64), spp=(128, 64),
+              r4=((64, 64, 32, 3), (96, 96, 48, 3), (128, 128, 64, 3), (96, 96, 48, 3), (64, 64, 32, 3), (96, 96, 48, 3), (128, 128, 64, 3))),
+    "s": dict(stem=(32, 64), l2=(64, 64, 32, None), down="aconv", downs=(128, 192, 256, 96, 128), spp=(256, 128),
+              r4=((128, 128, 64, 3), (192, 192, 96, 3), (256, 256, 128, 3), (192, 192, 96, 3), (128, 128, 64, 3), (192, 192, 96, 3),
+                  (256, 256, 128, 3))),
+    "m": dict(stem=(32, 64), l2=(128, 128, 64, 1), down="aconv", downs=(240, 360, 480, 184, 240), spp=(480, 240),
+              r4=((240, 240, 120, 1), (360, 360, 180, 1), (480, 480, 240, 1), (360, 360, 180, 1), (240, 240, 120, 1), (360, 360, 180, 1),
+                  (480, 480, 240, 1))),
+    "c": dict(stem=(64, 128), l2=(256, 128, 64, 1), down="adown", downs=(256, 512, 512, 256, 512), spp=(512, 256),
+              r4=((512, 256, 128, 1), (512, 512, 256, 1), (512, 512, 256, 1), (512, 512, 256, 1), (256, 256, 128, 1), (512, 512, 256, 1),
+                  (512, 512, 256, 1))),
+}
+
+
+def yolov9_conv_count(scale: str) -> int:
+    """Convolutions of the fused graph (RepConvN as one conv; the fixed DFL conv not counted).  A training-form file has one more per
+    RepConvN (its 1x1 branch): yolov9_repconvn_count(scale)."""
+    cfg = YOLOV9[scale]
+    n_r4 = lambda n: 10 + 4 * n                        # cv1, 2 x (RepNCSP: cv1, cv2, cv3, n x (RepConvN, Conv) + Conv 3x3), cv4
+    l2 = 4 if cfg["l2"][3] is None else n_r4(cfg["l2"][3])
+    down = 1 if cfg["down"] == "aconv" else 2
+    return 2 + l2 + 5 * down + sum(n_r4(r[3]) for r in cfg["r4"]) + 2 + 3 * 6
+
+
+def yolov9_repconvn_count(scale: str) -> int:
+    cfg = YOLOV9[scale]
+    return 2 * ((cfg["l2"][3] or 0) + sum(r[3] for r in cfg["r4"]))
+
+
+class Yolov9Packer:
+    """The GELAN blocks of YOLOv9 on a PlanBuilder.  A feature is (stored view, real channel segments ((offset in the view, count), ...)):
+    every concat member and chunk starts at a multiple of 8 channels (the GEMM's alignment).  A producer stores round_up(cout, 8)
+    channels, zero past cout; consumers' weights are scattered around those zero columns, and the first 1x1 conv of a RepNCSPELAN4 writes
+    its two chunks as two aligned row blocks of one GEMM.  Only YOLOv9-M has widths (180, 90, 60) that need it.  flops_per_img counts
+    the real channels only."""
+
+    def __init__(self, pb: PlanBuilder, W: Weights, down: str):
+        self.pb, self.W, self.down_kind, self.eps = pb, W, down, BN_EPS_YOLO
+
+    @staticmethod
+    def r8(c: int) -> int:
+        return (c + 7) // 8 * 8
+
+    @staticmethod
+    def feat(v: View, c: Optional[int] = None):
+        return (v, ((0, v.C if c is None else c),))
+
+    @staticmethod
+    def real(x) -> int:
+        return sum(n for _, n in x[1])
+
+    def conv(self, x, w: np.ndarray, b: np.ndarray, k: int, s: int = 1, out: Optional[View] = None, res: Optional[View] = None,
+             real_cout: Optional[int] = None):
+        """w [cout, real input channels, k, k] on x's segments (SiLU); returns the output feature."""
+        v, segs = x
+        cout = int(w.shape[0])
+        cin_real = int(w.shape[1])
+        if segs != ((0, v.C),):
+            wx = np.zeros((cout, v.C, k, k), np.float32)
+            j = 0
+            for off, n in segs:
+                wx[:, off:off + n] = w[:, j:j + n]
+                j += n
+            assert j == cin_real, (segs, w.shape)
+            w = wx
+        f0 = self.pb.flops_per_img
+        y = self.pb.conv(v, w, b, k, s, ACT_SILU, out=out, res=res)
+        self.pb.flops_per_img = f0 + 2 * y.H * y.W * (real_cout or cout) * cin_real * k * k
+        return self.feat(View(y.buf, y.coff, self.r8(cout), y.H, y.W), cout)
+
+    def conv_bn(self, name: str, cout: int, cin: int, k: int, res_branch: bool = False):
+        """Conv + BatchNorm, or its upstream-fused form (`conv.weight` + `conv.bias`, no `bn`)."""
+        W = self.W
+        if W.real and f"{name}.conv.bias" in W.state_dict and f"{name}.bn.weight" not in W.state_dict:
+            return W.conv_bias(f"{name}.conv", cout, cin, k)
+        return W.conv_bn(name, cout, cin, k, self.eps, res_branch=res_branch)
+
+    def cbs(self, name: str, x, cout: int, k: int, s: int = 1, out: Optional[View] = None, res: Optional[View] = None):
+        w, b = self.conv_bn(name, cout, self.real(x), k, res_branch=res is not None)
+        return self.conv(x, w, b, k, s, out=out, res=res)
+
+    def rep_ncsp(self, name: str, x, c2: int, n: int, out: Optional[View] = None):
+        """RepNCSP: cv3(cat(m(cv1(x)), cv2(x))), m = n x RepNBottleneck (RepConvN 3x3, Conv 3x3, residual add)."""
+        pb, r8 = self.pb, self.r8
+        c_ = c2 // 2
+        cat = pb.new_padded(x[0].H, x[0].W, 2 * r8(c_))
+        a = self.cbs(f"{name}.cv1", x, c_, 1)
+        for j in range(n):
+            w, b = self.W.repconvn(f"{name}.m.{j}.cv1", c_, c_, self.eps)
+            t = self.conv(a, w, b, 3)
+            a = self.cbs(f"{name}.m.{j}.cv2", t, c_, 3, out=pb.sub(cat, 0, r8(c_)) if j == n - 1 else None, res=a[0])
+        self.cbs(f"{name}.cv2", x, c_, 1, out=pb.sub(cat, r8(c_), r8(c_)))
+        return self.cbs(f"{name}.cv3", (cat, ((0, c_), (r8(c_), c_))), c2, 1, out=out)
+
+    def elan(self, name: str, x, c2: int, c3: int, c4: int, n: Optional[int], out: Optional[View] = None):
+        """RepNCSPELAN4 (n = RepNCSP depth) or ELAN1 (n None): cv4(cat(chunk0, chunk1, cv2(chunk1), cv3(cv2(...))))."""
+        pb, r8 = self.pb, self.r8
+        h = c3 // 2
+        o = (0, r8(h), 2 * r8(h), 2 * r8(h) + r8(c4))
+        cat = pb.new_padded(x[0].H, x[0].W, o[3] + r8(c4))
+        w, b = self.conv_bn(f"{name}.cv1", c3, self.real(x), 1)
+        if r8(h) != h:                                   # the two chunks as aligned row blocks of one GEMM
+            wz = np.zeros((2 * r8(h),) + w.shape[1:], np.float32)
+            bz = np.zeros(2 * r8(h), np.float32)
+            wz[:h], wz[r8(h):r8(h) + h], bz[:h], bz[r8(h):r8(h) + h] = w[:h], w[h:], b[:h], b[h:]
+            w, b = wz, bz
+        self.conv(x, w, b, 1, out=pb.sub(cat, 0, 2 * r8(h)), real_cout=c3)
+        t = (pb.sub(cat, o[1], r8(h)), ((0, h),))
+        for i, slot in ((2, o[2]), (3, o[3])):
+            if n is None:
+                t = self.cbs(f"{name}.cv{i}", t, c4, 3, out=pb.sub(cat, slot, r8(c4)))
+            else:
+                t = self.rep_ncsp(f"{name}.cv{i}.0", t, c4, n)
+                t = self.cbs(f"{name}.cv{i}.1", t, c4, 3, out=pb.sub(cat, slot, r8(c4)))
+        return self.cbs(f"{name}.cv4", (cat, ((0, h), (o[1], h), (o[2], c4), (o[3], c4))), c2, 1, out=out)
+
+    def down(self, name: str, x, c2: int, out: Optional[View] = None):
+        """AConv: cv1 (3x3 s2) of the 2x2 stride-1 average pool.  ADown: the pool's first half through cv1 (3x3 s2), its second half
+        through a 3x3 stride-2 max pool and cv2 (1x1), concatenated.  The pool is stored on the input's even H x W grid with a zero
+        (AConv, ADown's first half) or -inf (ADown's second half) last row and column (PlanBuilder.avgpool2)."""
+        pb = self.pb
+        v = x[0]
+        out = out if out is not None else pb.new_padded(v.H // 2, v.W // 2, self.r8(c2))
+        if self.down_kind == "aconv":
+            return self.cbs(f"{name}.cv1", (pb.avgpool2(v, 0), x[1]), c2, 3, 2, out=out)
+        half, c = self.real(x) // 2, c2 // 2
+        assert x[1] == ((0, v.C),) and half % 8 == 0 and c % 8 == 0, (name, x[1], c2)
+        p = pb.new_padded(v.H, v.W, v.C)
+        pb.avgpool2(pb.sub(v, 0, half), 0, out=pb.sub(p, 0, half))
+        pb.avgpool2(pb.sub(v, half, half), 1, out=pb.sub(p, half, half))
+        self.cbs(f"{name}.cv1", self.feat(pb.sub(p, 0, half)), c, 3, 2, out=pb.sub(out, 0, c))
+        self.cbs(f"{name}.cv2", self.feat(pb.maxpool(pb.sub(p, half, half), 3, 2, 1)), c, 1, out=pb.sub(out, c, c))
+        return self.feat(View(out.buf, out.coff, c2, out.H, out.W))
+
+    def sppelan(self, name: str, x, c2: int, c3: int, out: Optional[View] = None):
+        """SPPELAN: cv5(cat(y, p(y), p(p(y)), p(p(p(y))))), y = cv1(x), p = 5x5 stride-1 max pool."""
+        pb, r8 = self.pb, self.r8
+        sp = pb.new_padded(x[0].H, x[0].W, 4 * r8(c3))
+        y = self.cbs(f"{name}.cv1", x, c3, 1, out=pb.sub(sp, 0, r8(c3)))[0]
+        for i in range(1, 4):
+            y = pb.maxpool(y, 5, 1, 2, out=pb.sub(sp, i * r8(c3), r8(c3)))
+        return self.cbs(f"{name}.cv5", (sp, tuple((i * r8(c3), c3) for i in range(4))), c2, 1, out=out)
+
+
+def build_yolov9(weights: Weights, scale: str = "c", nc: int = 80, in_h: int = 640, in_w: int = 640) -> PlanBuilder:
+    """YOLOv9-T / S / M / C (GELAN graphs, upstream `model.<i>` names; Conv = Conv2d + BatchNorm + SiLU) with the DDetect head (model.22).
+    The output and its decode are YOLOv8's ([B, 4 + nc, A], MODEL_YOLOV8 kind).  Inputs are multiples of 32.
+
+    RepConvN is folded here in fp64 (training-form `conv1` / `conv2` keys) or taken fused (`conv.weight` + `conv.bias`); a Conv fused
+    upstream (`conv.bias`, no `bn`) is taken as it is.  ADown / AConv's 2x2 stride-1 average pool runs as OP_AVGPOOL2 on the input's grid,
+    so their stride-2 convs see even maps.  DDetect's grouped box convs pack as dense block-diagonal weights.  Channel layout: Yolov9Packer."""
+    assert scale in YOLOV9, f"YOLOv9 scale {scale!r}: 't', 's', 'm' or 'c' (YOLOv9-E / GELAN-E is not supported)"
+    assert in_h % 32 == 0 and in_w % 32 == 0, f"YOLOv9 input {in_h}x{in_w}: a multiple of 32"
+    cfg = YOLOV9[scale]
+    pb = PlanBuilder(MODEL_YOLOV8, 3, in_h, in_w)
+    g = Yolov9Packer(pb, weights, cfg["down"])
+    H, Wd = in_h, in_w
+    d, r, (s2, s3) = cfg["downs"], cfg["r4"], cfg["spp"]
+    assert all(c % 8 == 0 for c in d + (s2,) + tuple(x[0] for x in r)), scale     # the head's concat members are aligned as they are
+    cat11 = pb.new_padded(H // 16, Wd // 16, s2 + r[1][0])     # [up(9), 6]
+    cat14 = pb.new_padded(H // 8, Wd // 8, r[3][0] + r[0][0])  # [up(12), 4]
+    cat17 = pb.new_padded(H // 16, Wd // 16, d[3] + r[3][0])   # [16, 12]
+    cat20 = pb.new_padded(H // 32, Wd // 32, d[4] + s2)        # [19, 9]
+
+    x = g.cbs("model.0", (pb.image, ((0, 3),)), cfg["stem"][0], 3, 2)
+    x = g.cbs("model.1", x, cfg["stem"][1], 3, 2)
+    x = g.elan("model.2", x, *cfg["l2"])
+    x = g.down("model.3", x, d[0])
+    p3 = g.elan("model.4", x, *r[0], out=pb.sub(cat14, r[3][0], r[0][0]))
+    x = g.down("model.5", p3, d[1])
+    p4 = g.elan("model.6", x, *r[1], out=pb.sub(cat11, s2, r[1][0]))
+    x = g.down("model.7", p4, d[2])
+    x = g.elan("model.8", x, *r[2])
+    p5 = g.sppelan("model.9", x, s2, s3, out=pb.sub(cat20, d[4], s2))
+    pb.upsample2x(p5[0], pb.sub(cat11, 0, s2))
+    h12 = g.elan("model.12", g.feat(cat11), *r[3], out=pb.sub(cat17, d[3], r[3][0]))
+    pb.upsample2x(h12[0], pb.sub(cat14, 0, r[3][0]))
+    h15 = g.elan("model.15", g.feat(cat14), *r[4])
+    g.down("model.16", h15, d[3], out=pb.sub(cat17, 0, d[3]))
+    h18 = g.elan("model.18", g.feat(cat17), *r[5])
+    g.down("model.19", h18, d[4], out=pb.sub(cat20, 0, d[4]))
+    h21 = g.elan("model.21", g.feat(cat20), *r[6])
+    A = v8_detect(pb, weights, "model.22", (h15[0], h18[0], h21[0]), nc, box_groups=4, conv_bn=g.conv_bn)
+    pb.meta[0], pb.meta[1] = nc, A
     return pb
 
 

@@ -1,5 +1,5 @@
 """Per-layer table of a plan at real clocks: every launch replayed alone (CUDA events, L2-warm), GEMM shapes and tile choices.
-usage: python tools/op_table.py yolov8|ufldv2|yolov5|yolov7|yolov7-tiny|yolov7-w6|yolov7-e6|yolov7-d6|yolov7-e6e|yolov6n|yolov6s|yolov6m|yolov6l|yolov9-t|yolov9-s|yolov9-m|yolov9-c [batch] [iters]
+usage: python tools/op_table.py yolov8|ufldv2|yolov5|yolov7|yolov7-tiny|yolov7-w6|yolov7-e6|yolov7-d6|yolov7-e6e|yolov6n|yolov6s|yolov6m|yolov6l|yolov9-t|yolov9-s|yolov9-m|yolov9-c|yolov10n|yolov10s|yolov10m|yolov10b|yolov10l|yolov10x [batch] [iters]
 (the YOLOv7 P6 models run at 1280x1280)   (env switches of the library apply)"""
 import os, re, sys, tempfile
 R = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, R); sys.path.insert(0, os.path.join(R, "tests"))
@@ -15,6 +15,10 @@ elif kind.startswith("yolov6"):
     pb = plan.build_yolov6(plan.synth_weights("yolov6", 0, variant=kind[-1]), kind[-1])
     path = os.path.join(tempfile.mkdtemp(), kind + ".b200w")
     pb.write(path)
+elif kind.startswith("yolov10"):
+    pb = plan.build_yolov10(plan.synth_weights("yolov10", 0, variant=kind[-1]), kind[-1])
+    path = os.path.join(tempfile.mkdtemp(), kind + ".b200w")
+    pb.write(path)
 elif kind.startswith("yolov9"):
     pb = plan.build_yolov9(plan.synth_weights("yolov9", 0, variant=kind[-1]), kind[-1])
     path = os.path.join(tempfile.mkdtemp(), kind + ".b200w")
@@ -25,7 +29,7 @@ else:
 eng = _capi.Engine(path, 0, max_batch=B)
 eng.run(B)
 n = eng.num_steps(B)
-names = {1: "gemm", 2: "im2col", 3: "maxpool", 4: "upsample", 5: "layernorm", 6: "stempack", 7: "stemconv", 8: "avgpool2", 31: "(folded)"}
+names = {1: "gemm", 2: "im2col", 3: "maxpool", 4: "upsample", 5: "layernorm", 6: "stempack", 7: "stemconv", 8: "avgpool2", 9: "dwconv", 10: "attention", 31: "(folded)"}
 tot = 0.0; tot_g = 0.0; rows = []
 for i in range(n):
     ms, t, d = eng.time_step(B, i, iters)
@@ -39,7 +43,7 @@ for i in range(n):
             tf = f"{2.0 * M * N * K / ms / 1e9:7.1f} TF(incl halo)"
     rows.append((ms, i, names.get(t, str(t)), d, tf))
     print(f"{i:3d} {names.get(t, str(t)):9s} {ms * 1e3:8.1f} us {tf} {d}", flush=True)
-flops = (pb.flops_per_img - pb.stem_flops_per_img) * B      # the stem conv is not a GEMM launch
+flops = (pb.flops_per_img - pb.stem_flops_per_img - pb.dw_flops_per_img) * B      # the stem and depthwise convs are not GEMM launches
 print(f"TOTAL {kind} b{B}: sum of isolated launches {tot * 1e3:.1f} us (gemm {tot_g * 1e3:.1f} us) -> {flops / tot_g / 1e9:.1f} TFLOP/s algorithmic over GEMM time")
 ms_all, nl = eng.time_ops(B, 0xFFFFFFFF, 10)
 ms_g, ng = eng.time_ops(B, 1 << 1, 10)
@@ -48,4 +52,16 @@ print(f"back-to-back: all {ms_all * 1e3:.1f} us ({nl} launches), gemm only {ms_g
 ms_ap = sum(r[0] for r in rows if r[2] == "avgpool2")
 ms_ic = sum(r[0] for r in rows if r[2] == "im2col" and pb.ops[r[1]][1][2] < 64)        # one launch per plan op; im2col p[2] = Cin
 print(f"share of the sum of isolated launches: avgpool2 {100 * ms_ap / tot:.1f} %, im2col of convs with < 64 input channels {100 * ms_ic / tot:.1f} %")
+dw_rows = [r for r in rows if r[2] == "dwconv"]
+if dw_rows:
+    ms_dw = sum(r[0] for r in dw_rows)
+    ms_at = sum(r[0] for r in rows if r[2] == "attention")
+    dw_bytes = 0                              # fp16 input + output (+ residual) of every depthwise launch, weights once: computed from shapes
+    for r in dw_rows:
+        p = pb.ops[r[1]][1]
+        bi, bo = pb.buffers[p[0]], pb.buffers[p[8]]
+        C, k = p[2], p[3]
+        dw_bytes += 2 * B * C * (bi[3] * bi[4] + bo[3] * bo[4] * (2 if p[10] >= 0 else 1)) + C * (2 * k * k + 4)
+    print(f"share of the sum of isolated launches: dwconv {100 * ms_dw / tot:.1f} %, attention {100 * ms_at / tot:.1f} %; "
+          f"dwconv {dw_bytes / 1e6:.1f} MB in {ms_dw * 1e3:.1f} us -> {dw_bytes / ms_dw / 1e6:.0f} GB/s (HBM3 data sheet: 3350 GB/s)")
 eng.close()

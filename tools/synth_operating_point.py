@@ -1,7 +1,7 @@
 """Scan synthetic head operating points (gain, bias) on the CPU: fp32 oracle vs its fp16-storage emulation (oracle.nets.forward_fp16_emulated).
 Prints the probability / box error the device path will show, the candidates per frame at box_score 0.4 and how many sit within 1e-3 / 2e-3
 of the threshold.  Test infrastructure (uses oracle/):  python tools/synth_operating_point.py yolov8 l 45,-9 40,-8.2
-(yolov9 t|s|m|c: the scale's class bias; the head gains of plan.SYNTH_PROFILES["yolov9"] are kept)
+(yolov9 t|s|m|c, yolov10 n|s|m|b|l|x: the scale's class bias; the head gains of plan.SYNTH_PROFILES[kind] are kept)
 """
 import sys, os
 R = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, R); sys.path.insert(0, os.path.join(R, 'tests'))
@@ -12,7 +12,7 @@ from adas_b200 import plan
 from oracle import nets, post
 import synth
 kind, variant = sys.argv[1], sys.argv[2]
-builder = {"yolov8": plan.build_yolov8, "yolov9": plan.build_yolov9}.get(kind, plan.build_yolov5)
+builder = {"yolov8": plan.build_yolov8, "yolov9": plan.build_yolov9, "yolov10": plan.build_yolov10}.get(kind, plan.build_yolov5)
 x = torch.from_numpy(np.concatenate([post.yolo_prepare_input(synth.frame(s), 640, 640)[0] for s in (0,1,2,3,4,5,6,7)]))
 for a in sys.argv[3:]:
     g,b = map(float,a.split(','))
@@ -21,21 +21,28 @@ for a in sys.argv[3:]:
     elif kind=="yolov9":
         plan.SYNTH_PROFILES["yolov9"]={**plan.SYNTH_PROFILES["yolov9"], "gains":[(r"model\.22\.cv3\.\d\.2\.weight", g), (r"model\.22\.cv2\.\d\.2\.weight", 25.0)],
                                    "variants": {variant: {"fill": [(r"model\.22\.cv3\.\d\.2\.bias", b)]}}}
+    elif kind=="yolov10":
+        plan.SYNTH_PROFILES["yolov10"]={**plan.SYNTH_PROFILES["yolov10"], "gains":[(r"model\.23\.one2one_cv3\.\d\.2\.weight", g), (r"model\.23\.one2one_cv2\.\d\.2\.weight", 25.0)],
+                                    "variants": {variant: {"fill": [(r"model\.23\.one2one_cv3\.\d\.2\.bias", b)]}}}
     else:
         plan.SYNTH_PROFILES["yolov5"]={"gains":[(r"model\.24\.m\.\d\.weight", g)],"fill":[(r"model\.24\.m\.\d\.bias", b)]}
     W = plan.synth_weights(kind, 0, variant=variant); builder(W, variant)
     if kind=="yolov9":
         import yolov9_oracle
         md = yolov9_oracle.build(W.state_dict, variant)
+    elif kind=="yolov10":
+        import yolov10_oracle
+        md = yolov10_oracle.build(W.state_dict, variant)
     else:
         md = nets.build(kind, W.state_dict, scale=variant)
     with torch.no_grad():
-        ref = md(x).numpy(); emu = nets.forward_fp16_emulated(md, x).numpy()
-    if kind in ("yolov8", "yolov9"):
+        ref = md(x).numpy()
+        emu = (yolov10_oracle.forward_fp16_emulated if kind == "yolov10" else nets.forward_fp16_emulated)(md, x).numpy()
+    if kind in ("yolov8", "yolov9", "yolov10"):
         e=np.abs(ref[:,4:]-emu[:,4:]); mx=ref[:,4:].max(1); mg=emu[:,4:].max(1); eb=np.abs(ref[:,:4]-emu[:,:4]).max()
     else:
         e=np.abs(ref[...,4:]-emu[...,4:]); mx=(ref[...,5:]*ref[...,4:5]).max(2); mg=(emu[...,5:]*emu[...,4:5]).max(2); eb=np.abs(ref[...,:4]-emu[...,:4]).max()
     cand=mx>0.4
     print(f"g={g} b={b}: max prob err {e.max():.2e} box err {eb:.3f} | cands {cand.sum(1).tolist()} within1e-3 {(np.abs(mx-0.4)<1e-3).sum(1).tolist()} within2e-3 {int((np.abs(mx-0.4)<2e-3).sum())} flips {int((cand!=(mg>0.4)).sum())}", flush=True)
-    if kind in ("yolov8", "yolov9"): print("   per-frame max prob err", [f"{v:.2e}" for v in e.max(axis=(1,2))])
+    if kind in ("yolov8", "yolov9", "yolov10"): print("   per-frame max prob err", [f"{v:.2e}" for v in e.max(axis=(1,2))])
     else: print("   per-frame max prob err", [f"{v:.2e}" for v in e.reshape(e.shape[0],-1).max(1)])

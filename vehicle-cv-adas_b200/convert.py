@@ -11,6 +11,8 @@ and `TrafficLaneDetector/convertPytorchToONNX.py:77-87` (UFLD `.pth` checkpoint 
     python -m adas_b200.convert yolov7-w6.state_dict.pth --kind yolov7 --scale w6     # P6: w6 | e6 | d6 | e6e, 1280x1280
     python -m adas_b200.convert yolov6s.state_dict.pth --kind yolov6 --scale s
     python -m adas_b200.convert yolov9-c.state_dict.pth --kind yolov9 --scale c     # t | s | m | c
+    python -m adas_b200.convert yolov10s.state_dict.pth --kind yolov10 --scale s    # n | s | m | b | l | x
+    python -m adas_b200.convert yolov10s.onnx                                         # recognised, also with the top-k tail
 
 Upstream YOLOv6 checkpoints pickle the whole model; extract its parameters once, in the YOLOv6 repository:
     torch.save(torch.load("yolov6s.pt", map_location="cpu", weights_only=False)["model"].float().state_dict(), "yolov6s.state_dict.pth")
@@ -19,6 +21,11 @@ YOLOv9 checkpoints (WongKinYiu/yolov9) pickle the whole model too; extract the p
     torch.save(torch.load("yolov9-c-converted.pt", map_location="cpu", weights_only=False)["model"].float().state_dict(), "yolov9-c.state_dict.pth")
 Training-form (RepConvN conv1 / conv2 + BatchNorm) and fused (conv weight + bias) keys are both accepted; only the converted (GELAN)
 graphs are supported, not the training files with the auxiliary branch.
+YOLOv10 checkpoints (ultralytics 8.2.41) pickle the whole model; extract the parameters once, in an ultralytics checkout:
+    torch.save(torch.load("yolov10s.pt", map_location="cpu", weights_only=False)["model"].float().state_dict(), "yolov10s.state_dict.pth")
+Training-form (Conv + BatchNorm, RepVGGDW conv / conv1) and fused keys are both accepted.  Only the one-to-one head
+(`model.23.one2one_cv2` / `one2one_cv3`) is packed; the one-to-many head's keys are ignored.  The plan emits YOLOv8's [B, 4 + nc, A]
+output, decoded by the YOLOv8 path, not upstream's top-k [1, 300, 6] tail.
 
 Checkpoints hold un-fused Conv/BatchNorm parameters under the upstream key names (the names `plan.build_*` ask for), so BatchNorm
 is folded here in float64 exactly as for the seeded weights.  Only the parameter dictionary is read: pickled model objects
@@ -67,6 +74,8 @@ def plan_from_state_dict(sd: Dict[str, np.ndarray], kind: str, scale: str = "l",
         return plan.build_yolov6(w, scale, nc=nc)
     if kind == "yolov9":
         return plan.build_yolov9(w, scale, nc=nc)
+    if kind == "yolov10":
+        return plan.build_yolov10(w, scale, nc=nc)
     if kind == "ufldv2":
         return plan.build_ufldv2(w, backbone)
     raise Exception(f"unsupported model kind {kind}")
@@ -81,7 +90,7 @@ def convert(path: str, out: Optional[str] = None, kind: Optional[str] = None, sc
         pb = build_plan(model, recognise(model))
     else:
         if kind is None:
-            raise Exception("--kind is required for checkpoint files (yolov8 | yolov5 | yolov7 | yolov6 | yolov9 | ufldv2)")
+            raise Exception("--kind is required for checkpoint files (yolov8 | yolov5 | yolov7 | yolov6 | yolov9 | yolov10 | ufldv2)")
         pb = plan_from_state_dict(load_checkpoint_state_dict(path), kind, scale, backbone, nc)
     pb.write(out)
     return out
@@ -91,8 +100,8 @@ def main(argv=None) -> int:
     ap = argparse.ArgumentParser(description="convert an .onnx model or a state_dict checkpoint to a .b200w plan")
     ap.add_argument("model")
     ap.add_argument("--out", default=None)
-    ap.add_argument("--kind", default=None, choices=["yolov8", "yolov5", "yolov7", "yolov6", "yolov9", "ufldv2"])
-    ap.add_argument("--scale", default="l", help="YOLO scale letter (n | s | m | l for yolov6, t | s | m | c for yolov9), or tiny | base | w6 | e6 | d6 | e6e for yolov7 (checkpoints only; ONNX files are recognised)")
+    ap.add_argument("--kind", default=None, choices=["yolov8", "yolov5", "yolov7", "yolov6", "yolov9", "yolov10", "ufldv2"])
+    ap.add_argument("--scale", default="l", help="YOLO scale letter (n | s | m | l for yolov6, t | s | m | c for yolov9, n | s | m | b | l | x for yolov10), or tiny | base | w6 | e6 | d6 | e6e for yolov7 (checkpoints only; ONNX files are recognised)")
     ap.add_argument("--backbone", default="34", choices=["18", "34"], help="UFLDv2 ResNet depth (checkpoints only)")
     ap.add_argument("--nc", type=int, default=80)
     a = ap.parse_args(argv)

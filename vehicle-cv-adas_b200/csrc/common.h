@@ -124,6 +124,13 @@ int stem_conv_supported(int Cout, int k, int pad);
 int launch_stem_conv(const __half* img, int B, int H, int W, const __half* wq, const float* bias, int Cout, int k, int pad, int stride, int act,
                      __half* out, int out_ld, int Ho, int Wo, cudaStream_t st);
 int launch_zero_rows(__half* buf, int ld, int C, int row0, int nrows, cudaStream_t st);
+// dwconv.cu: depthwise k x k conv (k 3 / 7, stride 1 / 2) of a channel slice, out = act(acc + bias) (+ res)
+int launch_dwconv(const __half* in, int in_ld, int B, int H, int W, int C, int k, int stride, const __half* w, const float* bias, int act,
+                  const __half* res, int res_ld, __half* out, int out_ld, int Ho, int Wo, cudaStream_t st);
+// attention.cu: multi-head self-attention over the H*W pixels of each image (YOLOv10 PSA)
+int attention_supported(int nh, int kdp, int hd);
+int launch_attention(const __half* qkv, int in_ld, int B, int H, int W, int nh, int kdp, int hd, float scale, __half* out, int out_ld,
+                     cudaStream_t st);
 
 // ---- pre-processing (preprocess.cu) -----------------------------------------------------------
 struct LetterboxGeom {

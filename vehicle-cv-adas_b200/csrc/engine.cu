@@ -317,6 +317,40 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
                 prog->steps.push_back([=](cudaStream_t st) { return launch_avgpool2(in, in_ld, batch, H, W, C, out, out_ld, fill, st); });
                 break;
             }
+            case OP_DWCONV: {
+                const PlanBuffer& ib = e->bufs[p[0]];
+                const PlanBuffer& ob = e->bufs[p[8]];
+                const __half* in = static_cast<const __half*>(e->dbufs[p[0]].ptr) + p[1];
+                __half* out = static_cast<__half*>(e->dbufs[p[8]].ptr) + p[9];
+                const __half* res = p[10] >= 0 ? static_cast<const __half*>(e->dbufs[p[10]].ptr) + p[11] : nullptr;
+                const int res_ld = p[10] >= 0 ? (int)e->bufs[p[10]].C : 0;
+                const __half* w = static_cast<const __half*>(tensor_ptr(e, p[6]));
+                const float* bias = static_cast<const float*>(tensor_ptr(e, p[7]));
+                const int in_ld = (int)ib.C, H = (int)ib.H, W = (int)ib.W, C = p[2], k = p[3], s = p[4], act = p[5];
+                const int out_ld = (int)ob.C, Ho = (int)ob.H, Wo = (int)ob.W;
+                char d[128];
+                snprintf(d, sizeof(d), "dwconv %dx%d s%d C=%d, %dx%d -> %dx%d%s%s", k, k, s, C, H, W, Ho, Wo, act ? " silu" : "", res ? " +res" : "");
+                prog->step_desc.resize(prog->step_type.size());
+                prog->step_desc.back() = d;
+                prog->steps.push_back([=](cudaStream_t st) {
+                    return launch_dwconv(in, in_ld, batch, H, W, C, k, s, w, bias, act, res, res_ld, out, out_ld, Ho, Wo, st);
+                });
+                break;
+            }
+            case OP_ATTN: {
+                const PlanBuffer& ib = e->bufs[p[0]];
+                const PlanBuffer& ob = e->bufs[p[5]];
+                const __half* in = static_cast<const __half*>(e->dbufs[p[0]].ptr) + p[1];
+                __half* out = static_cast<__half*>(e->dbufs[p[5]].ptr) + p[6];
+                const int in_ld = (int)ib.C, H = (int)ib.H, W = (int)ib.W, nh = p[2], kdp = p[3], hd = p[4], out_ld = (int)ob.C;
+                const float scale = op.f[0];
+                char d[128];
+                snprintf(d, sizeof(d), "attention N=%d heads=%d kdp=%d hd=%d", H * W, nh, kdp, hd);
+                prog->step_desc.resize(prog->step_type.size());
+                prog->step_desc.back() = d;
+                prog->steps.push_back([=](cudaStream_t st) { return launch_attention(in, in_ld, batch, H, W, nh, kdp, hd, scale, out, out_ld, st); });
+                break;
+            }
             case OP_UPSAMPLE2X: {
                 const PlanBuffer& ib = e->bufs[p[0]];
                 const PlanBuffer& ob = e->bufs[p[3]];
@@ -616,6 +650,43 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
                 ADAS_CHECK(view_ok(p[0], p[1], p[2]) && view_ok(p[3], p[4], p[2]) && (p[0] != p[3] || p[4] >= p[1] + p[2] || p[1] >= p[4] + p[2]),
                            "plan %s: op %zu: avgpool2 channel slice exceeds its buffer or overlaps its input", path, oi);
                 ADAS_CHECK(p[5] == 0 || p[5] == 1, "plan %s: op %zu: avgpool2 fill %d (0: zero, 1: -inf)", path, oi, p[5]);
+                break;
+            }
+            case OP_DWCONV: {
+                const int C = p[2], k = p[3], s = p[4], act = p[5], rb = p[10];
+                ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[8]) && (rb == -1 || buf_ok(rb)), "plan %s: op %zu: dwconv buffer index out of range", path, oi);
+                const PlanBuffer &ib = e->bufs[p[0]], &ob = e->bufs[p[8]];
+                ADAS_CHECK(ib.dtype == 0 && ob.dtype == 0 && (rb < 0 || e->bufs[rb].dtype == 0), "plan %s: op %zu: dwconv buffers must be fp16", path, oi);
+                ADAS_CHECK((k == 3 && (s == 1 || s == 2)) || (k == 7 && s == 1), "plan %s: op %zu: dwconv k %d stride %d (3 s1 / s2, 7 s1)", path, oi, k, s);
+                ADAS_CHECK(act == 0 || act == 1, "plan %s: op %zu: dwconv act %d (0 none, 1 SiLU)", path, oi, act);
+                ADAS_CHECK(ib.H > 0 && ob.H > 0 && (int)ob.H == ((int)ib.H + 2 * (k / 2) - k) / s + 1 && (int)ob.W == ((int)ib.W + 2 * (k / 2) - k) / s + 1,
+                           "plan %s: op %zu: dwconv output geometry %ux%u does not match a %dx%d stride-%d conv of %ux%u", path, oi, ob.H, ob.W, k, k, s, ib.H, ib.W);
+                ADAS_CHECK(C >= 8 && C % 8 == 0 && p[1] % 8 == 0 && p[9] % 8 == 0 && (rb < 0 || (p[11] % 8 == 0 && e->bufs[rb].C % 8 == 0)) &&
+                           ib.C % 8 == 0 && ob.C % 8 == 0, "plan %s: op %zu: dwconv channels and offsets must be multiples of 8", path, oi);
+                ADAS_CHECK(tensor_ok(p[6], 0) && e->tensors[p[6]].dtype == 0 && e->tensors[p[6]].bytes == (uint64_t)C * k * k * 2,
+                           "plan %s: op %zu: dwconv weight tensor must be fp16 [k*k][C]", path, oi);
+                ADAS_CHECK(tensor_ok(p[7], 0) && e->tensors[p[7]].dtype == 1 && e->tensors[p[7]].bytes == (uint64_t)C * 4,
+                           "plan %s: op %zu: dwconv bias tensor must be fp32 [C]", path, oi);
+                ADAS_CHECK(rb < 0 || (e->bufs[rb].H == ob.H && e->bufs[rb].W == ob.W && view_ok(rb, p[11], C)),
+                           "plan %s: op %zu: dwconv residual slice must have the output's geometry and fit its buffer", path, oi);
+                ADAS_CHECK(view_ok(p[0], p[1], C) && view_ok(p[8], p[9], C) && (p[0] != p[8] || p[9] >= p[1] + C || p[1] >= p[9] + C) &&
+                           (rb != p[8] || p[11] == p[9] || p[11] >= p[9] + C || p[9] >= p[11] + C),
+                           "plan %s: op %zu: dwconv channel slice exceeds its buffer or overlaps its input", path, oi);
+                break;
+            }
+            case OP_ATTN: {
+                const int nh = p[2], kdp = p[3], hd = p[4];
+                ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[5]), "plan %s: op %zu: attention buffer index out of range", path, oi);
+                const PlanBuffer &ib = e->bufs[p[0]], &ob = e->bufs[p[5]];
+                ADAS_CHECK(ib.dtype == 0 && ob.dtype == 0, "plan %s: op %zu: attention buffers must be fp16", path, oi);
+                ADAS_CHECK(ib.H > 0 && ob.H == ib.H && ob.W == ib.W, "plan %s: op %zu: attention output must have its input's H x W", path, oi);
+                ADAS_CHECK(attention_supported(nh, kdp, hd), "plan %s: op %zu: attention heads %d, kdp %d (multiple of 16, <= 64), hd %d (multiple of 8, <= 128)",
+                           path, oi, nh, kdp, hd);
+                ADAS_CHECK(p[1] % 8 == 0 && p[6] % 8 == 0 && ib.C % 8 == 0 && ob.C % 8 == 0, "plan %s: op %zu: attention channels and offsets must be multiples of 8", path, oi);
+                const int cin = nh * (2 * kdp + hd), cout = nh * hd;
+                ADAS_CHECK(view_ok(p[0], p[1], cin) && view_ok(p[5], p[6], cout) && (p[0] != p[5] || p[6] >= p[1] + cin || p[1] >= p[6] + cout),
+                           "plan %s: op %zu: attention channel slice exceeds its buffer or overlaps its input", path, oi);
+                ADAS_CHECK(std::isfinite(op.f[0]) && op.f[0] > 0.f, "plan %s: op %zu: attention scale %g", path, oi, (double)op.f[0]);
                 break;
             }
             case OP_UPSAMPLE2X:

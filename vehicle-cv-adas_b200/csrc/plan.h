@@ -63,6 +63,11 @@ enum PlanOpType : uint32_t {
                        //    other d_len - d_norm slab entries are structural zeros with gamma = beta = 0)
     OP_AVGPOOL2 = 8,   // p: in_buf in_coff C out_buf out_coff fill : 2x2 stride-1 mean into a buffer of the input's H x W geometry;
                        //    row H-1 and column W-1 hold 0 (fill 0) or -inf (fill 1), see elementwise.cu avgpool2_kernel
+    OP_DWCONV = 9,     // p: in_buf in_coff C k stride act w_tensor bias_tensor out_buf out_coff res_buf res_coff : depthwise k x k conv
+                       //    (k 3 or 7, pad k/2, stride 1 or 2 with k 3), weights fp16 [k*k][C], bias fp32 [C], act 0 none / 1 SiLU;
+                       //    out = act(acc + bias) (+ res, res_buf -1: none), see dwconv.cu
+    OP_ATTN = 10,      // p: in_buf in_coff nh kdp hd out_buf out_coff ; f0 = softmax scale : multi-head self-attention over the H*W
+                       //    pixels; input channels [Q nh*kdp | K nh*kdp | V nh*hd], output nh*hd channels head-major, see attention.cu
 };
 
 }  // namespace adas

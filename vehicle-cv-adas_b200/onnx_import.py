@@ -4,7 +4,7 @@ The reference hands `.onnx` / `.trt` files to ONNXRuntime / TensorRT (coreEngine
 ultralytics / yolov5 exports (README.md:53-58) and from `TrafficLaneDetector/convertPytorchToONNX.py:60-87` (UFLD).  This module
 is the H100 replacement of that ingestion step (SURVEY 8f rank 2): it reads the ONNX protobuf directly (the `onnx` package is
 not a dependency -- the wire format is parsed here), recovers the convolution / linear / LayerNorm parameters, recognises the
-architecture (YOLOv8 / YOLOv5 / YOLOv6 / YOLOv7 / YOLOv9 / UFLDv2, scale, class count, input size) and drives the same `plan.build_*` builders that the
+architecture (YOLOv8 / YOLOv5 / YOLOv6 / YOLOv7 / YOLOv9 / YOLOv10 / UFLDv2, scale, class count, input size) and drives the same `plan.build_*` builders that the
 state_dict path uses.  Nothing here runs the network: the graph is only a parameter container plus a shape oracle.
 
 How parameters are matched to layers:
@@ -329,6 +329,20 @@ class OnnxWeights(plan.Weights):
         w[:, :, 1, 1] += w1[:, :, 0, 0]
         return w.astype(np.float32), (b3.astype(np.float64) + b1).astype(np.float32)
 
+    def repvggdw(self, prefix: str, c: int, eps: float):
+        """Fused (`conv.weight`) or named un-fused RepVGGDW as in plan.Weights; exporter-folded, its 7x7 and 3x3 depthwise branches are
+        two anonymous convolutions in graph order (a file fused upstream has the 7x7 alone), summed here in fp64."""
+        if f"{prefix}.conv.weight" in self.state_dict or f"{prefix}.conv.bn.running_var" in self.state_dict:
+            return super().repvggdw(prefix, c, eps)
+        w7, b7 = self.conv_bn(f"{prefix}.conv", c, 1, 7, eps)
+        nxt = next((i for i in range(len(self._anon)) if i not in self._anon_used), None)
+        if nxt is None or tuple(self._anon[nxt][1].shape) != (c, 1, 3, 3):
+            return w7, b7
+        w3, b3 = self.conv_bn(f"{prefix}.conv1", c, 1, 3, eps)
+        w = w7.astype(np.float64)
+        w[:, :, 2:5, 2:5] += w3
+        return w.astype(np.float32), (b7.astype(np.float64) + b3).astype(np.float32)
+
 
 def _is_module_name(name: str) -> bool:
     """True for exporter-kept parameter names (`model.0.conv.weight`, `pool.weight`), False for `onnx::Conv_123` and friends."""
@@ -340,7 +354,7 @@ def _is_module_name(name: str) -> bool:
 # ---------------------------------------------------------------------------------------------------------------
 @dataclass
 class ModelSpec:
-    kind: str                 # "yolov8" | "yolov5" | "yolov7" | "yolov6" | "yolov9" | "ufldv2"
+    kind: str                 # "yolov8" | "yolov5" | "yolov7" | "yolov6" | "yolov9" | "yolov10" | "ufldv2"
     scale: str                # YOLO scale letter ("tiny" / "base" for YOLOv7) or ResNet depth ("18" / "34")
     nc: int = 80
     in_h: int = 640
@@ -375,6 +389,8 @@ def recognise(model: OnnxModel) -> ModelSpec:
         return _recognise_yolov6(model, w, in_h, in_w)
     if _is_yolov7(model, w):
         return _recognise_yolov7(model, w, in_h, in_w)
+    if _is_yolov10(model):                                           # depthwise convs + PSA's softmax; v6-Lite is refused above
+        return _recognise_yolov10(model, w, in_h, in_w)
     cout0, k0 = first.shape[0], first.shape[2]
     if cout0 not in _V8_WIDTH:
         raise Exception(f"unrecognised YOLO width: first convolution has {cout0} output channels")
@@ -587,7 +603,7 @@ def _recognise_yolov6(model: OnnxModel, w: OnnxWeights, in_h: int, in_w: int) ->
 
 
 _V9_SUPPORTED = ("YOLOv9-T / S / M / C (WongKinYiu/yolov9 v0.1, the converted GELAN graphs with a DDetect head, exported with one output; "
-                 "YOLOv9-E / GELAN-E, files with the auxiliary branch, ultralytics' YOLOv9 and YOLOv10 are not supported)")
+                 "YOLOv9-E / GELAN-E, files with the auxiliary branch, ultralytics' YOLOv9 are not supported)")
 _V9_STEM = {16: ("t",), 32: ("s", "m"), 64: ("c",)}
 _V9_DOWN3 = {128: "s", 240: "m"}            # layer 3 (AConv) width tells S from M
 
@@ -638,6 +654,58 @@ def _recognise_yolov9(model: OnnxModel, w: OnnxWeights, in_h: int, in_w: int) ->
     return ModelSpec("yolov9", scale, nc, in_h or 640, in_w or 640)
 
 
+_V10_SUPPORTED = ("YOLOv10-N / S / M / B / L / X (ultralytics 8.2.41) with the one-to-one head, one output ([1, 4 + nc, A] or the "
+                  "top-k [1, 300, 6] tail), input a multiple of 32")
+_V10_STEM = {16: ("n",), 32: ("s",), 48: ("m",), 64: ("b", "l"), 80: ("x",)}
+
+
+def _is_yolov10(model: OnnxModel) -> bool:
+    """Depthwise convolutions (group = Cin = Cout > 1: SCDown, CIB, PSA's pe, the v10 class branch) together with a Softmax outside
+    the DFL decode (PSA's attention).  YOLOv8 files have the DFL softmax but no depthwise conv; YOLOv9's grouped convs have 4 groups."""
+    dw = any(n.op_type == "Conv" and int(n.attrs.get("group", 1)) > 1 and len(n.inputs) > 1 and n.inputs[1] in model.initializers
+             and model.initializers[n.inputs[1]].shape[1] == 1 and model.initializers[n.inputs[1]].shape[0] == int(n.attrs["group"])
+             for n in model.nodes)
+    return dw and any(n.op_type == "Softmax" for n in model.nodes)
+
+
+def _recognise_yolov10(model: OnnxModel, w: OnnxWeights, in_h: int, in_w: int) -> ModelSpec:
+    """YOLOv10-N / S / M / B / L / X: the stem width gives the scale (64: B or L by `model.2.m.2.*`, else by the convolution count).
+    Without module names the convolution count must be the scale's (fused, or with RepVGGDW's two branches apart): a file that also
+    carries the one-to-many head cannot be matched by order and is refused.  The class count comes from `model.23.one2one_cv3.*.2`."""
+    if len(model.outputs) != 1:
+        raise Exception(f"YOLOv10 file with {len(model.outputs)} outputs; supported: {_V10_SUPPORTED}")
+    if (in_h and in_h % 32) or (in_w and in_w % 32):
+        raise Exception(f"YOLOv10 file with a {in_h}x{in_w} input: a multiple of 32; supported: {_V10_SUPPORTED}")
+    first = w.convs[0][1]
+    cands = _V10_STEM.get(int(first.shape[0]), ()) if tuple(first.shape[1:]) == (3, 3, 3) else ()
+    if not cands:
+        raise Exception(f"YOLOv10 stem {tuple(first.shape)}: 16 (N), 32 (S), 48 (M), 64 (B / L) or 80 (X) channels; supported: {_V10_SUPPORTED}")
+    named = any(re.fullmatch(r"model\.23\.one2one_cv3\.\d+\.2\.weight", k) for k in model.initializers) and \
+        any(k.startswith("model.2.") for k in model.initializers)
+    n = sum(1 for _, cw, _ in w.convs if tuple(cw.shape) != (1, 16, 1, 1))        # upstream's fixed DFL conv is not counted
+    counts = {sc: (plan.yolov10_conv_count(sc), plan.yolov10_conv_count(sc) + plan.yolov10_repvggdw_count(sc)) for sc in cands}
+    if named:
+        scale = ("l" if any(k.startswith("model.2.m.2.") for k in model.initializers) else "b") if len(cands) > 1 else cands[0]
+    else:
+        fits = [sc for sc in cands if n in counts[sc]]
+        if not fits:
+            o2m = [sc for sc in cands if n - 24 in counts[sc]]
+            if o2m:
+                raise Exception(f"YOLOv10-{o2m[0].upper()} file without module names that also carries the one-to-many head ({n} "
+                                f"convolutions): its convolutions cannot be matched in order; export the model after upstream's fuse() "
+                                f"(which drops that head) or keep the module names; supported: {_V10_SUPPORTED}")
+            raise Exception(f"YOLOv10 file with {n} convolutions, " + ", ".join(f"YOLOv10-{sc.upper()} has {c[0]} ({c[1]} with RepVGGDW's "
+                            f"branches apart)" for sc, c in counts.items()) + f"; supported: {_V10_SUPPORTED}")
+        scale = fits[0]
+    nc = None
+    for name, cw, _ in w.convs:
+        if re.fullmatch(r"model\.23\.one2one_cv3\.\d+\.2\.weight", name):      # v10Detect.one2one_cv3[i][2]: Conv2d(c3, nc, 1)
+            nc = int(cw.shape[0])
+    if nc is None:                                               # names lost: the last 1x1 conv before the (optional) DFL conv
+        nc = int([cw.shape[0] for _, cw, _ in w.convs if cw.shape[2:] == (1, 1) and cw.shape[0] != 1][-1])
+    return ModelSpec("yolov10", scale, nc, in_h or 640, in_w or 640)
+
+
 def build_plan(model: OnnxModel, spec: Optional[ModelSpec] = None) -> "plan.PlanBuilder":
     spec = spec or recognise(model)
     w = OnnxWeights(model)
@@ -649,6 +717,8 @@ def build_plan(model: OnnxModel, spec: Optional[ModelSpec] = None) -> "plan.Plan
         return plan.build_yolov7(w, spec.scale, nc=spec.nc, in_h=spec.in_h, in_w=spec.in_w, act=spec.act, anchors=spec.anchors)
     if spec.kind == "yolov9":
         return plan.build_yolov9(w, spec.scale, nc=spec.nc, in_h=spec.in_h, in_w=spec.in_w)
+    if spec.kind == "yolov10":
+        return plan.build_yolov10(w, spec.scale, nc=spec.nc, in_h=spec.in_h, in_w=spec.in_w)
     if spec.kind == "yolov6":
         body, neck, head = spec.acts or (None, "relu", "silu")
         return plan.build_yolov6(w, spec.scale, nc=spec.nc, in_h=spec.in_h, in_w=spec.in_w, act_body=body, act_neck=neck, act_head=head,

@@ -34,6 +34,7 @@ MODEL_YOLOV8, MODEL_YOLOV5, MODEL_UFLDV2, MODEL_UFLDV1 = 0, 1, 2, 4      # 3 = A
 MODEL_YOLOV6 = 5                                                         # anchor-free head, [B, 8400, 5 + nc] output; meta[2] = reg_max
 OP_GEMM, OP_IM2COL, OP_MAXPOOL, OP_UPSAMPLE2X, OP_LAYERNORM, OP_STEMPACK, OP_STEMCONV = 1, 2, 3, 4, 5, 6, 7
 OP_AVGPOOL2 = 8
+OP_DWCONV, OP_ATTN = 9, 10
 ACT_NONE, ACT_SILU, ACT_RELU, ACT_LEAKY = 0, 1, 2, 3          # ACT_LEAKY: LeakyReLU(0.1)
 PLAN_VERSION = 1
 
@@ -184,6 +185,16 @@ class Weights:
         w3[:, :, 1, 1] += w1[:, :, 0, 0]
         return w3.astype(np.float32), (b3 + b1).astype(np.float32)
 
+    def repvggdw(self, prefix: str, c: int, eps: float):
+        """YOLOv10 RepVGGDW: dw7x7+BN (`conv`) + dw3x3+BN (`conv1`), folded in fp64 into one depthwise 7x7 (the 3x3 on the centre taps).
+        A file fused upstream carries `conv.weight` + `conv.bias` instead."""
+        if f"{prefix}.conv.weight" in self.state_dict:
+            return self.conv_bias(f"{prefix}.conv", c, 1, 7)
+        w7, b7 = self._conv_bn64(f"{prefix}.conv", c, 1, 7, eps)
+        w3, b3 = self._conv_bn64(f"{prefix}.conv1", c, 1, 3, eps)
+        w7[:, :, 2:5, 2:5] += w3
+        return w7.astype(np.float32), (b7 + b3).astype(np.float32)
+
     def implicit_head(self, prefix: str, li: int, no: int, cin: int):
         """YOLOv7 IDetect level li: im * (m(x + ia)) folded into the 1x1 conv, w' = im * w, b' = im * (b + w @ ia) in fp64.  Files
         fused upstream (IDetect.fuse) carry the folded m.li conv and no implicit tensors."""
@@ -231,6 +242,15 @@ SYNTH_PROFILES = {
                "fill": [(r"model\.22\.cv3\.\d\.2\.bias", -3.5)],
                "variants": {sc: {"fill": [(r"model\.22\.cv3\.\d\.2\.bias", -3.5 - d)]}
                             for sc, d in (("t", 0.53), ("s", -0.31), ("m", 0.04), ("c", 0.05))}},
+    # YOLOv10 N/S/M/B/L/X: YOLOv8's head gains on the one-to-one head (CPU fp16 emulation, q / k / v and the attention output rounded
+    # too: probability error 2.5-3.7e-4, box error 0.13-0.23 px on 4 frames).  The class bias of each scale puts ~100 of the 8400
+    # anchors per frame above box_score = 0.4 (fp32 oracle, synthetic frames 0-3: at bias -3.5 the 100th-highest max-class logit sits
+    # -0.80 (N), 0.05 (S), 0.11 (M), 0.10 (B), 0.49 (L), 0.53 (X) from logit(0.4)).  The seeded PSA attention is not peaky (mean
+    # largest softmax weight 0.003 over 400 tokens), so its qkv weights are not damped.
+    "yolov10": {"gains": [(r"model\.23\.one2one_cv3\.\d\.2\.weight", 16.0), (r"model\.23\.one2one_cv2\.\d\.2\.weight", 25.0)],
+                "fill": [(r"model\.23\.one2one_cv3\.\d\.2\.bias", -3.5)],
+                "variants": {sc: {"fill": [(r"model\.23\.one2one_cv3\.\d\.2\.bias", -3.5 - d)]}
+                             for sc, d in (("n", -0.804), ("s", 0.054), ("m", 0.112), ("b", 0.099), ("l", 0.485), ("x", 0.534))}},
     # YOLOv7 base (model.105, SiLU) and tiny (model.77, LeakyReLU).  The tiny net's activations are not damped layer by layer as with
     # SiLU: its fp16 noise at the head is ~50x larger, so its head gain is 0.3, its objectness / class biases (-0.2) set the operating
     # point and its box biases sit at -3, where the xywh sigmoids are flat (box noise 0.4 px -> 0.01 px).  CPU fp16 emulation on
@@ -268,7 +288,7 @@ SYNTH_PROFILES_WORKLOAD = {
 
 
 def synth_weights(kind: str, seed: int = 0, variant: Optional[str] = None, workload: bool = False) -> "Weights":
-    """Seeded synthetic weights.  A profile's `variants` entry (YOLOv6, YOLOv9) adds per-variant `fill` rules ahead of the shared ones; other
+    """Seeded synthetic weights.  A profile's `variants` entry (YOLOv6, YOLOv9, YOLOv10) adds per-variant `fill` rules ahead of the shared ones; other
     kinds ignore `variant`."""
     prof = SYNTH_PROFILES_WORKLOAD.get(kind, SYNTH_PROFILES[kind]) if workload else SYNTH_PROFILES[kind]
     extra = prof.get("variants", {}).get(variant)
@@ -299,6 +319,7 @@ class PlanBuilder:
         self.meta = [0] * 16
         self.flops_per_img = 0   # 2*MAC of the convs/FCs as mathematically defined (no padding waste)
         self.stem_flops_per_img = 0   # the part of flops_per_img that runs in stem_conv.cu (mma.sync) rather than in the wgmma GEMM launches
+        self.dw_flops_per_img = 0     # the part of flops_per_img that runs in dwconv.cu (depthwise convs) rather than in the GEMM launches
         self.stem_direct = os.environ.get("ADAS_B200_STEMCONV", "1") != "0"
         self.strided_tma = os.environ.get("ADAS_B200_STRIDED_TMA", "1") != "0"
         # buffer 0: the network input image, padded NHWC with C=4 (R,G,B,0)
@@ -461,6 +482,41 @@ class PlanBuilder:
         assert out.H == x.H and out.W == x.W and x.C % 8 == 0 and x.coff % 8 == 0 and out.coff % 8 == 0 and fill in (0, 1)
         self._op(OP_AVGPOOL2, [x.buf, x.coff, x.C, out.buf, out.coff, fill])
         return View(out.buf, out.coff, x.C, x.H, x.W)
+
+    def dwconv(self, x: View, w: np.ndarray, b: np.ndarray, k: int, s: int, act: int, out: Optional[View] = None,
+               res: Optional[View] = None) -> View:
+        """Depthwise k x k conv (pad k/2; k 3 stride 1 / 2, k 7 stride 1) of x's channels: w [C_real, 1, k, k] fp32, b [C_real];
+        x.C may exceed C_real (zero-padded channels get zero weights and bias).  out = act(conv + b) (+ res).  Weights are packed
+        [k*k][C] fp16 so one tap of 8 channels is one 16-byte load (dwconv.cu)."""
+        c_real = int(w.shape[0])
+        assert w.shape[1:] == (1, k, k) and c_real <= x.C and x.C % 8 == 0 and x.coff % 8 == 0, (w.shape, x)
+        assert (k == 3 and s in (1, 2)) or (k == 7 and s == 1), (k, s)
+        Ho = (x.H + 2 * (k // 2) - k) // s + 1
+        Wo = (x.W + 2 * (k // 2) - k) // s + 1
+        if out is None:
+            out = self.new_padded(Ho, Wo, x.C)
+        assert out.H == Ho and out.W == Wo and out.coff % 8 == 0, (out, Ho, Wo)
+        assert res is None or (res.H == Ho and res.W == Wo and res.coff % 8 == 0), res
+        wk = np.zeros((k * k, x.C), np.float32)
+        wk[:, :c_real] = w.reshape(c_real, k * k).T
+        bk = np.zeros(x.C, np.float32)
+        bk[:c_real] = b
+        f = 2 * Ho * Wo * c_real * k * k
+        self.flops_per_img += f
+        self.dw_flops_per_img += f
+        self._op(OP_DWCONV, [x.buf, x.coff, x.C, k, s, act, self.tensor(wk.astype(np.float16)), self.tensor(bk), out.buf, out.coff,
+                             res.buf if res is not None else -1, res.coff if res is not None else 0])
+        return View(out.buf, out.coff, x.C, Ho, Wo)
+
+    def attention(self, qkv: View, nh: int, kdp: int, hd: int, scale: float, out: Optional[View] = None) -> View:
+        """Multi-head self-attention over the H*W pixels (attention.cu).  qkv holds [Q nh*kdp | K nh*kdp | V nh*hd] channels; the
+        output holds nh*hd channels, head-major: softmax(Q K^T * scale) V of head h in channels [h*hd, (h+1)*hd)."""
+        assert qkv.C == nh * (2 * kdp + hd) and kdp % 16 == 0 and hd % 8 == 0 and qkv.coff % 8 == 0 and math.isfinite(scale) and scale > 0
+        if out is None:
+            out = self.new_padded(qkv.H, qkv.W, nh * hd)
+        assert out.H == qkv.H and out.W == qkv.W and out.coff % 8 == 0, out
+        self._op(OP_ATTN, [qkv.buf, qkv.coff, nh, kdp, hd, out.buf, out.coff], [scale])
+        return View(out.buf, out.coff, nh * hd, qkv.H, qkv.W)
 
     def upsample2x(self, x: View, out: View) -> View:
         assert out.H == 2 * x.H and out.W == 2 * x.W and x.C % 8 == 0
@@ -1350,6 +1406,214 @@ def build_yolov9(weights: Weights, scale: str = "c", nc: int = 80, in_h: int = 6
     g.down("model.19", h18, d[4], out=pb.sub(cat20, 0, d[4]))
     h21 = g.elan("model.21", g.feat(cat20), *r[6])
     A = v8_detect(pb, weights, "model.22", (h15[0], h18[0], h21[0]), nc, box_groups=4, conv_bn=g.conv_bn)
+    pb.meta[0], pb.meta[1] = nc, A
+    return pb
+
+
+# ---------------------------------------------------------------------------------------------
+# YOLOv10 (ultralytics 8.2.41 `yolov10{n,s,m,b,l,x}.yaml`; the one-to-one head)
+# ---------------------------------------------------------------------------------------------
+# depth, width, max_channels; the C2f layers that are C2fCIB, mapped to lk (the 7x7 RepVGGDW in the CIB's middle conv)
+YOLOV10_SCALES = {"n": (0.33, 0.25, 1024), "s": (0.33, 0.50, 1024), "m": (0.67, 0.75, 768), "b": (0.67, 1.00, 512),
+                  "l": (1.00, 1.00, 512), "x": (1.00, 1.25, 512)}
+YOLOV10_CIB = {"n": {22: True}, "s": {8: True, 22: True}, "m": {8: False, 19: False, 22: False},
+               "b": {8: False, 13: False, 19: False, 22: False}, "l": {8: False, 13: False, 19: False, 22: False},
+               "x": {6: False, 8: False, 13: False, 19: False, 22: False}}
+
+
+def yolov10_conv_count(scale: str) -> int:
+    """Convolutions of the fused one-to-one graph (RepVGGDW as one conv; the fixed DFL conv not counted): stem and layers 1, 3, 17;
+    three SCDowns; SPPF; PSA (cv1, qkv, pe, proj, two ffn convs, cv2); the C2f / C2fCIB layers (cv1, cv2 and 2 convs per Bottleneck,
+    5 per CIB); the head (3 box and 5 class convs per level).  A training-form file has one more per RepVGGDW
+    (yolov10_repvggdw_count), one with the one-to-many head 24 more."""
+    depth = YOLOV10_SCALES[scale][0]
+    cibs = YOLOV10_CIB[scale]
+    reps = {2: 3, 4: 6, 6: 6, 8: 3, 13: 3, 16: 3, 19: 3, 22: 3}
+    c2f = sum(2 + _v8_n(n, depth) * (5 if li in cibs else 2) for li, n in reps.items())
+    return 4 + 3 * 2 + 2 + 7 + c2f + 3 * 8
+
+
+def yolov10_repvggdw_count(scale: str) -> int:
+    depth = YOLOV10_SCALES[scale][0]
+    return sum(_v8_n(3, depth) for lk in YOLOV10_CIB[scale].values() if lk)     # every C2fCIB layer repeats 3 (x depth) blocks
+
+
+def yolov10_attention_dims(c: int) -> Tuple[int, int, int, int]:
+    """PSA Attention(dim = c): (heads, key dim, head dim, key dim padded to 16) -- nh = c // 64, hd = c // nh, kd = hd // 2."""
+    nh = c // 64
+    hd = c // nh
+    kd = hd // 2
+    return nh, kd, hd, (kd + 15) // 16 * 16
+
+
+class Yolov10Packer:
+    """The YOLOv10 blocks on a PlanBuilder.  Conv = Conv2d + BatchNorm (eps 1e-3) folded in fp64, or a Conv fused upstream (`conv.bias`,
+    no `bn`) taken as it is.  Depthwise convs run as OP_DWCONV, PSA's attention as OP_ATTN; everything else is the GEMM."""
+
+    def __init__(self, pb: PlanBuilder, W: Weights):
+        self.pb, self.W = pb, W
+
+    def conv_bn(self, name: str, cout: int, cin: int, k: int, res_branch: bool = False):
+        W = self.W
+        if W.real and f"{name}.conv.bias" in W.state_dict and f"{name}.bn.weight" not in W.state_dict:
+            return W.conv_bias(f"{name}.conv", cout, cin, k)
+        return W.conv_bn(name, cout, cin, k, BN_EPS_YOLO, res_branch=res_branch)
+
+    def cbs(self, x: View, name: str, cout: int, k: int, s: int = 1, act: int = ACT_SILU, out: Optional[View] = None,
+            res: Optional[View] = None, cin: Optional[int] = None) -> View:
+        w, b = self.conv_bn(name, cout, cin if cin is not None else x.C, k, res_branch=res is not None)
+        return self.pb.conv(x, w, b, k, s, act, out=out, res=res)
+
+    def dw(self, x: View, name: str, c: int, k: int, s: int = 1, act: int = ACT_SILU, out: Optional[View] = None,
+           res: Optional[View] = None) -> View:
+        w, b = self.conv_bn(name, c, 1, k, res_branch=res is not None)
+        return self.pb.dwconv(x, w, b, k, s, act, out=out, res=res)
+
+    def repvggdw(self, x: View, name: str, c: int) -> View:
+        """RepVGGDW as one folded depthwise 7x7 with SiLU (Weights.repvggdw)."""
+        w, b = self.W.repvggdw(name, c, BN_EPS_YOLO)
+        return self.pb.dwconv(x, w, b, 7, 1, ACT_SILU)
+
+    def scdown(self, x: View, name: str, c2: int, out: Optional[View] = None) -> View:
+        """SCDown: 1x1 Conv (c1 -> c2), then a 3x3 stride-2 depthwise Conv without activation."""
+        t = self.cbs(x, f"{name}.cv1", c2, 1)
+        return self.dw(t, f"{name}.cv2", c2, 3, 2, act=ACT_NONE, out=out)
+
+    def cib(self, x: View, name: str, c: int, shortcut: bool, lk: bool, out: Optional[View] = None) -> View:
+        """CIB(c, c, e=1): x (+) [dw3x3, 1x1 c->2c, (RepVGGDW 7x7 | dw3x3), 1x1 2c->c, dw3x3], every conv SiLU."""
+        t = self.dw(x, f"{name}.cv1.0", c, 3)
+        t = self.cbs(t, f"{name}.cv1.1", 2 * c, 1)
+        t = self.repvggdw(t, f"{name}.cv1.2", 2 * c) if lk else self.dw(t, f"{name}.cv1.2", 2 * c, 3)
+        t = self.cbs(t, f"{name}.cv1.3", c, 1)
+        return self.dw(t, f"{name}.cv1.4", c, 3, out=out, res=x if shortcut else None)
+
+    def c2f(self, x: View, name: str, c2: int, n: int, shortcut: bool, cib: Optional[bool] = None, out: Optional[View] = None) -> View:
+        """C2f (cib None) or C2fCIB (cib = lk): cv2(cat(chunk0, chunk1, m0(chunk1), m1(m0(...)), ...))."""
+        pb = self.pb
+        c = c2 // 2
+        cat = pb.new_padded(x.H, x.W, (2 + n) * c)
+        self.cbs(x, f"{name}.cv1", 2 * c, 1, out=pb.sub(cat, 0, 2 * c))
+        for i in range(n):
+            src, dst = pb.sub(cat, (1 + i) * c, c), pb.sub(cat, (2 + i) * c, c)
+            if cib is None:
+                t = self.cbs(src, f"{name}.m.{i}.cv1", c, 3)
+                self.cbs(t, f"{name}.m.{i}.cv2", c, 3, out=dst, res=src if shortcut else None)
+            else:
+                self.cib(src, f"{name}.m.{i}", c, shortcut, cib, out=dst)
+        return self.cbs(cat, f"{name}.cv2", c2, 1, out=out)
+
+    def psa(self, x: View, name: str, out: Optional[View] = None) -> View:
+        """PSA(c1): a, b = cv1(x).split(c); b += attn(b); b += ffn(b); cv2(cat(a, b)).  attn(b) = proj(attention(q, k, v) + pe(v)):
+        the qkv conv's rows are permuted from upstream's per-head [q kd | k kd | v hd] into [Q all heads | K all heads | V all heads],
+        each q / k padded to kdp rows with zero weights and biases; V then is the c-channel tensor upstream's pe conv reads."""
+        pb, c1 = self.pb, x.C
+        c = c1 // 2
+        nh, kd, hd, kdp = yolov10_attention_dims(c)
+        ab = pb.new_padded(x.H, x.W, 2 * c)
+        self.cbs(x, f"{name}.cv1", 2 * c, 1, out=ab)
+        b = pb.sub(ab, c, c)
+        w, bias = self.conv_bn(f"{name}.attn.qkv", c + 2 * nh * kd, c, 1)
+        wq, bq = qkv_permute(w, bias, nh, kd, hd)
+        f0 = pb.flops_per_img
+        qkv = pb.conv(b, wq, bq, 1, 1, ACT_NONE)
+        pb.flops_per_img = f0 + 2 * x.H * x.W * (c + 2 * nh * kd) * c           # the kdp - kd zero rows are not counted
+        att = pb.attention(qkv, nh, kdp, hd, float(kd) ** -0.5)
+        u = self.dw(pb.sub(qkv, 2 * nh * kdp, c), f"{name}.attn.pe", c, 3, act=ACT_NONE, res=att)
+        b2 = self.cbs(u, f"{name}.attn.proj", c, 1, act=ACT_NONE, res=b)
+        f = self.cbs(b2, f"{name}.ffn.0", 2 * c, 1)
+        self.cbs(f, f"{name}.ffn.1", c, 1, act=ACT_NONE, out=b, res=b2)
+        return self.cbs(ab, f"{name}.cv2", c1, 1, out=out)
+
+
+def qkv_permute(w: np.ndarray, b: np.ndarray, nh: int, kd: int, hd: int) -> Tuple[np.ndarray, np.ndarray]:
+    """Rows of PSA's qkv conv from upstream's per-head [q kd | k kd | v hd] order into [Q | K | V], all heads each, q / k padded to
+    kdp = round_up(kd, 16) rows per head with zero weights and biases (zeros change no q . k product)."""
+    kdp = (kd + 15) // 16 * 16
+    per = 2 * kd + hd
+    assert w.shape[0] == nh * per, (w.shape, nh, kd, hd)
+    wo = np.zeros((nh * (2 * kdp + hd),) + w.shape[1:], np.float32)
+    bo = np.zeros(nh * (2 * kdp + hd), np.float32)
+    for h in range(nh):
+        src = h * per
+        for part, (s0, n, d0) in enumerate(((0, kd, h * kdp), (kd, kd, nh * kdp + h * kdp), (2 * kd, hd, 2 * nh * kdp + h * hd))):
+            wo[d0:d0 + n] = w[src + s0:src + s0 + n]
+            bo[d0:d0 + n] = b[src + s0:src + s0 + n]
+    return wo, bo
+
+
+def v10_detect(pb: PlanBuilder, g: Yolov10Packer, name: str, feats, nc: int) -> int:
+    """YOLOv10 v10Detect, the one-to-one branch (`one2one_cv2` / `one2one_cv3`) on the P3 / P4 / P5 views; returns the anchor count.
+    Writes YOLOv8's f32 head buffers and outputs ([64 DFL logits | nc class logits] per pixel), so the kind-0 decode reads them.  The box
+    branch is YOLOv8's; the class branch is [dw3x3, 1x1 -> c3], [dw3x3, 1x1 c3 -> c3], 1x1 -> nc, c3 = max(ch0, min(nc, 100))."""
+    reg_max = 16
+    cb = max(16, feats[0].C // 4, reg_max * 4)
+    c3 = max(feats[0].C, min(nc, 100))
+    A = 0
+    for li, (feat, stride) in enumerate(zip(feats, (8, 16, 32))):
+        cin = feat.C
+        b2, b3 = f"{name}.one2one_cv2.{li}", f"{name}.one2one_cv3.{li}"
+        head = pb.new_padded(feat.H, feat.W, 4 * reg_max + (nc + 7) // 8 * 8, f32=True)
+        tb = g.cbs(g.cbs(feat, f"{b2}.0", cb, 3), f"{b2}.1", cb, 3)
+        wbx, bbx = g.W.conv_bias(f"{b2}.2", 4 * reg_max, cb, 1)
+        pb.conv(tb, wbx, bbx, 1, 1, ACT_NONE, out=pb.sub(head, 0, 4 * reg_max), out_f32=True)
+        r8 = lambda v: View(v.buf, v.coff, (v.C + 7) // 8 * 8, v.H, v.W)     # c3 may not be a multiple of 8: zero channels follow
+        t = r8(g.cbs(g.dw(feat, f"{b3}.0.0", cin, 3), f"{b3}.0.1", c3, 1))
+        t = r8(g.cbs(g.dw(t, f"{b3}.1.0", c3, 3), f"{b3}.1.1", c3, 1, cin=c3))
+        wcl, bcl = g.W.conv_bias(f"{b3}.2", nc, c3, 1)
+        pb.conv(t, wcl, bcl, 1, 1, ACT_NONE, out=pb.sub(head, 4 * reg_max, (nc + 7) // 8 * 8), out_f32=True)
+        pb.outputs.append((head.buf, 0, head.C, stride))
+        A += feat.H * feat.W
+    return A
+
+
+def build_yolov10(weights: Weights, scale: str = "n", nc: int = 80, in_h: int = 640, in_w: int = 640) -> PlanBuilder:
+    """YOLOv10-N / S / M / B / L / X (upstream `model.<i>` names, head `model.23`) with the one-to-one head; the one-to-many head's
+    keys are never read.  The output and its decode are YOLOv8's ([B, 4 + nc, A], MODEL_YOLOV8 kind), not upstream's top-k tail.
+    Inputs are multiples of 32."""
+    assert scale in YOLOV10_SCALES, f"YOLOv10 scale {scale!r}: one of {sorted(YOLOV10_SCALES)}"
+    assert in_h % 32 == 0 and in_w % 32 == 0, f"YOLOv10 input {in_h}x{in_w}: a multiple of 32"
+    depth, width, max_ch = YOLOV10_SCALES[scale]
+    cibs = YOLOV10_CIB[scale]
+    ch = lambda c: _v8_ch(c, width, max_ch)
+    rep = lambda n: _v8_n(n, depth)
+    pb = PlanBuilder(MODEL_YOLOV8, 3, in_h, in_w)
+    g = Yolov10Packer(pb, weights)
+
+    def c2f(x, li, c2, n, shortcut, out=None):
+        return g.c2f(x, f"model.{li}", c2, n, shortcut or li in cibs, cibs.get(li), out=out)
+
+    c1, c2_, c3, c4, c5 = ch(64), ch(128), ch(256), ch(512), ch(1024)
+    H, Wd = in_h, in_w
+    cat12 = pb.new_padded(H // 16, Wd // 16, c5 + c4)      # [up(10), 6]
+    cat15 = pb.new_padded(H // 8, Wd // 8, c4 + c3)        # [up(13), 4]
+    cat18 = pb.new_padded(H // 16, Wd // 16, c3 + c4)      # [17, 13]
+    cat21 = pb.new_padded(H // 32, Wd // 32, c4 + c5)      # [20, 10]
+
+    x = g.cbs(pb.image, "model.0", c1, 3, 2, cin=3)
+    x = g.cbs(x, "model.1", c2_, 3, 2)
+    x = c2f(x, 2, c2_, rep(3), True)
+    x = g.cbs(x, "model.3", c3, 3, 2)
+    p3 = c2f(x, 4, c3, rep(6), True, out=pb.sub(cat15, c4, c3))
+    x = g.scdown(p3, "model.5", c4)
+    p4 = c2f(x, 6, c4, rep(6), True, out=pb.sub(cat12, c5, c4))
+    x = g.scdown(p4, "model.7", c5)
+    x = c2f(x, 8, c5, rep(3), True)
+    ch_ = c5 // 2                                           # SPPF
+    sp = pb.new_padded(x.H, x.W, 4 * ch_)
+    y = g.cbs(x, "model.9.cv1", ch_, 1, out=pb.sub(sp, 0, ch_))
+    for i in range(3):
+        y = pb.maxpool(y, 5, 1, 2, out=pb.sub(sp, (i + 1) * ch_, ch_))
+    x = g.cbs(sp, "model.9.cv2", c5, 1)
+    p5 = g.psa(x, "model.10", out=pb.sub(cat21, c4, c5))
+    pb.upsample2x(p5, pb.sub(cat12, 0, c5))
+    h13 = c2f(cat12, 13, c4, rep(3), False, out=pb.sub(cat18, c3, c4))
+    pb.upsample2x(h13, pb.sub(cat15, 0, c4))
+    h16 = c2f(cat15, 16, c3, rep(3), False)
+    g.cbs(h16, "model.17", c3, 3, 2, out=pb.sub(cat18, 0, c3))
+    h19 = c2f(cat18, 19, c4, rep(3), False)
+    g.scdown(h19, "model.20", c4, out=pb.sub(cat21, 0, c4))
+    h22 = c2f(cat21, 22, c5, rep(3), False)
+    A = v10_detect(pb, g, "model.23", (h16, h19, h22), nc)
     pb.meta[0], pb.meta[1] = nc, A
     return pb
 

@@ -229,36 +229,44 @@ int launch_upsample2x(const __half* in, int in_ld, int B, int H, int W, int C, _
 }
 
 // ---- LayerNorm over a feature row (one CTA per row), fp32 statistics ------------------------------
+// Block-wide sum in a fixed order (per-thread strided run, xor tree over lanes, then over warps): every row is reduced by the same
+// instruction sequence whatever the batch.
+__device__ __forceinline__ float block_sum(float v, float* red) {
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+    __syncthreads();                                   // red is free (a previous block_sum has been read)
+    if (l == 0) red[w] = v;
+    __syncthreads();
+    if (w == 0) {
+        v = (l < (int)(blockDim.x >> 5)) ? red[l] : 0.f;
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if (l == 0) red[32] = v;
+    }
+    __syncthreads();
+    return red[32];
+}
+
+// Two passes over the row (at most a few KB, L1-resident): the mean, then the sum of (x - mean)^2.  A one-pass E[x^2] - mean^2
+// cancels catastrophically when |mean| >> std (its error grows with (mean / std)^2).  The D - Dn structural entries are exact
+// zeros scattered through the row, so the second pass sums the nonzero entries and adds mean^2 once per zero entry that is not
+// structural (zeros counted exactly): every term is non-negative, nothing cancels.
 __global__ void layernorm_kernel(const __half* __restrict__ in, int in_ld, int D, int Dn, const float* __restrict__ gamma,
                                  const float* __restrict__ beta, float eps, __half* __restrict__ out, int out_ld) {
     const int row = blockIdx.x;
     const __half* x = in + (size_t)row * in_ld;
-    __shared__ float red[2][32];
-    float s = 0.f, ss = 0.f;
+    __shared__ float red[33];
+    float s = 0.f;
+    for (int i = threadIdx.x; i < D; i += blockDim.x) s += __half2float(x[i]);
+    const float mean = block_sum(s, red) / Dn;
+    float ss = 0.f, nz = 0.f;
     for (int i = threadIdx.x; i < D; i += blockDim.x) {
         const float v = __half2float(x[i]);
-        s += v;
-        ss += v * v;
+        if (v != 0.f) { const float d = v - mean; ss = fmaf(d, d, ss); }
+        else nz += 1.f;
     }
-    for (int o = 16; o > 0; o >>= 1) {
-        s += __shfl_xor_sync(0xffffffffu, s, o);
-        ss += __shfl_xor_sync(0xffffffffu, ss, o);
-    }
-    const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-    if (l == 0) { red[0][w] = s; red[1][w] = ss; }
-    __syncthreads();
-    if (w == 0) {
-        s = (l < (int)(blockDim.x >> 5)) ? red[0][l] : 0.f;
-        ss = (l < (int)(blockDim.x >> 5)) ? red[1][l] : 0.f;
-        for (int o = 16; o > 0; o >>= 1) {
-            s += __shfl_xor_sync(0xffffffffu, s, o);
-            ss += __shfl_xor_sync(0xffffffffu, ss, o);
-        }
-        if (l == 0) { red[0][0] = s; red[1][0] = ss; }
-    }
-    __syncthreads();
-    const float mean = red[0][0] / Dn;
-    const float var = fmaxf(red[1][0] / Dn - mean * mean, 0.f);
+    ss = block_sum(ss, red);
+    const float zeros = fmaxf(block_sum(nz, red) - (float)(D - Dn), 0.f);     // exact: counts < 2^24
+    const float var = fmaf(zeros, mean * mean, ss) / Dn;
     const float rstd = rsqrtf(var + eps);
     for (int i = threadIdx.x; i < D; i += blockDim.x) {
         const float v = (__half2float(x[i]) - mean) * rstd * gamma[i] + beta[i];

@@ -359,7 +359,12 @@ class PlanBuilder:
         res_scale: out = act(conv) + res_scale * res (YOLOv6 BottleRep's alpha); None = a plain residual add (op f[0] = 0).
         no_slab (test hook): a 3x3 stride-1 conv loads one activation tile per tap instead of one slab per (dy, k-block).
         wide_stem: an 80 / 96-channel image conv also runs in stem_conv.cu (the YOLOv7 P6 stems); without it those widths keep the
-        im2col + GEMM route, so the 80-channel stems of YOLOv5x / YOLOv8x pack as before."""
+        im2col + GEMM route, so the 80-channel stems of YOLOv5x / YOLOv8x pack as before.
+        Cout % 8 != 0: the epilogue stores 8-channel vectors, so the conv owns n_store = round_up(Cout, 8) channels
+        [out.coff, out.coff + n_store) of `out` (a concat neighbour starts at out.coff + n_store); channels [Cout, n_store) hold
+        act(0) = 0 (zero weights and bias) plus the residual's channels [Cout, n_store).  A residual therefore owns n_store channels
+        too, with zeros past Cout -- as every output of such a conv has, so a residual written by a conv of the same Cout (the
+        YOLOv9 GELAN blocks) keeps the tail exactly zero."""
         assert res_scale is None or (res is not None and not res_pre_act and math.isfinite(res_scale) and res_scale != 0.0), res_scale
         cout, cin_real = int(w.shape[0]), int(w.shape[1])
         pad = k // 2 if pad is None else pad

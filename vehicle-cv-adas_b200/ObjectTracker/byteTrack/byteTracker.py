@@ -111,7 +111,7 @@ class BYTETracker(ObjectTrackBase):
         cnt = self._capi.NativeTracker.count()
         return [t.get_track_message(cnt) for t in self.tracked_stracks]
 
-    def update_batch(self, frames_dets, max_out: int = 256):
+    def update_batch(self, frames_dets):
         """All frames of a pipeline step in ONE library call (no interpreter work between frames).
         frames_dets: sequence of (bboxes xyxy [n,4], scores [n], class_ids [n]) per frame, in time order.
         Returns one TRACK_DTYPE record array per frame (the tracked_stracks of that frame); `messages(recs)` turns a record array into
@@ -128,13 +128,13 @@ class BYTETracker(ObjectTrackBase):
                 scores[o:o + n] = np.asarray(sc, dtype=np.float64)
                 ids[o:o + n] = [self._cid(c) for c in (cl.tolist() if hasattr(cl, "tolist") else cl)]
             o += n
-        recs = self._nt.update_batch(counts, boxes, scores, ids, max_out)
+        recs = self._nt.update_batch(counts, boxes, scores, ids)
         self.frame_id += len(frames_dets)
         if recs:
             self.tracked_stracks = [self._view(r, None) for r in recs[-1]]
         return recs
 
-    def update_batch_arrays(self, counts, xyxy, scores, class_ids, max_out: int = 256):
+    def update_batch_arrays(self, counts, xyxy, scores, class_ids):
         """update_batch on already concatenated arrays (the pipeline's hot path): counts [F] int, xyxy [sum, 4], scores [sum],
         class_ids [sum] integer labels.  Labels are mapped to the tracker's class slots in first-seen order like `update` does."""
         cl = np.asarray(class_ids)
@@ -146,7 +146,7 @@ class BYTETracker(ObjectTrackBase):
             ids = lut[np.searchsorted(uniq, cl)]
         else:
             ids = np.zeros(0, np.int32)
-        recs = self._nt.update_batch(counts, xyxy, scores, ids, max_out)
+        recs = self._nt.update_batch(counts, xyxy, scores, ids)
         self.frame_id += len(counts)
         if recs:
             self.tracked_stracks = [self._view(r, None) for r in recs[-1]]

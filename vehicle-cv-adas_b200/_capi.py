@@ -71,8 +71,9 @@ assert TRACK_DTYPE.itemsize == C.sizeof(TrackRec)
 
 
 class NativeTracker:
-    """Owns one adas_tracker handle (native ByteTrack; association stages on the device)."""
-    MAX_OUT = 1024
+    """Owns one adas_tracker handle (native ByteTrack; association stages on the device).  Every call returns every record: the
+    output rows grow with the number of tracks, there is no track limit."""
+    MAX_OUT = 1024                      # initial rows of the per-frame output buffer
 
     def __init__(self, device=0, track_thresh=0.5, track_buffer=30, match_thresh=0.8, frame_rate=30):
         self._h = C.c_void_p()
@@ -99,9 +100,16 @@ class NativeTracker:
         s = as_c(scores, np.float64)
         c = as_c(class_ids, np.int32)
         n = C.c_int()
-        check(lib().adas_tracker_update(self._h, int(b.shape[0]), _p(b, C.c_double), _p(s, C.c_double), _p(c, C.c_int32), self.MAX_OUT,
+        check(lib().adas_tracker_update(self._h, int(b.shape[0]), _p(b, C.c_double), _p(s, C.c_double), _p(c, C.c_int32), len(self._out),
                                         self._out.ctypes.data_as(C.c_void_p), C.byref(n)))
-        return self._out[:min(n.value, self.MAX_OUT)].copy()
+        if n.value > len(self._out):    # more tracks than rows: the update is done, read the tracked list again (no second update)
+            return self.get(0)
+        return self._out[:n.value].copy()
+
+    def _count(self, which: int) -> int:
+        n = C.c_int()
+        check(lib().adas_tracker_get(self._h, which, 0, None, C.byref(n)))
+        return int(n.value)
 
     def stats(self):
         """{frames, total_ms, wait_ms, launches} of update_batch since creation (wait_ms = launch -> result of the association kernel)."""
@@ -109,25 +117,31 @@ class NativeTracker:
         check(lib().adas_tracker_stats(self._h, o))
         return {"frames": int(o[0]), "total_ms": float(o[1]), "wait_ms": float(o[2]), "launches": int(o[3])}
 
-    def update_batch(self, counts, boxes_xyxy, scores, class_ids, max_out: int = 256):
-        """All frames of a step in one library call -> list (per frame) of TRACK_DTYPE record arrays."""
+    def update_batch(self, counts, boxes_xyxy, scores, class_ids):
+        """All frames of a step in one library call -> list (per frame) of TRACK_DTYPE record arrays.
+        The output rows per frame are sized from a bound that always holds: the tracks after frame f are at most the tracks tracked
+        before the call plus the detections of frames 0..f.  So the call never runs out of rows after the tracker has advanced."""
         cnt = as_c(counts, np.int32)
         nf = int(cnt.shape[0])
         b = as_c(np.asarray(boxes_xyxy, np.float64).reshape(-1, 4), np.float64)
         s = as_c(scores, np.float64)
         c = as_c(class_ids, np.int32)
+        max_out = max(1, self._count(0) + int(cnt.sum()))
         out = np.zeros((nf, max_out), TRACK_DTYPE)
         n_out = np.zeros(nf, np.int32)
         check(lib().adas_tracker_update_batch(self._h, nf, _p(cnt, C.c_int32), _p(b, C.c_double), _p(s, C.c_double), _p(c, C.c_int32), int(max_out),
                                               out.ctypes.data_as(C.c_void_p), _p(n_out, C.c_int32)))
-        if int(n_out.max(initial=0)) > max_out:          # rare: more live tracks than the caller-sized output rows; redo nothing, tell the caller
-            raise Exception(f"adas_tracker_update_batch: {int(n_out.max())} tracks exceed max_out {max_out}")
+        if int(n_out.max(initial=0)) > max_out:
+            raise Exception(f"adas_tracker_update_batch: {int(n_out.max())} tracks exceed the row bound {max_out}")
         return [out[f, :int(n_out[f])] for f in range(nf)]
 
     def get(self, which: int) -> np.ndarray:
-        n = C.c_int()
-        check(lib().adas_tracker_get(self._h, which, self.MAX_OUT, self._out.ctypes.data_as(C.c_void_p), C.byref(n)))
-        return self._out[:min(n.value, self.MAX_OUT)].copy()
+        """records of the tracked (0), lost (1) or removed (2) list"""
+        n = self._count(which)
+        if n > len(self._out):
+            self._out = np.zeros(max(n, 2 * len(self._out)), TRACK_DTYPE)
+        check(lib().adas_tracker_get(self._h, which, len(self._out), self._out.ctypes.data_as(C.c_void_p), C.byref(C.c_int())))
+        return self._out[:n].copy()
 
     @staticmethod
     def count() -> int:

@@ -66,13 +66,13 @@ __device__ __forceinline__ double lap_cost(const double* C, int D, int T, double
 }
 
 // Exact assignment of one problem by ONE WARP (all 32 lanes call it together).  C: T x D cost matrix; X[T] / Y[D] receive the matched
-// column / row or -1.  Scratch: v, minv (m + 1 doubles), p / way / used (3 x (LAP_MAX_COLS + 1) int32), u (shared, T + 1 doubles).
+// column / row or -1.  Scratch: v, minv (m + 1 doubles), p / way / used (3 x ws int32, ws >= m + 1), u (T + 1 doubles).
 __device__ void lap_solve(const double* __restrict__ C, int T, int D, double thresh, int32_t* __restrict__ X, int32_t* __restrict__ Y,
-                          double* __restrict__ v, double* __restrict__ minv, int32_t* __restrict__ p, double* u) {
+                          double* __restrict__ v, double* __restrict__ minv, int32_t* __restrict__ p, int ws, double* u) {
     const int lane = threadIdx.x & 31;
     const int m = D + T;
-    int32_t* way = p + (LAP_MAX_COLS + 1);
-    int32_t* used = way + (LAP_MAX_COLS + 1);
+    int32_t* way = p + ws;
+    int32_t* used = way + ws;
     for (int j = lane; j <= m; j += 32) { v[j] = 0.0; p[j] = 0; way[j] = 0; }
     for (int i = lane; i <= T; i += 32) u[i] = 0.0;
     __syncwarp();
@@ -141,7 +141,7 @@ __global__ void lap_kernel(const double* __restrict__ cost, const int64_t* __res
     const int pr = blockIdx.x;
     __shared__ double u[LAP_MAX_COLS / 2 + 1];   // row potentials (T <= 1024)
     lap_solve(cost + cost_off[pr], Ts[pr], Ds[pr], threshs[pr], x + x_off[pr], y + y_off[pr], work_v + (size_t)pr * (LAP_MAX_COLS + 1),
-              work_minv + (size_t)pr * (LAP_MAX_COLS + 1), work_i + (size_t)pr * 3 * (LAP_MAX_COLS + 1), u);
+              work_minv + (size_t)pr * (LAP_MAX_COLS + 1), work_i + (size_t)pr * 3 * (LAP_MAX_COLS + 1), LAP_MAX_COLS + 1, u);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -161,10 +161,12 @@ __global__ void lap_kernel(const double* __restrict__ cost, const int64_t* __res
 // fence -- the host spins on that word (tracker.cu) instead of paying two copy-engine transfers and a stream synchronisation per frame.
 // Row potentials live in shared memory only up to ASSOC_SMEM_ROWS rows (1 KB): next to a conv CTA that holds ~224 KB of an SM's shared
 // memory this block still fits, so it starts at once instead of waiting for a conv CTA to retire; larger problems use global scratch.
+// The column scratch (v, minv: ws doubles; p / way / used: 3 x ws int32) is sized by the host for the largest stage of the frame
+// (ws > max(P + D, P + D2, U + D)), so the fused association has no size limit of its own -- like the reference.
 static constexpr int ASSOC_SMEM_ROWS = 120;
 
 __device__ void assoc3_body(const double* __restrict__ in, int32_t* __restrict__ out, double* __restrict__ cost, double* __restrict__ work_v,
-                            double* __restrict__ work_minv, int32_t* __restrict__ work_i, int32_t* __restrict__ lists, double* u) {
+                            double* __restrict__ work_minv, int32_t* __restrict__ work_i, int ws, int32_t* __restrict__ lists, double* u) {
     const int lane = threadIdx.x;
     const int P = (int)in[0], U = (int)in[1], D = (int)in[2], D2 = (int)in[3];
     const double match_thresh = in[4];
@@ -190,7 +192,7 @@ __device__ void assoc3_body(const double* __restrict__ in, int32_t* __restrict__
     if (P > 0 && D > 0) {
         for (int i = lane; i < P * D; i += 32) cost[i] = assoc_cost(pool, det, dsc, 1, i / D, i % D);
         __syncwarp();
-        lap_solve(cost, P, D, match_thresh, m1, ys, work_v, work_minv, work_i, u);
+        lap_solve(cost, P, D, match_thresh, m1, ys, work_v, work_minv, work_i, ws, u);
     }
     // rem = unmatched pool rows that are Tracked; left = unmatched detections (both ascending)
     int R = 0, L = 0;
@@ -207,7 +209,7 @@ __device__ void assoc3_body(const double* __restrict__ in, int32_t* __restrict__
         __syncwarp();
         for (int i = lane; i < R * D2; i += 32) cost[i] = assoc_cost(rbox, det2, nullptr, 0, i / D2, i % D2);
         __syncwarp();
-        lap_solve(cost, R, D2, 0.5, xs, ys, work_v, work_minv, work_i, u);
+        lap_solve(cost, R, D2, 0.5, xs, ys, work_v, work_minv, work_i, ws, u);
         for (int k = lane; k < R; k += 32) m2[rem[k]] = xs[k];
         __syncwarp();
     }
@@ -222,7 +224,7 @@ __device__ void assoc3_body(const double* __restrict__ in, int32_t* __restrict__
         __syncwarp();
         for (int i = lane; i < U * L; i += 32) cost[i] = assoc_cost(unconf, lbox, lsc, 1, i / L, i % L);
         __syncwarp();
-        lap_solve(cost, U, L, 0.7, xs, ys, work_v, work_minv, work_i, u);
+        lap_solve(cost, U, L, 0.7, xs, ys, work_v, work_minv, work_i, ws, u);
         for (int k = lane; k < U; k += 32) m3[k] = xs[k] >= 0 ? left[xs[k]] : -1;
         for (int j = lane; j < L; j += 32) if (ys[j] < 0) free3[left[j]] = 1;
     } else {
@@ -232,14 +234,14 @@ __device__ void assoc3_body(const double* __restrict__ in, int32_t* __restrict__
 
 __global__ void assoc3_kernel(const double* __restrict__ in_host, int n_in, double* __restrict__ in_dev, int32_t* __restrict__ out_host, int n_out,
                               int32_t* __restrict__ out_dev, volatile int32_t* done_host, int32_t seq, double* __restrict__ cost,
-                              double* __restrict__ work_v, double* __restrict__ work_minv, int32_t* __restrict__ work_i, int32_t* __restrict__ lists,
-                              double* __restrict__ work_u) {
+                              double* __restrict__ work_v, double* __restrict__ work_minv, int32_t* __restrict__ work_i, int ws,
+                              int32_t* __restrict__ lists, double* __restrict__ work_u) {
     __shared__ double u_s[ASSOC_SMEM_ROWS + 1];
     const int lane = threadIdx.x;
     for (int i = lane; i < n_in; i += 32) in_dev[i] = in_host[i];
     __syncwarp();
     const int P = (int)in_dev[0], U = (int)in_dev[1];
-    assoc3_body(in_dev, out_dev, cost, work_v, work_minv, work_i, lists, (P <= ASSOC_SMEM_ROWS && U <= ASSOC_SMEM_ROWS) ? u_s : work_u);
+    assoc3_body(in_dev, out_dev, cost, work_v, work_minv, work_i, ws, lists, (P <= ASSOC_SMEM_ROWS && U <= ASSOC_SMEM_ROWS) ? u_s : work_u);
     __syncwarp();
     for (int i = lane; i < n_out; i += 32) out_host[i] = out_dev[i];
     __threadfence_system();
@@ -248,8 +250,8 @@ __global__ void assoc3_kernel(const double* __restrict__ in_host, int n_in, doub
 }
 
 int launch_assoc3(const double* in_host, int n_in, double* in_dev, int32_t* out_host, int n_out, int32_t* out_dev, int32_t* done_host, int32_t seq,
-                  double* cost, double* work_v, double* work_minv, int32_t* work_i, int32_t* lists, double* work_u, cudaStream_t st) {
-    assoc3_kernel<<<1, 32, 0, st>>>(in_host, n_in, in_dev, out_host, n_out, out_dev, done_host, seq, cost, work_v, work_minv, work_i, lists, work_u);
+                  double* cost, double* work_v, double* work_minv, int32_t* work_i, int ws, int32_t* lists, double* work_u, cudaStream_t st) {
+    assoc3_kernel<<<1, 32, 0, st>>>(in_host, n_in, in_dev, out_host, n_out, out_dev, done_host, seq, cost, work_v, work_minv, work_i, ws, lists, work_u);
     count_launch();
     ADAS_CUDA(cudaGetLastError());
     return 0;

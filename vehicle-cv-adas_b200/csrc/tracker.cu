@@ -24,7 +24,7 @@ int launch_lap(int problems, const double* cost, const int64_t* cost_off, const 
                double* work_minv, int32_t* work_i, cudaStream_t st);
 int lap_max_cols();
 int launch_assoc3(const double* in_host, int n_in, double* in_dev, int32_t* out_host, int n_out, int32_t* out_dev, int32_t* done_host, int32_t seq,
-                  double* cost, double* work_v, double* work_minv, int32_t* work_i, int32_t* lists, double* work_u, cudaStream_t st);
+                  double* cost, double* work_v, double* work_minv, int32_t* work_i, int ws, int32_t* lists, double* work_u, cudaStream_t st);
 
 enum { ST_NEW = 0, ST_TRACKED = 1, ST_LOST = 2, ST_REMOVED = 3 };
 static std::atomic<int> g_track_count{0};          // BaseTrack._count: process-global (base_track.py:12,33-36)
@@ -141,6 +141,7 @@ struct adas_tracker {
     double* h3_in_dev = nullptr; int32_t* h3_out_dev = nullptr;   // their device-side addresses
     int32_t* h_done = nullptr; int32_t* h_done_dev = nullptr; int32_t seq = 0;   // completion word the host spins on
     double* d_u = nullptr;                                    // row potentials of problems beyond the kernel's shared-memory budget
+    size_t cap_ws = 0;                                        // entries of d_v / d_mv / d_u and of each third of d_wi (column scratch)
     // wall-clock accounting of the update path (adas_tracker_stats): frames, total ns, ns between launch and result, launches
     uint64_t st_frames = 0, st_total_ns = 0, st_wait_ns = 0, st_launches = 0;
     double* d3_in = nullptr; int32_t* d3_out = nullptr; double* d3_cost = nullptr; int32_t* d3_lists = nullptr;
@@ -160,6 +161,7 @@ static int ensure_scratch(adas_tracker* t, size_t nb, size_t nc) {
         ADAS_CUDA(cudaMalloc(&t->d_th, 8)); ADAS_CUDA(cudaMalloc(&t->d_v, wc * 8)); ADAS_CUDA(cudaMalloc(&t->d_mv, wc * 8));
         ADAS_CUDA(cudaMalloc(&t->d_wi, wc * 12)); ADAS_CUDA(cudaMalloc(&t->d_meta, 32)); ADAS_CUDA(cudaMalloc(&t->d_co, 16));
         ADAS_CUDA(cudaMalloc(&t->d_u, wc * 8));
+        t->cap_ws = wc;
         ADAS_CUDA(cudaHostAlloc(&t->h_done, 64, cudaHostAllocMapped));
         *t->h_done = 0;
         ADAS_CUDA(cudaHostGetDevicePointer(&t->h_done_dev, t->h_done, 0));
@@ -224,6 +226,16 @@ namespace adas {
 // scratch of the fused association, sized for this frame (called before any tracker state is touched)
 static int assoc3_prepare(adas_tracker* t, int P, int U, int D, int D2) {
     if (ensure_scratch(t, 1, 1)) return 1;
+    // column scratch of the largest stage: stage 1 is P x (D + P), stage 2 R x (D2 + R) with R <= P, stage 3 U x (D + U)
+    const size_t ws = (size_t)std::max({P + D, P + D2, U + D}) + 1;
+    if (ws > t->cap_ws) {
+        cudaFree(t->d_v); cudaFree(t->d_mv); cudaFree(t->d_wi); cudaFree(t->d_u);
+        t->d_v = t->d_mv = t->d_u = nullptr; t->d_wi = nullptr; t->cap_ws = 0;
+        const size_t wc = ws * 2;
+        ADAS_CUDA(cudaMalloc(&t->d_v, wc * 8)); ADAS_CUDA(cudaMalloc(&t->d_mv, wc * 8));
+        ADAS_CUDA(cudaMalloc(&t->d_wi, wc * 12)); ADAS_CUDA(cudaMalloc(&t->d_u, wc * 8));
+        t->cap_ws = wc;
+    }
     const size_t mr = (size_t)std::max(P, U), mc = (size_t)std::max(D, D2);
     const size_t n_in = 5 + (size_t)P * 5 + (size_t)U * 4 + (size_t)D * 5 + (size_t)D2 * 4, n_out = (size_t)2 * P + U + D + 4;
     const size_t n_cost = mr * mc + (size_t)D * 5 + (size_t)P * 4 + 8, n_lists = (size_t)P + D + mr + mc + 8;
@@ -275,7 +287,7 @@ static int assoc3_run(adas_tracker* t, const std::vector<TrackP>& pool, const st
     const int32_t seq = ++t->seq;
     const uint64_t w0 = now_ns();
     if (launch_assoc3(t->h3_in_dev, (int)n_in, t->d3_in, t->h3_out_dev, (int)n_out, t->d3_out, t->h_done_dev, seq, t->d3_cost, t->d_v, t->d_mv, t->d_wi,
-                      t->d3_lists, t->d_u, t->st)) return 1;
+                      (int)t->cap_ws, t->d3_lists, t->d_u, t->st)) return 1;
     {
         volatile int32_t* done = t->h_done;
         uint32_t spins = 0;
@@ -349,10 +361,9 @@ static int update_one(adas_tracker* t, int n, const double* boxes_xyxy, const do
     std::vector<TrackP> unconfirmed, confirmed;
     for (auto& x : t->tracked) (x->activated ? confirmed : unconfirmed).push_back(x);
     std::vector<TrackP> pool = joint(confirmed, t->lost);
-    // sizes are validated BEFORE any state is touched: a failed frame leaves the tracker exactly as it was (advisor finding, r01)
+    // the association has no size limit (its scratch grows with the frame, like the reference's); scratch is allocated BEFORE any
+    // state is touched, so a failed frame leaves the tracker exactly as it was
     const int P = (int)pool.size(), U = (int)unconfirmed.size(), D = (int)dets.size(), D2 = (int)dets2.size();
-    ADAS_CHECK(P + D <= lap_max_cols() && P + D2 <= lap_max_cols() && U + D <= lap_max_cols() && P <= lap_max_cols() / 2 && U <= lap_max_cols() / 2,
-               "tracker: association too large (pool %d, unconfirmed %d, detections %d + %d)", P, U, D, D2);
     std::vector<int32_t> m1, m2, m3, free3;
     const bool need_dev = (P > 0 || U > 0) && (D > 0 || D2 > 0);
     if (need_dev && assoc3_prepare(t, P, U, D, D2)) return 1;
@@ -405,8 +416,10 @@ static int update_one(adas_tracker* t, int n, const double* boxes_xyxy, const do
         for (size_t j = 0; j < nb; ++j) if (!db[j]) rb.push_back(t->lost[j]);
         t->tracked.swap(ra); t->lost.swap(rb);
     }
-    // removed tracks are never read again: keep only their ids' worth of memory bounded
-    if (t->removed.size() > 4096) t->removed.erase(t->removed.begin(), t->removed.begin() + 2048);
+    // keep `removed` bounded by trimming its oldest entries, but never this frame's: a lost track that aged out in this frame is still in
+    // `lost` until the next frame's sub(lost, removed) drops it
+    if (t->removed.size() > 4096)
+        t->removed.erase(t->removed.begin(), t->removed.begin() + std::min<size_t>(2048, t->removed.size() - removed_now.size()));
     int k = 0;
     for (auto& x : t->tracked) { if (out && k < max_out) fill_out(*x, &out[k]); ++k; }
     if (n_out) *n_out = k;

@@ -149,7 +149,8 @@ typedef struct adas_lane_geom {
     int32_t area_status;   /* LaneInfo.area_status: both ego lanes detected */
     int32_t n_area;        /* points of the ego-lane polygon: left ++ flipud(right) */
     int32_t n_bird[4];     /* bird-view points per lane (0 when no matrix was given) */
-    int32_t direction;     /* curvature_direction: -1 "L", 0 "F", 1 "R", 2 = None (an ego lane is missing) */
+    int32_t direction;     /* curvature_direction: -1 "L", 0 "F", 1 "R", 2 = None (an ego lane has fewer than 3 bird-view points,
+                              or bird_h < 720, where the reference's leftx[719] raises) */
     int32_t pad;
     double curvature;      /* metres; valid when direction != 2 */
     double offset;         /* distance_from_center, metres; valid when direction != 2 */
@@ -157,7 +158,8 @@ typedef struct adas_lane_geom {
 
 /* From host arrays shaped like adas_ufld_detect's outputs: pts [batch,4,max_pts,2] int32, npts [batch,4], status [batch,4].
  * M: [batch,9] row-major float64 frontal->bird-view matrices (PerspectiveTransformation.M after updateTransformParams) or NULL to
- * skip the bird view.  area: [batch,cap_area,2] (cap_area >= 2*max_pts, and >= 2*img_h with adjust_lanes), bird: [batch,4,max_pts,2]. */
+ * skip the bird view; with a matrix, bird_h may be at most 2160.  area: [batch,cap_area,2] (cap_area >= 2*max_pts, and >= 2*img_h
+ * with adjust_lanes), bird: [batch,4,max_pts,2]. */
 int adas_lane_geometry(int device, const int32_t* pts, const int32_t* npts, const uint8_t* status, int batch, int max_pts, int img_w,
                        int img_h, int adjust_lanes, const double* M, int bird_w, int bird_h, int32_t* area, int cap_area, int32_t* bird,
                        adas_lane_geom* out);

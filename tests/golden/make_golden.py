@@ -292,7 +292,84 @@ def gen_birdview():
     print("birdview.npz:", len(out), "arrays")
 
 
+def gen_lane_conformance():
+    """The reference's own __process_output (v2 and v1), __adjust_lanes_points, transformToBirdViewPoints and calcCurveAndOffset on the
+    crafted heads and lanes of tests/lane_conformance_cases.py -> lane_conformance.npz."""
+    import lane_conformance_cases as lc
+    import TrafficLaneDetector.ufldDetector.ultrafastLaneDetector as v1mod
+    from TrafficLaneDetector.ufldDetector.core import LaneDetectBase
+    from TrafficLaneDetector.ufldDetector.perspectiveTransformation import PerspectiveTransformation
+    res = {}
+    for ds, mt in (("culane", LaneModelType.UFLDV2_CULANE), ("tusimple", LaneModelType.UFLDV2_TUSIMPLE)):
+        ngr, ncr, ngc, ncc = lc.V2_GOLDEN_DIMS[ds]
+        shapes = [[1, ngr, ncr, 4], [1, ngc, ncc, 4], [1, 2, ncr, 4], [1, 2, ncc, 4]]
+        umod.OnnxEngine = lambda p, shapes=shapes: ref_shims.FakeEngine([1, 3, 320, 800], shapes, ["loc_row", "loc_col", "exist_row", "exist_col"],
+                                                                      lambda x: None)
+        det = umod.UltrafastLaneDetectorV2("fake.onnx", mt, None)
+        for i, heads in enumerate(lc.v2_golden_heads(ds)):
+            for w, h in lc.FRAME_SIZES:
+                det.img_width, det.img_height = w, h
+                lanes, status = det._UltrafastLaneDetectorV2__process_output(heads, det.cfg)
+                key = f"v2_{ds}_{i}_{w}x{h}"
+                for l in range(4):
+                    res[f"{key}_lane{l}"] = np.array(lanes[l], np.int32).reshape(-1, 2)
+                res[key + "_status"] = np.array(status, np.uint8)
+    for ds, G, R in lc.V1_GOLDEN:
+        mt = LaneModelType.UFLD_TUSIMPLE if ds == "tusimple" else LaneModelType.UFLD_CULANE
+        v1mod.OnnxEngine = lambda p, G=G, R=R: ref_shims.FakeEngine([1, 3, 288, 800], [[1, G + 1, R, 4]], ["output"], lambda x: None)
+        det = v1mod.UltrafastLaneDetector("fake.onnx", mt, None)
+        for i, head in enumerate(lc.v1_golden_heads(G, R)):
+            for w, h in lc.FRAME_SIZES:
+                det.img_height, det.img_width = h, w
+                det.h_ratio, det.w_ratio = h / det.cfg.img_h, w / det.cfg.img_w
+                lanes, status = det._UltrafastLaneDetector__process_output([head], det.cfg)
+                key = f"v1_{ds}_{i}_{w}x{h}"
+                for l in range(4):
+                    res[f"{key}_lane{l}"] = np.array(lanes[l], np.int32).reshape(-1, 2)
+                res[key + "_status"] = np.array([bool(v) for v in status], np.uint8)
+    res["M_default"] = PerspectiveTransformation((1280, 720)).M
+    for c in lc.geom_cases():
+        key = "geom_" + c["name"]
+        left, right = [tuple(p) for p in c["left"]], [tuple(p) for p in c["right"]]
+        if len(left) > 10 and len(right) > 10:
+            al, ar = LaneDetectBase._LaneDetectBase__adjust_lanes_points(left, right, c["img_wh"][1])
+            res[key + "_area_adj"] = np.vstack((al, np.flipud(ar))).astype(np.int32)
+        if c["M"] is not None:
+            t = PerspectiveTransformation((1280, 720))
+            if c["M"] == "identity":
+                t.M = np.eye(3)
+            bl, br = t.transformToBirdViewPoints(left), t.transformToBirdViewPoints(right)
+            res[key + "_bl"], res[key + "_br"] = np.asarray(bl, np.int64), np.asarray(br, np.int64)
+            bw, bh = c["bird_wh"]
+            try:
+                (d, curv), off = t.calcCurveAndOffset(np.zeros((bh, bw, 3), np.uint8), bl, br)
+                res[key + "_curve"] = np.array([{"L": -1.0, "F": 0.0, "R": 1.0}[d], curv, off])
+            except IndexError:
+                res[key + "_curve"] = np.array([np.nan, np.nan, np.nan])          # leftx[719] past a bird view under 720 rows
+    np.savez_compressed(os.path.join(OUT, "lane_conformance.npz"), **res)
+    print("lane_conformance.npz:", len(res), "arrays")
+
+
+def gen_warp_edges():
+    """cv2.warpPerspective (the library the reference calls in transformToBirdView) on the edge cases of
+    tests/lane_conformance_cases.py: sha256 of every output -> warp_edges.npz."""
+    import cv2
+    import lane_conformance_cases as lc
+    res = {}
+    for name, seed, (h, w), mname, dsize in lc.warp_cases():
+        res[name] = lc.sha(cv2.warpPerspective(lc.warp_source(seed, h, w), lc.WARP_MATRICES[mname], dsize, flags=cv2.INTER_LINEAR))
+    Ms = lc.warp_batch_matrices()
+    for b in range(len(Ms)):
+        res[f"batch_{b}"] = lc.sha(cv2.warpPerspective(lc.warp_source(100 + b, 480, 640), Ms[b], (333, 97), flags=cv2.INTER_LINEAR))
+    np.savez_compressed(os.path.join(OUT, "warp_edges.npz"), **res)
+    print("warp_edges.npz:", len(res), "hashes")
+
+
 if __name__ == "__main__":
+    if len(sys.argv) > 1 and sys.argv[1] == "lanes":
+        gen_lane_conformance()
+        gen_warp_edges()
+        sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == "birdview":
         gen_birdview()
         sys.exit(0)
@@ -315,3 +392,5 @@ if __name__ == "__main__":
     gen_track()
     gen_ufld_net_pin()
     gen_birdview()
+    gen_lane_conformance()
+    gen_warp_edges()

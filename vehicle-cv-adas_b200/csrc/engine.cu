@@ -1143,8 +1143,7 @@ int adas_ufld_lane_geometry(adas_engine* e, int batch, int img_w, int img_h, int
     ADAS_CUDA(cudaSetDevice(e->device));
     const int mp = e->ufld_max_pts;
     if (e->d_geom == nullptr || e->geom_cap_area < cap_area) {
-        cudaFree(e->d_warp); cudaFree(e->d_warpM);
-    cudaFree(e->d_area); cudaFree(e->d_bird); cudaFree(e->d_geom); cudaFree(e->d_M);
+        cudaFree(e->d_area); cudaFree(e->d_bird); cudaFree(e->d_geom); cudaFree(e->d_M);
         e->d_area = nullptr; e->d_bird = nullptr; e->d_geom = nullptr; e->d_M = nullptr;
         ADAS_CUDA(cudaMalloc(&e->d_area, (size_t)e->max_batch * cap_area * 8));
         ADAS_CUDA(cudaMalloc(&e->d_bird, (size_t)e->max_batch * 4 * mp * 8));

@@ -12,8 +12,9 @@
 //
 // np.polyfit(x, y, 2) = least squares on the Vandermonde matrix [x^2, x, 1] with columns scaled to unit 2-norm (numpy/lib/
 // polynomial.py: lhs /= scale; lstsq; c /= scale).  numpy solves the scaled system by SVD (LAPACK gelsd); here it is Householder QR in
-// float64 on the same scaled matrix -- the same least-squares solution up to rounding (agreement ~1e-12 relative on these problems;
-// the tests compare integer points exactly away from integer boundaries, coefficients-derived reals to 1e-8).  All float64
+// float64 on the same scaled matrix -- the same least-squares solution up to rounding: both are backward stable, so they differ by at
+// most the conditioning bound of tests/lane_conformance_cases.py polyfit_perturbation, which the tests carry through to the integer
+// points (exact away from integer boundaries) and to curvature / offset.  All float64
 // arithmetic that feeds an int() truncation follows numpy's operation order with _rn intrinsics (this file is built with -fmad=false).
 #include "common.h"
 #include "../../include/adas_b200.h"
@@ -23,7 +24,9 @@
 namespace adas {
 
 static constexpr int LG_THREADS = 128;
-static constexpr int LG_MAX_N = 1100;          // rows of the largest fit: the bird-view image height (720 in the reference's demo)
+// rows of the largest fit: the bird-view image height (720 in the reference's demo; 2160 covers a 4K-tall bird view).  Six such
+// float64 columns are the block's dynamic shared memory: 101.25 KB, within sm_90's 227 KB opt-in.
+static constexpr int LG_MAX_N = 2160;
 
 // deterministic block-wide sum (fixed order: per-thread strided partials -> warp shuffle tree -> warps in order)
 __device__ double block_sum(double v, double* red) {
@@ -178,7 +181,9 @@ __global__ void __launch_bounds__(LG_THREADS) lane_geom_kernel(const LaneGeomPar
             }
         __syncthreads();
         const int nl = N[1], nr = N[2];
-        if (nl >= 3 && nr >= 3 && p.bird_h >= 720 && p.bird_h <= LG_MAX_N) {
+        // below 720 rows the reference's leftx[719] raises IndexError: no curvature / offset ("None"), like a missing lane.  Two
+        // points make a rank-deficient fit (numpy's minimum-norm answer is not reproduced): also "None".
+        if (nl >= 3 && nr >= 3 && p.bird_h >= 720) {
             const int32_t* L = B + (size_t)1 * p.max_pts * 2;
             const int32_t* Rr = B + (size_t)2 * p.max_pts * 2;
             double lf[3], rf[3], lc[3], rc[3];
@@ -227,10 +232,11 @@ int launch_lane_geom(const int32_t* pts, const int32_t* npts, const uint8_t* sta
                      int adjust, int bird_w, int bird_h, int32_t* area, int cap_area, int32_t* bird, adas_lane_geom* out, cudaStream_t st) {
     ADAS_CHECK(max_pts >= 1 && max_pts <= LG_MAX_N && img_h >= 2 && cap_area >= 2 * max_pts, "lane_geometry: bad sizes (max_pts %d, img_h %d, cap_area %d)", max_pts, img_h, cap_area);
     ADAS_CHECK(!adjust || cap_area >= 2 * img_h, "lane_geometry: adjust_lanes needs room for 2 x image_height area points (cap_area %d)", cap_area);
+    ADAS_CHECK(M == nullptr || bird_h <= LG_MAX_N, "lane_geometry: bird view of %d rows, at most %d are supported", bird_h, LG_MAX_N);
     LaneGeomParams p;
     p.pts = pts; p.npts = npts; p.status = status; p.M = M; p.area = area; p.bird = bird; p.out = out;
     p.max_pts = max_pts; p.img_w = img_w; p.img_h = img_h; p.adjust = adjust; p.bird_w = bird_w; p.bird_h = bird_h; p.cap_area = cap_area;
-    const int smem = 6 * LG_MAX_N * 8;                      // 52.8 KB: needs the opt-in
+    const int smem = 6 * LG_MAX_N * 8;                      // 101.25 KB: needs the opt-in
     static std::mutex mu;
     static bool set_for[64] = {};
     int dev = 0;

@@ -164,6 +164,9 @@ __global__ void yolo_pre_kernel(const uint8_t* __restrict__ frames, int B, Lette
 
 int launch_yolo_pre(const uint8_t* frames, int B, const LetterboxGeom& g, __half* img_padded, int img_ld,
                     float* blob_nchw, cudaStream_t st) {
+    // a frame more than in_w (or in_h) times taller than wide letterboxes to 0 columns (rows): nothing to resize into
+    ADAS_CHECK(g.new_w >= 1 && g.new_h >= 1, "yolo_pre: a %d x %d frame letterboxes to %d x %d inside %d x %d", g.src_h, g.src_w, g.new_h,
+               g.new_w, g.in_h, g.in_w);
     ResizeTab t;
     if (get_resize_tab(g.src_w, g.src_h, g.new_w, g.new_h, &t)) return 1;
     const long long total = (long long)B * g.in_h * g.in_w;

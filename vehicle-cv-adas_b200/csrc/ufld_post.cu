@@ -100,6 +100,8 @@ int launch_ufld_post(const float* heads, int ld, int B, UfldDims d, int img_w, i
                      cudaStream_t st) {
     ADAS_CHECK(d.nl == 4, "ufld_post: num_lanes must be 4 (got %d)", d.nl);
     ADAS_CHECK(d.ncr <= UFLD_MAX_ANCH && d.ncc <= UFLD_MAX_ANCH, "ufld_post: too many anchors");
+    // the expectation divides by num_grid - 1: a 1-cell grid has no coordinate (the reference's int() of the infinity raises)
+    ADAS_CHECK(d.ngr >= 2 && d.ngc >= 2, "ufld_post: grids of %d x %d cells, need at least 2 each", d.ngr, d.ngc);
     ufld_post_kernel<<<B, UFLD_THREADS, 0, st>>>(heads, ld, d, img_w, img_h, row_anchor, col_anchor, pts, npts, status, coords,
                                                 max_pts);
     count_launch();

@@ -96,8 +96,9 @@ conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         }
     };
     // Programmatic dependent launch: everything above overlapped the tail of the previous kernel in the stream; its results may
-    // only be touched after `griddepcontrol.wait`.  Weights do not depend on the previous kernel: the producer arms the first
-    // pipeline stages and fetches their weight tiles BEFORE the wait, so only the activation tiles see the dependency.
+    // only be touched after `griddepcontrol.wait`.  The B operand holds the weights for a conv (A = activations): the producer arms
+    // the first pipeline stages and fetches their B tiles BEFORE the wait, so only the A tiles see the dependency.  In swap-AB mode
+    // (p.transposed) B is the activation, so gemm_v3_config turns the prefetch off there.
     int pre = 0;                                          // pipeline steps whose weight tiles were fetched ahead of the wait
     if (threadIdx.x == 0 && g.pdl && g.prefetch_w && (int)blockIdx.x < g.total_tiles) {
         const int steps_tile = o_cnt * p.kpt * i_cnt;
@@ -392,7 +393,7 @@ int gemm_v3_config(const GemmParams& p_in, GemmV3* g) {
     g->fd_bw = make_fastdiv(p.s2 ? p.s2_bw : 1);
     g->pdl = 0;
     static const int no_prefetch = env_int("ADAS_B200_NO_WPREFETCH", 0);
-    g->prefetch_w = no_prefetch ? 0 : 1;
+    g->prefetch_w = (no_prefetch || p.transposed) ? 0 : 1;     // swap-AB: B is the previous kernel's output, not the weights
     return 0;
 }
 
@@ -511,9 +512,9 @@ int gemm_v3_run(void* opaque, cudaStream_t st) { return gemm_v3_launch(*static_c
 void gemm_v3_free(void* opaque) { delete static_cast<GemmV3Launch*>(opaque); }
 void gemm_v3_describe(const void* opaque, char* out, int cap) {
     const GemmV3& g = static_cast<const GemmV3Launch*>(opaque)->g;
-    snprintf(out, (size_t)cap, "M=%d N=%d K=%d taps=%d act=%d res=%d f32=%d s2=%d tr=%d up2=%d | v3 BN=%d MT=%d slab=%d stages=%d tiles=%d", g.p.M,
+    snprintf(out, (size_t)cap, "M=%d N=%d K=%d taps=%d act=%d res=%d f32=%d s2=%d tr=%d up2=%d | v3 BN=%d MT=%d slab=%d stages=%d tiles=%d wpre=%d", g.p.M,
              g.p.N, g.p.Kc * g.p.ntaps, g.p.ntaps, g.p.act, g.p.res ? (g.p.res_ld < 0 ? -1 : 1) : 0, g.p.out_f32, g.p.s2, g.p.transposed, g.p.up2,
-             g.p.BN, g.MT, g.slab, g.stages, g.total_tiles);
+             g.p.BN, g.MT, g.slab, g.stages, g.total_tiles, g.prefetch_w);
 }
 
 }  // namespace adas

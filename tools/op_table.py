@@ -1,5 +1,5 @@
 """Per-layer table of a plan at real clocks: every launch replayed alone (CUDA events, L2-warm), GEMM shapes and tile choices.
-usage: python tools/op_table.py yolov8|ufldv2|yolov5|yolov7|yolov7-tiny|yolov7-w6|yolov7-e6|yolov7-d6|yolov7-e6e|yolov6n|yolov6s|yolov6m|yolov6l|yolov9-t|yolov9-s|yolov9-m|yolov9-c|yolov10n|yolov10s|yolov10m|yolov10b|yolov10l|yolov10x [batch] [iters]
+usage: python tools/op_table.py yolov8|ufldv2|yolov5|yolov7|yolov7-tiny|yolov7-w6|yolov7-e6|yolov7-d6|yolov7-e6e|yolov6n|yolov6s|yolov6m|yolov6l|yolov9-t|yolov9-s|yolov9-m|yolov9-c|yolov9-e|yolov10n|yolov10s|yolov10m|yolov10b|yolov10l|yolov10x [batch] [iters]
 (the YOLOv7 P6 models run at 1280x1280)   (env switches of the library apply)"""
 import os, re, sys, tempfile
 R = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, R); sys.path.insert(0, os.path.join(R, "tests"))
@@ -29,7 +29,8 @@ else:
 eng = _capi.Engine(path, 0, max_batch=B)
 eng.run(B)
 n = eng.num_steps(B)
-names = {1: "gemm", 2: "im2col", 3: "maxpool", 4: "upsample", 5: "layernorm", 6: "stempack", 7: "stemconv", 8: "avgpool2", 9: "dwconv", 10: "attention", 31: "(folded)"}
+names = {1: "gemm", 2: "im2col", 3: "maxpool", 4: "upsample", 5: "layernorm", 6: "stempack", 7: "stemconv", 8: "avgpool2", 9: "dwconv", 10: "attention",
+         11: "cbfuse", 31: "(folded)"}
 tot = 0.0; tot_g = 0.0; rows = []
 for i in range(n):
     ms, t, d = eng.time_step(B, i, iters)
@@ -64,4 +65,14 @@ if dw_rows:
         dw_bytes += 2 * B * C * (bi[3] * bi[4] + bo[3] * bo[4] * (2 if p[10] >= 0 else 1)) + C * (2 * k * k + 4)
     print(f"share of the sum of isolated launches: dwconv {100 * ms_dw / tot:.1f} %, attention {100 * ms_at / tot:.1f} %; "
           f"dwconv {dw_bytes / 1e6:.1f} MB in {ms_dw * 1e3:.1f} us -> {dw_bytes / ms_dw / 1e6:.0f} GB/s (HBM3 data sheet: 3350 GB/s)")
+cb_rows = [r for r in rows if r[2] == "cbfuse"]
+if cb_rows:
+    ms_cb = sum(r[0] for r in cb_rows)
+    cb_bytes = 0                              # fp16: the target read and written once, each source read once at its own resolution
+    for r in cb_rows:
+        p = pb.ops[r[1]][1]
+        ob = pb.buffers[p[0]]
+        cb_bytes += 2 * B * p[2] * ob[3] * ob[4] * 2 + sum(2 * B * p[2] * pb.buffers[p[6 + 3 * s]][3] * pb.buffers[p[6 + 3 * s]][4] for s in range(p[5]))
+    print(f"share of the sum of isolated launches: cbfuse {100 * ms_cb / tot:.1f} %; cbfuse {cb_bytes / 1e6:.1f} MB in {ms_cb * 1e3:.1f} us -> "
+          f"{cb_bytes / ms_cb / 1e6:.0f} GB/s (HBM3 data sheet: 3350 GB/s)")
 eng.close()

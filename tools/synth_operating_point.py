@@ -1,7 +1,7 @@
 """Scan synthetic head operating points (gain, bias) on the CPU: fp32 oracle vs its fp16-storage emulation (oracle.nets.forward_fp16_emulated).
 Prints the probability / box error the device path will show, the candidates per frame at box_score 0.4 and how many sit within 1e-3 / 2e-3
 of the threshold.  Test infrastructure (uses oracle/):  python tools/synth_operating_point.py yolov8 l 45,-9 40,-8.2
-(yolov9 t|s|m|c, yolov10 n|s|m|b|l|x: the scale's class bias; the head gains of plan.SYNTH_PROFILES[kind] are kept)
+(yolov9 t|s|m|c|e, yolov10 n|s|m|b|l|x: the scale's class bias; the head gains of plan.SYNTH_PROFILES[kind] are kept)
 """
 import sys, os
 R = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, R); sys.path.insert(0, os.path.join(R, 'tests'))
@@ -19,8 +19,9 @@ for a in sys.argv[3:]:
     if kind=="yolov8":
         plan.SYNTH_PROFILES["yolov8"]={"gains":[(r"model\.22\.cv3\.\d\.2\.weight", g), (r"model\.22\.cv2\.\d\.2\.weight", 25.0)],"fill":[(r"model\.22\.cv3\.\d\.2\.bias", b)]}
     elif kind=="yolov9":
-        plan.SYNTH_PROFILES["yolov9"]={**plan.SYNTH_PROFILES["yolov9"], "gains":[(r"model\.22\.cv3\.\d\.2\.weight", g), (r"model\.22\.cv2\.\d\.2\.weight", 25.0)],
-                                   "variants": {variant: {"fill": [(r"model\.22\.cv3\.\d\.2\.bias", b)]}}}
+        hd, bg = ("model\\.42", 12.0) if variant == "e" else ("model\\.22", 25.0)      # YOLOv9-E's head is model.42 (box gain 12)
+        plan.SYNTH_PROFILES["yolov9"]={**plan.SYNTH_PROFILES["yolov9"], "gains":[(hd + r"\.cv3\.\d\.2\.weight", g), (hd + r"\.cv2\.\d\.2\.weight", bg)],
+                                   "variants": {variant: {"fill": [(hd + r"\.cv3\.\d\.2\.bias", b)]}}}
     elif kind=="yolov10":
         plan.SYNTH_PROFILES["yolov10"]={**plan.SYNTH_PROFILES["yolov10"], "gains":[(r"model\.23\.one2one_cv3\.\d\.2\.weight", g), (r"model\.23\.one2one_cv2\.\d\.2\.weight", 25.0)],
                                     "variants": {variant: {"fill": [(r"model\.23\.one2one_cv3\.\d\.2\.bias", b)]}}}
@@ -28,8 +29,8 @@ for a in sys.argv[3:]:
         plan.SYNTH_PROFILES["yolov5"]={"gains":[(r"model\.24\.m\.\d\.weight", g)],"fill":[(r"model\.24\.m\.\d\.bias", b)]}
     W = plan.synth_weights(kind, 0, variant=variant); builder(W, variant)
     if kind=="yolov9":
-        import yolov9_oracle
-        md = yolov9_oracle.build(W.state_dict, variant)
+        import yolov9_oracle, yolov9e_oracle
+        md = yolov9e_oracle.build(W.state_dict) if variant == "e" else yolov9_oracle.build(W.state_dict, variant)
     elif kind=="yolov10":
         import yolov10_oracle
         md = yolov10_oracle.build(W.state_dict, variant)

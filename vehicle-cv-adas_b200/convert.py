@@ -10,7 +10,7 @@ and `TrafficLaneDetector/convertPytorchToONNX.py:77-87` (UFLD `.pth` checkpoint 
     python -m adas_b200.convert yolov7-tiny.state_dict.pth --kind yolov7 --scale tiny
     python -m adas_b200.convert yolov7-w6.state_dict.pth --kind yolov7 --scale w6     # P6: w6 | e6 | d6 | e6e, 1280x1280
     python -m adas_b200.convert yolov6s.state_dict.pth --kind yolov6 --scale s
-    python -m adas_b200.convert yolov9-c.state_dict.pth --kind yolov9 --scale c     # t | s | m | c
+    python -m adas_b200.convert yolov9-c.state_dict.pth --kind yolov9 --scale c     # t | s | m | c | e
     python -m adas_b200.convert yolov10s.state_dict.pth --kind yolov10 --scale s    # n | s | m | b | l | x
     python -m adas_b200.convert yolov10s.onnx                                         # recognised, also with the top-k tail
 
@@ -101,7 +101,7 @@ def main(argv=None) -> int:
     ap.add_argument("model")
     ap.add_argument("--out", default=None)
     ap.add_argument("--kind", default=None, choices=["yolov8", "yolov5", "yolov7", "yolov6", "yolov9", "yolov10", "ufldv2"])
-    ap.add_argument("--scale", default="l", help="YOLO scale letter (n | s | m | l for yolov6, t | s | m | c for yolov9, n | s | m | b | l | x for yolov10), or tiny | base | w6 | e6 | d6 | e6e for yolov7 (checkpoints only; ONNX files are recognised)")
+    ap.add_argument("--scale", default="l", help="YOLO scale letter (n | s | m | l for yolov6, t | s | m | c | e for yolov9, n | s | m | b | l | x for yolov10), or tiny | base | w6 | e6 | d6 | e6e for yolov7 (checkpoints only; ONNX files are recognised)")
     ap.add_argument("--backbone", default="34", choices=["18", "34"], help="UFLDv2 ResNet depth (checkpoints only)")
     ap.add_argument("--nc", type=int, default=80)
     a = ap.parse_args(argv)

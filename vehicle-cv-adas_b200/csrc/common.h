@@ -108,6 +108,17 @@ int launch_maxpool(const __half* in, int in_ld, int B, int H, int W, int C, int 
 int launch_avgpool2(const __half* in, int in_ld, int B, int H, int W, int C, __half* out, int out_ld, int fill, cudaStream_t st);
 int launch_upsample2x(const __half* in, int in_ld, int B, int H, int W, int C, __half* out, int out_ld,
                       cudaStream_t st);
+// CBFuse (YOLOv9-E): out = base + sum of nearest-upsampled channel slices of n_src sources, each on an (H >> shift) x (W >> shift)
+// padded grid; fp32 sum in the listed order, one rounding, interior pixels only.  base may be out (in place).
+static const int kCbfuseMaxSrc = 5;
+struct CbfuseSrc { const __half* ptr; int ld; int shift; };
+struct CbfuseParams {
+    __half* out; int out_ld;
+    const __half* base; int base_ld;
+    int B, H, W, C, n_src;
+    CbfuseSrc src[kCbfuseMaxSrc];
+};
+int launch_cbfuse(const CbfuseParams& p, cudaStream_t st);
 int launch_layernorm(const __half* in, int in_ld, int rows, int d_len, int d_norm, const float* gamma,
                      const float* beta, float eps, __half* out, int out_ld, cudaStream_t st);
 int launch_fc_stream(const __half* x, int x_ld, int batch, const __half* W, int K, int N, const float* bias, int act, void* out, int out_ld,

@@ -228,6 +228,60 @@ int launch_upsample2x(const __half* in, int in_ld, int B, int H, int W, int C, _
     return 0;
 }
 
+// ---- CBFuse: base + nearest-upsampled channel slices of up to 5 sources (YOLOv9-E's dual-backbone routing) -------------------
+// out(y, x, c) = base(y, x, c) + sum_i src_i(y >> shift_i, x >> shift_i, c): fp32 sum in a fixed order (base, then the sources as
+// listed), one rounding.  Interior pixels only, so the halo stays zero.  `base` may be `out` itself (in place): every thread reads
+// its own 16 bytes before it writes them, so base and out are not __restrict__.
+__global__ void cbfuse_kernel(CbfuseParams p) {
+    const int c8 = p.C >> 3;
+    const long long total = (long long)p.B * p.H * p.W * c8;
+    const int Hp = p.H + 2, Wp = p.W + 2;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int cg = (int)(i % c8);
+        long long t = i / c8;
+        const int x = (int)(t % p.W); t /= p.W;
+        const int y = (int)(t % p.H);
+        const int b = (int)(t / p.H);
+        const size_t r = ((size_t)b * Hp + (y + 1)) * Wp + (x + 1);
+        const uint4 bv = *reinterpret_cast<const uint4*>(p.base + r * p.base_ld + cg * 8);
+        const __half2* bh = reinterpret_cast<const __half2*>(&bv);
+        float2 acc[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[j] = __half22float2(bh[j]);
+        for (int s = 0; s < p.n_src; ++s) {
+            const CbfuseSrc& q = p.src[s];
+            const int Hs = p.H >> q.shift, Ws = p.W >> q.shift;
+            const size_t rs = ((size_t)b * (Hs + 2) + ((y >> q.shift) + 1)) * (Ws + 2) + ((x >> q.shift) + 1);
+            const uint4 sv = __ldg(reinterpret_cast<const uint4*>(q.ptr + rs * q.ld + cg * 8));
+            const __half2* sh = reinterpret_cast<const __half2*>(&sv);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const float2 f = __half22float2(sh[j]);
+                acc[j].x += f.x;
+                acc[j].y += f.y;
+            }
+        }
+        uint4 o;
+        __half2* oh = reinterpret_cast<__half2*>(&o);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) oh[j] = __floats2half2_rn(acc[j].x, acc[j].y);
+        *reinterpret_cast<uint4*>(p.out + r * p.out_ld + cg * 8) = o;
+    }
+}
+
+int launch_cbfuse(const CbfuseParams& p, cudaStream_t st) {
+    ADAS_CHECK(p.n_src >= 1 && p.n_src <= kCbfuseMaxSrc && p.C % 8 == 0 && p.out_ld % 8 == 0 && p.base_ld % 8 == 0, "cbfuse: sources / channel alignment");
+    for (int s = 0; s < p.n_src; ++s)
+        ADAS_CHECK(p.src[s].shift >= 0 && p.src[s].shift <= 4 && p.src[s].ld % 8 == 0, "cbfuse: source %d shift / alignment", s);
+    const long long total = (long long)p.B * p.H * p.W * (p.C / 8);
+    int blocks = grid_for(total, 256);
+    if (blocks > 132 * 32) blocks = 132 * 32;
+    cbfuse_kernel<<<blocks, 256, 0, st>>>(p);
+    count_launch();
+    ADAS_CUDA(cudaGetLastError());
+    return 0;
+}
+
 // ---- LayerNorm over a feature row (one CTA per row), fp32 statistics ------------------------------
 // Block-wide sum in a fixed order (per-thread strided run, xor tree over lanes, then over warps): every row is reduced by the same
 // instruction sequence whatever the batch.

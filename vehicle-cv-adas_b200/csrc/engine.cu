@@ -361,6 +361,29 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
                 prog->steps.push_back([=](cudaStream_t st) { return launch_upsample2x(in, in_ld, batch, H, W, C, out, out_ld, st); });
                 break;
             }
+            case OP_CBFUSE: {
+                const PlanBuffer& ob = e->bufs[p[0]];
+                const PlanBuffer& bb = e->bufs[p[3]];
+                CbfuseParams cp;
+                memset(&cp, 0, sizeof(cp));
+                cp.out = static_cast<__half*>(e->dbufs[p[0]].ptr) + p[1];
+                cp.out_ld = (int)ob.C;
+                cp.base = static_cast<const __half*>(e->dbufs[p[3]].ptr) + p[4];
+                cp.base_ld = (int)bb.C;
+                cp.B = batch; cp.H = (int)ob.H; cp.W = (int)ob.W; cp.C = p[2]; cp.n_src = p[5];
+                for (int s = 0; s < cp.n_src; ++s) {
+                    const int* q = p + 6 + 3 * s;
+                    cp.src[s].ptr = static_cast<const __half*>(e->dbufs[q[0]].ptr) + q[1];
+                    cp.src[s].ld = (int)e->bufs[q[0]].C;
+                    cp.src[s].shift = q[2];
+                }
+                char d[128];
+                snprintf(d, sizeof(d), "cbfuse C=%d %dx%d sources=%d%s", cp.C, cp.H, cp.W, cp.n_src, (p[0] == p[3] && p[1] == p[4]) ? " in place" : "");
+                prog->step_desc.resize(prog->step_type.size());
+                prog->step_desc.back() = d;
+                prog->steps.push_back([=](cudaStream_t st) { return launch_cbfuse(cp, st); });
+                break;
+            }
             case OP_STEMPACK: {
                 const PlanBuffer& ib = e->bufs[p[0]];
                 const PlanBuffer& ob = e->bufs[p[1]];
@@ -693,6 +716,36 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
                 ADAS_CHECK(view_ok(p[0], p[1], p[2]) && view_ok(p[3], p[4], p[2]) && e->bufs[p[0]].H > 0 && e->bufs[p[3]].H == 2 * e->bufs[p[0]].H && e->bufs[p[3]].W == 2 * e->bufs[p[0]].W,
                            "plan %s: op %zu: bad upsample", path, oi);
                 break;
+            case OP_CBFUSE: {
+                const int C = p[2], n_src = p[5];
+                ADAS_CHECK(n_src >= 1 && n_src <= kCbfuseMaxSrc, "plan %s: op %zu: cbfuse with %d sources (1 to %d)", path, oi, n_src, kCbfuseMaxSrc);
+                ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[3]), "plan %s: op %zu: cbfuse buffer index out of range", path, oi);
+                for (int s = 0; s < n_src; ++s)
+                    ADAS_CHECK(buf_ok(p[6 + 3 * s]), "plan %s: op %zu: cbfuse buffer index out of range", path, oi);
+                const PlanBuffer &ob = e->bufs[p[0]], &bb = e->bufs[p[3]];
+                bool f16 = ob.dtype == 0 && bb.dtype == 0;
+                for (int s = 0; s < n_src; ++s) f16 = f16 && e->bufs[p[6 + 3 * s]].dtype == 0;
+                ADAS_CHECK(f16, "plan %s: op %zu: cbfuse buffers must be fp16", path, oi);
+                ADAS_CHECK(ob.H > 0 && bb.H == ob.H && bb.W == ob.W, "plan %s: op %zu: cbfuse base must have the output's H x W", path, oi);
+                for (int s = 0; s < n_src; ++s) {
+                    const int* q = p + 6 + 3 * s;
+                    const PlanBuffer& sb = e->bufs[q[0]];
+                    ADAS_CHECK(q[2] >= 0 && q[2] <= 4, "plan %s: op %zu: cbfuse source %d shift %d (0 to 4)", path, oi, s, q[2]);
+                    ADAS_CHECK(sb.H > 0 && ((uint64_t)sb.H << q[2]) == ob.H && ((uint64_t)sb.W << q[2]) == ob.W,
+                               "plan %s: op %zu: cbfuse source %d geometry %ux%u << %d is not the output's %ux%u", path, oi, s, sb.H, sb.W, q[2], ob.H, ob.W);
+                }
+                bool al = C >= 8 && C % 8 == 0 && p[1] % 8 == 0 && p[4] % 8 == 0 && ob.C % 8 == 0 && bb.C % 8 == 0;
+                for (int s = 0; s < n_src; ++s) al = al && p[7 + 3 * s] % 8 == 0 && e->bufs[p[6 + 3 * s]].C % 8 == 0;
+                ADAS_CHECK(al, "plan %s: op %zu: cbfuse channels and offsets must be multiples of 8", path, oi);
+                bool fits = view_ok(p[0], p[1], C) && view_ok(p[3], p[4], C);
+                for (int s = 0; s < n_src; ++s) fits = fits && view_ok(p[6 + 3 * s], p[7 + 3 * s], C);
+                ADAS_CHECK(fits, "plan %s: op %zu: cbfuse channel slice exceeds its buffer", path, oi);
+                auto apart = [&](int b, int coff) { return b != p[0] || coff >= p[1] + C || p[1] >= coff + C; };
+                bool sep = apart(p[3], p[4]) || p[4] == p[1];
+                for (int s = 0; s < n_src; ++s) sep = sep && apart(p[6 + 3 * s], p[7 + 3 * s]);
+                ADAS_CHECK(sep, "plan %s: op %zu: cbfuse source slice overlaps the output (only the base may be the output slice itself)", path, oi);
+                break;
+            }
             case OP_STEMPACK:
                 ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[1]) && e->bufs[p[0]].H > 0 && e->bufs[p[1]].H > 0 && e->bufs[p[0]].C == 4 && e->bufs[p[1]].C == 64, "plan %s: op %zu: bad stem re-layout", path, oi);
                 break;

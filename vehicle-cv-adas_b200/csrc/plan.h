@@ -68,6 +68,10 @@ enum PlanOpType : uint32_t {
                        //    out = act(acc + bias) (+ res, res_buf -1: none), see dwconv.cu
     OP_ATTN = 10,      // p: in_buf in_coff nh kdp hd out_buf out_coff ; f0 = softmax scale : multi-head self-attention over the H*W
                        //    pixels; input channels [Q nh*kdp | K nh*kdp | V nh*hd], output nh*hd channels head-major, see attention.cu
+    OP_CBFUSE = 11,    // p: out_buf out_coff C base_buf base_coff n_src, then n_src x (src_buf src_coff shift) : YOLOv9-E CBFuse,
+                       //    out(y, x, c) = base(y, x, c) + sum_i src_i(y >> shift_i, x >> shift_i, src_coff_i + c) over the output's
+                       //    interior (n_src 1..5, shift 0..4, src H x W << shift == out H x W); fp32 sum in the listed order, one
+                       //    rounding; base may be the output slice itself (in place), see elementwise.cu cbfuse_kernel
 };
 
 }  // namespace adas

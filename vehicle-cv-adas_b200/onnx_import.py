@@ -602,8 +602,8 @@ def _recognise_yolov6(model: OnnxModel, w: OnnxWeights, in_h: int, in_w: int) ->
                      acts=(roles.get("body", "relu"), roles.get("neck", "relu"), roles.get("head", "silu")))
 
 
-_V9_SUPPORTED = ("YOLOv9-T / S / M / C (WongKinYiu/yolov9 v0.1, the converted GELAN graphs with a DDetect head, exported with one output; "
-                 "YOLOv9-E / GELAN-E, files with the auxiliary branch, ultralytics' YOLOv9 are not supported)")
+_V9_SUPPORTED = ("YOLOv9-T / S / M / C / E (WongKinYiu/yolov9 v0.1, the converted GELAN graphs with a DDetect head, exported with one "
+                 "output; files with the auxiliary branch and ultralytics' YOLOv9 are not supported)")
 _V9_STEM = {16: ("t",), 32: ("s", "m"), 64: ("c",)}
 _V9_DOWN3 = {128: "s", 240: "m"}            # layer 3 (AConv) width tells S from M
 
@@ -615,13 +615,20 @@ def _is_yolov9(model: OnnxModel) -> bool:
 
 def _recognise_yolov9(model: OnnxModel, w: OnnxWeights, in_h: int, in_w: int) -> ModelSpec:
     """YOLOv9-T / S / M / C: the stem width gives the scale (32: S or M by layer 3's width), the head must have DDetect's grouped box
-    convolutions, and the convolution count must be the scale's (fused, or with RepConvN's two branches apart)."""
+    convolutions, and the convolution count must be the scale's (fused, or with RepConvN's two branches apart).  YOLOv9-E: two
+    [64, 3, 3, 3] convolutions read the image (its two backbones, model.1 and model.15); the same head and count checks follow."""
     if len(model.outputs) != 1:
         raise Exception(f"YOLOv9 file with {len(model.outputs)} outputs (an auxiliary-branch training file?); supported: {_V9_SUPPORTED}")
     first = w.convs[0][1]
-    cands = _V9_STEM.get(int(first.shape[0]), ()) if tuple(first.shape[1:]) == (3, 3, 3) else ()
+    image = model.inputs[0][0] if model.inputs else None
+    image_convs = [model.initializers.get(n.inputs[1]) for n in model.nodes if n.op_type == "Conv" and n.inputs and n.inputs[0] == image]
+    if len(image_convs) == 2 and all(c is not None and tuple(c.shape) == (64, 3, 3, 3) for c in image_convs):
+        cands = ("e",)
+    else:
+        cands = _V9_STEM.get(int(first.shape[0]), ()) if tuple(first.shape[1:]) == (3, 3, 3) else ()
     if not cands:
-        raise Exception(f"YOLOv9 stem {tuple(first.shape)}: 16 (T), 32 (S / M) or 64 (C) channels; supported: {_V9_SUPPORTED}")
+        raise Exception(f"YOLOv9 stem {tuple(first.shape)}: 16 (T), 32 (S / M) or 64 (C) channels, or two 64-channel image convolutions (E); "
+                        f"supported: {_V9_SUPPORTED}")
     grouped = [n for n in model.nodes if n.op_type == "Conv" and int(n.attrs.get("group", 1)) == 4]
     if len(grouped) != 6:
         raise Exception(f"YOLOv9 file with {len(grouped)} group-4 convolutions: a head without DDetect's grouped box convolutions "
@@ -646,8 +653,9 @@ def _recognise_yolov9(model: OnnxModel, w: OnnxWeights, in_h: int, in_w: int) ->
         raise Exception(f"YOLOv9 file with {n} convolutions, YOLOv9-{scale.upper()} has {fused} ({fused + plan.yolov9_repconvn_count(scale)} with "
                         f"RepConvN's branches apart); supported: {_V9_SUPPORTED}")
     nc = None
+    head = "model.42" if scale == "e" else "model.22"
     for name, cw, _ in w.convs:
-        if re.fullmatch(r"model\.22\.cv3\.\d+\.2\.weight", name):      # DDetect.cv3[i][2]: Conv2d(c3, nc, 1)
+        if re.fullmatch(re.escape(head) + r"\.cv3\.\d+\.2\.weight", name):      # DDetect.cv3[i][2]: Conv2d(c3, nc, 1)
             nc = int(cw.shape[0])
     if nc is None:                                               # names lost: the last 1x1 conv before the (optional) DFL conv
         nc = int([cw.shape[0] for _, cw, _ in w.convs if cw.shape[2:] == (1, 1) and cw.shape[0] != 1][-1])

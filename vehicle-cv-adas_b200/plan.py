@@ -26,7 +26,7 @@ import re
 import struct
 import zlib
 from dataclasses import dataclass
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -35,6 +35,7 @@ MODEL_YOLOV6 = 5                                                         # ancho
 OP_GEMM, OP_IM2COL, OP_MAXPOOL, OP_UPSAMPLE2X, OP_LAYERNORM, OP_STEMPACK, OP_STEMCONV = 1, 2, 3, 4, 5, 6, 7
 OP_AVGPOOL2 = 8
 OP_DWCONV, OP_ATTN = 9, 10
+OP_CBFUSE = 11
 ACT_NONE, ACT_SILU, ACT_RELU, ACT_LEAKY = 0, 1, 2, 3          # ACT_LEAKY: LeakyReLU(0.1)
 PLAN_VERSION = 1
 
@@ -238,10 +239,19 @@ SYNTH_PROFILES = {
     # YOLOv9 T/S/M/C: YOLOv8's head gains (CPU fp16 emulation: probability error 2-4e-4, box error 0.1 px on 8 frames); the class bias
     # of each scale puts ~100 of the 8400 anchors per frame above box_score = 0.4 (fp32 oracle, synthetic frames 0-3: at bias -3.5 the
     # 100th-highest max-class logit sits 0.53 (T), -0.31 (S), 0.04 (M), 0.05 (C) from logit(0.4); per-anchor spread 0.16-0.47).
-    "yolov9": {"gains": [(r"model\.22\.cv3\.\d\.2\.weight", 16.0), (r"model\.22\.cv2\.\d\.2\.weight", 25.0)],
+    # YOLOv9-E (head model.42): at YOLOv8's gains the CPU fp16 emulation (plan_interp.interpret, every op rounded to fp16) was 5.9e-3
+    # off in probability on frame 0 (4: 1.3e-3) and 0.42 px on boxes: its 261-conv graph and the CBFuse sums leave large per-frame
+    # offsets on the class logits.  Class gain 2 and box gain 12 gave 7.6e-4 / 3.3e-4 and 0.22 / 0.13 px on frames 0 / 1, but 1.0e-3 on
+    # the device at 384x640 (H100), so the class gain is 1.5: device 7.1e-4 / 0.26 px at 640x640 and 6.9e-4 / 0.26 px at 384x640 on
+    # frames 0 / 1; `tools/synth_operating_point.py yolov9 e 1.5,-1.25` gives 5.6e-4 / 2.2e-4 there and up to 1.02e-3 on frame 2.  Class
+    # bias -1.25 puts 183, 9, 274, 53 anchors of synthetic frames 0-3 above box_score = 0.4 (fp32 oracle, 640x640); the per-frame spread
+    # is wide, and frames 4, 6, 7 have none.
+    "yolov9": {"gains": [(r"model\.22\.cv3\.\d\.2\.weight", 16.0), (r"model\.22\.cv2\.\d\.2\.weight", 25.0),
+                         (r"model\.42\.cv3\.\d\.2\.weight", 1.5), (r"model\.42\.cv2\.\d\.2\.weight", 12.0)],
                "fill": [(r"model\.22\.cv3\.\d\.2\.bias", -3.5)],
-               "variants": {sc: {"fill": [(r"model\.22\.cv3\.\d\.2\.bias", -3.5 - d)]}
-                            for sc, d in (("t", 0.53), ("s", -0.31), ("m", 0.04), ("c", 0.05))}},
+               "variants": {**{sc: {"fill": [(r"model\.22\.cv3\.\d\.2\.bias", -3.5 - d)]}
+                               for sc, d in (("t", 0.53), ("s", -0.31), ("m", 0.04), ("c", 0.05))},
+                            "e": {"fill": [(r"model\.42\.cv3\.\d\.2\.bias", -1.25)]}}},
     # YOLOv10 N/S/M/B/L/X: YOLOv8's head gains on the one-to-one head (CPU fp16 emulation, q / k / v and the attention output rounded
     # too: probability error 2.5-3.7e-4, box error 0.13-0.23 px on 4 frames).  The class bias of each scale puts ~100 of the 8400
     # anchors per frame above box_score = 0.4 (fp32 oracle, synthetic frames 0-3: at bias -3.5 the 100th-highest max-class logit sits
@@ -527,6 +537,20 @@ class PlanBuilder:
         assert out.H == 2 * x.H and out.W == 2 * x.W and x.C % 8 == 0
         self._op(OP_UPSAMPLE2X, [x.buf, x.coff, x.C, out.buf, out.coff])
         return View(out.buf, out.coff, x.C, out.H, out.W)
+
+    def cbfuse(self, base: View, srcs: Sequence[Tuple[View, int]], out: Optional[View] = None) -> View:
+        """YOLOv9-E CBFuse: out = base + sum of the nearest-upsampled source slices, source i read at (y >> shift_i, x >> shift_i)
+        (fp32 sum in the listed order, one rounding).  out None: in place on `base`."""
+        out = base if out is None else out
+        assert 1 <= len(srcs) <= 5 and base.C == out.C and base.C % 8 == 0 and base.coff % 8 == 0 and out.coff % 8 == 0, (base, out)
+        assert (base.H, base.W) == (out.H, out.W), (base, out)
+        p = [out.buf, out.coff, out.C, base.buf, base.coff, len(srcs)]
+        for v, shift in srcs:
+            assert v.C == out.C and v.coff % 8 == 0 and 0 <= shift <= 4 and (v.H << shift, v.W << shift) == (out.H, out.W), (v, shift, out)
+            assert v.buf != out.buf or v.coff >= out.coff + out.C or out.coff >= v.coff + v.C, (v, out)
+            p += [v.buf, v.coff, shift]
+        self._op(OP_CBFUSE, p)
+        return View(out.buf, out.coff, out.C, out.H, out.W)
 
     def layernorm(self, in_buf: int, d_len: int, d_norm: int, gamma: np.ndarray, beta: np.ndarray, eps: float, out_buf: int) -> None:
         self._op(OP_LAYERNORM, [in_buf, d_len, self.tensor(gamma.astype(np.float32)), self.tensor(beta.astype(np.float32)), out_buf, d_norm],
@@ -1242,17 +1266,33 @@ YOLOV9 = {
 }
 
 
+# YOLOv9-E (GELAN-E, upstream `models/detect/gelan-e.yaml`): two backbones.  model.0 is Silence (the image passes through), so
+# model.1 and model.15 both read the image.  `elan`: RepNCSPELAN4 (c2, c3, c4, n) of layers 3, 5, 7, 9 (again as 19, 22, 25, 28 in the
+# second backbone); `downs`: ADown widths of layers 4, 6, 8 (20, 23, 26); `cbl`: CBLinear groups of layers 10-14, which read layers 1,
+# 3, 5, 7, 9; `spp`: SPPELAN (c2, c3) of layer 29; `head`: RepNCSPELAN4 of layers 32, 35, 38, 41; `head_downs`: ADown widths of layers
+# 36, 39.  CBFuse (16, 18, 21, 24, 27) adds group `level` of every CBLinear from layer 10 + level on, nearest-upsampled, to the output
+# of layer 15, 17, 20, 23 or 26.  The head is DDetect (model.42) on layers 35, 38, 41.
+YOLOV9_E = dict(stem=(64, 128), elan=((256, 128, 64, 2), (512, 256, 128, 2), (1024, 512, 256, 2), (1024, 512, 256, 2)),
+                downs=(256, 512, 1024), cbl=((64,), (64, 128), (64, 128, 256), (64, 128, 256, 512), (64, 128, 256, 512, 1024)),
+                spp=(512, 256), head=((512, 512, 256, 2), (256, 256, 128, 2), (512, 512, 256, 2), (512, 1024, 512, 2)), head_downs=(256, 512))
+
+
 def yolov9_conv_count(scale: str) -> int:
     """Convolutions of the fused graph (RepConvN as one conv; the fixed DFL conv not counted).  A training-form file has one more per
     RepConvN (its 1x1 branch): yolov9_repconvn_count(scale)."""
-    cfg = YOLOV9[scale]
     n_r4 = lambda n: 10 + 4 * n                        # cv1, 2 x (RepNCSP: cv1, cv2, cv3, n x (RepConvN, Conv) + Conv 3x3), cv4
+    if scale == "e":                                   # 4 stem convs, 12 ELANs, 8 ADowns, 5 CBLinears, SPPELAN, DDetect
+        e = YOLOV9_E
+        return 4 + 2 * sum(n_r4(r[3]) for r in e["elan"]) + sum(n_r4(r[3]) for r in e["head"]) + 2 * 8 + len(e["cbl"]) + 2 + 3 * 6
+    cfg = YOLOV9[scale]
     l2 = 4 if cfg["l2"][3] is None else n_r4(cfg["l2"][3])
     down = 1 if cfg["down"] == "aconv" else 2
     return 2 + l2 + 5 * down + sum(n_r4(r[3]) for r in cfg["r4"]) + 2 + 3 * 6
 
 
 def yolov9_repconvn_count(scale: str) -> int:
+    if scale == "e":
+        return 2 * (2 * sum(r[3] for r in YOLOV9_E["elan"]) + sum(r[3] for r in YOLOV9_E["head"]))
     cfg = YOLOV9[scale]
     return 2 * ((cfg["l2"][3] or 0) + sum(r[3] for r in cfg["r4"]))
 
@@ -1378,9 +1418,12 @@ def build_yolov9(weights: Weights, scale: str = "c", nc: int = 80, in_h: int = 6
 
     RepConvN is folded here in fp64 (training-form `conv1` / `conv2` keys) or taken fused (`conv.weight` + `conv.bias`); a Conv fused
     upstream (`conv.bias`, no `bn`) is taken as it is.  ADown / AConv's 2x2 stride-1 average pool runs as OP_AVGPOOL2 on the input's grid,
-    so their stride-2 convs see even maps.  DDetect's grouped box convs pack as dense block-diagonal weights.  Channel layout: Yolov9Packer."""
-    assert scale in YOLOV9, f"YOLOv9 scale {scale!r}: 't', 's', 'm' or 'c' (YOLOv9-E / GELAN-E is not supported)"
+    so their stride-2 convs see even maps.  DDetect's grouped box convs pack as dense block-diagonal weights.  Channel layout: Yolov9Packer.
+    YOLOv9-E: build_yolov9e."""
+    assert scale in YOLOV9 or scale == "e", f"YOLOv9 scale {scale!r}: 't', 's', 'm', 'c' or 'e'"
     assert in_h % 32 == 0 and in_w % 32 == 0, f"YOLOv9 input {in_h}x{in_w}: a multiple of 32"
+    if scale == "e":
+        return build_yolov9e(weights, nc, in_h, in_w)
     cfg = YOLOV9[scale]
     pb = PlanBuilder(MODEL_YOLOV8, 3, in_h, in_w)
     g = Yolov9Packer(pb, weights, cfg["down"])
@@ -1411,6 +1454,69 @@ def build_yolov9(weights: Weights, scale: str = "c", nc: int = 80, in_h: int = 6
     g.down("model.19", h18, d[4], out=pb.sub(cat20, 0, d[4]))
     h21 = g.elan("model.21", g.feat(cat20), *r[6])
     A = v8_detect(pb, weights, "model.22", (h15[0], h18[0], h21[0]), nc, box_groups=4, conv_bn=g.conv_bn)
+    pb.meta[0], pb.meta[1] = nc, A
+    return pb
+
+
+def build_yolov9e(weights: Weights, nc: int = 80, in_h: int = 640, in_w: int = 640, cbfuse_in_place: bool = True) -> PlanBuilder:
+    """YOLOv9-E (GELAN-E, YOLOV9_E), ops emitted and weights requested in upstream's execution order (1-9, 10-14, 15, ...), so files
+    whose names were lost are consumed in graph order.  Each CBLinear (`model.{10..14}.conv`, biased 1x1, no BN, no activation) is one
+    GEMM writing all its groups into one buffer; each CBFuse is one OP_CBFUSE on the slice that conv 15 / 17 or ADown 20 / 23 / 26 has
+    just written (cbfuse_in_place False: into a buffer of its own, so that every op's inputs survive the run).  The two image convs
+    run in stem_conv.cu.  Inputs are multiples of 32, so every source's nearest-upsampling factor is an exact power of two."""
+    assert in_h % 32 == 0 and in_w % 32 == 0, f"YOLOv9 input {in_h}x{in_w}: a multiple of 32"
+    cfg = YOLOV9_E
+    pb = PlanBuilder(MODEL_YOLOV8, 3, in_h, in_w)
+    g = Yolov9Packer(pb, weights, "adown")
+    H, Wd = in_h, in_w
+    el, (h32, h35, h38, h41), (s2, s3), (d36, d39) = cfg["elan"], cfg["head"], cfg["spp"], cfg["head_downs"]
+    cat31 = pb.new_padded(H // 16, Wd // 16, s2 + el[2][0])     # [up(29), 25]
+    cat34 = pb.new_padded(H // 8, Wd // 8, h32[0] + el[1][0])   # [up(32), 22]
+    cat37 = pb.new_padded(H // 16, Wd // 16, d36 + h32[0])      # [36, 32]
+    cat40 = pb.new_padded(H // 32, Wd // 32, d39 + s2)          # [39, 29]
+    image = (pb.image, ((0, 3),))
+
+    # first backbone (1-9) and the CBLinear projections of layers 1, 3, 5, 7, 9 (10-14)
+    x1 = g.cbs("model.1", image, cfg["stem"][0], 3, 2)
+    x3 = g.elan("model.3", g.cbs("model.2", x1, cfg["stem"][1], 3, 2), *el[0])
+    x5 = g.elan("model.5", g.down("model.4", x3, cfg["downs"][0]), *el[1])
+    x7 = g.elan("model.7", g.down("model.6", x5, cfg["downs"][1]), *el[2])
+    x9 = g.elan("model.9", g.down("model.8", x7, cfg["downs"][2]), *el[3])
+    lin = []
+    for i, (x, groups) in enumerate(zip((x1, x3, x5, x7, x9), cfg["cbl"])):
+        assert all(c % 8 == 0 for c in groups) and x[1] == ((0, x[0].C),)
+        w, b = weights.conv_bias(f"model.{10 + i}.conv", sum(groups), x[0].C, 1)
+        lin.append(pb.conv(x[0], w, b, 1, 1, ACT_NONE))
+
+    def cbfuse(y, level):
+        """CBFuse of level `level` (output stride 2 << level): group `level` of CBLinear 10 + k, k >= level, upsampled by 2^(k - level)."""
+        w = cfg["cbl"][level][level]
+        srcs = [(pb.sub(lin[k], sum(cfg["cbl"][k][:level]), w), k - level) for k in range(level, len(lin))]
+        v = y[0]
+        assert y[1] == ((0, v.C),) and v.C == w, (y, w)
+        return g.feat(pb.cbfuse(v, srcs, out=None if cbfuse_in_place else pb.new_padded(v.H, v.W, v.C)))
+
+    # second backbone (15-28): its five stages each fused with the CBLinear groups of their resolution
+    y = cbfuse(g.cbs("model.15", image, cfg["stem"][0], 3, 2), 0)                 # 16
+    y = cbfuse(g.cbs("model.17", y, cfg["stem"][1], 3, 2), 1)                     # 18
+    y = cbfuse(g.down("model.20", g.elan("model.19", y, *el[0]), cfg["downs"][0]), 2)       # 21
+    y22 = g.elan("model.22", y, *el[1], out=pb.sub(cat34, h32[0], el[1][0]))
+    y = cbfuse(g.down("model.23", y22, cfg["downs"][1]), 3)                       # 24
+    y25 = g.elan("model.25", y, *el[2], out=pb.sub(cat31, s2, el[2][0]))
+    y = cbfuse(g.down("model.26", y25, cfg["downs"][2]), 4)                       # 27
+    y28 = g.elan("model.28", y, *el[3])
+
+    # head (29-41)
+    p29 = g.sppelan("model.29", y28, s2, s3, out=pb.sub(cat40, d39, s2))
+    pb.upsample2x(p29[0], pb.sub(cat31, 0, s2))                                   # 30, 31
+    p32 = g.elan("model.32", g.feat(cat31), *h32, out=pb.sub(cat37, d36, h32[0]))
+    pb.upsample2x(p32[0], pb.sub(cat34, 0, h32[0]))                               # 33, 34
+    p35 = g.elan("model.35", g.feat(cat34), *h35)
+    g.down("model.36", p35, d36, out=pb.sub(cat37, 0, d36))                       # 36, 37
+    p38 = g.elan("model.38", g.feat(cat37), *h38)
+    g.down("model.39", p38, d39, out=pb.sub(cat40, 0, d39))                       # 39, 40
+    p41 = g.elan("model.41", g.feat(cat40), *h41)
+    A = v8_detect(pb, weights, "model.42", (p35[0], p38[0], p41[0]), nc, box_groups=4, conv_bn=g.conv_bn)
     pb.meta[0], pb.meta[1] = nc, A
     return pb
 

@@ -1,6 +1,6 @@
 """Per-layer table of a plan at real clocks: every launch replayed alone (CUDA events, L2-warm), GEMM shapes and tile choices.
-usage: python tools/op_table.py yolov8|ufldv2|yolov5|yolov7|yolov7-tiny|yolov7-w6|yolov7-e6|yolov7-d6|yolov7-e6e|yolov6n|yolov6s|yolov6m|yolov6l|yolov9-t|yolov9-s|yolov9-m|yolov9-c|yolov9-e|yolov10n|yolov10s|yolov10m|yolov10b|yolov10l|yolov10x [batch] [iters]
-(the YOLOv7 P6 models run at 1280x1280)   (env switches of the library apply)"""
+usage: python tools/op_table.py yolov8|ufldv2|yolov5|yolov7|yolov7-tiny|yolov7-w6|yolov7-e6|yolov7-d6|yolov7-e6e|yolov6n|yolov6s|yolov6m|yolov6l|yolov6lite-s|yolov6lite-m|yolov6lite-l|yolov9-t|yolov9-s|yolov9-m|yolov9-c|yolov9-e|yolov10n|yolov10s|yolov10m|yolov10b|yolov10l|yolov10x [batch] [iters]
+(the YOLOv7 P6 models run at 1280x1280, YOLOv6-Lite at 320x320)   (env switches of the library apply)"""
 import os, re, sys, tempfile
 R = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, R); sys.path.insert(0, os.path.join(R, "tests"))
 import adas_b200
@@ -9,6 +9,10 @@ from gpu_util import cached_plan
 kind = sys.argv[1]; B = int(sys.argv[2]) if len(sys.argv) > 2 else 8; iters = int(sys.argv[3]) if len(sys.argv) > 3 else 20
 if kind.startswith("yolov7"):        # built fresh: ADAS_B200_STEMCONV decides at pack time where the stem runs
     pb = plan.build_yolov7(plan.synth_weights("yolov7", 0), {"yolov7": "base", "yolov7-tiny": "tiny"}.get(kind, kind[7:]))
+    path = os.path.join(tempfile.mkdtemp(), kind + ".b200w")
+    pb.write(path)
+elif kind.startswith("yolov6lite"):
+    pb = plan.build_yolov6_lite(plan.synth_weights("yolov6lite", 0, variant=kind[-1]), kind[-1])
     path = os.path.join(tempfile.mkdtemp(), kind + ".b200w")
     pb.write(path)
 elif kind.startswith("yolov6"):
@@ -30,7 +34,7 @@ eng = _capi.Engine(path, 0, max_batch=B)
 eng.run(B)
 n = eng.num_steps(B)
 names = {1: "gemm", 2: "im2col", 3: "maxpool", 4: "upsample", 5: "layernorm", 6: "stempack", 7: "stemconv", 8: "avgpool2", 9: "dwconv", 10: "attention",
-         11: "cbfuse", 31: "(folded)"}
+         11: "cbfuse", 12: "se", 13: "shuffle2", 31: "(folded)"}
 tot = 0.0; tot_g = 0.0; rows = []
 for i in range(n):
     ms, t, d = eng.time_step(B, i, iters)
@@ -75,4 +79,18 @@ if cb_rows:
         cb_bytes += 2 * B * p[2] * ob[3] * ob[4] * 2 + sum(2 * B * p[2] * pb.buffers[p[6 + 3 * s]][3] * pb.buffers[p[6 + 3 * s]][4] for s in range(p[5]))
     print(f"share of the sum of isolated launches: cbfuse {100 * ms_cb / tot:.1f} %; cbfuse {cb_bytes / 1e6:.1f} MB in {ms_cb * 1e3:.1f} us -> "
           f"{cb_bytes / ms_cb / 1e6:.0f} GB/s (HBM3 data sheet: 3350 GB/s)")
+se_rows = [r for r in rows if r[2] in ("se", "shuffle2")]
+if se_rows:
+    share = {k: sum(r[0] for r in rows if r[2] == k) for k in ("se", "shuffle2", "dwconv", "gemm")}
+    print("share of the sum of isolated launches: " + ", ".join(f"{k} {100 * v / tot:.1f} %" for k, v in share.items()))
+    for k in ("se", "shuffle2"):              # bytes from shapes: SE reads its fp16 slice twice (mean, then scale), writes it once and reads
+        nbytes = 0                            # its fp32 FC weights once per image; SHUFFLE2 reads two n-channel slices and writes 2n channels
+        for r in (r for r in rows if r[2] == k):
+            p = pb.ops[r[1]][1]
+            b = pb.buffers[p[0]]
+            nbytes += 2 * B * b[3] * b[4] * 3 * p[2] + B * 4 * (2 * p[2] * p[3] + p[2] + p[3]) if k == "se" else 2 * B * b[3] * b[4] * 4 * p[4]
+        print(f"{k}: {nbytes / 1e6:.2f} MB in {share[k] * 1e3:.1f} us -> {nbytes / share[k] / 1e6:.0f} GB/s (HBM3 data sheet: 3350 GB/s)")
+    act = sum(B * rows_ * C * (4 if f32 else 2) for rows_, C, f32, _, _, _ in pb.buffers)
+    wts = sum(t.nbytes for t in pb.tensors)
+    print(f"device memory of the plan at batch {B}: activations {act / 1e6:.1f} MB, weights {wts / 1e6:.2f} MB")
 eng.close()

@@ -2,6 +2,8 @@
 Prints the probability / box error the device path will show, the candidates per frame at box_score 0.4 and how many sit within 1e-3 / 2e-3
 of the threshold.  Test infrastructure (uses oracle/):  python tools/synth_operating_point.py yolov8 l 45,-9 40,-8.2
 (yolov9 t|s|m|c|e, yolov10 n|s|m|b|l|x: the scale's class bias; the head gains of plan.SYNTH_PROFILES[kind] are kept)
+(yolov6lite s|m|l: 320x320, gain = the class-logit gain, bias = the scale's class bias; the fp16 emulation is plan_interp's rounded run of
+the plan itself, tests/plan_interp_lite.py)
 """
 import sys, os
 R = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, R); sys.path.insert(0, os.path.join(R, 'tests'))
@@ -13,9 +15,26 @@ from oracle import nets, post
 import synth
 kind, variant = sys.argv[1], sys.argv[2]
 builder = {"yolov8": plan.build_yolov8, "yolov9": plan.build_yolov9, "yolov10": plan.build_yolov10}.get(kind, plan.build_yolov5)
-x = torch.from_numpy(np.concatenate([post.yolo_prepare_input(synth.frame(s), 640, 640)[0] for s in (0,1,2,3,4,5,6,7)]))
+size = 320 if kind == "yolov6lite" else 640
+x = torch.from_numpy(np.concatenate([post.yolo_prepare_input(synth.frame(s), size, size)[0] for s in (0,1,2,3,4,5,6,7)]))
 for a in sys.argv[3:]:
     g,b = map(float,a.split(','))
+    if kind=="yolov6lite":
+        import yolov6_lite_oracle, plan_interp_lite, test_yolov6_lite_cpu
+        from gpu_util import to_padded
+        plan.SYNTH_PROFILES["yolov6lite"]={**plan.SYNTH_PROFILES["yolov6lite"], "gains":[(r"detect\.cls_preds\.\d\.weight", g)],
+                                       "variants": {variant: {"fill": [(r"detect\.cls_preds\.\d\.bias", b)]}}}
+        W = plan.synth_weights(kind, 0, variant=variant); pb = plan.build_yolov6_lite(W, variant)
+        with torch.no_grad():
+            ref = yolov6_lite_oracle.build(W.state_dict, variant)(x).numpy()
+        emu = np.stack([test_yolov6_lite_cpu._decode(pb, plan_interp_lite.interpret(pb, to_padded(x[i:i + 1].numpy(), 4), 1, round_to_plan=True))
+                        for i in range(len(x))])
+        ref = np.concatenate([ref[..., :4], ref[..., 5:]], -1)
+        e=np.abs(ref[...,4:]-emu[...,4:]); mx=ref[...,4:].max(2); mg=emu[...,4:].max(2); eb=np.abs(ref[...,:4]-emu[...,:4]).max()
+        cand=mx>0.4
+        print(f"g={g} b={b}: max prob err {e.max():.2e} box err {eb:.3f} | cands {cand.sum(1).tolist()} within1e-3 {(np.abs(mx-0.4)<1e-3).sum(1).tolist()} flips {int((cand!=(mg>0.4)).sum())}", flush=True)
+        print("   per-frame max prob err", [f"{v:.2e}" for v in e.reshape(e.shape[0],-1).max(1)])
+        continue
     if kind=="yolov8":
         plan.SYNTH_PROFILES["yolov8"]={"gains":[(r"model\.22\.cv3\.\d\.2\.weight", g), (r"model\.22\.cv2\.\d\.2\.weight", 25.0)],"fill":[(r"model\.22\.cv3\.\d\.2\.bias", b)]}
     elif kind=="yolov9":

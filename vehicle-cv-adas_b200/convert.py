@@ -10,6 +10,7 @@ and `TrafficLaneDetector/convertPytorchToONNX.py:77-87` (UFLD `.pth` checkpoint 
     python -m adas_b200.convert yolov7-tiny.state_dict.pth --kind yolov7 --scale tiny
     python -m adas_b200.convert yolov7-w6.state_dict.pth --kind yolov7 --scale w6     # P6: w6 | e6 | d6 | e6e, 1280x1280
     python -m adas_b200.convert yolov6s.state_dict.pth --kind yolov6 --scale s
+    python -m adas_b200.convert yolov6lite_s.state_dict.pth --kind yolov6-lite --scale s    # s | m | l, 320x320
     python -m adas_b200.convert yolov9-c.state_dict.pth --kind yolov9 --scale c     # t | s | m | c | e
     python -m adas_b200.convert yolov10s.state_dict.pth --kind yolov10 --scale s    # n | s | m | b | l | x
     python -m adas_b200.convert yolov10s.onnx                                         # recognised, also with the top-k tail
@@ -17,6 +18,8 @@ and `TrafficLaneDetector/convertPytorchToONNX.py:77-87` (UFLD `.pth` checkpoint 
 Upstream YOLOv6 checkpoints pickle the whole model; extract its parameters once, in the YOLOv6 repository:
     torch.save(torch.load("yolov6s.pt", map_location="cpu", weights_only=False)["model"].float().state_dict(), "yolov6s.state_dict.pth")
 Training-form (rbr_dense / rbr_1x1 / rbr_identity + BatchNorm) and deployed (rbr_reparam, fused conv biases) keys are both accepted.
+YOLOv6-Lite checkpoints are extracted the same way; training-form (ConvBNHS / DPBlock with their BatchNorms) and fused keys are both
+accepted.  YOLOv6-Lite .onnx files are recognised like the other families.
 YOLOv9 checkpoints (WongKinYiu/yolov9) pickle the whole model too; extract the parameters once, in the YOLOv9 repository:
     torch.save(torch.load("yolov9-c-converted.pt", map_location="cpu", weights_only=False)["model"].float().state_dict(), "yolov9-c.state_dict.pth")
 Training-form (RepConvN conv1 / conv2 + BatchNorm) and fused (conv weight + bias) keys are both accepted; only the converted (GELAN)
@@ -72,6 +75,8 @@ def plan_from_state_dict(sd: Dict[str, np.ndarray], kind: str, scale: str = "l",
         return plan.build_yolov7(w, scale, nc=nc)
     if kind == "yolov6":
         return plan.build_yolov6(w, scale, nc=nc)
+    if kind == "yolov6-lite":
+        return plan.build_yolov6_lite(w, scale, nc=nc)
     if kind == "yolov9":
         return plan.build_yolov9(w, scale, nc=nc)
     if kind == "yolov10":
@@ -90,7 +95,7 @@ def convert(path: str, out: Optional[str] = None, kind: Optional[str] = None, sc
         pb = build_plan(model, recognise(model))
     else:
         if kind is None:
-            raise Exception("--kind is required for checkpoint files (yolov8 | yolov5 | yolov7 | yolov6 | yolov9 | yolov10 | ufldv2)")
+            raise Exception("--kind is required for checkpoint files (yolov8 | yolov5 | yolov7 | yolov6 | yolov6-lite | yolov9 | yolov10 | ufldv2)")
         pb = plan_from_state_dict(load_checkpoint_state_dict(path), kind, scale, backbone, nc)
     pb.write(out)
     return out
@@ -100,8 +105,8 @@ def main(argv=None) -> int:
     ap = argparse.ArgumentParser(description="convert an .onnx model or a state_dict checkpoint to a .b200w plan")
     ap.add_argument("model")
     ap.add_argument("--out", default=None)
-    ap.add_argument("--kind", default=None, choices=["yolov8", "yolov5", "yolov7", "yolov6", "yolov9", "yolov10", "ufldv2"])
-    ap.add_argument("--scale", default="l", help="YOLO scale letter (n | s | m | l for yolov6, t | s | m | c | e for yolov9, n | s | m | b | l | x for yolov10), or tiny | base | w6 | e6 | d6 | e6e for yolov7 (checkpoints only; ONNX files are recognised)")
+    ap.add_argument("--kind", default=None, choices=["yolov8", "yolov5", "yolov7", "yolov6", "yolov6-lite", "yolov9", "yolov10", "ufldv2"])
+    ap.add_argument("--scale", default="l", help="YOLO scale letter (n | s | m | l for yolov6, s | m | l for yolov6-lite, t | s | m | c | e for yolov9, n | s | m | b | l | x for yolov10), or tiny | base | w6 | e6 | d6 | e6e for yolov7 (checkpoints only; ONNX files are recognised)")
     ap.add_argument("--backbone", default="34", choices=["18", "34"], help="UFLDv2 ResNet depth (checkpoints only)")
     ap.add_argument("--nc", type=int, default=80)
     a = ap.parse_args(argv)

@@ -62,7 +62,7 @@ struct GemmParams {
     int kpt;        // k-blocks (of 64) per tap = ceil(Kc/64)
     int BN;         // tile width (multiple of 16, <= 256)
     int stages;     // smem pipeline depth
-    int act;        // 0 none, 1 SiLU, 2 ReLU, 3 LeakyReLU(0.1)
+    int act;        // 0 none, 1 SiLU, 2 ReLU, 3 LeakyReLU(0.1), 5 Hardswish
     int out_f32;    // 0: fp16 out, 1: fp32 out
     int out_ld;     // row stride of out, elements
     int res_ld;     // row stride of res, elements; NEGATIVE = add the residual before the activation (ResNet)
@@ -138,6 +138,19 @@ int launch_zero_rows(__half* buf, int ld, int C, int row0, int nrows, cudaStream
 // dwconv.cu: depthwise k x k conv (k 3 / 7, stride 1 / 2) of a channel slice, out = act(acc + bias) (+ res)
 int launch_dwconv(const __half* in, int in_ld, int B, int H, int W, int C, int k, int stride, const __half* w, const float* bias, int act,
                   const __half* res, int res_ld, __half* out, int out_ld, int Ho, int Wo, cudaStream_t st);
+// lite_ops.cu: squeeze-excite of a channel slice (YOLOv6-Lite SEBlock), gate = hardsigmoid(W2 relu(W1 mean + b1) + b2), one CTA per
+// image; W1 fp32 [hid][C], W2 fp32 [C][hid].  out may be in (in place).
+static const int kSeMaxC = 1024;
+struct SeParams {
+    const __half* in; int in_ld;
+    __half* out; int out_ld;
+    const float *w1, *b1, *w2, *b2;
+    int B, H, W, C, hid;
+};
+int se_supported(int C, int hid);
+int launch_se(const SeParams& p, cudaStream_t st);
+// lite_ops.cu: out(2j) = a(j), out(2j + 1) = b(j), j < n (concat + channel_shuffle(2)), interior pixels of an H x W padded grid
+int launch_shuffle2(const __half* a, int a_ld, const __half* b, int b_ld, __half* out, int out_ld, int B, int H, int W, int n, cudaStream_t st);
 // attention.cu: multi-head self-attention over the H*W pixels of each image (YOLOv10 PSA)
 int attention_supported(int nh, int kdp, int hd);
 int launch_attention(const __half* qkv, int in_ld, int B, int H, int W, int nh, int kdp, int hd, float scale, __half* out, int out_ld,
@@ -165,7 +178,7 @@ int launch_yolov5_head_decode(const YoloLevel* lv /*n_levels*/, int n_levels /*3
 int launch_yolov5_lite_post(float* raw /*[B,A,5+nc], in place*/, int B, int A, int nc, int in_h, int in_w, cudaStream_t st);
 // YOLOv6 level columns: 4 * (reg_max + 1) box columns (stored as 8-column groups), the nc class logits from the next multiple of 8 on
 __host__ __device__ inline unsigned yolov6_cls_col(unsigned reg_max) { return (4u * (reg_max + 1u) + 7u) / 8u * 8u; }
-int launch_yolov6_head_decode(const YoloLevel* lv /*3*/, int B, int nc, int reg_max, float* raw /*[B,A,5+nc]*/, int A, cudaStream_t st);
+int launch_yolov6_head_decode(const YoloLevel* lv /*n_levels*/, int n_levels /*3, or 4 (YOLOv6-Lite)*/, int B, int nc, int reg_max, float* raw /*[B,A,5+nc]*/, int A, cudaStream_t st);
 struct YoloPostBufs {
     // device scratch, sized for max_batch
     int32_t* flags;      // [B, A] candidate flag

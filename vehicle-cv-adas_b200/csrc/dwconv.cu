@@ -1,14 +1,17 @@
-// dwconv.cu -- depthwise k x k convolution (k = 3 or 7, stride 1 or 2) of a channel slice of a padded-NHWC fp16 buffer (OP_DWCONV).
+// dwconv.cu -- depthwise k x k convolution (k = 3 or 5, stride 1 or 2; k = 7, stride 1) of a channel slice of a padded-NHWC fp16 buffer
+// (OP_DWCONV).
 //
-// YOLOv10's SCDown, CIB, RepVGGDW (folded to one 7x7), PSA's positional conv and the v10 classification head.  Packing these as dense
+// YOLOv10's SCDown, CIB, RepVGGDW (folded to one 7x7), PSA's positional conv and the v10 classification head; YOLOv6-Lite's 3x3 and 5x5
+// (DPBlock) depthwise convs.  Packing these as dense
 // block-diagonal GEMMs would do C times the work and read C times the weight bytes, so they run here instead:
 //   one thread = 8 channels (one 16-byte vector) x DW_TX consecutive output pixels of one output row;
 //   per filter row the (DW_TX - 1) * S + K input pixels that the DW_TX windows cover are loaded once into registers and shared by all
 //   DW_TX outputs; the K input rows a thread reads are also read by the K - 1 neighbouring output rows, which run in the same or the
 //   next few CTAs, so those re-reads are served by L1 / L2 rather than HBM;
 //   weights are packed [k*k][C] fp16 (one tap of 8 channels = one 16-byte load), bias fp32, accumulation fp32 in a fixed tap order;
-//   epilogue: out = act(acc + bias) (+ res), rounded to fp16 once.
-// Taps are bound-checked against the H x W interior: the buffer's halo is one pixel wide and a 7x7 window reaches three pixels out, so
+//   epilogue: out = act(acc + bias) (+ res), rounded to fp16 once (act 0 none, 1 SiLU, 5 Hardswish).
+// Taps are bound-checked against the H x W interior: the buffer's halo is one pixel wide and a 5x5 / 7x7 window reaches two / three pixels
+// out, so
 // an unchecked tap would read the neighbouring row of the padded matrix (or the next image) instead of zero.  Only interior pixels of
 // the output slice are written; its halo stays zero.
 #include "common.h"
@@ -109,7 +112,7 @@ __global__ void __launch_bounds__(DW_THREADS) dwconv_kernel(const DwParams p) {
 int launch_dwconv(const __half* in, int in_ld, int B, int H, int W, int C, int k, int stride, const __half* w, const float* bias, int act,
                   const __half* res, int res_ld, __half* out, int out_ld, int Ho, int Wo, cudaStream_t st) {
     ADAS_CHECK(C % 8 == 0 && in_ld % 8 == 0 && out_ld % 8 == 0 && (res == nullptr || res_ld % 8 == 0), "dwconv: channel alignment");
-    ADAS_CHECK((k == 3 && (stride == 1 || stride == 2)) || (k == 7 && stride == 1), "dwconv: k %d stride %d (3 s1/s2, 7 s1)", k, stride);
+    ADAS_CHECK(((k == 3 || k == 5) && (stride == 1 || stride == 2)) || (k == 7 && stride == 1), "dwconv: k %d stride %d (3 / 5 s1 / s2, 7 s1)", k, stride);
     ADAS_CHECK(Ho == (H + 2 * (k / 2) - k) / stride + 1 && Wo == (W + 2 * (k / 2) - k) / stride + 1, "dwconv: output geometry %dx%d of %dx%d", Ho, Wo, H, W);
     DwParams p;
     p.in = in; p.in_ld = in_ld; p.w = w; p.bias = bias; p.res = res; p.res_ld = res_ld; p.out = out; p.out_ld = out_ld;
@@ -118,6 +121,8 @@ int launch_dwconv(const __half* in, int in_ld, int B, int H, int W, int C, int k
     long long blocks = (total + DW_THREADS - 1) / DW_THREADS;
     if (blocks > 132 * 16) blocks = 132 * 16;
     if (k == 7) dwconv_kernel<7, 1><<<(int)blocks, DW_THREADS, 0, st>>>(p);
+    else if (k == 5 && stride == 2) dwconv_kernel<5, 2><<<(int)blocks, DW_THREADS, 0, st>>>(p);
+    else if (k == 5) dwconv_kernel<5, 1><<<(int)blocks, DW_THREADS, 0, st>>>(p);
     else if (stride == 2) dwconv_kernel<3, 2><<<(int)blocks, DW_THREADS, 0, st>>>(p);
     else dwconv_kernel<3, 1><<<(int)blocks, DW_THREADS, 0, st>>>(p);
     count_launch();

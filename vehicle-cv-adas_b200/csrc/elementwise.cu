@@ -491,6 +491,7 @@ fc_stream_kernel(const __half* __restrict__ x, int x_ld, int batch, const __half
             if (act == 1) v = v / (1.f + __expf(-v));
             else if (act == 2) v = fmaxf(v, 0.f);
             else if (act == 3) v = v >= 0.f ? v : v * 0.1f;
+            else if (act == 5) v = v * fminf(fmaxf(v + 3.f, 0.f), 6.f) * (1.f / 6.f);     // Hardswish, as tc_common.cuh hardswish()
             const size_t o = (size_t)(b0 + b) * out_ld + n;
             if (out_f32) reinterpret_cast<float*>(out)[o] = v;
             else reinterpret_cast<__half*>(out)[o] = __float2half_rn(v);

@@ -329,7 +329,7 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
                 const int in_ld = (int)ib.C, H = (int)ib.H, W = (int)ib.W, C = p[2], k = p[3], s = p[4], act = p[5];
                 const int out_ld = (int)ob.C, Ho = (int)ob.H, Wo = (int)ob.W;
                 char d[128];
-                snprintf(d, sizeof(d), "dwconv %dx%d s%d C=%d, %dx%d -> %dx%d%s%s", k, k, s, C, H, W, Ho, Wo, act ? " silu" : "", res ? " +res" : "");
+                snprintf(d, sizeof(d), "dwconv %dx%d s%d C=%d, %dx%d -> %dx%d%s%s", k, k, s, C, H, W, Ho, Wo, act == 5 ? " hardswish" : act ? " silu" : "", res ? " +res" : "");
                 prog->step_desc.resize(prog->step_type.size());
                 prog->step_desc.back() = d;
                 prog->steps.push_back([=](cudaStream_t st) {
@@ -382,6 +382,35 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
                 prog->step_desc.resize(prog->step_type.size());
                 prog->step_desc.back() = d;
                 prog->steps.push_back([=](cudaStream_t st) { return launch_cbfuse(cp, st); });
+                break;
+            }
+            case OP_SE: {
+                const PlanBuffer& ib = e->bufs[p[0]];
+                const PlanBuffer& ob = e->bufs[p[8]];
+                SeParams sp;
+                sp.in = static_cast<const __half*>(e->dbufs[p[0]].ptr) + p[1]; sp.in_ld = (int)ib.C;
+                sp.out = static_cast<__half*>(e->dbufs[p[8]].ptr) + p[9]; sp.out_ld = (int)ob.C;
+                sp.w1 = static_cast<const float*>(tensor_ptr(e, p[4])); sp.b1 = static_cast<const float*>(tensor_ptr(e, p[5]));
+                sp.w2 = static_cast<const float*>(tensor_ptr(e, p[6])); sp.b2 = static_cast<const float*>(tensor_ptr(e, p[7]));
+                sp.B = batch; sp.H = (int)ib.H; sp.W = (int)ib.W; sp.C = p[2]; sp.hid = p[3];
+                char d[128];
+                snprintf(d, sizeof(d), "se C=%d hidden=%d %dx%d%s", sp.C, sp.hid, sp.H, sp.W, (p[0] == p[8] && p[1] == p[9]) ? " in place" : "");
+                prog->step_desc.resize(prog->step_type.size());
+                prog->step_desc.back() = d;
+                prog->steps.push_back([=](cudaStream_t st) { return launch_se(sp, st); });
+                break;
+            }
+            case OP_SHUFFLE2: {
+                const PlanBuffer& ob = e->bufs[p[5]];
+                const __half* a = static_cast<const __half*>(e->dbufs[p[0]].ptr) + p[1];
+                const __half* b = static_cast<const __half*>(e->dbufs[p[2]].ptr) + p[3];
+                __half* out = static_cast<__half*>(e->dbufs[p[5]].ptr) + p[6];
+                const int a_ld = (int)e->bufs[p[0]].C, b_ld = (int)e->bufs[p[2]].C, out_ld = (int)ob.C, H = (int)ob.H, W = (int)ob.W, n = p[4];
+                char d[128];
+                snprintf(d, sizeof(d), "shuffle2 2x%d channels %dx%d", n, H, W);
+                prog->step_desc.resize(prog->step_type.size());
+                prog->step_desc.back() = d;
+                prog->steps.push_back([=](cudaStream_t st) { return launch_shuffle2(a, a_ld, b, b_ld, out, out_ld, batch, H, W, n, st); });
                 break;
             }
             case OP_STEMPACK: {
@@ -475,13 +504,14 @@ static const float* yolo_anchors(const adas_engine* e) {
 }
 
 // A YOLOv5-layout (non-lite) head may have a fourth, stride-64 level (the P6 models); every other head has 3.
-static bool yolo_four_levels_ok(const PlanHeader& h) { return h.model_kind == ADAS_MODEL_YOLOV5 && h.meta[2] == 0; }
+// A YOLOv6 head may have one too (YOLOv6-Lite).
+static bool yolo_four_levels_ok(const PlanHeader& h) { return (h.model_kind == ADAS_MODEL_YOLOV5 && h.meta[2] == 0) || h.model_kind == ADAS_MODEL_YOLOV6; }
 
 static int head_decode(adas_engine* e, int batch) {
     if (is_ufld(e->hdr.model_kind)) return 0;   // heads are the raw FC output buffer
     YoloLevel lv[kYoloMaxLevels];
     const int nl = (int)e->outs.size();
-    ADAS_CHECK(nl == 3 || (nl == kYoloMaxLevels && yolo_four_levels_ok(e->hdr)), "YOLO plan must declare 3 output levels (4 for a YOLOv5-layout P6 head)");
+    ADAS_CHECK(nl == 3 || (nl == kYoloMaxLevels && yolo_four_levels_ok(e->hdr)), "YOLO plan must declare 3 output levels (4 for a YOLOv5-layout P6 head or a YOLOv6-Lite head)");
     for (int i = 0; i < nl; ++i) {
         const PlanOutput& o = e->outs[i];
         const PlanBuffer& b = e->bufs[o.buffer];
@@ -491,7 +521,7 @@ static int head_decode(adas_engine* e, int batch) {
     }
     const int nc = (int)e->hdr.meta[0], A = (int)e->hdr.meta[1];
     if (e->hdr.model_kind == ADAS_MODEL_YOLOV8) return launch_yolov8_head_decode(lv, batch, nc, e->d_raw, A, e->stream);
-    if (e->hdr.model_kind == ADAS_MODEL_YOLOV6) return launch_yolov6_head_decode(lv, batch, nc, (int)e->hdr.meta[2], e->d_raw, A, e->stream);
+    if (e->hdr.model_kind == ADAS_MODEL_YOLOV6) return launch_yolov6_head_decode(lv, nl, batch, nc, (int)e->hdr.meta[2], e->d_raw, A, e->stream);
     return launch_yolov5_head_decode(lv, nl, batch, nc, e->d_raw, A, (int)e->hdr.meta[2], yolo_anchors(e), e->stream);
 }
 // YOLOV5_LITE plans (meta[2] != 0): the network output is the sigmoid-only head; the fused detect calls apply
@@ -601,6 +631,16 @@ static const UfldDataset* ufld_dataset(const PlanHeader& h) {
 
 // Every index, offset and size of a plan file is checked before anything is allocated or launched: a plan is input data (the
 // reference trusts its .trt / .onnx files to TensorRT / ONNXRuntime, which validate them; here that job is ours).
+// Activation codes of plan.h: 0 none, 1 SiLU, 2 ReLU, 3 LeakyReLU(0.1), 5 Hardswish; 4 is unused.
+static bool act_code_ok(int act) { return (act >= 0 && act <= 3) || act == 5; }
+
+// A YOLOv6 head has 3 levels (strides 8 / 16 / 32), or 4 with a stride-64 level (YOLOv6-Lite); level i has stride 8 << i and a
+// ceil(H / stride) x ceil(W / stride) grid (a stride-2 conv of an odd-sized map rounds up).
+static bool yolov6_level_ok(const PlanHeader& h, const PlanOutput& o, const PlanBuffer& b, size_t i) {
+    const uint32_t s = 8u << i;
+    return o.stride == s && b.H == (h.in_h + s - 1) / s && b.W == (h.in_w + s - 1) / s;
+}
+
 static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* path) {
     const PlanHeader& h = e->hdr;
     const uint64_t rec_bytes = sizeof(PlanHeader) + (uint64_t)h.n_buffers * sizeof(PlanBuffer) + (uint64_t)h.n_ops * sizeof(PlanOp) +
@@ -650,7 +690,7 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
                 ADAS_CHECK(p[5] < 0 || (tensor_ok(p[5], (uint64_t)N * 4) && e->tensors[p[5]].dtype == 1), "plan %s: op %zu: bias tensor missing or too small", path, oi);
                 ADAS_CHECK(p[8] < 0 || (!transposed && view_ok(p[8], p[9], N) && e->bufs[p[8]].dtype == 0), "plan %s: op %zu: residual slice exceeds its buffer", path, oi);
                 ADAS_CHECK(p[15] >= 0 && p[15] <= 256 && p[17] >= 0 && p[17] <= 4 && (p[18] == 0 || p[18] == 1), "plan %s: op %zu: bad forced tile shape", path, oi);
-                ADAS_CHECK(p[7] >= 0 && p[7] <= 3, "plan %s: op %zu: unknown activation %d", path, oi, p[7]);
+                ADAS_CHECK(act_code_ok(p[7]), "plan %s: op %zu: unknown activation %d", path, oi, p[7]);
                 break;
             }
             case OP_IM2COL:
@@ -680,14 +720,14 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
                 ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[8]) && (rb == -1 || buf_ok(rb)), "plan %s: op %zu: dwconv buffer index out of range", path, oi);
                 const PlanBuffer &ib = e->bufs[p[0]], &ob = e->bufs[p[8]];
                 ADAS_CHECK(ib.dtype == 0 && ob.dtype == 0 && (rb < 0 || e->bufs[rb].dtype == 0), "plan %s: op %zu: dwconv buffers must be fp16", path, oi);
-                ADAS_CHECK((k == 3 && (s == 1 || s == 2)) || (k == 7 && s == 1), "plan %s: op %zu: dwconv k %d stride %d (3 s1 / s2, 7 s1)", path, oi, k, s);
-                ADAS_CHECK(act == 0 || act == 1, "plan %s: op %zu: dwconv act %d (0 none, 1 SiLU)", path, oi, act);
+                ADAS_CHECK(((k == 3 || k == 5) && (s == 1 || s == 2)) || (k == 7 && s == 1), "plan %s: op %zu: dwconv k %d stride %d (3 / 5 s1 / s2, 7 s1)", path, oi, k, s);
+                ADAS_CHECK(act == 0 || act == 1 || act == 5, "plan %s: op %zu: dwconv act %d (0 none, 1 SiLU, 5 Hardswish)", path, oi, act);
                 ADAS_CHECK(ib.H > 0 && ob.H > 0 && (int)ob.H == ((int)ib.H + 2 * (k / 2) - k) / s + 1 && (int)ob.W == ((int)ib.W + 2 * (k / 2) - k) / s + 1,
                            "plan %s: op %zu: dwconv output geometry %ux%u does not match a %dx%d stride-%d conv of %ux%u", path, oi, ob.H, ob.W, k, k, s, ib.H, ib.W);
                 ADAS_CHECK(C >= 8 && C % 8 == 0 && p[1] % 8 == 0 && p[9] % 8 == 0 && (rb < 0 || (p[11] % 8 == 0 && e->bufs[rb].C % 8 == 0)) &&
                            ib.C % 8 == 0 && ob.C % 8 == 0, "plan %s: op %zu: dwconv channels and offsets must be multiples of 8", path, oi);
                 ADAS_CHECK(tensor_ok(p[6], 0) && e->tensors[p[6]].dtype == 0 && e->tensors[p[6]].bytes == (uint64_t)C * k * k * 2,
-                           "plan %s: op %zu: dwconv weight tensor must be fp16 [k*k][C]", path, oi);
+                           "plan %s: op %zu: dwconv k %d: the weight tensor must be fp16 [k*k][C] (%llu bytes)", path, oi, k, (unsigned long long)C * k * k * 2);
                 ADAS_CHECK(tensor_ok(p[7], 0) && e->tensors[p[7]].dtype == 1 && e->tensors[p[7]].bytes == (uint64_t)C * 4,
                            "plan %s: op %zu: dwconv bias tensor must be fp32 [C]", path, oi);
                 ADAS_CHECK(rb < 0 || (e->bufs[rb].H == ob.H && e->bufs[rb].W == ob.W && view_ok(rb, p[11], C)),
@@ -746,12 +786,44 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
                 ADAS_CHECK(sep, "plan %s: op %zu: cbfuse source slice overlaps the output (only the base may be the output slice itself)", path, oi);
                 break;
             }
+            case OP_SE: {
+                const int C = p[2], hid = p[3];
+                ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[8]), "plan %s: op %zu: se buffer index out of range", path, oi);
+                const PlanBuffer &ib = e->bufs[p[0]], &ob = e->bufs[p[8]];
+                ADAS_CHECK(ib.dtype == 0 && ob.dtype == 0, "plan %s: op %zu: se buffers must be fp16", path, oi);
+                ADAS_CHECK(ib.H > 0 && ob.H == ib.H && ob.W == ib.W, "plan %s: op %zu: se output must have its input's H x W", path, oi);
+                ADAS_CHECK(se_supported(C, hid), "plan %s: op %zu: se with %d channels and %d hidden (C a multiple of 8 up to %d, 1 to %d hidden)", path, oi, C, hid,
+                           kSeMaxC, kSeMaxC / 4);
+                ADAS_CHECK(p[1] % 8 == 0 && p[9] % 8 == 0 && ib.C % 8 == 0 && ob.C % 8 == 0, "plan %s: op %zu: se channels and offsets must be multiples of 8", path, oi);
+                const uint64_t sz[4] = {(uint64_t)hid * C * 4, (uint64_t)hid * 4, (uint64_t)C * hid * 4, (uint64_t)C * 4};
+                for (int t = 0; t < 4; ++t)
+                    ADAS_CHECK(tensor_ok(p[4 + t], 0) && e->tensors[p[4 + t]].dtype == 1 && e->tensors[p[4 + t]].bytes == sz[t],
+                               "plan %s: op %zu: se tensor %d must be fp32 of %llu bytes (w1 [hid][C], b1 [hid], w2 [C][hid], b2 [C])", path, oi, t,
+                               (unsigned long long)sz[t]);
+                ADAS_CHECK(view_ok(p[0], p[1], C) && view_ok(p[8], p[9], C) && (p[0] != p[8] || p[1] == p[9] || p[9] >= p[1] + C || p[1] >= p[9] + C),
+                           "plan %s: op %zu: se channel slice exceeds its buffer or partly overlaps its input (in place or apart)", path, oi);
+                break;
+            }
+            case OP_SHUFFLE2: {
+                const int n = p[4];
+                ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[2]) && buf_ok(p[5]), "plan %s: op %zu: shuffle2 buffer index out of range", path, oi);
+                const PlanBuffer &ab = e->bufs[p[0]], &bb = e->bufs[p[2]], &ob = e->bufs[p[5]];
+                ADAS_CHECK(ab.dtype == 0 && bb.dtype == 0 && ob.dtype == 0, "plan %s: op %zu: shuffle2 buffers must be fp16", path, oi);
+                ADAS_CHECK(ob.H > 0 && ab.H == ob.H && ab.W == ob.W && bb.H == ob.H && bb.W == ob.W, "plan %s: op %zu: shuffle2 sources must have the output's H x W", path, oi);
+                ADAS_CHECK(n >= 8 && n % 8 == 0 && p[1] % 8 == 0 && p[3] % 8 == 0 && p[6] % 8 == 0 && ab.C % 8 == 0 && bb.C % 8 == 0 && ob.C % 8 == 0,
+                           "plan %s: op %zu: shuffle2 channels and offsets must be multiples of 8", path, oi);
+                ADAS_CHECK(view_ok(p[0], p[1], n) && view_ok(p[2], p[3], n) && (uint64_t)n * 2 <= (1u << 20) && view_ok(p[5], p[6], 2 * n),
+                           "plan %s: op %zu: shuffle2 channel slice exceeds its buffer", path, oi);
+                auto apart = [&](int b, int coff) { return b != p[5] || coff >= p[6] + 2 * n || p[6] >= coff + n; };
+                ADAS_CHECK(apart(p[0], p[1]) && apart(p[2], p[3]), "plan %s: op %zu: shuffle2 output overlaps a source", path, oi);
+                break;
+            }
             case OP_STEMPACK:
                 ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[1]) && e->bufs[p[0]].H > 0 && e->bufs[p[1]].H > 0 && e->bufs[p[0]].C == 4 && e->bufs[p[1]].C == 64, "plan %s: op %zu: bad stem re-layout", path, oi);
                 break;
             case OP_STEMCONV: {
                 const int Cout = p[3], k = p[4], s = p[9] == 0 ? 2 : p[9];          // p[9] = 0: stride 2 (plans without the field)
-                ADAS_CHECK(p[6] >= 0 && p[6] <= 3, "plan %s: op %zu: unknown activation %d", path, oi, p[6]);
+                ADAS_CHECK(act_code_ok(p[6]), "plan %s: op %zu: unknown activation %d", path, oi, p[6]);
                 ADAS_CHECK((s == 1 || s == 2) && buf_ok(p[0]) && e->bufs[p[0]].H > 0 && e->bufs[p[0]].C == 4 && stem_conv_supported(Cout, k, p[5]) &&
                            view_ok(p[7], p[8], Cout) && e->bufs[p[7]].H > 0 && tensor_ok(p[1], (uint64_t)Cout * k * ((4 * k + 15) / 16 * 16) * 2) &&
                            (p[2] < 0 || tensor_ok(p[2], (uint64_t)Cout * 4)) &&
@@ -801,11 +873,15 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
         if (h.model_kind == ADAS_MODEL_YOLOV6) {
             const uint32_t reg_max = h.meta[2];
             ADAS_CHECK(reg_max == 0 || reg_max == 16, "plan %s: YOLOv6 reg_max %u (0: raw distances, 16: 17-bin DFL)", path, reg_max);
-            ADAS_CHECK(h.n_outputs == 3, "plan %s: a YOLOv6 head has 3 levels", path);
+            const bool four = h.n_outputs == 4 && e->outs[3].stride == 64 && yolov6_level_ok(h, e->outs[3], e->bufs[e->outs[3].buffer], 3);
+            ADAS_CHECK(h.n_outputs == 3 || four, "plan %s: a YOLOv6 head has 3 levels, or 4 with a stride-64 level of ceil(H/64) x ceil(W/64) cells "
+                       "(the plan declares %u)", path, h.n_outputs);
             uint64_t A = 0;
             for (size_t i = 0; i < e->outs.size(); ++i) {
                 const PlanOutput& o = e->outs[i];
                 const PlanBuffer& b = e->bufs[o.buffer];
+                ADAS_CHECK(!four || yolov6_level_ok(h, o, b, i), "plan %s: YOLOv6 level %zu has stride %u and a %ux%u grid; stride %u of a %ux%u input needs "
+                           "ceil(H / stride) x ceil(W / stride) cells", path, i, o.stride, b.H, b.W, 8u << i, h.in_h, h.in_w);
                 ADAS_CHECK(b.dtype == 1 && b.H > 0 && o.C >= yolov6_cls_col(reg_max) + h.meta[0], "plan %s: YOLOv6 level %zu is %u columns wide; reg_max %u and %u classes need %u",
                            path, i, o.C, reg_max, h.meta[0], yolov6_cls_col(reg_max) + h.meta[0]);
                 A += (uint64_t)b.H * b.W;

@@ -33,7 +33,15 @@ namespace adas {
 
 // UP2: the 2x2 transposed-conv store (GemmParams::up2).  A separate instantiation (BN 64 / 128 / 256 only): its address arithmetic in the
 // unrolled epilogue costs the other instantiations spill slots, so they are compiled without it.
-template <int BN, bool UP2>
+// HS: the Hardswish epilogue (act 5), a separate instantiation for the same reason: one more activation branch in the shared epilogue
+// cost the BN 128 / 256 kernels 4 to 8 bytes of spill loads and YOLOv8-L ~3 % of its end-to-end rate on the H100.
+template <bool HS>
+__device__ __forceinline__ float v3_act(float x, int act) {
+    if constexpr (HS) return hardswish(x);
+    else return act_apply_base(x, act);
+}
+
+template <int BN, bool UP2, bool HS>
 __global__ void __launch_bounds__(V3_THREADS, 1)
 conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmV3 g) {
     constexpr int MTX = V3_ACC_COLS / BN >= 4 ? 4 : V3_ACC_COLS / BN >= 1 ? V3_ACC_COLS / BN : 1;   // sub-tiles held in registers
@@ -236,7 +244,7 @@ conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                             for (int e = 0; e < 2; ++e) {
                                 const int col = n0 + 8 * j + c0 + e;
                                 if (col < p.N) {
-                                    const float x = act_apply(acc[mt][4 * j + 2 * h + e] + row_bias, p.act);
+                                    const float x = v3_act<HS>(acc[mt][4 * j + 2 * h + e] + row_bias, p.act);
                                     if (p.out_f32) reinterpret_cast<float*>(p.out)[(size_t)col * (size_t)p.out_ld + row] = x;
                                     else reinterpret_cast<__half*>(p.out)[(size_t)col * (size_t)p.out_ld + row] = __float2half_rn(x);
                                 }
@@ -259,7 +267,7 @@ conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                             if (n0 + 8 * j >= p.N) break;
                             float x0 = acc[mt][4 * j + 2 * h], x1 = acc[mt][4 * j + 2 * h + 1];
                             if (p.bias != nullptr) { x0 += __ldg(p.bias + n); x1 += __ldg(p.bias + n + 1); }
-                            x0 = act_apply(x0, p.act); x1 = act_apply(x1, p.act);
+                            x0 = v3_act<HS>(x0, p.act); x1 = v3_act<HS>(x1, p.act);
                             const int q = (n >= co) + (n >= 2 * co) + (n >= 3 * co);
                             const size_t o = (size_t)(up_row + (q >> 1) * Wo2 + (q & 1)) * (size_t)p.out_ld + (n - q * co);
                             if (p.out_f32) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + o) = make_float2(x0, x1);
@@ -277,7 +285,8 @@ conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                         float2 rv = make_float2(0.f, 0.f);
                         if (rp != nullptr) rv = __half22float2(*reinterpret_cast<const __half2*>(rp + n));
                         if (p.res_ld < 0) { x0 += rv.x; x1 += rv.y; }
-                        if (p.act == 1) silu2(x0, x1);
+                        if constexpr (HS) { x0 = hardswish(x0); x1 = hardswish(x1); }
+                        else if (p.act == 1) silu2(x0, x1);
                         else if (p.act >= 2) { x0 = relu_leaky(x0, neg_slope); x1 = relu_leaky(x1, neg_slope); }
                         if (p.res_ld > 0) { x0 += p.res_scale * rv.x; x1 += p.res_scale * rv.y; }   // scale 1: the bits of a plain add
                         if (p.out_f32) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + (size_t)row * (size_t)p.out_ld + n) = make_float2(x0, x1);
@@ -293,21 +302,25 @@ conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
 // BN is a template parameter (the accumulator array and the wgmma widths are static): every multiple of 16 up to 256.
 #define V3_FOR_EACH_BN(X) X(16) X(32) X(48) X(64) X(80) X(96) X(112) X(128) X(144) X(160) X(176) X(192) X(208) X(224) X(240) X(256)
 
-static const void* v3_kernel(int BN, bool up2 = false) {
+template <bool HS>
+static const void* v3_kernel_act(int BN, bool up2) {
     if (up2) {
         switch (BN) {
-            case 64: return reinterpret_cast<const void*>(&conv_gemm_v3_kernel<64, true>);
-            case 128: return reinterpret_cast<const void*>(&conv_gemm_v3_kernel<128, true>);
-            case 256: return reinterpret_cast<const void*>(&conv_gemm_v3_kernel<256, true>);
+            case 64: return reinterpret_cast<const void*>(&conv_gemm_v3_kernel<64, true, HS>);
+            case 128: return reinterpret_cast<const void*>(&conv_gemm_v3_kernel<128, true, HS>);
+            case 256: return reinterpret_cast<const void*>(&conv_gemm_v3_kernel<256, true, HS>);
             default: return nullptr;
         }
     }
     switch (BN) {
-#define V3_CASE(b) case b: return reinterpret_cast<const void*>(&conv_gemm_v3_kernel<b, false>);
+#define V3_CASE(b) case b: return reinterpret_cast<const void*>(&conv_gemm_v3_kernel<b, false, HS>);
         V3_FOR_EACH_BN(V3_CASE)
 #undef V3_CASE
         default: return nullptr;
     }
+}
+static const void* v3_kernel(int BN, bool up2 = false, bool hswish = false) {
+    return hswish ? v3_kernel_act<true>(BN, up2) : v3_kernel_act<false>(BN, up2);
 }
 static bool v3_up2_tile(int BN) { return BN == 64 || BN == 128 || BN == 256; }
 
@@ -323,8 +336,10 @@ static int v3_device_state(int* num_sms) {
     V3Device& d = g_v3_dev[dev];
     if (!d.attr_set) {
         // function attributes are per device: set them once for every device an engine runs on
-        for (int bn = 16; bn <= 256; bn += 16) ADAS_CUDA(cudaFuncSetAttribute(v3_kernel(bn), cudaFuncAttributeMaxDynamicSharedMemorySize, V3_DYN_SMEM_MAX));
-        for (int bn = 64; bn <= 256; bn *= 2) ADAS_CUDA(cudaFuncSetAttribute(v3_kernel(bn, true), cudaFuncAttributeMaxDynamicSharedMemorySize, V3_DYN_SMEM_MAX));
+        for (int hs = 0; hs < 2; ++hs) {
+            for (int bn = 16; bn <= 256; bn += 16) ADAS_CUDA(cudaFuncSetAttribute(v3_kernel(bn, false, hs), cudaFuncAttributeMaxDynamicSharedMemorySize, V3_DYN_SMEM_MAX));
+            for (int bn = 64; bn <= 256; bn *= 2) ADAS_CUDA(cudaFuncSetAttribute(v3_kernel(bn, true, hs), cudaFuncAttributeMaxDynamicSharedMemorySize, V3_DYN_SMEM_MAX));
+        }
         ADAS_CUDA(cudaDeviceGetAttribute(&d.num_sms, cudaDevAttrMultiProcessorCount, dev));
         d.attr_set = true;
     }
@@ -405,7 +420,7 @@ int gemm_v3_launch(const GemmV3Launch& L, cudaStream_t st) {
     static const int pdl = env_int("ADAS_B200_PDL", 1);
     GemmV3 gp = L.g;
     gp.pdl = pdl ? 1 : 0;
-    const void* fn = v3_kernel(gp.p.BN, gp.p.up2 != 0);
+    const void* fn = v3_kernel(gp.p.BN, gp.p.up2 != 0, gp.p.act == 5);
     ADAS_CHECK(fn != nullptr, "gemm_v3: no kernel for BN %d%s", gp.p.BN, gp.p.up2 ? " with the transposed-conv store" : "");
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(gp.total_tiles < num_sms ? gp.total_tiles : num_sms, 1, 1);

@@ -44,7 +44,7 @@ struct PlanOutput {
 #pragma pack(pop)
 
 enum PlanOpType : uint32_t {
-    OP_GEMM = 1,       // act: 0 none, 1 SiLU, 2 ReLU, 3 LeakyReLU(0.1)
+    OP_GEMM = 1,       // act: 0 none, 1 SiLU, 2 ReLU, 3 LeakyReLU(0.1), 5 Hardswish x * clamp(x + 3, 0, 6) / 6 (4 is unused and rejected)
                        // p: a_buf a_coff Kc ntaps w_tensor bias_tensor N act res_buf res_coff res_pre_act out_buf out_coff masked transposed BN s2 MT no_slab
                        //    up2
                        //    (BN / MT > 0 force the tile shape, no_slab = 1 one activation tile per 3x3 tap: test hooks;
@@ -64,7 +64,7 @@ enum PlanOpType : uint32_t {
     OP_AVGPOOL2 = 8,   // p: in_buf in_coff C out_buf out_coff fill : 2x2 stride-1 mean into a buffer of the input's H x W geometry;
                        //    row H-1 and column W-1 hold 0 (fill 0) or -inf (fill 1), see elementwise.cu avgpool2_kernel
     OP_DWCONV = 9,     // p: in_buf in_coff C k stride act w_tensor bias_tensor out_buf out_coff res_buf res_coff : depthwise k x k conv
-                       //    (k 3 or 7, pad k/2, stride 1 or 2 with k 3), weights fp16 [k*k][C], bias fp32 [C], act 0 none / 1 SiLU;
+                       //    (k 3, 5 or 7, pad k/2, stride 1 or 2 with k 3 / 5), weights fp16 [k*k][C], bias fp32 [C], act 0 none / 1 SiLU / 5 Hardswish;
                        //    out = act(acc + bias) (+ res, res_buf -1: none), see dwconv.cu
     OP_ATTN = 10,      // p: in_buf in_coff nh kdp hd out_buf out_coff ; f0 = softmax scale : multi-head self-attention over the H*W
                        //    pixels; input channels [Q nh*kdp | K nh*kdp | V nh*hd], output nh*hd channels head-major, see attention.cu
@@ -72,6 +72,13 @@ enum PlanOpType : uint32_t {
                        //    out(y, x, c) = base(y, x, c) + sum_i src_i(y >> shift_i, x >> shift_i, src_coff_i + c) over the output's
                        //    interior (n_src 1..5, shift 0..4, src H x W << shift == out H x W); fp32 sum in the listed order, one
                        //    rounding; base may be the output slice itself (in place), see elementwise.cu cbfuse_kernel
+    OP_SE = 12,        // p: in_buf in_coff C hid w1 b1 w2 b2 out_buf out_coff : YOLOv6-Lite SEBlock over the interior of a C-channel slice,
+                       //    gate = hardsigmoid(w2 relu(w1 mean(x) + b1) + b2), out = x * gate (one fp16 rounding); fp32 tensors w1 [hid][C],
+                       //    b1 [hid], w2 [C][hid], b2 [C]; C % 8 == 0, C <= 1024, 1 <= hid <= 256; out == in slice (in place) or disjoint
+                       //    from it, see lite_ops.cu se_kernel
+    OP_SHUFFLE2 = 13,  // p: a_buf a_coff b_buf b_coff n out_buf out_coff : concat + channel_shuffle(2) of two n-channel slices,
+                       //    out(y, x, 2j) = a(y, x, j), out(y, x, 2j + 1) = b(y, x, j) over the interior (n % 8 == 0; all three on one
+                       //    H x W grid; the 2n-channel output slice overlaps neither source), see lite_ops.cu shuffle2_kernel
 };
 
 }  // namespace adas

@@ -125,7 +125,7 @@ __global__ void __launch_bounds__(STEM_THREADS) stem_conv_kernel(const StemParam
 }
 
 int stem_conv_supported(int Cout, int k, int pad) {
-    return (Cout == 16 || Cout == 32 || Cout == 48 || Cout == 64 || Cout == 80 || Cout == 96) && k >= 3 && k <= 7 && pad >= 0 && pad <= 3;
+    return (Cout == 16 || Cout == 24 || Cout == 32 || Cout == 48 || Cout == 64 || Cout == 80 || Cout == 96) && k >= 3 && k <= 7 && pad >= 0 && pad <= 3;
 }
 
 // The 80 / 96-channel stems (YOLOv7-E6 / E6E / D6, ReOrg + 3x3 folded into a 6x6 stride-2 conv) stage more than 48 KB: the kernel opts
@@ -173,6 +173,7 @@ int launch_stem_conv(const __half* img, int B, int H, int W, const __half* wq, c
     if (blocks > cap) blocks = cap;
     switch (Cout / 8) {
         case 2: stem_conv_kernel<2><<<blocks, STEM_THREADS, smem, st>>>(p); break;
+        case 3: stem_conv_kernel<3><<<blocks, STEM_THREADS, smem, st>>>(p); break;      // YOLOv6-Lite's 24-channel stem
         case 4: stem_conv_kernel<4><<<blocks, STEM_THREADS, smem, st>>>(p); break;
         case 6: stem_conv_kernel<6><<<blocks, STEM_THREADS, smem, st>>>(p); break;
         case 10: stem_conv_kernel<10><<<blocks, STEM_THREADS, smem, st>>>(p); break;

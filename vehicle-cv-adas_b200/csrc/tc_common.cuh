@@ -123,11 +123,19 @@ struct WgmmaCols<OFF, 0> {
 // (x * 0 = -0) into +0, the bits fmaxf(x, 0) gives.
 __device__ __forceinline__ float relu_leaky(float x, float s) { return fmaxf(x, x * s) + 0.0f; }
 
-__device__ __forceinline__ float act_apply(float x, int act) {
+// Hardswish (torch.nn.Hardswish): x * clamp(x + 3, 0, 6) / 6 in fp32, the division as a product with fp32(1/6) (within one fp32 ulp of
+// the quotient; a true IEEE division inlines a slow-path subroutine).
+__device__ __forceinline__ float hardswish(float x) { return x * fminf(fmaxf(x + 3.0f, 0.0f), 6.0f) * (1.0f / 6.0f); }
+
+// Activation codes 0 none, 1 SiLU, 2 ReLU, 3 LeakyReLU(0.1); the GEMM kernel's instantiations without Hardswish use this alone.
+__device__ __forceinline__ float act_apply_base(float x, int act) {
     if (act == 1) return __fdividef(x, 1.0f + __expf(-x));   // SiLU
     if (act >= 2) return relu_leaky(x, act == 3 ? 0.1f : 0.0f);   // ReLU, LeakyReLU(0.1)
     return x;
 }
+
+// Activation codes of plan.h: 0 none, 1 SiLU, 2 ReLU, 3 LeakyReLU(0.1), 5 Hardswish (4 is unused).
+__device__ __forceinline__ float act_apply(float x, int act) { return act == 5 ? hardswish(x) : act_apply_base(x, act); }
 
 __device__ __forceinline__ float ex2_approx(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float rcp_approx(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }

@@ -65,14 +65,20 @@ int launch_yolov8_head_decode(const YoloLevel* lv, int B, int nc, float* raw, in
 // x R+1 bins; R = reg_max), class logits from yolov6_cls_col(R).  R = 0: the four columns are the distances; R = 16: softmax over the 17
 // bins projected on 0..16 (the fixed proj_conv).  raw[b][a][5+nc], a = level offset + y*W + x: cx, cy, w, h (input pixels), 1.0, the class
 // sigmoids -- the YOLOv5 layout, so `conf = cls * obj` of the v5 post-processing is exactly the class probability.
-__global__ void yolov6_decode_kernel(YoloLevel l0, YoloLevel l1, YoloLevel l2, int B, int nc, int reg_max, float* __restrict__ raw, int A) {
+// Up to four head levels by value (strides 8 / 16 / 32 / 64 of the P6 models), n of them in use.
+struct YoloLevels { YoloLevel l[kYoloMaxLevels]; int n; };
+
+// 3 levels, or 4 with a stride-64 level (YOLOv6-Lite); the per-anchor arithmetic does not depend on the level count.
+__global__ void yolov6_decode_kernel(const YoloLevels L, int B, int nc, int reg_max, float* __restrict__ raw, int A) {
     const long long total = (long long)B * A;
     const int nb = reg_max + 1, cc = (int)yolov6_cls_col((unsigned)reg_max);
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const int b = (int)(i / A);
         int a = (int)(i % A);
-        YoloLevel lv = l0;
-        if (a >= l0.H * l0.W) { a -= l0.H * l0.W; lv = l1; if (a >= l1.H * l1.W) { a -= l1.H * l1.W; lv = l2; } }
+        YoloLevel lv = L.l[0];
+#pragma unroll
+        for (int j = 1; j < kYoloMaxLevels; ++j)
+            if (j < L.n && a >= lv.H * lv.W) { a -= lv.H * lv.W; lv = L.l[j]; }
         const int y = a / lv.W, x = a % lv.W;
         const float* p = lv.ptr + ((size_t)b * lv.rows_per_img + (size_t)(y + 1) * (lv.W + 2) + (x + 1)) * lv.ld;
         float d[4];
@@ -102,10 +108,14 @@ __global__ void yolov6_decode_kernel(YoloLevel l0, YoloLevel l1, YoloLevel l2, i
     }
 }
 
-int launch_yolov6_head_decode(const YoloLevel* lv, int B, int nc, int reg_max, float* raw, int A, cudaStream_t st) {
+int launch_yolov6_head_decode(const YoloLevel* lv, int n_levels, int B, int nc, int reg_max, float* raw, int A, cudaStream_t st) {
+    ADAS_CHECK(n_levels == 3 || n_levels == kYoloMaxLevels, "YOLOv6 decode: %d levels (3 or 4)", n_levels);
+    YoloLevels L;
+    for (int j = 0; j < kYoloMaxLevels; ++j) L.l[j] = lv[j < n_levels ? j : 0];
+    L.n = n_levels;
     const long long total = (long long)B * A;
     int blocks = (int)((total + 127) / 128);
-    yolov6_decode_kernel<<<blocks, 128, 0, st>>>(lv[0], lv[1], lv[2], B, nc, reg_max, raw, A);
+    yolov6_decode_kernel<<<blocks, 128, 0, st>>>(L, B, nc, reg_max, raw, A);
     count_launch();
     ADAS_CUDA(cudaGetLastError());
     return 0;
@@ -115,9 +125,6 @@ int launch_yolov6_head_decode(const YoloLevel* lv, int B, int nc, int reg_max, f
 // raw[b][idx][5+nc], idx = level offset + anchor*H*W + y*W + x  (yoloDetector.py:45-48 ordering).
 // Anchor (w, h) pairs [level][anchor]: the plan's own table (YOLOv7; 3 or 4 levels) or, without one, the YOLOv5 table below (3 levels).
 __constant__ float c_v5_anchors[18] = {10, 13, 16, 30, 33, 23, 30, 61, 62, 45, 59, 119, 116, 90, 156, 198, 373, 326};
-
-// Up to four head levels by value (strides 8 / 16 / 32 / 64 of the P6 models), n of them in use.
-struct YoloLevels { YoloLevel l[kYoloMaxLevels]; int n; };
 
 // lite != 0: the head of a YOLOv5-lite export -- sigmoid only, grid/anchor decode left to lite_postprocess (yoloDetector.py:36-50).
 __global__ void yolov5_decode_kernel(const YoloLevels L, int B, int nc, float* __restrict__ raw, int A, int lite, const float* __restrict__ anchors) {

@@ -354,7 +354,7 @@ def _is_module_name(name: str) -> bool:
 # ---------------------------------------------------------------------------------------------------------------
 @dataclass
 class ModelSpec:
-    kind: str                 # "yolov8" | "yolov5" | "yolov7" | "yolov6" | "yolov9" | "yolov10" | "ufldv2"
+    kind: str                 # "yolov8" | "yolov5" | "yolov7" | "yolov6" | "yolov6-lite" | "yolov9" | "yolov10" | "ufldv2"
     scale: str                # YOLO scale letter ("tiny" / "base" for YOLOv7) or ResNet depth ("18" / "34")
     nc: int = 80
     in_h: int = 640
@@ -387,9 +387,11 @@ def recognise(model: OnnxModel) -> ModelSpec:
         return _recognise_yolov9(model, w, in_h, in_w)
     if any(n.op_type == "ConvTranspose" for n in model.nodes):       # YOLOv6's BiFusion; v5 / v7 / v8 upsample with Resize
         return _recognise_yolov6(model, w, in_h, in_w)
+    if _is_yolov6_lite(model):                                       # depthwise convs + SEBlock's HardSigmoid, no transposed conv
+        return _recognise_yolov6_lite(model, w, in_h, in_w)
     if _is_yolov7(model, w):
         return _recognise_yolov7(model, w, in_h, in_w)
-    if _is_yolov10(model):                                           # depthwise convs + PSA's softmax; v6-Lite is refused above
+    if _is_yolov10(model):                                           # depthwise convs + PSA's softmax; v6-Lite is taken above
         return _recognise_yolov10(model, w, in_h, in_w)
     cout0, k0 = first.shape[0], first.shape[2]
     if cout0 not in _V8_WIDTH:
@@ -527,7 +529,9 @@ def _recognise_yolov7_p6(model: OnnxModel, w: OnnxWeights, stem, heads, in_h: in
     return ModelSpec("yolov7", scales[0], no // 3 - 5, in_h or 1280, in_w or 1280, act, _v7_anchors(model, 4))
 
 
-_V6_SUPPORTED = "YOLOv6-N / S / M / L (release 0.4.0, P5, 3 detection levels; YOLOv6-Lite, the P6 models and the 2.x models are not supported)"
+_V6_SUPPORTED = ("YOLOv6-N / S / M / L (release 0.4.0, P5, 3 detection levels, BiFusion's transposed convs) and YOLOv6-Lite-S / M / L "
+                 "(4 detection levels, depthwise convs and SEBlock, no transposed conv, input a multiple of 32); the P6 models and the 2.x "
+                 "models are not supported")
 _V6_WIDTH = {16: "n", 32: "s", 48: "m", 64: "l"}
 
 
@@ -569,7 +573,8 @@ def _v6_role(name: str) -> Optional[str]:
 def _recognise_yolov6(model: OnnxModel, w: OnnxWeights, in_h: int, in_w: int) -> ModelSpec:
     grouped = [n.inputs[1] for n in model.nodes if n.op_type == "Conv" and int(n.attrs.get("group", 1)) > 1]
     if grouped:
-        raise Exception(f"YOLOv6 file with grouped / depthwise convolutions ({grouped[0]}: a YOLOv6-Lite model); supported: {_V6_SUPPORTED}")
+        raise Exception(f"YOLOv6 file with grouped / depthwise convolutions ({grouped[0]}) and transposed convolutions: neither "
+                        f"YOLOv6-N / S / M / L nor YOLOv6-Lite; supported: {_V6_SUPPORTED}")
     named = {k for k in model.initializers if _is_module_name(k)}
     cls = sorted((k for k in named if re.fullmatch(r"detect\.cls_preds\.\d+\.weight", k)), key=lambda k: int(k.split(".")[2]))
     reg = sorted((k for k in named if re.fullmatch(r"detect\.reg_preds\.\d+\.weight", k)), key=lambda k: int(k.split(".")[2]))
@@ -600,6 +605,42 @@ def _recognise_yolov6(model: OnnxModel, w: OnnxWeights, in_h: int, in_w: int) ->
                             "a graph the packer cannot represent")
     return ModelSpec("yolov6", scale, nc, in_h or 640, in_w or 640, reg_max=0 if nbox == 4 else 16,
                      acts=(roles.get("body", "relu"), roles.get("neck", "relu"), roles.get("head", "silu")))
+
+
+_V6_LITE_WIDTH = {176: "s", 288: "m", 384: "l"}      # stage-4 output width (plan.yolov6_lite_widths)
+
+
+def _depthwise(model: OnnxModel) -> bool:
+    """Any depthwise convolution: group = Cin = Cout > 1."""
+    return any(n.op_type == "Conv" and int(n.attrs.get("group", 1)) > 1 and len(n.inputs) > 1 and n.inputs[1] in model.initializers
+               and model.initializers[n.inputs[1]].shape[1] == 1 and model.initializers[n.inputs[1]].shape[0] == int(n.attrs["group"])
+               for n in model.nodes)
+
+
+def _is_yolov6_lite(model: OnnxModel) -> bool:
+    """Depthwise convolutions together with SEBlock's HardSigmoid gate (Hardswish itself exports as HardSwish at opset >= 14, as
+    HardSigmoid + Mul at opset 12).  YOLOv10 files have depthwise convs but no HardSigmoid; no other supported family has one."""
+    return _depthwise(model) and any(n.op_type == "HardSigmoid" for n in model.nodes)
+
+
+def _recognise_yolov6_lite(model: OnnxModel, w: OnnxWeights, in_h: int, in_w: int) -> ModelSpec:
+    """YOLOv6-Lite-S / M / L: the scale comes from the stage-4 output width (the widest convolution outside the class predictions:
+    176 / 288 / 384), the class count from `detect.cls_preds.0`, which must have kept its module name."""
+    named = {k for k in model.initializers if _is_module_name(k)}
+    cls = sorted((k for k in named if re.fullmatch(r"detect\.cls_preds\.\d+\.weight", k)), key=lambda k: int(k.split(".")[2]))
+    if not cls:
+        raise Exception("YOLOv6-Lite file without its module names (detect.cls_preds.*): export the model with torch.onnx.export, which "
+                        f"keeps them; supported: {_V6_SUPPORTED}")
+    if len(cls) != 4:
+        raise Exception(f"YOLOv6-Lite file with {len(cls)} detection levels (4: strides 8 / 16 / 32 / 64); supported: {_V6_SUPPORTED}")
+    if len(model.outputs) != 1:
+        raise Exception(f"YOLOv6-Lite file with {len(model.outputs)} outputs; supported: {_V6_SUPPORTED}")
+    if (in_h and in_h % 32) or (in_w and in_w % 32):
+        raise Exception(f"YOLOv6-Lite file with a {in_h}x{in_w} input: a multiple of 32; supported: {_V6_SUPPORTED}")
+    width = max(int(cw.shape[0]) for name, cw, _ in w.convs if not name.startswith("detect.cls_preds."))
+    if width not in _V6_LITE_WIDTH:
+        raise Exception(f"YOLOv6-Lite file with a stage-4 width of {width} channels (176: S, 288: M, 384: L); supported: {_V6_SUPPORTED}")
+    return ModelSpec("yolov6-lite", _V6_LITE_WIDTH[width], int(model.initializers[cls[0]].shape[0]), in_h or 320, in_w or 320)
 
 
 _V9_SUPPORTED = ("YOLOv9-T / S / M / C / E (WongKinYiu/yolov9 v0.1, the converted GELAN graphs with a DDetect head, exported with one "
@@ -670,10 +711,7 @@ _V10_STEM = {16: ("n",), 32: ("s",), 48: ("m",), 64: ("b", "l"), 80: ("x",)}
 def _is_yolov10(model: OnnxModel) -> bool:
     """Depthwise convolutions (group = Cin = Cout > 1: SCDown, CIB, PSA's pe, the v10 class branch) together with a Softmax outside
     the DFL decode (PSA's attention).  YOLOv8 files have the DFL softmax but no depthwise conv; YOLOv9's grouped convs have 4 groups."""
-    dw = any(n.op_type == "Conv" and int(n.attrs.get("group", 1)) > 1 and len(n.inputs) > 1 and n.inputs[1] in model.initializers
-             and model.initializers[n.inputs[1]].shape[1] == 1 and model.initializers[n.inputs[1]].shape[0] == int(n.attrs["group"])
-             for n in model.nodes)
-    return dw and any(n.op_type == "Softmax" for n in model.nodes)
+    return _depthwise(model) and any(n.op_type == "Softmax" for n in model.nodes)
 
 
 def _recognise_yolov10(model: OnnxModel, w: OnnxWeights, in_h: int, in_w: int) -> ModelSpec:
@@ -731,6 +769,8 @@ def build_plan(model: OnnxModel, spec: Optional[ModelSpec] = None) -> "plan.Plan
         body, neck, head = spec.acts or (None, "relu", "silu")
         return plan.build_yolov6(w, spec.scale, nc=spec.nc, in_h=spec.in_h, in_w=spec.in_w, act_body=body, act_neck=neck, act_head=head,
                                  reg_max=spec.reg_max)
+    if spec.kind == "yolov6-lite":
+        return plan.build_yolov6_lite(w, spec.scale, nc=spec.nc, in_h=spec.in_h, in_w=spec.in_w)
     if spec.kind == "ufldv2":
         # the dataset follows from the input binding (ModelConfig: CULane 320x1600, TuSimple 320x800); the engine rejects any other
         cfg = dict(plan.UFLD_TUSIMPLE if (spec.in_h, spec.in_w) == (320, 800) else plan.UFLD_CULANE)

@@ -36,7 +36,9 @@ OP_GEMM, OP_IM2COL, OP_MAXPOOL, OP_UPSAMPLE2X, OP_LAYERNORM, OP_STEMPACK, OP_STE
 OP_AVGPOOL2 = 8
 OP_DWCONV, OP_ATTN = 9, 10
 OP_CBFUSE = 11
+OP_SE, OP_SHUFFLE2 = 12, 13
 ACT_NONE, ACT_SILU, ACT_RELU, ACT_LEAKY = 0, 1, 2, 3          # ACT_LEAKY: LeakyReLU(0.1)
+ACT_HSWISH = 5                                                # Hardswish x * clamp(x + 3, 0, 6) / 6; code 4 is unused
 PLAN_VERSION = 1
 
 
@@ -285,6 +287,18 @@ SYNTH_PROFILES = {
                "fill": [(r"detect\.reg_preds\.\d\.bias", 2.0)],
                "variants": {sc: {"fill": [(r"detect\.cls_preds\.\d\.bias", -3.0 + d)]}
                             for sc, d in (("n", -0.135), ("s", -0.177), ("m", -0.30), ("l", 0.595))}},
+    # YOLOv6-Lite S/M/L: Hardswish halves small activations (slope 1/2 at 0) and grows large ones quadratically, so a random net either
+    # forgets its input or blows up: at conv gain 1.0 the neck outputs of two synthetic frames differ by 0.1-5 %, at 1.2 S's neck
+    # reaches |x| ~ 10 and L's ~ 100, at 1.3 ~ 1e5 (fp32 oracle, frames 0-3).  Near that edge the net also amplifies rounding: at gain
+    # 1.15 the CPU fp16 emulation (plan_interp.interpret, every op rounded to its buffer dtype) was up to 8.5e-3 off in probability with
+    # YOLOv6's class gain 12.  Gain 1.1 (neck maps differ by 1-22 % between frames) with class gain 8 gives 3.3e-4 (S) to 7.0e-4 (L) on
+    # frames 0-3.  Box biases of 2 grid cells keep the raw l, t, r, b distances positive.  The class bias of each scale puts ~50 of the
+    # 2125 anchors (320 x 320) per frame above box_score = 0.4: at bias 0 the 50th-highest max-class logit sits 1.65 (S), 1.60 (M), 1.62
+    # (L) above 0, so the bias is -0.405 minus that; the per-anchor spread of the max-class logit is small (std 0.12).
+    "yolov6lite": {"conv_gain": 1.1,
+                   "gains": [(r"detect\.cls_preds\.\d\.weight", 8.0)],
+                   "fill": [(r"detect\.reg_preds\.\d\.bias", 2.0)],
+                   "variants": {sc: {"fill": [(r"detect\.cls_preds\.\d\.bias", -0.405 - d)]} for sc, d in (("s", 1.65), ("m", 1.60), ("l", 1.62))}},
 }
 
 
@@ -298,7 +312,7 @@ SYNTH_PROFILES_WORKLOAD = {
 
 
 def synth_weights(kind: str, seed: int = 0, variant: Optional[str] = None, workload: bool = False) -> "Weights":
-    """Seeded synthetic weights.  A profile's `variants` entry (YOLOv6, YOLOv9, YOLOv10) adds per-variant `fill` rules ahead of the shared ones; other
+    """Seeded synthetic weights.  A profile's `variants` entry (YOLOv6, YOLOv6-Lite, YOLOv9, YOLOv10) adds per-variant `fill` rules ahead of the shared ones; other
     kinds ignore `variant`."""
     prof = SYNTH_PROFILES_WORKLOAD.get(kind, SYNTH_PROFILES[kind]) if workload else SYNTH_PROFILES[kind]
     extra = prof.get("variants", {}).get(variant)
@@ -391,7 +405,7 @@ class PlanBuilder:
         if out is None:
             out = self.new_padded(Ho, Wo, n_store, f32=out_f32)
         assert out.H == Ho and out.W == Wo, (out, Ho, Wo)
-        stem_couts = (16, 32, 48, 64, 80, 96) if wide_stem else (16, 32, 48, 64)
+        stem_couts = (16, 24, 32, 48, 64, 80, 96) if wide_stem else (16, 24, 32, 48, 64)
         if (self.stem_direct and x.buf == self.image.buf and x.C == 4 and s in (1, 2) and 3 <= k <= 7 and cout in stem_couts and res is None
                 and not out_f32 and tile is None and out.coff % 8 == 0):
             return self.stem_conv(x, w, b, k, s, pad, act, out)
@@ -500,12 +514,13 @@ class PlanBuilder:
 
     def dwconv(self, x: View, w: np.ndarray, b: np.ndarray, k: int, s: int, act: int, out: Optional[View] = None,
                res: Optional[View] = None) -> View:
-        """Depthwise k x k conv (pad k/2; k 3 stride 1 / 2, k 7 stride 1) of x's channels: w [C_real, 1, k, k] fp32, b [C_real];
+        """Depthwise k x k conv (pad k/2; k 3 / 5 stride 1 / 2, k 7 stride 1) of x's channels: w [C_real, 1, k, k] fp32, b [C_real];
         x.C may exceed C_real (zero-padded channels get zero weights and bias).  out = act(conv + b) (+ res).  Weights are packed
         [k*k][C] fp16 so one tap of 8 channels is one 16-byte load (dwconv.cu)."""
         c_real = int(w.shape[0])
         assert w.shape[1:] == (1, k, k) and c_real <= x.C and x.C % 8 == 0 and x.coff % 8 == 0, (w.shape, x)
-        assert (k == 3 and s in (1, 2)) or (k == 7 and s == 1), (k, s)
+        assert (k in (3, 5) and s in (1, 2)) or (k == 7 and s == 1), (k, s)
+        assert act in (ACT_NONE, ACT_SILU, ACT_HSWISH), act
         Ho = (x.H + 2 * (k // 2) - k) // s + 1
         Wo = (x.W + 2 * (k // 2) - k) // s + 1
         if out is None:
@@ -551,6 +566,36 @@ class PlanBuilder:
             p += [v.buf, v.coff, shift]
         self._op(OP_CBFUSE, p)
         return View(out.buf, out.coff, out.C, out.H, out.W)
+
+    def se(self, x: View, w1: np.ndarray, b1: np.ndarray, w2: np.ndarray, b2: np.ndarray, out: Optional[View] = None) -> View:
+        """Squeeze-excite (YOLOv6-Lite SEBlock): out = x * hardsigmoid(w2 relu(w1 mean(x) + b1) + b2), mean over the H x W interior.
+        w1 [hid, C_real(, 1, 1)], b1 [hid], w2 [C_real, hid(, 1, 1)], b2 [C_real] (1x1 convs with bias), kept fp32.  x.C may exceed
+        C_real: the padded channels get zero FC weights, so they read as zero means and, being zero, stay zero.  out None: in place."""
+        hid, c_real = int(w1.shape[0]), int(w1.shape[1])
+        assert x.C % 8 == 0 and x.coff % 8 == 0 and c_real <= x.C and tuple(w2.shape[:2]) == (c_real, hid), (x, w1.shape, w2.shape)
+        out = x if out is None else out
+        assert (out.H, out.W, out.C) == (x.H, x.W, x.C) and out.coff % 8 == 0, (out, x)
+        w1p = np.zeros((hid, x.C), np.float32)
+        w1p[:, :c_real] = w1.reshape(hid, c_real)
+        w2p = np.zeros((x.C, hid), np.float32)
+        w2p[:c_real] = w2.reshape(c_real, hid)
+        b2p = np.zeros(x.C, np.float32)
+        b2p[:c_real] = b2
+        self._op(OP_SE, [x.buf, x.coff, x.C, hid, self.tensor(w1p), self.tensor(np.asarray(b1, np.float32).reshape(hid)),
+                         self.tensor(w2p), self.tensor(b2p), out.buf, out.coff])
+        return View(out.buf, out.coff, x.C, x.H, x.W)
+
+    def shuffle2(self, a: View, b: View, out: Optional[View] = None) -> View:
+        """torch.cat([a, b], 1) then channel_shuffle(groups = 2): out(2j) = a(j), out(2j + 1) = b(j); a.C == b.C, a multiple of 8."""
+        n = a.C
+        assert b.C == n and n % 8 == 0 and a.coff % 8 == 0 and b.coff % 8 == 0 and (a.H, a.W) == (b.H, b.W), (a, b)
+        if out is None:
+            out = self.new_padded(a.H, a.W, 2 * n)
+        assert out.C == 2 * n and (out.H, out.W) == (a.H, a.W) and out.coff % 8 == 0, out
+        for v in (a, b):
+            assert v.buf != out.buf or v.coff >= out.coff + 2 * n or out.coff >= v.coff + n, (v, out)
+        self._op(OP_SHUFFLE2, [a.buf, a.coff, b.buf, b.coff, n, out.buf, out.coff])
+        return View(out.buf, out.coff, 2 * n, a.H, a.W)
 
     def layernorm(self, in_buf: int, d_len: int, d_norm: int, gamma: np.ndarray, beta: np.ndarray, eps: float, out_buf: int) -> None:
         self._op(OP_LAYERNORM, [in_buf, d_len, self.tensor(gamma.astype(np.float32)), self.tensor(beta.astype(np.float32)), out_buf, d_norm],
@@ -1241,6 +1286,178 @@ def build_yolov6(weights: Weights, scale: str = "n", nc: int = 80, in_h: int = 6
         pb.outputs.append((head.buf, 0, head.C, stride))
         A += feat.H * feat.W
     pb.meta[0], pb.meta[1], pb.meta[2] = nc, A, reg_max
+    return pb
+
+
+# ---------------------------------------------------------------------------------------------
+# YOLOv6-Lite (meituan/YOLOv6 release 0.4.0, configs/yolov6_lite/yolov6_lite_{s,m,l}.py: Lite_EffiBackbone, Lite_EffiNeck,
+# Lite_EffideHead).  Restated from the upstream configs; no upstream file is available here, so the widths are pinned by the published
+# parameter counts (tests/test_yolov6_lite_cpu.py).
+# ---------------------------------------------------------------------------------------------
+YOLOV6_LITE_SCALES = {"s": 0.7, "m": 1.1, "l": 1.5}      # width_multiple
+YOLOV6_LITE_BLOCKS = (1, 3, 7, 3)                          # Lite_EffiBlockS2 + (n - 1) x Lite_EffiBlockS1 per stage
+YOLOV6_LITE_NECK = 96                                      # unified neck / head width
+YOLOV6_LITE_PARAMS = {"s": 0.55e6, "m": 0.79e6, "l": 1.09e6}   # published (README of release 0.4.0)
+
+
+def _make_divisible_mobile(v: float, d: int) -> int:
+    """Upstream `make_divisible` of the Lite models (MobileNet rounding): nearest multiple of d, at least d, and not below 0.9 v."""
+    n = max(d, int(v + d / 2) // d * d)
+    return n + d if n < 0.9 * v else n
+
+
+def yolov6_lite_widths(scale: str) -> Tuple[List[int], List[int], List[int]]:
+    """(backbone out_channels [stem, stage 1-4], mid_channels [stem slot unused, stage 1-4], neck inputs [P5, P4, P3])."""
+    assert scale in YOLOV6_LITE_SCALES, f"YOLOv6-Lite scale {scale!r}: 's', 'm' or 'l'"
+    w = YOLOV6_LITE_SCALES[scale]
+    out = [_make_divisible_mobile(c * w, 16) for c in (24, 32, 64, 128, 256)]
+    mid = [_make_divisible_mobile(int(c * 0.5), 8) for c in out]
+    out[0] = 24                                            # the stem is fixed at 24 channels
+    neck_in = [_make_divisible_mobile(c * w, 16) for c in (256, 128, 64)]
+    return out, mid, neck_in
+
+
+def _r8(v: View) -> View:
+    """The view widened to the 8-channel-aligned width its producer owns (a conv of Cout % 8 != 0 stores zero channels up to it)."""
+    return View(v.buf, v.coff, (v.C + 7) // 8 * 8, v.H, v.W)
+
+
+def build_yolov6_lite(weights: Weights, scale: str = "s", nc: int = 80, in_h: int = 320, in_w: int = 320, se_in_place: bool = True) -> PlanBuilder:
+    """YOLOv6-Lite-S/M/L under upstream module names (`backbone.conv_0`, `backbone.lite_effiblock_{1..4}.{j}`, `neck.reduce_layer{0,1,2}`,
+    `neck.Csp_{p4,p3,n3,n4}`, `neck.downsample{2,1}`, `neck.p6_conv_{1,2}`, `detect.{stems,cls_convs,reg_convs,cls_preds,reg_preds}.{0..3}`).
+    Output [B, A, 5 + nc] (MODEL_YOLOV6, reg_max 0) over four levels, strides 8 / 16 / 32 / 64; level i has ceil(H / s) x ceil(W / s) cells.
+
+    Every activation is Hardswish (ACT_HSWISH).  ConvBNHS / ConvBN (`name.block.conv` + `name.block.bn`) and DPBlock (`conv_dw_1` + `bn_1`,
+    `conv_pw_1` + `bn_2`, convs with bias) are folded in fp64; a deployed file carries the fused convs with a bias and no BatchNorm.
+    Depthwise convs run in dwconv.cu, SEBlock as OP_SE (in place), the concat + channel shuffle of Lite_EffiBlockS1 as OP_SHUFFLE2; the
+    split is a channel slice.  Channel widths that are not multiples of 8 (the S2 blocks' mid / 2 branch) are carried zero-padded.
+    se_in_place False: every SE writes a buffer of its own (same results; every op's inputs then survive the run, for per-op checks)."""
+    out_c, mid_c, neck_in = yolov6_lite_widths(scale)
+    assert in_h % 32 == 0 and in_w % 32 == 0, f"YOLOv6-Lite input {in_h}x{in_w}: a multiple of 32 in each dimension"
+    pb = PlanBuilder(MODEL_YOLOV6, 3, in_h, in_w)
+    W = weights
+    eps = BN_EPS_YOLO
+    U = YOLOV6_LITE_NECK
+    HS = ACT_HSWISH
+
+    def fold(name: str, conv: str, bn: str, cout: int, cin: int, k: int, conv_bias: bool):
+        """conv (+ its bias) then BatchNorm, folded in fp64; the fused form is `conv` with a bias and no `bn`."""
+        if W.real and f"{name}.{bn}.weight" not in W.state_dict:
+            return W.conv_bias(f"{name}.{conv}", cout, cin, k)
+        w = W.get(f"{name}.{conv}.weight", (cout, cin, k, k), "conv").astype(np.float64)
+        cb = np.zeros(cout)
+        if conv_bias and (not W.real or f"{name}.{conv}.bias" in W.state_dict):
+            cb = W.get(f"{name}.{conv}.bias", (cout,), "bias").astype(np.float64)
+        g = W.get(f"{name}.{bn}.weight", (cout,), "bn_gamma").astype(np.float64)
+        be = W.get(f"{name}.{bn}.bias", (cout,), "bn_beta").astype(np.float64)
+        m = W.get(f"{name}.{bn}.running_mean", (cout,), "bn_mean").astype(np.float64)
+        v = W.get(f"{name}.{bn}.running_var", (cout,), "bn_var").astype(np.float64)
+        if not W.real and f"{name}.{bn}.num_batches_tracked" not in W.state_dict:
+            W.state_dict[f"{name}.{bn}.num_batches_tracked"] = np.zeros((), dtype=np.int64)
+        sc = g / np.sqrt(v + eps)
+        return (w * sc[:, None, None, None]).astype(np.float32), ((cb - m) * sc + be).astype(np.float32)
+
+    def cbn(x: View, name: str, cout: int, k: int, s: int = 1, act: int = HS, dw: bool = False, out: Optional[View] = None,
+            cin: Optional[int] = None) -> View:
+        """ConvBNHS (act) / ConvBN (act none): `name.block.conv` + `name.block.bn`, no conv bias."""
+        cin = cout if dw else (cin if cin is not None else x.C)
+        w, b = fold(f"{name}.block", "conv", "bn", cout, 1 if dw else cin, k, False)
+        xa = x if x.buf == pb.image.buf else _r8(x)         # the image buffer carries a zero fourth channel
+        if dw:
+            return pb.dwconv(xa, w, b, k, s, act, out=out)
+        return pb.conv(xa, w, b, k, s, act, out=out)
+
+    def dp(x: View, name: str, c: int, k: int = 5, s: int = 1, out: Optional[View] = None, res: Optional[View] = None) -> View:
+        """DPBlock: depthwise k x k (stride s) + BN + Hardswish, then 1x1 + BN + Hardswish (+ res after the activation)."""
+        wd, bd = fold(name, "conv_dw_1", "bn_1", c, 1, k, True)
+        t = pb.dwconv(x, wd, bd, k, s, HS)
+        wp, bp = fold(name, "conv_pw_1", "bn_2", c, c, 1, True)
+        return pb.conv(t, wp, bp, 1, 1, HS, out=out, res=res)
+
+    def se(x: View, name: str, c: int) -> View:
+        hid = c // 4
+        w1, b1 = W.conv_bias(f"{name}.conv1", hid, c, 1)
+        w2, b2 = W.conv_bias(f"{name}.conv2", c, hid, 1)
+        x = _r8(x)
+        return pb.se(x, w1, b1, w2, b2, out=None if se_in_place else pb.new_padded(x.H, x.W, x.C))
+
+    def block_s1(x: View, name: str, mid: int, cout: int) -> View:
+        h = cout // 2
+        t = cbn(pb.sub(x, h, h), f"{name}.conv_pw_1", mid, 1)
+        t = cbn(t, f"{name}.conv_dw_1", mid, 3, act=ACT_NONE, dw=True)
+        t = se(t, f"{name}.se", mid)
+        t = cbn(t, f"{name}.conv_1", h, 1, cin=mid)
+        return pb.shuffle2(pb.sub(x, 0, h), t)
+
+    def block_s2(x: View, name: str, cin: int, mid: int, cout: int) -> View:
+        h, m2 = cout // 2, mid // 2
+        Ho, Wo = (x.H - 1) // 2 + 1, (x.W - 1) // 2 + 1
+        cat = pb.new_padded(Ho, Wo, cout)
+        t = cbn(x, f"{name}.conv_dw_1", cin, 3, 2, act=ACT_NONE, dw=True)
+        cbn(t, f"{name}.conv_1", h, 1, cin=cin, out=pb.sub(cat, 0, h))
+        t = cbn(x, f"{name}.conv_pw_2", m2, 1, cin=cin)
+        t = cbn(t, f"{name}.conv_dw_2", m2, 3, 2, act=ACT_NONE, dw=True)
+        t = se(t, f"{name}.se", m2)
+        cbn(t, f"{name}.conv_2", h, 1, cin=m2, out=pb.sub(cat, h, h))
+        t = cbn(cat, f"{name}.conv_dw_3", cout, 3, dw=True)
+        return cbn(t, f"{name}.conv_pw_3", cout, 1)
+
+    def csp(x: View, name: str, out: Optional[View] = None) -> View:
+        """CSPBlock(2U, U, k=5): conv_3(cat(blocks(conv_1(x)), conv_2(x))), blocks = DarknetBlock (1x1 HS, then DPBlock k=5)."""
+        m = U // 2
+        cat = pb.new_padded(x.H, x.W, 2 * m)
+        t = cbn(x, f"{name}.conv_1", m, 1)
+        t = cbn(t, f"{name}.blocks.conv_1", m, 1)
+        dp(t, f"{name}.blocks.conv_2", m, out=pb.sub(cat, 0, m))
+        cbn(x, f"{name}.conv_2", m, 1, out=pb.sub(cat, m, m))
+        return cbn(cat, f"{name}.conv_3", U, 1, out=out)
+
+    # backbone
+    x = cbn(pb.image, "backbone.conv_0", out_c[0], 3, 2, cin=3)
+    feats = []
+    for i, n in enumerate(YOLOV6_LITE_BLOCKS):
+        nm = f"backbone.lite_effiblock_{i + 1}"
+        x = block_s2(x, f"{nm}.0", out_c[i], mid_c[i + 1], out_c[i + 1])
+        for j in range(1, n):
+            x = block_s1(x, f"{nm}.{j}", mid_c[i + 1], out_c[i + 1])
+        if i:
+            feats.append(x)
+    x2, x1, x0 = feats
+    assert (x0.C, x1.C, x2.C) == tuple(neck_in), ((x0.C, x1.C, x2.C), neck_in)
+    # neck; the PAN concats are allocated up front and their producers write their slices
+    cat_p4 = pb.new_padded(x1.H, x1.W, 2 * U)          # [upsample(fpn_out0), reduce_layer1(x1)]
+    cat_p3 = pb.new_padded(x2.H, x2.W, 2 * U)          # [upsample(f_out1), reduce_layer2(x2)]
+    cat_n3 = pb.new_padded(x1.H, x1.W, 2 * U)          # [downsample2(pan_out3), f_out1]
+    cat_n4 = pb.new_padded(x0.H, x0.W, 2 * U)          # [downsample1(pan_out2), fpn_out0]
+    fpn0 = cbn(x0, "neck.reduce_layer0", U, 1, out=pb.sub(cat_n4, U, U))
+    pb.upsample2x(fpn0, pb.sub(cat_p4, 0, U))
+    cbn(x1, "neck.reduce_layer1", U, 1, out=pb.sub(cat_p4, U, U))
+    f_out1 = csp(cat_p4, "neck.Csp_p4", out=pb.sub(cat_n3, U, U))
+    pb.upsample2x(f_out1, pb.sub(cat_p3, 0, U))
+    cbn(x2, "neck.reduce_layer2", U, 1, out=pb.sub(cat_p3, U, U))
+    pan3 = csp(cat_p3, "neck.Csp_p3")
+    dp(pan3, "neck.downsample2", U, s=2, out=pb.sub(cat_n3, 0, U))
+    pan2 = csp(cat_n3, "neck.Csp_n3")
+    dp(pan2, "neck.downsample1", U, s=2, out=pb.sub(cat_n4, 0, U))
+    pan1 = csp(cat_n4, "neck.Csp_n4")
+    top = dp(fpn0, "neck.p6_conv_1", U, s=2)
+    pan0 = dp(pan1, "neck.p6_conv_2", U, s=2, res=top)     # p6_conv_1(fpn_out0) + p6_conv_2(pan_out1), after both activations
+    # Lite_EffideHead: reg_max 0, box distances in columns 0-3, class logits from column 8
+    cls_col = 8
+    A = 0
+    for li, (feat, stride) in enumerate(((pan3, 8), (pan2, 16), (pan1, 32), (pan0, 64))):
+        assert (feat.H, feat.W) == (-(-in_h // stride), -(-in_w // stride)), (li, feat)
+        t = dp(feat, f"detect.stems.{li}", U)
+        tc = dp(t, f"detect.cls_convs.{li}", U)
+        tr = dp(t, f"detect.reg_convs.{li}", U)
+        head = pb.new_padded(feat.H, feat.W, cls_col + (nc + 7) // 8 * 8, f32=True)
+        wrp, brp = W.conv_bias(f"detect.reg_preds.{li}", 4, U, 1)
+        wcp, bcp = W.conv_bias(f"detect.cls_preds.{li}", nc, U, 1)
+        pb.conv(tr, wrp, brp, 1, 1, ACT_NONE, out=pb.sub(head, 0, cls_col), out_f32=True)
+        pb.conv(tc, wcp, bcp, 1, 1, ACT_NONE, out=pb.sub(head, cls_col, (nc + 7) // 8 * 8), out_f32=True)
+        pb.outputs.append((head.buf, 0, head.C, stride))
+        A += feat.H * feat.W
+    pb.meta[0], pb.meta[1], pb.meta[2] = nc, A, 0
     return pb
 
 

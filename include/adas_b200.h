@@ -255,6 +255,8 @@ int adas_engine_buffer_info(const adas_engine* e, int idx, int64_t info[5] /* ro
 int adas_engine_write_buffer(adas_engine* e, int idx, const void* host, int64_t bytes);
 int adas_engine_read_buffer(adas_engine* e, int idx, void* host, int64_t bytes);
 int adas_engine_run(adas_engine* e, int batch);   /* replay the plan on whatever buffer 0 holds; synchronous */
+/* parse and validate a plan file exactly as adas_engine_create does, without touching a device: 0 = the plan would load */
+int adas_plan_validate(const char* plan_path);
 
 /* ---- timing hooks (bench.py): CUDA events on the handle's own stream (torch.cuda.Event only sees torch's stream).
  * adas_engine_event_record records event `slot` (0..3) on e's stream; adas_event_elapsed_ms synchronises on both

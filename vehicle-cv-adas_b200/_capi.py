@@ -23,7 +23,7 @@ SYMBOLS = [
     "adas_engine_infer", "adas_engine_infer_dev", "adas_yolo_detect", "adas_yolo_postprocess", "adas_yolo_preprocess",
     "adas_ufld_detect", "adas_ufld_postprocess", "adas_ufld_v1_postprocess", "adas_lane_geometry", "adas_ufld_lane_geometry", "adas_warp_perspective", "adas_engine_warp_perspective", "adas_ufld_preprocess", "adas_iou_cost", "adas_lap", "adas_associate",
     "adas_engine_stream", "adas_engine_num_buffers", "adas_engine_buffer_info", "adas_engine_write_buffer", "adas_engine_read_buffer",
-    "adas_engine_run", "adas_engine_event_record", "adas_event_elapsed_ms", "adas_engine_time_ops", "adas_engine_num_steps", "adas_engine_time_step", "adas_detect_pair",
+    "adas_engine_run", "adas_plan_validate", "adas_engine_event_record", "adas_event_elapsed_ms", "adas_engine_time_ops", "adas_engine_num_steps", "adas_engine_time_step", "adas_detect_pair",
     "adas_comm_unique_id", "adas_comm_create", "adas_comm_destroy", "adas_comm_all_gather", "adas_comm_sync", "adas_comm_read", "adas_comm_info",
     "adas_tracker_create", "adas_tracker_destroy", "adas_tracker_reset", "adas_tracker_update", "adas_tracker_update_batch", "adas_tracker_get", "adas_tracker_count", "adas_tracker_stats",
 ]
@@ -45,6 +45,11 @@ def lib() -> C.CDLL:
 def check(rc: int) -> None:
     if rc != 0:
         raise Exception(lib().adas_last_error().decode("utf-8", "replace"))
+
+
+def plan_validate(path: str) -> None:
+    """Parse and validate a plan file as the engine loader does, on the host only; raises with the loader's message."""
+    check(lib().adas_plan_validate(os.fsencode(path)))
 
 
 def launch_count() -> int:

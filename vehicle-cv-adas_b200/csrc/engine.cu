@@ -655,6 +655,9 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
         ADAS_CHECK(b.rows_per_img >= 1 && b.C >= 1 && b.C <= (1u << 20) && b.dtype <= 1 && (uint64_t)b.rows_per_img * b.C <= (1ull << 31), "plan %s: buffer %d has a bad shape", path, i);
         ADAS_CHECK((b.H == 0 && b.W == 0) || (b.H >= 1 && b.W >= 1 && (uint64_t)(b.H + 2) * (b.W + 2) == b.rows_per_img), "plan %s: buffer %d: rows_per_img != (H+2)*(W+2)", path, i);
     }
+    // the input staging kernels write 4 fp16 channels per pixel of buffer 0 at the header's in_h x in_w padded geometry
+    ADAS_CHECK(nb >= 1 && e->bufs[0].dtype == 0 && e->bufs[0].H == h.in_h && e->bufs[0].W == h.in_w && e->bufs[0].C >= 4,
+               "plan %s: buffer 0 must be the fp16 padded %ux%u input image with at least 4 channels", path, h.in_h, h.in_w);
     for (int i = 0; i < nt; ++i) {
         const PlanTensor& t = e->tensors[i];
         ADAS_CHECK(t.offset <= h.blob_bytes && t.bytes <= h.blob_bytes - t.offset && t.offset % 16 == 0 && t.dtype <= 1, "plan %s: tensor %d lies outside the weight blob", path, i);
@@ -691,15 +694,29 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
                 ADAS_CHECK(p[8] < 0 || (!transposed && view_ok(p[8], p[9], N) && e->bufs[p[8]].dtype == 0), "plan %s: op %zu: residual slice exceeds its buffer", path, oi);
                 ADAS_CHECK(p[15] >= 0 && p[15] <= 256 && p[17] >= 0 && p[17] <= 4 && (p[18] == 0 || p[18] == 1), "plan %s: op %zu: bad forced tile shape", path, oi);
                 ADAS_CHECK(act_code_ok(p[7]), "plan %s: op %zu: unknown activation %d", path, oi, p[7]);
+                // the launch-time preconditions of build_program, checked here too so that a plan accepted at load runs in bounds
+                const PlanBuffer &ab = e->bufs[p[0]], &ob = e->bufs[p[11]];
+                ADAS_CHECK(ab.dtype == 0, "plan %s: op %zu: GEMM input buffer must be fp16", path, oi);
+                ADAS_CHECK(Kc % 8 == 0 && p[1] % 8 == 0 && ab.C % 8 == 0, "plan %s: op %zu: GEMM K, input offset and row stride must be multiples of 8", path, oi);
+                ADAS_CHECK(ntaps == 1 || (Kc % 64 == 0 && ab.W > 0), "plan %s: op %zu: tap mode needs Cin %% 64 == 0 on a padded grid", path, oi);
+                ADAS_CHECK(!p[16] || (Kc % 64 == 0 && ab.W > 0 && ob.W > 0 && !transposed), "plan %s: op %zu: stride-2 mode needs Cin %% 64 == 0 on padded grids", path, oi);
+                ADAS_CHECK(transposed || p[16] || up2 || ob.rows_per_img == ab.rows_per_img, "plan %s: op %zu: GEMM in/out row geometry differs", path, oi);
+                ADAS_CHECK(!p[13] || ob.H > 0, "plan %s: op %zu: masked store into a dense buffer", path, oi);
+                ADAS_CHECK(!transposed || ((uint64_t)ab.rows_per_img * ab.C) % 8 == 0, "plan %s: op %zu: FC input slab must be a multiple of 8 elements", path, oi);
+                // the epilogue reads the residual at the output's row index
+                ADAS_CHECK(p[8] < 0 || (e->bufs[p[8]].rows_per_img == ob.rows_per_img && e->bufs[p[8]].H == ob.H && e->bufs[p[8]].W == ob.W),
+                           "plan %s: op %zu: GEMM residual slice must have the output's geometry", path, oi);
                 break;
             }
             case OP_IM2COL:
                 ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[7]) && view_ok(p[0], p[1], p[2]) && e->bufs[p[0]].H > 0 && e->bufs[p[7]].H > 0 && p[3] >= 1 && p[3] <= 7 && p[4] >= 1 && p[4] <= 7 &&
-                           p[5] >= 1 && p[5] <= 4 && p[6] >= 0 && p[6] <= 3 && (uint64_t)p[2] * p[3] * p[4] <= e->bufs[p[7]].C,
+                           p[5] >= 1 && p[5] <= 4 && p[6] >= 0 && p[6] <= 3 && (uint64_t)p[2] * p[3] * p[4] <= e->bufs[p[7]].C &&
+                           e->bufs[p[0]].dtype == 0 && e->bufs[p[7]].dtype == 0,
                            "plan %s: op %zu: bad im2col", path, oi);
                 break;
             case OP_MAXPOOL:
-                ADAS_CHECK(view_ok(p[0], p[1], p[2]) && view_ok(p[6], p[7], p[2]) && e->bufs[p[0]].H > 0 && e->bufs[p[6]].H > 0 && p[3] >= 1 && p[3] <= 7 && p[4] >= 1 && p[4] <= 4 && p[5] >= 0 && p[5] <= 3,
+                ADAS_CHECK(view_ok(p[0], p[1], p[2]) && view_ok(p[6], p[7], p[2]) && e->bufs[p[0]].H > 0 && e->bufs[p[6]].H > 0 && p[3] >= 1 && p[3] <= 7 && p[4] >= 1 && p[4] <= 4 && p[5] >= 0 && p[5] <= 3 &&
+                           e->bufs[p[0]].dtype == 0 && e->bufs[p[6]].dtype == 0,
                            "plan %s: op %zu: bad maxpool", path, oi);
                 break;
             case OP_AVGPOOL2: {
@@ -753,7 +770,8 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
                 break;
             }
             case OP_UPSAMPLE2X:
-                ADAS_CHECK(view_ok(p[0], p[1], p[2]) && view_ok(p[3], p[4], p[2]) && e->bufs[p[0]].H > 0 && e->bufs[p[3]].H == 2 * e->bufs[p[0]].H && e->bufs[p[3]].W == 2 * e->bufs[p[0]].W,
+                ADAS_CHECK(view_ok(p[0], p[1], p[2]) && view_ok(p[3], p[4], p[2]) && e->bufs[p[0]].H > 0 && e->bufs[p[3]].H == 2 * e->bufs[p[0]].H && e->bufs[p[3]].W == 2 * e->bufs[p[0]].W &&
+                           e->bufs[p[0]].dtype == 0 && e->bufs[p[3]].dtype == 0,
                            "plan %s: op %zu: bad upsample", path, oi);
                 break;
             case OP_CBFUSE: {
@@ -819,12 +837,15 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
                 break;
             }
             case OP_STEMPACK:
-                ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[1]) && e->bufs[p[0]].H > 0 && e->bufs[p[1]].H > 0 && e->bufs[p[0]].C == 4 && e->bufs[p[1]].C == 64, "plan %s: op %zu: bad stem re-layout", path, oi);
+                ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[1]) && e->bufs[p[0]].H > 0 && e->bufs[p[1]].H > 0 && e->bufs[p[0]].C == 4 && e->bufs[p[1]].C == 64 &&
+                           e->bufs[p[0]].dtype == 0 && e->bufs[p[1]].dtype == 0 && e->bufs[p[1]].H * 2 == e->bufs[p[0]].H && e->bufs[p[1]].W * 2 == e->bufs[p[0]].W,
+                           "plan %s: op %zu: bad stem re-layout", path, oi);
                 break;
             case OP_STEMCONV: {
                 const int Cout = p[3], k = p[4], s = p[9] == 0 ? 2 : p[9];          // p[9] = 0: stride 2 (plans without the field)
                 ADAS_CHECK(act_code_ok(p[6]), "plan %s: op %zu: unknown activation %d", path, oi, p[6]);
-                ADAS_CHECK((s == 1 || s == 2) && buf_ok(p[0]) && e->bufs[p[0]].H > 0 && e->bufs[p[0]].C == 4 && stem_conv_supported(Cout, k, p[5]) &&
+                ADAS_CHECK((s == 1 || s == 2) && buf_ok(p[0]) && e->bufs[p[0]].H > 0 && e->bufs[p[0]].C == 4 && e->bufs[p[0]].dtype == 0 && stem_conv_supported(Cout, k, p[5]) &&
+                           buf_ok(p[7]) && e->bufs[p[7]].dtype == 0 && p[8] % 8 == 0 && e->bufs[p[7]].C % 8 == 0 &&
                            view_ok(p[7], p[8], Cout) && e->bufs[p[7]].H > 0 && tensor_ok(p[1], (uint64_t)Cout * k * ((4 * k + 15) / 16 * 16) * 2) &&
                            (p[2] < 0 || tensor_ok(p[2], (uint64_t)Cout * 4)) &&
                            e->bufs[p[7]].H == (e->bufs[p[0]].H + 2 * p[5] - k) / s + 1 && e->bufs[p[7]].W == (e->bufs[p[0]].W + 2 * p[5] - k) / s + 1,
@@ -832,7 +853,8 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
                 break;
             }
             case OP_LAYERNORM: {
-                ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[4]) && p[1] >= 1 && p[5] >= 1 && p[5] <= p[1], "plan %s: op %zu: bad layernorm", path, oi);
+                ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[4]) && p[1] >= 1 && p[5] >= 1 && p[5] <= p[1] && e->bufs[p[0]].dtype == 0 && e->bufs[p[4]].dtype == 0,
+                           "plan %s: op %zu: bad layernorm", path, oi);
                 const PlanBuffer &ib = e->bufs[p[0]], &ob = e->bufs[p[4]];
                 ADAS_CHECK((uint64_t)p[1] <= (uint64_t)ib.rows_per_img * ib.C && (uint64_t)p[1] <= (uint64_t)ob.rows_per_img * ob.C && tensor_ok(p[2], (uint64_t)p[1] * 4) && tensor_ok(p[3], (uint64_t)p[1] * 4),
                            "plan %s: op %zu: layernorm vector exceeds its buffers", path, oi);
@@ -852,19 +874,28 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
                    (h.model_kind == ADAS_MODEL_YOLOV5 && h.meta[2] == 0 && (h.n_outputs == 3 || h.n_outputs == 4) && tensor_ok((int)h.meta[3] - 1, 0) &&
                     e->tensors[h.meta[3] - 1].bytes == (uint64_t)h.n_outputs * 6 * 4 && e->tensors[h.meta[3] - 1].dtype == 1),
                "plan %s: anchor table (meta[3] = %u) is not an fp32 tensor of %u x 3 x 2 values of a YOLOv5-layout head", path, h.meta[3], h.n_outputs);
+    // adas_engine_create sets up the lane decode from the dataset for every UFLD plan, with or without outputs
+    ADAS_CHECK(h.model_kind != ADAS_MODEL_UFLDV2 || ufld_dataset(h) != nullptr,
+               "plan %s: unknown UFLD dataset id %u (0 = CULane, 1 = TuSimple; CurveLanes is rejected like the reference does)", path, h.meta[6]);
+    ADAS_CHECK(h.model_kind != ADAS_MODEL_UFLDV1 || ufld_v1_dataset(h) != nullptr, "plan %s: unknown UFLD v1 dataset id %u (0 = CULane, 1 = TuSimple)", path, h.meta[6]);
     if (h.n_outputs == 0) return 0;          // single-layer plans of the kernel tests: no network outputs, no head geometry
+    if (is_ufld(h.model_kind)) {
+        // the lane decode and the output copies read total_dim fp32 values per image at an image stride of the buffer's C
+        const PlanOutput& o = e->outs[0];
+        const PlanBuffer& b = e->bufs[o.buffer];
+        ADAS_CHECK(h.n_outputs == 1 && b.dtype == 1 && b.H == 0 && b.rows_per_img == 1 && o.C >= h.meta[5],
+                   "plan %s: a UFLD head is one output of %u values on a dense fp32 buffer of one row per image", path, h.meta[5]);
+    }
     if (h.model_kind == ADAS_MODEL_UFLDV2) {
         const uint64_t ngr = h.meta[0], ncr = h.meta[1], ngc = h.meta[2], ncc = h.meta[3], nl = h.meta[4];
         ADAS_CHECK(nl == 4 && ngr >= 2 && ncr >= 1 && ngc >= 2 && ncc >= 1 && ngr <= 1024 && ngc <= 1024 && ncr <= 1024 && ncc <= 1024, "plan %s: bad UFLD head dimensions", path);
         ADAS_CHECK(h.meta[5] == ngr * ncr * nl + ngc * ncc * nl + 2 * ncr * nl + 2 * ncc * nl, "plan %s: UFLD total_dim does not match the head dimensions", path);
-        const UfldDataset* ds = ufld_dataset(h);
-        ADAS_CHECK(ds != nullptr, "plan %s: unknown UFLD dataset id %u (0 = CULane, 1 = TuSimple; CurveLanes is rejected like the reference does)", path, h.meta[6]);
+        const UfldDataset* ds = ufld_dataset(h);          // known: checked above
         ADAS_CHECK((int)ngr == ds->ngr && (int)ncr == ds->ncr && (int)ngc == ds->ngc && (int)ncc == ds->ncc && (int)h.in_h == ds->in_h && (int)h.in_w == ds->in_w,
                    "plan %s: head %llux%llu / %llux%llu at %ux%u is not the %s geometry its header names", path, (unsigned long long)ngr, (unsigned long long)ncr,
                    (unsigned long long)ngc, (unsigned long long)ncc, h.in_h, h.in_w, ds->name);
     } else if (h.model_kind == ADAS_MODEL_UFLDV1) {
-        const UfldV1Dataset* ds = ufld_v1_dataset(h);
-        ADAS_CHECK(ds != nullptr, "plan %s: unknown UFLD v1 dataset id %u (0 = CULane, 1 = TuSimple)", path, h.meta[6]);
+        const UfldV1Dataset* ds = ufld_v1_dataset(h);     // known: checked above
         ADAS_CHECK((int)h.meta[0] == ds->G && (int)h.meta[1] == ds->R && h.meta[4] == 4 && h.meta[5] == (uint64_t)(ds->G + 1) * ds->R * 4 && h.in_h == 288 && h.in_w == 800,
                    "plan %s: head %ux%u at %ux%u is not the UFLD v1 %s geometry its header names", path, h.meta[0], h.meta[1], h.in_h, h.in_w, ds->name);
     } else {
@@ -888,7 +919,20 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
             }
             ADAS_CHECK(A == h.meta[1], "plan %s: YOLOv6 levels hold %llu anchors, the header %u", path, (unsigned long long)A, h.meta[1]);
         } else if (h.model_kind == ADAS_MODEL_YOLOV8) {
+            // level i: stride 8 << i, an in / stride grid of fp32 cells holding 64 DFL bins and nc class logits from the output's offset
             ADAS_CHECK(h.n_outputs == 3, "plan %s: a YOLOv8 head has 3 levels, the plan declares %u", path, h.n_outputs);
+            uint64_t A = 0;
+            for (size_t i = 0; i < e->outs.size(); ++i) {
+                const PlanOutput& o = e->outs[i];
+                const PlanBuffer& b = e->bufs[o.buffer];
+                const uint32_t s = 8u << i;
+                ADAS_CHECK(o.stride == s && b.H > 0 && b.H == h.in_h / s && b.W == h.in_w / s, "plan %s: YOLOv8 level %zu has stride %u and a %ux%u grid; "
+                           "stride %u of a %ux%u input needs %ux%u", path, i, o.stride, b.H, b.W, s, h.in_h, h.in_w, h.in_h / s, h.in_w / s);
+                ADAS_CHECK(b.dtype == 1 && o.C >= 64 + h.meta[0], "plan %s: YOLOv8 level %zu is %u %s columns wide; 64 DFL bins and %u classes need %u fp32 columns",
+                           path, i, o.C, b.dtype == 1 ? "fp32" : "fp16", h.meta[0], 64 + h.meta[0]);
+                A += (uint64_t)b.H * b.W;
+            }
+            ADAS_CHECK(A == h.meta[1], "plan %s: YOLOv8 levels hold %llu anchors, the header %u", path, (unsigned long long)A, h.meta[1]);
         } else {
             // YOLOv5 layout: 3 levels (strides 8 / 16 / 32), or 4 (+ 64) for a non-lite head with its own anchor table (the YOLOv5 table
             // has 3 levels); level i is the in / stride grid and holds 3 anchors per cell
@@ -903,6 +947,8 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
                 const uint32_t s = 8u << i;
                 ADAS_CHECK(o.stride == s && b.H > 0 && b.H == h.in_h / s && b.W == h.in_w / s, "plan %s: YOLO level %zu has stride %u and a %ux%u grid; "
                            "stride %u of a %ux%u input needs %ux%u", path, i, o.stride, b.H, b.W, s, h.in_h, h.in_w, h.in_h / s, h.in_w / s);
+                ADAS_CHECK(b.dtype == 1 && o.C >= 3 * (5 + h.meta[0]), "plan %s: YOLO level %zu is %u %s columns wide; 3 anchors of %u classes need %u fp32 columns",
+                           path, i, o.C, b.dtype == 1 ? "fp32" : "fp16", h.meta[0], 3 * (5 + h.meta[0]));
                 A += 3ull * b.H * b.W;
             }
             ADAS_CHECK(A == h.meta[1], "plan %s: YOLOv5-layout levels hold %llu anchors, the header %u", path, (unsigned long long)A, h.meta[1]);
@@ -911,18 +957,11 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
     return 0;
 }
 
-int adas_engine_create(const char* plan_path, int device, int max_batch, int conv_impl, adas_engine** out) {
-    ADAS_CHECK(out != nullptr && plan_path != nullptr, "adas_engine_create: null argument");
-    *out = nullptr;
+// Reads and validates the plan's records into e and, when blob is given, its weight blob; touches no device.
+static int load_plan(adas_engine* e, const char* plan_path, std::vector<uint8_t>* blob) {
     FILE* f = fopen(plan_path, "rb");
     // same wording class as EngineBase.__init__ (coreEngine.py:12-13)
     ADAS_CHECK(f != nullptr, "The model path [%s] can't not found!", plan_path);
-    std::unique_ptr<adas_engine> e(new adas_engine());
-    e->device = device; e->max_batch = max_batch; e->conv_impl = conv_impl;
-    const char* ng = getenv("ADAS_B200_NO_GRAPH");
-    e->use_graph = !(ng && ng[0] == '1');
-    const char* at = getenv("ADAS_B200_AUTOTUNE");
-    e->autotune = !(at && at[0] == '0');
     bool ok = fread(&e->hdr, sizeof(PlanHeader), 1, f) == 1 && memcmp(e->hdr.magic, kPlanMagic, 8) == 0 && e->hdr.version == kPlanVersion;
     if (!ok) { fclose(f); ADAS_CHECK(false, "Parameters must be a .b200w plan file (bad magic/version): %s", plan_path); }
     if (e->hdr.n_buffers > 65536 || e->hdr.n_ops > 65536 || e->hdr.n_tensors > 65536 || e->hdr.n_outputs > 64) { fclose(f); ADAS_CHECK(false, "plan %s: implausible record counts", plan_path); }
@@ -934,19 +973,45 @@ int adas_engine_create(const char* plan_path, int device, int max_batch, int con
     if (!ok) { fclose(f); ADAS_CHECK(false, "truncated plan file %s", plan_path); }
     fseek(f, 0, SEEK_END);
     const uint64_t file_bytes = (uint64_t)ftell(f);
-    if (validate_plan(e.get(), file_bytes, plan_path)) { fclose(f); return 1; }
-    std::vector<uint8_t> blob(e->hdr.blob_bytes);
-    fseek(f, (long)e->hdr.blob_offset, SEEK_SET);
-    ok = fread(blob.data(), 1, blob.size(), f) == blob.size();
+    if (validate_plan(e, file_bytes, plan_path)) { fclose(f); return 1; }
+    const bool anchors = !is_ufld(e->hdr.model_kind) && e->hdr.meta[3] != 0;
+    float anc[kYoloMaxLevels * 6];
+    const int n_anc = (int)e->hdr.n_outputs * 6;              // validated: 3 or 4 levels, tensor of exactly this size
+    if (blob) {
+        blob->resize(e->hdr.blob_bytes);
+        fseek(f, (long)e->hdr.blob_offset, SEEK_SET);
+        ok = fread(blob->data(), 1, blob->size(), f) == blob->size();
+        if (ok && anchors) memcpy(anc, blob->data() + e->tensors[e->hdr.meta[3] - 1].offset, n_anc * sizeof(float));
+    } else if (anchors) {                                      // validation only: read the anchor table alone
+        fseek(f, (long)(e->hdr.blob_offset + e->tensors[e->hdr.meta[3] - 1].offset), SEEK_SET);
+        ok = fread(anc, sizeof(float), n_anc, f) == (size_t)n_anc;
+    }
     fclose(f);
     ADAS_CHECK(ok, "truncated plan blob in %s", plan_path);
-    if (!is_ufld(e->hdr.model_kind) && e->hdr.meta[3] != 0) {
-        float anc[kYoloMaxLevels * 6];
-        const int n_anc = (int)e->hdr.n_outputs * 6;          // validated: 3 or 4 levels, tensor of exactly this size
-        memcpy(anc, blob.data() + e->tensors[e->hdr.meta[3] - 1].offset, n_anc * sizeof(float));
+    if (anchors) {
         for (int i = 0; i < n_anc; ++i)
             ADAS_CHECK(isfinite(anc[i]) && anc[i] > 0.f, "plan %s: anchor %d of the head's table is %g (finite and positive required)", plan_path, i, (double)anc[i]);
     }
+    return 0;
+}
+
+int adas_plan_validate(const char* plan_path) {
+    ADAS_CHECK(plan_path != nullptr, "adas_plan_validate: null argument");
+    std::unique_ptr<adas_engine> e(new adas_engine());
+    return load_plan(e.get(), plan_path, nullptr);
+}
+
+int adas_engine_create(const char* plan_path, int device, int max_batch, int conv_impl, adas_engine** out) {
+    ADAS_CHECK(out != nullptr && plan_path != nullptr, "adas_engine_create: null argument");
+    *out = nullptr;
+    std::unique_ptr<adas_engine> e(new adas_engine());
+    e->device = device; e->max_batch = max_batch; e->conv_impl = conv_impl;
+    const char* ng = getenv("ADAS_B200_NO_GRAPH");
+    e->use_graph = !(ng && ng[0] == '1');
+    const char* at = getenv("ADAS_B200_AUTOTUNE");
+    e->autotune = !(at && at[0] == '0');
+    std::vector<uint8_t> blob;
+    if (load_plan(e.get(), plan_path, &blob)) return 1;
 
     int ndev = 0;
     cudaError_t ce = cudaGetDeviceCount(&ndev);
@@ -1065,8 +1130,15 @@ int adas_engine_output_shape(const adas_engine* e, int idx, int64_t s[4], int* r
 }
 int adas_engine_stream(const adas_engine* e, void** st) { *st = (void*)e->stream; return 0; }
 
+// single-op plans (no network outputs) only run through adas_engine_run: the decodes and copies read e->outs[0]
+static int check_has_outputs(const adas_engine* e, const char* fn) {
+    ADAS_CHECK(!e->outs.empty(), "%s: the plan declares no network outputs", fn);
+    return 0;
+}
+
 static int infer_common(adas_engine* e, const float* input, int batch, float* const* outs, bool on_device) {
     ADAS_CHECK(e != nullptr, "null engine");
+    if (check_has_outputs(e, "adas_engine_infer")) return 1;
     ADAS_CHECK(batch >= 1 && batch <= e->max_batch, "batch %d outside [1, %d]", batch, e->max_batch);
     ADAS_CUDA(cudaSetDevice(e->device));
     const size_t in_elems = (size_t)e->hdr.in_c * e->hdr.in_h * e->hdr.in_w;
@@ -1131,6 +1203,7 @@ int adas_yolo_detect(adas_engine* e, const uint8_t* frames, int frames_on_device
                      int32_t* counts, int32_t* n_candidates) {
     ADAS_CHECK(e != nullptr, "null engine");
     ADAS_CHECK(!is_ufld(e->hdr.model_kind), "adas_yolo_detect on a UFLD plan");
+    if (check_has_outputs(e, "adas_yolo_detect")) return 1;
     ADAS_CHECK(batch >= 1 && batch <= e->max_batch, "batch %d outside [1, %d]", batch, e->max_batch);
     ADAS_CUDA(cudaSetDevice(e->device));
     const int nc = (int)e->hdr.meta[0], A = (int)e->hdr.meta[1];
@@ -1218,6 +1291,7 @@ int adas_ufld_detect(adas_engine* e, const uint8_t* frames, int frames_on_device
                      uint8_t* status, double* coords_f) {
     ADAS_CHECK(e != nullptr, "null engine");
     ADAS_CHECK(is_ufld(e->hdr.model_kind), "adas_ufld_detect on a YOLO plan");
+    if (check_has_outputs(e, "adas_ufld_detect")) return 1;
     ADAS_CHECK(batch >= 1 && batch <= e->max_batch, "batch %d outside [1, %d]", batch, e->max_batch);
     ADAS_CUDA(cudaSetDevice(e->device));
     const uint8_t* dfr = nullptr;
@@ -1295,6 +1369,9 @@ int adas_detect_pair(adas_engine* yolo, adas_engine* ufld, const uint8_t* frames
                      double nms_iou, int max_det, float* boxes_xywh, float* scores, int32_t* class_ids, int32_t* cand_index, int32_t* counts,
                      int32_t* n_candidates, int32_t* pts, int32_t* npts, uint8_t* status) {
     NvtxRange nv("adas_detect_pair");
+    ADAS_CHECK(yolo != nullptr && ufld != nullptr, "null engine");
+    ADAS_CHECK(!is_ufld(yolo->hdr.model_kind) && is_ufld(ufld->hdr.model_kind), "adas_detect_pair needs a YOLO and a UFLD engine");
+    if (check_has_outputs(yolo, "adas_detect_pair") || check_has_outputs(ufld, "adas_detect_pair")) return 1;
     static int conc = -1;
     if (conc < 0) { const char* c = getenv("ADAS_B200_CONCURRENT"); conc = (c && c[0] == '0') ? 0 : 1; }
     if (!conc || yolo->device != ufld->device) {

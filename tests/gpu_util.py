@@ -1,11 +1,11 @@
-"""Helpers for the GPU parity tests: padded-NHWC packing and cached plan files."""
+"""Helpers for the GPU parity tests: padded-NHWC packing, cached plan files and network inputs."""
 import os
 
 import numpy as np
 
 import adas_b200  # noqa: F401
 from adas_b200 import plan
-
+from oracle import post
 
 
 def to_padded(x_nchw: np.ndarray, C: int) -> np.ndarray:
@@ -28,23 +28,25 @@ def halo_is_zero(buf: np.ndarray, B: int, H: int, W: int) -> bool:
 
 
 def cached_plan(kind: str, seed: int = 0, **kw):
-    """Build (once per process tree) the synthetic plan + return (path, Weights-like state_dict)."""
-    CACHE = plan.cache_dir()
+    """Build the seeded synthetic plan of one network and write it to the plan cache: (path, state_dict, PlanBuilder).
+
+    `kind` names the builder (`plan.build_<kind>`: "yolov5", "yolov6", "yolov6_lite", "yolov7", "yolov8", "yolov9", "yolov10", "ufldv1",
+    "ufldv2"; YOLOv9-E is "yolov9" with scale "e") and `kw` are its arguments.  The file is rewritten from this build on every call,
+    through a temporary name of this process, so it never holds a plan an older builder wrote, nor a mix of two processes' writes."""
     import zlib
-    prof = zlib.crc32(repr((plan.SYNTH_PROFILES.get("ufldv2" if kind == "ufldv1" else kind), plan.PLAN_VERSION)).encode()) & 0xffff      # a changed operating point is a new plan
+    synth = {"ufldv1": "ufldv2", "yolov6_lite": "yolov6lite"}.get(kind, kind)
+    prof = zlib.crc32(repr((plan.SYNTH_PROFILES[synth], plan.PLAN_VERSION)).encode()) & 0xffff      # a changed operating point is a new plan
     tag = kind + "_" + "_".join(f"{k}{v}" for k, v in sorted(kw.items())) + f"_s{seed}_{prof:04x}"
-    path = os.path.join(CACHE, tag + ".b200w")
+    path = os.path.join(plan.cache_dir(), tag + ".b200w")
     variant = kw.get("scale", kw.get("backbone"))             # calibrated BatchNorm statistics exist for the tested variants
-    W = plan.synth_weights("ufldv2" if kind == "ufldv1" else kind, seed, variant=variant)
-    if kind == "yolov8":
-        pb = plan.build_yolov8(W, **kw)
-    elif kind == "yolov5":
-        pb = plan.build_yolov5(W, **kw)
-    elif kind == "ufldv1":
-        pb = plan.build_ufldv1(W, **kw)
-    else:
-        pb = plan.build_ufldv2(W, **kw)
-    if not os.path.isfile(path):
-        pb.write(path + ".tmp")
-        os.replace(path + ".tmp", path)
+    W = plan.synth_weights(synth, seed, variant=variant)
+    pb = getattr(plan, "build_" + kind)(W, **kw)
+    tmp = f"{path}.{os.getpid()}.tmp"
+    pb.write(tmp)
+    os.replace(tmp, path)
     return path, W.state_dict, pb
+
+
+def yolo_blob(frames, h: int = 640, w: int = 640) -> np.ndarray:
+    """The letterboxed [B, 3, h, w] float32 network input of a list of frames (the oracle's pre-processing)."""
+    return np.concatenate([post.yolo_prepare_input(f, h, w)[0] for f in frames])

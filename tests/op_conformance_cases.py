@@ -53,13 +53,17 @@ def view(pb, H, W, C, off, f32=False):
 
 
 def act64(a: np.ndarray, act: int, slope: float = LEAKY) -> np.ndarray:
+    if act == plan.ACT_NONE:
+        return a
     if act == 1:
         return a / (1.0 + np.exp(-a))
     if act == 2:
         return np.maximum(a, 0.0)
     if act == 3:
         return np.where(a >= 0, a, slope * a)
-    return a
+    if act == plan.ACT_HSWISH:
+        return a * np.clip(a + 3.0, 0.0, 6.0) / 6.0
+    raise ValueError(f"unknown activation code {act}")
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
@@ -72,13 +76,21 @@ def gemm_bound(ref, S, K, act, a, res_post=None, out_f32=False):
     order of K products (exact: fp16 x fp16 fits fp32) and the bias has error <= gamma_K * S <= K * 2^-24 * S; 2^-23 doubles it for
     the bias / pre-activation residual adds and for tensor-core accumulators that truncate instead of rounding.  The activation has
     Lipschitz constant 1 (none, ReLU, LeakyReLU) or 1.1 (SiLU) and SiLU's fp32 evaluation (exp, divide) adds 2^-20 |a|; LeakyReLU's
-    fp32 slope adds 2^-22 |a|.  A residual added after the activation costs one product and one add: 2^-24 |alpha r| + 2^-24 |ref|.
-    The fp16 store rounds to nearest: 2^-11 |ref| relative plus 2^-24 absolute below the normal range."""
+    fp32 slope adds 2^-22 |a|.  Hardswish has Lipschitz constant 1.5 (slope (2x + 3) / 6 on [-3, 3], 0 or 1 outside); its fp32
+    evaluation -- x + 3, the clamp (exact), the product with x and the product with fp32(1/6) -- adds four roundings of at most
+    |x| (|x| + 3) / 6 each (which bounds |x + 3| |x| / 6 and every intermediate): 2^-21 |a| (|a| + 3) / 6.  A residual added after the
+    activation costs one product and one add: 2^-24 |alpha r| + 2^-24 |ref|.  The fp16 store rounds to nearest: 2^-11 |ref| relative
+    plus 2^-24 absolute below the normal range."""
     E = K * 2.0 ** -23 * S
     if act == 1:
         E = 1.1 * E + 2.0 ** -20 * np.abs(a)
     elif act == 3:
         E = E + 2.0 ** -22 * np.abs(a)
+    elif act == plan.ACT_HSWISH:
+        a = np.abs(a)
+        E = 1.5 * E + 2.0 ** -21 * a * (a + 3.0) / 6.0
+    elif act not in (plan.ACT_NONE, plan.ACT_RELU):
+        raise ValueError(f"unknown activation code {act}")
     if res_post is not None:
         E = E + U32 * np.abs(res_post) + U32 * np.abs(ref)
     if out_f32:

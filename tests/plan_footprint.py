@@ -52,6 +52,24 @@ class Plan:
     def out_off(self, i): return self.ten_off(len(self.tensors)) + i * OUT_SIZE
 
 
+def corrupt(raw: bytes, off: int, fmt: str, value) -> bytes:
+    """`raw` with `value` packed in struct format `fmt` at byte `off` (a record field: Plan.buf_off / op_off / ten_off / out_off)."""
+    b = bytearray(raw)
+    struct.pack_into(fmt, b, off, value)
+    return bytes(b)
+
+
+def engine_error(path) -> Optional[str]:
+    """The error loading the plan file at `path` raises, None if it loads.  The loader validates the whole plan before any device work,
+    so without a GPU a valid plan fails only for the missing device."""
+    from adas_b200 import _capi
+    try:
+        _capi.Engine(str(path))
+    except Exception as e:
+        return str(e)
+    return None
+
+
 def parse(raw: bytes) -> Plan:
     h = list(struct.unpack_from(HDR_FMT, raw, 0))
     nb, no, nt, nout = h[6:10]

@@ -31,7 +31,7 @@ class Region(NamedTuple):
 
 OP_NAMES = {plan.OP_GEMM: "gemm", plan.OP_IM2COL: "im2col", plan.OP_MAXPOOL: "maxpool", plan.OP_UPSAMPLE2X: "upsample",
             plan.OP_LAYERNORM: "layernorm", plan.OP_STEMPACK: "stempack", plan.OP_STEMCONV: "stemconv", plan.OP_AVGPOOL2: "avgpool2",
-            plan.OP_DWCONV: "dwconv", plan.OP_ATTN: "attention"}
+            plan.OP_DWCONV: "dwconv", plan.OP_ATTN: "attention", plan.OP_CBFUSE: "cbfuse", plan.OP_SE: "se", plan.OP_SHUFFLE2: "shuffle2"}
 
 
 def geom(pb, buf):
@@ -69,8 +69,13 @@ def op_kind(pb, i) -> str:
     return OP_NAMES[t]
 
 
+def cbfuse_sources(p) -> List[Tuple[int, int, int]]:
+    """(buffer, channel offset, shift) of each source of an OP_CBFUSE op, in summation order."""
+    return [tuple(p[6 + 3 * s:9 + 3 * s]) for s in range(p[5])]
+
+
 def op_regions(pb, i) -> Tuple[List[Region], List[Region]]:
-    """(writes, reads) of op i."""
+    """(writes, reads) of op i.  An in-place CBFuse or SE reads its own write region."""
     t, p, _ = pb.ops[i]
     if t == plan.OP_GEMM:
         a, acoff, Kc, N, out, ocoff = p[0], p[1], p[2], p[6], p[11], p[12]
@@ -96,6 +101,14 @@ def op_regions(pb, i) -> Tuple[List[Region], List[Region]]:
     if t == plan.OP_ATTN:
         nh, kdp, hd = p[2], p[3], p[4]
         return [Region(p[5], p[6], p[6] + nh * hd)], [Region(p[0], p[1], p[1] + nh * (2 * kdp + hd))]
+    if t == plan.OP_CBFUSE:
+        C = p[2]
+        return [Region(p[0], p[1], p[1] + C)], [Region(p[3], p[4], p[4] + C)] + [Region(q[0], q[1], q[1] + C) for q in cbfuse_sources(p)]
+    if t == plan.OP_SE:
+        return [Region(p[8], p[9], p[9] + p[2])], [Region(p[0], p[1], p[1] + p[2])]
+    if t == plan.OP_SHUFFLE2:
+        n = p[4]
+        return [Region(p[5], p[6], p[6] + 2 * n)], [Region(p[0], p[1], p[1] + n), Region(p[2], p[3], p[3] + n)]
     raise ValueError(f"op {i}: unknown type {t}")
 
 
@@ -218,13 +231,17 @@ def new_buffers(pb, mb, dtype=None) -> Dict[int, np.ndarray]:
 # references
 # ---------------------------------------------------------------------------------------------------------------------------
 def _act(a: torch.Tensor, act: int) -> torch.Tensor:
+    if act == plan.ACT_NONE:
+        return a
     if act == 1:
         return a * torch.sigmoid(a)
     if act == 2:
         return torch.clamp_min(a, 0.0)
     if act == 3:
         return torch.where(a >= 0, a, oc.LEAKY * a)
-    return a
+    if act == plan.ACT_HSWISH:
+        return a * torch.clamp(a + 3.0, 0.0, 6.0) / 6.0
+    raise ValueError(f"unknown activation code {act}")
 
 
 def _np(t: torch.Tensor) -> np.ndarray:
@@ -389,6 +406,65 @@ def _layernorm_ref(pb, p, fl, bufs, B, want_bound):
     return ref, bnd
 
 
+def _cbfuse_ref(pb, p, bufs, B, dev, want_bound):
+    """base + sum of the sources, each repeated 2^shift times along H and W.  The kernel sums in fp32 (base first, then the sources
+    in order) and rounds once: within n_src * 2^-24 * (|base| + sum |src|) of the exact sum, then half an fp16 ulp."""
+    C = p[2]
+    refs, bnds = [], []
+    for b in range(B):
+        acc = image_view(pb, bufs, p[3], b, p[4], p[4] + C, dev)
+        S = acc.abs()
+        for buf, coff, s in cbfuse_sources(p):
+            v = image_view(pb, bufs, buf, b, coff, coff + C, dev).repeat_interleave(1 << s, 2).repeat_interleave(1 << s, 3)
+            acc = acc + v
+            S = S + v.abs()
+        refs.append(_np(acc))
+        if want_bound:
+            e32 = p[5] * 2.0 ** -24 * _np(S)
+            bnds.append(e32 + 0.5 * np.spacing((np.abs(refs[-1]) + e32).astype(np.float16)).astype(np.float64))
+    return np.concatenate(refs), (np.concatenate(bnds) if want_bound else None)
+
+
+def _se_ref(pb, p, bufs, B, dev, want_bound):
+    """x * hardsigmoid(W2 relu(W1 mean(x) + b1) + b2) per image, and its bound.  The kernel (lite_ops.cu): the mean is an fp32 sum of HW
+    terms and a division, within (HW + 1) 2^-24 mean|x|; each FC is an fp32 dot product with a bias, within n 2^-24 (|b| + sum |w| |v|)
+    of its fp32 inputs plus the propagated input error (ReLU: Lipschitz 1); hardsigmoid (Lipschitz 1/6, then + 3 and / 6 in fp32) adds
+    2^-23; the product x * g adds 2^-24 |x g|; the fp16 store 2^-11 |ref| + 2^-24.  Each 2^-24 is doubled below for margin."""
+    in_buf, coff, C, hid = p[:4]
+    w1, b1, w2, b2 = (pb.tensors[t].astype(np.float64) for t in p[4:8])
+    w1, w2 = w1.reshape(hid, C), w2.reshape(C, hid)
+    refs, bnds = [], []
+    for b in range(B):
+        x = _np(image_view(pb, bufs, in_buf, b, coff, coff + C, dev))[0]              # [C, H, W]
+        HW = x.shape[1] * x.shape[2]
+        m = x.reshape(C, HW).mean(1)
+        pre_h = b1 + w1 @ m
+        h = np.maximum(pre_h, 0.0)
+        pre_g = b2 + w2 @ h
+        g = np.clip(pre_g + 3.0, 0.0, 6.0) / 6.0
+        y = x * g[:, None, None]
+        refs.append(y[None])
+        if want_bound:
+            u = 2.0 ** -23
+            dm = (HW + 1) * u * np.abs(x).reshape(C, HW).mean(1)
+            dh = np.abs(w1) @ dm + C * u * (np.abs(b1) + np.abs(w1) @ np.abs(m))
+            dg = (np.abs(w2) @ dh + hid * u * (np.abs(b2) + np.abs(w2) @ np.abs(h))) / 6.0 + u
+            E = np.abs(x) * dg[:, None, None] + u * np.abs(y)
+            bnds.append((oc.U16 * np.abs(y) + (1 + oc.U16) * E + oc.U32)[None])
+    return np.concatenate(refs), (np.concatenate(bnds) if want_bound else None)
+
+
+def _shuffle2_ref(pb, p, bufs, B, dev):
+    """cat(a, b) with the channels interleaved (a0, b0, a1, b1, ...): ShuffleNetV2's channel_shuffle of two groups."""
+    n = p[4]
+    res = []
+    for b in range(B):
+        a = image_view(pb, bufs, p[0], b, p[1], p[1] + n, dev)
+        c = image_view(pb, bufs, p[2], b, p[3], p[3] + n, dev)
+        res.append(_np(torch.stack([a, c], 2).reshape(1, 2 * n, a.shape[2], a.shape[3])))
+    return np.concatenate(res)
+
+
 def op_ref(pb, i, bufs, B, device="cpu", want_bound=True) -> Tuple[np.ndarray, Optional[np.ndarray]]:
     """(reference, bound) of op i for images < B from `bufs`, in read_out's layout.  bound None: bit-exact."""
     t, p, fl = pb.ops[i]
@@ -432,6 +508,12 @@ def op_ref(pb, i, bufs, B, device="cpu", want_bound=True) -> Tuple[np.ndarray, O
                 refs.append(r)
                 bnds.append(bd)
             return np.concatenate(refs), (np.concatenate(bnds) if want_bound else None)
+        if t == plan.OP_CBFUSE:
+            return _cbfuse_ref(pb, p, bufs, B, dev, want_bound)
+        if t == plan.OP_SE:
+            return _se_ref(pb, p, bufs, B, dev, want_bound)
+        if t == plan.OP_SHUFFLE2:
+            return _shuffle2_ref(pb, p, bufs, B, dev), None
     raise ValueError(f"op {i}: unknown type {t}")
 
 

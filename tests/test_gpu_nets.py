@@ -15,15 +15,11 @@ import synth
 import adas_b200  # noqa: F401
 from adas_b200 import _capi, plan
 from adas_b200.coreEngine import B200Engine
-from gpu_util import cached_plan
+from gpu_util import cached_plan, yolo_blob
 from oracle import nets, post
 
 pytestmark = pytest.mark.gpu
 torch.set_num_threads(min(16, max(1, os.cpu_count() or 1)))   # oneDNN collapses under 100+ threads
-
-
-def _blob(frames):
-    return np.concatenate([post.yolo_prepare_input(f, 640, 640)[0] for f in frames])
 
 
 def _report(name, got, ref):
@@ -37,7 +33,7 @@ def test_yolov5n_engine_vs_oracle(impl):
     path, sd, _ = cached_plan("yolov5", scale="n")
     eng = _capi.Engine(path, 0, max_batch=2, conv_impl=impl)
     frames = [synth.frame(s) for s in (0, 1)]
-    x = _blob(frames)
+    x = yolo_blob(frames)
     raw = eng.infer(x)[0]
     model = nets.build("yolov5", sd, scale="n")
     with torch.no_grad():
@@ -56,7 +52,7 @@ def test_yolov8l_batch8_and_batch32_equal_batch1():
     path, sd, _ = cached_plan("yolov8", scale="l")
     eng = _capi.Engine(path, 0, max_batch=32)
     frames = [synth.frame(s % 8) if s < 24 else synth.frame(100 + s) for s in range(32)]
-    x = _blob(frames)
+    x = yolo_blob(frames)
     raw32 = eng.infer(x)[0]
     raw8 = eng.infer(x[8:16])[0]
     assert np.array_equal(raw8, raw32[8:16])
@@ -80,7 +76,7 @@ def test_yolov8l_engine_vs_oracle_and_batch_invariance():
     path, sd, _ = cached_plan("yolov8", scale="l")
     eng = _capi.Engine(path, 0, max_batch=4)
     frames = [synth.frame(s) for s in (0, 1, 2, 3)]
-    x = _blob(frames)
+    x = yolo_blob(frames)
     raw4 = eng.infer(x)[0]
     model = nets.build("yolov8", sd, scale="l")
     with torch.no_grad():
@@ -109,7 +105,7 @@ def test_yolov8l_fused_detect_matches_reference_postprocessing():
     boxes, scores, cls, idx, counts, ncand = eng.yolo_detect(frames, 0.4, 0.45, max_det=1024)
     # (a) pre-processing inside the fused path is the bit-exact blob, so engine_inference on it gives the same raw tensor
     x = _capi.yolo_preprocess(frames, (640, 640))
-    assert np.array_equal(x, _blob(frames))
+    assert np.array_equal(x, yolo_blob(frames))
     raw = eng.infer(x)[0]
     geom = post.letterbox_geom(720, 1280, 640, 640)
     total = 0
@@ -272,7 +268,7 @@ def test_yolov5_lite_plan_matches_decoded_plan():
     for ra, rb in zip(a, b):
         assert key(ra) == key(rb)
     # raw tensors: same logits, decoded vs sigmoid-only boxes
-    x = _blob(frames)
+    x = yolo_blob(frames)
     raw, raw_l = det.engine.engine_inference(x)[0], det_l.engine.engine_inference(x)[0]
     assert np.array_equal(raw[..., 4:], raw_l[..., 4:]) and raw_l[..., :4].max() <= 1.0 and raw[..., :4].max() > 1.0
     for i in range(2):
@@ -499,7 +495,7 @@ def test_two_devices_in_one_process():
     path, _, _ = cached_plan("yolov8", scale="l")
     upath, _, _ = cached_plan("ufldv2", backbone="18", cfg="tusimple")
     frames = np.stack([synth.frame(70 + s) for s in range(2)])
-    x = _blob(list(frames))
+    x = yolo_blob(list(frames))
     res = []
     for dev in (0, 1):
         eng = _capi.Engine(path, dev, max_batch=2)
@@ -549,7 +545,7 @@ def test_engine_from_onnx_file_matches_state_dict_plan(tmp_path):
     e_sd = B200Engine(path, device=0, max_batch=2)
     assert e_onnx.get_engine_input_shape() == e_sd.get_engine_input_shape() == [1, 3, 640, 640]
     assert e_onnx.get_engine_output_shape() == e_sd.get_engine_output_shape()
-    x = _blob([synth.frame(s) for s in (0, 1)])
+    x = yolo_blob([synth.frame(s) for s in (0, 1)])
     a, b = e_onnx.engine_inference(x)[0], e_sd.engine_inference(x)[0]
     with torch.no_grad():
         ref = model(torch.from_numpy(x)).numpy()

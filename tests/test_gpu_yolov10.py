@@ -2,7 +2,6 @@
 against the oracle's modules, and YOLOv10-N/S/M/B/L/X end to end against the fp32 oracle (tests/yolov10_oracle.py) through YOLOv8's head
 decode, candidate selection and NMS."""
 import os
-import zlib
 
 import numpy as np
 import pytest
@@ -12,7 +11,7 @@ import torch.nn.functional as F
 import synth
 import adas_b200  # noqa: F401
 from adas_b200 import _capi, plan
-from gpu_util import from_padded, halo_is_zero, to_padded
+from gpu_util import cached_plan, from_padded, halo_is_zero, to_padded, yolo_blob
 from oracle import post
 import yolov10_oracle as o10
 
@@ -204,28 +203,12 @@ def test_v10_head_matches_the_oracle(tmp_path, nc):
             assert err < 3e-3, (li, float(err))
 
 
-def v10_plan(scale, seed=0, in_h=640, in_w=640):
-    """Seeded synthetic YOLOv10 plan, cached per operating point: (path, state_dict)."""
-    prof = zlib.crc32(repr((plan.SYNTH_PROFILES["yolov10"], plan.PLAN_VERSION)).encode()) & 0xffff
-    path = os.path.join(plan.cache_dir(), f"yolov10_{scale}_{in_h}x{in_w}_s{seed}_{prof:04x}.b200w")
-    W = plan.synth_weights("yolov10", seed, variant=scale)
-    pb = plan.build_yolov10(W, scale, in_h=in_h, in_w=in_w)
-    if not os.path.isfile(path):
-        pb.write(path + ".tmp")
-        os.replace(path + ".tmp", path)
-    return path, W.state_dict
-
-
-def _blob(frames, h=640, w=640):
-    return np.concatenate([post.yolo_prepare_input(f, h, w)[0] for f in frames])
-
-
 @pytest.mark.parametrize("impl", [0, 1])
 @pytest.mark.parametrize("scale", ["n", "s", "m", "b", "l", "x"])
 def test_yolov10_engine_vs_oracle_and_batch_invariance(scale, impl):
-    path, sd = v10_plan(scale)
+    path, sd, _ = cached_plan("yolov10", scale=scale)
     eng = _capi.Engine(path, 0, max_batch=3, conv_impl=impl)
-    x = _blob([synth.frame(s) for s in (0, 1, 2)])
+    x = yolo_blob([synth.frame(s) for s in (0, 1, 2)])
     raw = eng.infer(x)[0]
     with torch.no_grad():
         ref = o10.build(sd, scale)(torch.from_numpy(x[:2])).numpy()
@@ -243,9 +226,9 @@ def test_yolov10_engine_vs_oracle_and_batch_invariance(scale, impl):
 @pytest.mark.parametrize("in_h,in_w", [(1280, 1280), (480, 640)])
 def test_yolov10n_at_other_input_sizes(in_h, in_w):
     """1600 attention tokens at 1280x1280; a non-square 640x480 letterbox."""
-    path, sd = v10_plan("n", in_h=in_h, in_w=in_w)
+    path, sd, _ = cached_plan("yolov10", scale="n", in_h=in_h, in_w=in_w)
     eng = _capi.Engine(path, 0, max_batch=2)
-    x = _blob([synth.frame(s) for s in (0, 1)], in_h, in_w)
+    x = yolo_blob([synth.frame(s) for s in (0, 1)], in_h, in_w)
     raw = eng.infer(x)[0]
     eng.close()
     with torch.no_grad():
@@ -261,7 +244,7 @@ def test_yolov10n_at_other_input_sizes(in_h, in_w):
 @pytest.mark.parametrize("scale", ["n", "m"])
 def test_yolov10_fused_detect_matches_reference_postprocessing(scale):
     """The device decode + candidate selection + NMS equals the reference's v8 host post-processing of the engine's own output."""
-    path, _ = v10_plan(scale)
+    path, _, _ = cached_plan("yolov10", scale=scale)
     eng = _capi.Engine(path, 0, max_batch=2)
     frames = np.stack([synth.frame(s) for s in (4, 5)])
     total = 0
@@ -284,9 +267,9 @@ def test_yolov10_fused_detect_matches_reference_postprocessing(scale):
 def test_yolov10_candidate_sets_follow_the_margin_rule(scale):
     """Candidates (max class probability > 0.4) agree with the fp32 oracle's wherever the oracle's score is more than 1e-3 from the
     threshold, and within 1e-3 of it where they do not."""
-    path, sd = v10_plan(scale)
+    path, sd, _ = cached_plan("yolov10", scale=scale)
     eng = _capi.Engine(path, 0, max_batch=4)
-    x = _blob([synth.frame(s) for s in (4, 5, 6, 7)])
+    x = yolo_blob([synth.frame(s) for s in (4, 5, 6, 7)])
     raw = eng.infer(x)[0]
     eng.close()
     with torch.no_grad():
@@ -320,7 +303,7 @@ def test_yolo_detector_runs_a_yolov10_onnx_file(tmp_path):
     finally:
         os.environ.pop("ADAS_B200_PLAN_CACHE", None)
     assert det.engine.handle.model_kind == plan.MODEL_YOLOV8
-    out = det.engine.engine_inference(_blob([synth.frame(3)]))
+    out = det.engine.engine_inference(yolo_blob([synth.frame(3)]))
     assert out[0].shape == (1, 84, 8400)
     fr = [synth.frame(3), synth.frame(4)]
     det.DetectFrame(fr[0])

@@ -1,7 +1,6 @@
 """GPU: YOLOv6 on the device -- the 2x2 transposed-conv store and the scaled residual of both GEMM epilogues, and YOLOv6-N/S/M/L end to
 end against the fp32 oracle (tests/yolov6_oracle.py) through the anchor-free v6 head decode."""
 import os
-import zlib
 
 import numpy as np
 import pytest
@@ -11,7 +10,7 @@ import torch.nn.functional as F
 import synth
 import adas_b200  # noqa: F401
 from adas_b200 import _capi, plan
-from gpu_util import from_padded, halo_is_zero, to_padded
+from gpu_util import cached_plan, from_padded, halo_is_zero, to_padded, yolo_blob
 from oracle import post
 import yolov6_oracle as o6
 
@@ -99,28 +98,12 @@ def test_residual_scale_one_is_the_plain_residual(tmp_path, impl):
         assert np.array_equal(a.view(np.uint16), b.view(np.uint16)), k
 
 
-def v6_plan(scale, seed=0):
-    """Seeded synthetic YOLOv6 plan, cached per operating point: (path, state_dict)."""
-    prof = zlib.crc32(repr((plan.SYNTH_PROFILES["yolov6"], plan.PLAN_VERSION)).encode()) & 0xffff
-    path = os.path.join(plan.cache_dir(), f"yolov6_{scale}_s{seed}_{prof:04x}.b200w")
-    W = plan.synth_weights("yolov6", seed, variant=scale)
-    pb = plan.build_yolov6(W, scale)
-    if not os.path.isfile(path):
-        pb.write(path + ".tmp")
-        os.replace(path + ".tmp", path)
-    return path, W.state_dict
-
-
-def _blob(frames):
-    return np.concatenate([post.yolo_prepare_input(f, 640, 640)[0] for f in frames])
-
-
 @pytest.mark.parametrize("impl", [0, 1])
 @pytest.mark.parametrize("scale", ["n", "s", "m", "l"])
 def test_yolov6_engine_vs_oracle_and_batch_invariance(scale, impl):
-    path, sd = v6_plan(scale)
+    path, sd, _ = cached_plan("yolov6", scale=scale)
     eng = _capi.Engine(path, 0, max_batch=3, conv_impl=impl)
-    x = _blob([synth.frame(s) for s in (0, 1, 2)])
+    x = yolo_blob([synth.frame(s) for s in (0, 1, 2)])
     raw = eng.infer(x)[0]
     with torch.no_grad():
         ref = o6.build(sd, scale)(torch.from_numpy(x[:2])).numpy()
@@ -139,7 +122,7 @@ def test_yolov6_engine_vs_oracle_and_batch_invariance(scale, impl):
 @pytest.mark.parametrize("scale", ["n", "m"])
 def test_yolov6_fused_detect_matches_reference_postprocessing(scale):
     """The device decode + candidate selection + NMS equals the reference's v5/v6/v7 host post-processing of the engine's own output."""
-    path, _ = v6_plan(scale)
+    path, _, _ = cached_plan("yolov6", scale=scale)
     eng = _capi.Engine(path, 0, max_batch=2)
     frames = np.stack([synth.frame(s) for s in (4, 5)])
     for score in (0.4, 0.05):
@@ -159,9 +142,9 @@ def test_yolov6_fused_detect_matches_reference_postprocessing(scale):
 def test_yolov6_candidate_sets_follow_the_margin_rule(scale):
     """Candidates (max class probability > 0.4) agree with the fp32 oracle's wherever the oracle's score is more than 1e-3 from the
     threshold, and few of them sit inside that margin."""
-    path, sd = v6_plan(scale)
+    path, sd, _ = cached_plan("yolov6", scale=scale)
     eng = _capi.Engine(path, 0, max_batch=4)
-    x = _blob([synth.frame(s) for s in (4, 5, 6, 7)])
+    x = yolo_blob([synth.frame(s) for s in (4, 5, 6, 7)])
     raw = eng.infer(x)[0]
     eng.close()
     with torch.no_grad():
@@ -198,7 +181,7 @@ def test_yolo_detector_runs_a_yolov6_onnx_file(tmp_path):
     finally:
         os.environ.pop("ADAS_B200_PLAN_CACHE", None)
     assert det.engine.handle.model_kind == plan.MODEL_YOLOV6
-    out = det.engine.engine_inference(_blob([synth.frame(3)]))
+    out = det.engine.engine_inference(yolo_blob([synth.frame(3)]))
     assert out[0].shape == (1, 8400, 85)
     fr = [synth.frame(3), synth.frame(4)]
     det.DetectFrame(fr[0])
@@ -210,7 +193,7 @@ def test_yolo_detector_runs_a_yolov6_onnx_file(tmp_path):
 def test_model_type_pairing_for_yolov6_plans(tmp_path):
     """The detector's existing pairing rule: a kind-5 plan runs as YOLOV5 / YOLOV6 / YOLOV7 and is refused for YOLOV5_LITE and the v8 layout."""
     from adas_b200.ObjectDetector import YoloDetector, ObjectModelType
-    path, _ = v6_plan("n")
+    path, _, _ = cached_plan("yolov6", scale="n")
     for mt, ok in ((ObjectModelType.YOLOV6, True), (ObjectModelType.YOLOV5, True), (ObjectModelType.YOLOV7, True),
                    (ObjectModelType.YOLOV5_LITE, False), (ObjectModelType.YOLOV8, False), (ObjectModelType.YOLOV10, False)):
         YoloDetector.set_defaults({"model_path": path, "model_type": mt, "classes_path": None, "box_score": 0.4, "box_nms_iou": 0.45})

@@ -6,7 +6,6 @@ consecutive batches, the fused detect against host post-processing, and YoloDete
 .onnx file."""
 import functools
 import os
-import zlib
 
 import numpy as np
 import pytest
@@ -15,10 +14,10 @@ import torch
 import synth
 import adas_b200  # noqa: F401
 from adas_b200 import _capi, plan
-from gpu_util import halo_is_zero
+from gpu_util import cached_plan, halo_is_zero, yolo_blob
 from oracle import post
 import op_conformance_cases as oc
-import plan_interp_lite as pl
+import plan_interp as pi
 import tile_space_cases as ts
 import yolov6_lite_oracle as ol
 
@@ -49,8 +48,8 @@ def _up2_hs(sweep_case, case, seed=0):
     for q in range(4):
         S[:, :, q // 2::2, q % 2::2] = np.einsum("nk,bkhw->bnhw", np.abs(w[q * cout:(q + 1) * cout]), np.abs(x))
     S += np.abs(sw.pb.tensors[sw.pb.ops[sw.ops[0][0]][1][5]][:cout].astype(np.float64))[None, :, None, None]
-    sw.ref = pl.hardswish(a)
-    sw.bound = pl.hardswish_bound(sw.ref, S, oc.r8(cin), a)
+    sw.ref = oc.act64(a, HS)
+    sw.bound = oc.gemm_bound(sw.ref, S, oc.r8(cin), HS, a)
     return sw
 
 
@@ -61,8 +60,7 @@ def test_hardswish_every_route_and_tile(tmp_path, monkeypatch, case):
     import test_gpu_tile_space as tgt
     if case[1] == "up2":
         monkeypatch.setattr(ts, "sweep_case", functools.partial(_up2_hs, ts.sweep_case))
-    with pl.extended():
-        tgt.test_tile_sweep(tmp_path, case)
+    tgt.test_tile_sweep(tmp_path, case)
 
 
 @pytest.mark.parametrize("route", ["tr", "stream"])
@@ -72,8 +70,7 @@ def test_hardswish_fully_connected(tmp_path, monkeypatch, route):
     monkeypatch.setattr(ts, "fc_sweep", functools.partial(ts.fc_sweep, act=HS))
     K, N = ts.FC_TR if route == "tr" else ts.FC_STREAM
     batches = (1, 16, 17, 48) if route == "tr" else ts.FC_STREAM_BATCHES
-    with pl.extended():
-        tgt._fc_batches(tmp_path, K, N, max(batches), [1, 2], batches, route).close()
+    tgt._fc_batches(tmp_path, K, N, max(batches), [1, 2], batches, route).close()
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
@@ -84,7 +81,7 @@ def _host(pb, B, mb, seed, scale=3.0, zero=()):
     channels, images >= B), the sentinel in its output buffer outside what it reads; zero halos.  `zero`: (buffer, lo, hi) regions
     that hold structural zeros (padded channels)."""
     rng = np.random.default_rng(seed)
-    writes, reads = pl.op_regions(pb, 0)
+    writes, reads = pi.op_regions(pb, 0)
     out_buf = writes[0].buf
     bufs = {}
     for i, (rows, C, _, H, W, _) in enumerate(pb.buffers):
@@ -110,8 +107,8 @@ def _check_op(tmp_path, pb, B=2, mb=3, seed=0, scale=3.0, zero=(), name="op"):
     path = str(tmp_path / f"{name}.b200w")
     pb.write(path)
     eng = _capi.Engine(path, device=0, max_batch=mb)
-    w = pl.out_region(pb, 0)
-    rows, C, _, H, W = pl.geom(pb, w.buf)
+    w = pi.out_region(pb, 0)
+    rows, C, _, H, W = pi.geom(pb, w.buf)
     results = []
     for r in range(3):
         host = _host(pb, B, mb, seed, scale, zero)
@@ -120,9 +117,9 @@ def _check_op(tmp_path, pb, B=2, mb=3, seed=0, scale=3.0, zero=(), name="op"):
         eng.run(B)
         got_buf = eng.read_buffer(w.buf, mb).copy()
         results.append(got_buf)
-        ref, bnd = pl.op_ref(pb, 0, host, B)
-        got = pl.read_out(pb, 0, {w.buf: got_buf}, B)
-        ratio, nbad = pl.excess(got, ref, bnd)
+        ref, bnd = pi.op_ref(pb, 0, host, B)
+        got = pi.read_out(pb, 0, {w.buf: got_buf}, B)
+        ratio, nbad = pi.excess(got, ref, bnd)
         assert nbad == 0, (name, r, ratio)
         assert halo_is_zero(got_buf, mb, H, W), f"{name} wrote into the zero halo"
         v = got_buf.reshape(mb, H + 2, W + 2, C)[:, 1:-1, 1:-1]
@@ -210,27 +207,13 @@ def test_shuffle2_bit_exact(tmp_path, n, H, W, same_buf):
 # ---------------------------------------------------------------------------------------------------------------------------
 # whole networks
 # ---------------------------------------------------------------------------------------------------------------------------
-def lite_plan(scale, seed=0, in_h=320, in_w=320):
-    """Seeded synthetic YOLOv6-Lite plan, cached per operating point: (path, state_dict)."""
-    prof = zlib.crc32(repr((plan.SYNTH_PROFILES["yolov6lite"], plan.PLAN_VERSION)).encode()) & 0xffff
-    path = os.path.join(plan.cache_dir(), f"yolov6lite_{scale}_{in_h}x{in_w}_s{seed}_{prof:04x}.b200w")
-    W = plan.synth_weights("yolov6lite", seed, variant=scale)
-    pb = plan.build_yolov6_lite(W, scale, in_h=in_h, in_w=in_w)
-    if not os.path.isfile(path):
-        pb.write(path + ".tmp")
-        os.replace(path + ".tmp", path)
-    return path, W.state_dict
-
-
-def _blob(frames, h, w):
-    return np.concatenate([post.yolo_prepare_input(f, h, w)[0] for f in frames])
 
 
 @pytest.mark.parametrize("impl", [0, 1])
 @pytest.mark.parametrize("scale,h,w", [("s", 320, 320), ("m", 320, 320), ("l", 320, 320), ("l", 224, 128), ("s", 320, 192)])
 def test_yolov6_lite_engine_vs_oracle_and_batch_invariance(scale, h, w, impl):
-    path, sd = lite_plan(scale, in_h=h, in_w=w)
-    x = _blob([synth.frame(s) for s in range(3)], h, w)
+    path, sd, _ = cached_plan("yolov6_lite", scale=scale, in_h=h, in_w=w)
+    x = yolo_blob([synth.frame(s) for s in range(3)], h, w)
     xb = np.concatenate([x] * 11)[:32]                           # frame k of a 32-image batch
     eng = _capi.Engine(path, 0, max_batch=32, conv_impl=impl)
     raw = eng.infer(x)[0]
@@ -260,9 +243,8 @@ def test_every_op_of_the_lite_plan_matches_float64(tmp_path, scale):
     import test_gpu_plan_conformance as gpc
     W = plan.synth_weights("yolov6lite", 0, variant=scale)
     apart = plan.build_yolov6_lite(W, scale, se_in_place=False)
-    assert not pl.stale_reads(apart) and not pl.overwritten(apart) and not pl.dataflow_violations(apart)
-    with pl.extended():
-        kinds, steps = gpc.run_aba(apart, "yolov6", {}, 2, 2, str(tmp_path / f"lite_{scale}_apart.b200w"))
+    assert not pi.stale_reads(apart) and not pi.overwritten(apart) and not pi.dataflow_violations(apart)
+    kinds, steps = gpc.run_aba(apart, "yolov6", {}, 2, 2, str(tmp_path / f"lite_{scale}_apart.b200w"))
     gpc.check_steps(kinds, steps)
     n_s1 = sum(n - 1 for n in plan.YOLOV6_LITE_BLOCKS)
     assert kinds.count("se") == n_s1 + 4 and kinds.count("shuffle2") == n_s1
@@ -270,7 +252,7 @@ def test_every_op_of_the_lite_plan_matches_float64(tmp_path, scale):
     eng = _capi.Engine(str(tmp_path / f"lite_{scale}_apart.b200w"), 0, max_batch=2)
     a = eng.infer(x)[0]
     eng.close()
-    path, _ = lite_plan(scale)
+    path, _, _ = cached_plan("yolov6_lite", scale=scale)
     eng = _capi.Engine(path, 0, max_batch=2)
     b = eng.infer(x)[0]
     descs = [eng.time_step(2, i, 1)[2] for i in range(eng.num_steps(2))]
@@ -281,7 +263,7 @@ def test_every_op_of_the_lite_plan_matches_float64(tmp_path, scale):
 
 @pytest.mark.parametrize("scale", ["s", "l"])
 def test_yolov6_lite_fused_detect_matches_reference_postprocessing(scale):
-    path, _ = lite_plan(scale)
+    path, _, _ = cached_plan("yolov6_lite", scale=scale)
     eng = _capi.Engine(path, 0, max_batch=2)
     frames = np.stack([synth.frame(s) for s in (4, 5)])
     total = 0
@@ -303,12 +285,12 @@ def test_yolov6_lite_fused_detect_matches_reference_postprocessing(scale):
 def test_yolo_detector_runs_a_yolov6_lite_plan(tmp_path):
     """YoloDetector(ObjectModelType.YOLOV6) on a YOLOv6-Lite-S .b200w plan: loaded, run and decoded like any YOLOv6 model."""
     from adas_b200.ObjectDetector import YoloDetector, ObjectModelType
-    path, _ = lite_plan("s")
+    path, _, _ = cached_plan("yolov6_lite", scale="s")
     YoloDetector.set_defaults({"model_path": path, "model_type": ObjectModelType.YOLOV6, "classes_path": None, "box_score": 0.4,
                                "box_nms_iou": 0.45})
     det = YoloDetector(logger=None, max_batch=2)
     assert det.engine.handle.model_kind == plan.MODEL_YOLOV6
-    out = det.engine.engine_inference(_blob([synth.frame(0)], 320, 320))
+    out = det.engine.engine_inference(yolo_blob([synth.frame(0)], 320, 320))
     assert out[0].shape == (1, 2125, 85)
     fr = [synth.frame(0), synth.frame(2)]
     det.DetectFrame(fr[0])
@@ -322,7 +304,7 @@ def test_yolo_detector_runs_a_yolov6_lite_onnx_file(tmp_path):
     and its network output equal to the plan built from the same state_dict."""
     from adas_b200.ObjectDetector import YoloDetector, ObjectModelType
     import test_yolov6_lite_cpu as tlc
-    path, sd = lite_plan("m")
+    path, sd, _ = cached_plan("yolov6_lite", scale="m")
     onnx_path = str(tmp_path / "yolov6lite_m.onnx")
     tlc._export(ol.build(sd, "m").fuse(), (1, 3, 320, 320), onnx_path, 14)
     os.environ["ADAS_B200_PLAN_CACHE"] = str(tmp_path / "cache")
@@ -333,7 +315,7 @@ def test_yolo_detector_runs_a_yolov6_lite_onnx_file(tmp_path):
     finally:
         os.environ.pop("ADAS_B200_PLAN_CACHE", None)
     assert det.engine.handle.model_kind == plan.MODEL_YOLOV6
-    x = _blob([synth.frame(0)], 320, 320)
+    x = yolo_blob([synth.frame(0)], 320, 320)
     out = det.engine.engine_inference(x)
     assert out[0].shape == (1, 2125, 85)
     eng = _capi.Engine(path, 0, max_batch=1)

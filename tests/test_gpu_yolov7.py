@@ -1,7 +1,6 @@
 """GPU: YOLOv7 / YOLOv7-tiny on the device -- the LeakyReLU(0.1) epilogue of every conv kernel, the stride-1 direct image stem, and
 both networks end to end against the fp32 oracle (tests/yolov7_oracle.py) with the plan-carried anchor table."""
 import os
-import zlib
 
 import numpy as np
 import pytest
@@ -11,7 +10,7 @@ import torch.nn.functional as F
 import synth
 import adas_b200  # noqa: F401
 from adas_b200 import _capi, plan
-from gpu_util import from_padded, halo_is_zero, to_padded
+from gpu_util import cached_plan, from_padded, halo_is_zero, to_padded, yolo_blob
 from oracle import post
 import yolov7_oracle as o7
 
@@ -135,28 +134,12 @@ def test_stem_conv_direct_stride1(tmp_path, cout, act):
         eng1.close(); eng.close()
 
 
-def v7_plan(scale, seed=0):
-    """Seeded synthetic YOLOv7 plan, cached per operating point: (path, state_dict)."""
-    prof = zlib.crc32(repr((plan.SYNTH_PROFILES["yolov7"], plan.PLAN_VERSION)).encode()) & 0xffff
-    path = os.path.join(plan.cache_dir(), f"yolov7_{scale}_s{seed}_{prof:04x}.b200w")
-    W = plan.synth_weights("yolov7", seed)
-    pb = plan.build_yolov7(W, scale)
-    if not os.path.isfile(path):
-        pb.write(path + ".tmp")
-        os.replace(path + ".tmp", path)
-    return path, W.state_dict
-
-
-def _blob(frames):
-    return np.concatenate([post.yolo_prepare_input(f, 640, 640)[0] for f in frames])
-
-
 @pytest.mark.parametrize("impl", [0, 1])
 @pytest.mark.parametrize("scale", ["tiny", "base"])
 def test_yolov7_engine_vs_oracle_and_batch_invariance(scale, impl):
-    path, sd = v7_plan(scale)
+    path, sd, _ = cached_plan("yolov7", scale=scale)
     eng = _capi.Engine(path, 0, max_batch=3, conv_impl=impl)
-    x = _blob([synth.frame(s) for s in (0, 1, 2)])
+    x = yolo_blob([synth.frame(s) for s in (0, 1, 2)])
     raw = eng.infer(x)[0]
     with torch.no_grad():
         ref = o7.build(sd, scale)(torch.from_numpy(x[:2])).numpy()
@@ -173,7 +156,7 @@ def test_yolov7_engine_vs_oracle_and_batch_invariance(scale, impl):
 
 @pytest.mark.parametrize("scale", ["tiny", "base"])
 def test_yolov7_fused_detect_matches_reference_postprocessing(scale):
-    path, sd = v7_plan(scale)
+    path, sd, _ = cached_plan("yolov7", scale=scale)
     eng = _capi.Engine(path, 0, max_batch=4)
     frames = np.stack([synth.frame(s) for s in (4, 5, 6, 7)])
     boxes, scores, cls, idx, counts, ncand = eng.yolo_detect(frames, 0.4, 0.45, max_det=1024)
@@ -218,7 +201,7 @@ def test_yolo_detector_runs_a_yolov7_onnx_file(tmp_path):
         det = YoloDetector(logger=None, max_batch=2)
     finally:
         os.environ.pop("ADAS_B200_PLAN_CACHE", None)
-    out = det.engine.engine_inference(_blob([synth.frame(3)]))
+    out = det.engine.engine_inference(yolo_blob([synth.frame(3)]))
     assert out[0].shape == (1, 25200, 85)
     fr = [synth.frame(3), synth.frame(4)]
     det.DetectFrame(fr[0])

@@ -1,7 +1,6 @@
 """GPU: YOLOv7 P6 models (W6 / E6 / D6 / E6E) on the device -- the 80 / 96-channel direct stem, the four-level YOLOv5-layout decode, and the
 networks end to end against the fp32 oracle (tests/yolov7_p6_oracle.py) with the plan-carried 4-level anchor table."""
 import os
-import zlib
 
 import numpy as np
 import pytest
@@ -11,7 +10,7 @@ import torch.nn.functional as F
 import synth
 import adas_b200  # noqa: F401
 from adas_b200 import _capi, plan
-from gpu_util import from_padded, halo_is_zero, to_padded
+from gpu_util import cached_plan, from_padded, halo_is_zero, to_padded, yolo_blob
 from oracle import post
 import yolov7_p6_oracle as o6
 
@@ -56,18 +55,6 @@ def test_stem_conv_6x6_s2_wide(tmp_path, cout):
         eng.close()
 
 
-def p6_plan(scale, size, seed=0):
-    """Seeded synthetic P6 plan, cached per operating point: (path, state_dict)."""
-    prof = zlib.crc32(repr((plan.SYNTH_PROFILES["yolov7"], plan.PLAN_VERSION)).encode()) & 0xffff
-    path = os.path.join(plan.cache_dir(), f"yolov7_{scale}_{size}_s{seed}_{prof:04x}.b200w")
-    W = plan.synth_weights("yolov7", seed)
-    pb = plan.build_yolov7(W, scale, in_h=size, in_w=size)
-    if not os.path.isfile(path):
-        pb.write(path + ".tmp")
-        os.replace(path + ".tmp", path)
-    return path, W.state_dict, pb
-
-
 def _host_v5_decode(heads, anchors, nc):
     """The YOLOv5-layout decode in numpy float32 from the raw head levels [(grid [B, H, W, C], stride)] and the plan's [L, 3, 2] anchors."""
     no, out = 5 + nc, []
@@ -88,7 +75,7 @@ def _host_v5_decode(heads, anchors, nc):
 def test_four_level_decode_matches_host_decode():
     """The engine's [B, A, 85] output against the host decode of its own head levels with the plan's 4 x 3 x 2 anchor table: the same rows
     in the same order (level -> anchor -> y -> x).  The sigmoid's expf is the only non-numpy operation (a few ulp)."""
-    path, _, pb = p6_plan("w6", 256)
+    path, _, pb = cached_plan("yolov7", scale="w6", in_h=256, in_w=256)
     eng = _capi.Engine(path, 0, max_batch=2)
     x = np.stack([post.yolo_prepare_input(synth.frame(s), 256, 256)[0][0] for s in (0, 1)])
     raw = eng.infer(x)[0]
@@ -108,16 +95,12 @@ def test_four_level_decode_matches_host_decode():
     eng.close()
 
 
-def _blob(frames, size):
-    return np.concatenate([post.yolo_prepare_input(f, size, size)[0] for f in frames])
-
-
 @pytest.mark.parametrize("impl", [0, 1])
 @pytest.mark.parametrize("scale,size", [("w6", 640), ("e6", 640), ("d6", 640), ("e6e", 640), ("w6", 1280)])
 def test_p6_engine_vs_oracle_and_batch_invariance(scale, size, impl):
-    path, sd, _ = p6_plan(scale, size)
+    path, sd, _ = cached_plan("yolov7", scale=scale, in_h=size, in_w=size)
     eng = _capi.Engine(path, 0, max_batch=3, conv_impl=impl)
-    x = _blob([synth.frame(s) for s in (0, 1, 2)], size)
+    x = yolo_blob([synth.frame(s) for s in (0, 1, 2)], size, size)
     raw = eng.infer(x)[0]
     with torch.no_grad():
         ref = o6.build(sd, scale)(torch.from_numpy(x[:2])).numpy()
@@ -134,7 +117,7 @@ def test_p6_engine_vs_oracle_and_batch_invariance(scale, size, impl):
 
 def test_w6_fused_detect_at_1280_matches_host_postprocessing():
     """A 1280x720 frame letterboxed to 1280x1280 (the resized image is 1280x721: the reference's +1) through the fused detect."""
-    path, sd, _ = p6_plan("w6", 1280)
+    path, sd, _ = cached_plan("yolov7", scale="w6", in_h=1280, in_w=1280)
     eng = _capi.Engine(path, 0, max_batch=2)
     frames = np.stack([synth.frame(s) for s in (4, 5)])
     geom = post.letterbox_geom(720, 1280, 1280, 1280)
@@ -178,7 +161,7 @@ def test_yolo_detector_runs_a_yolov7_w6_onnx_file(tmp_path):
         det = YoloDetector(logger=None, max_batch=2)
     finally:
         os.environ.pop("ADAS_B200_PLAN_CACHE", None)
-    out = det.engine.engine_inference(_blob([synth.frame(3)], 640))
+    out = det.engine.engine_inference(yolo_blob([synth.frame(3)], 640, 640))
     assert out[0].shape == (1, 3 * (80 * 80 + 40 * 40 + 20 * 20 + 10 * 10), 85)
     fr = [synth.frame(3), synth.frame(4)]
     det.DetectFrame(fr[0])

@@ -1,7 +1,6 @@
 """GPU: YOLOv9 on the device -- the 2x2 stride-1 average pool (OP_AVGPOOL2), the ADown / AConv blocks built on it, and YOLOv9-T/S/M/C
 end to end against the fp32 oracle (tests/yolov9_oracle.py) through YOLOv8's head decode, candidate selection and NMS."""
 import os
-import zlib
 
 import numpy as np
 import pytest
@@ -11,7 +10,7 @@ import torch.nn.functional as F
 import synth
 import adas_b200  # noqa: F401
 from adas_b200 import _capi, plan
-from gpu_util import from_padded, halo_is_zero, to_padded
+from gpu_util import cached_plan, from_padded, halo_is_zero, to_padded, yolo_blob
 from oracle import post
 import yolov9_oracle as o9
 
@@ -94,28 +93,12 @@ def test_adown_aconv_blocks_match_torch(tmp_path, impl, kind, c1, c2, H, W):
     assert err[..., -1, :].max() < 3e-3 and err[..., :, -1].max() < 3e-3
 
 
-def v9_plan(scale, seed=0):
-    """Seeded synthetic YOLOv9 plan, cached per operating point: (path, state_dict)."""
-    prof = zlib.crc32(repr((plan.SYNTH_PROFILES["yolov9"], plan.PLAN_VERSION)).encode()) & 0xffff
-    path = os.path.join(plan.cache_dir(), f"yolov9_{scale}_s{seed}_{prof:04x}.b200w")
-    W = plan.synth_weights("yolov9", seed, variant=scale)
-    pb = plan.build_yolov9(W, scale)
-    if not os.path.isfile(path):
-        pb.write(path + ".tmp")
-        os.replace(path + ".tmp", path)
-    return path, W.state_dict
-
-
-def _blob(frames):
-    return np.concatenate([post.yolo_prepare_input(f, 640, 640)[0] for f in frames])
-
-
 @pytest.mark.parametrize("impl", [0, 1])
 @pytest.mark.parametrize("scale", ["t", "s", "m", "c"])
 def test_yolov9_engine_vs_oracle_and_batch_invariance(scale, impl):
-    path, sd = v9_plan(scale)
+    path, sd, _ = cached_plan("yolov9", scale=scale)
     eng = _capi.Engine(path, 0, max_batch=3, conv_impl=impl)
-    x = _blob([synth.frame(s) for s in (0, 1, 2)])
+    x = yolo_blob([synth.frame(s) for s in (0, 1, 2)])
     raw = eng.infer(x)[0]
     with torch.no_grad():
         ref = o9.build(sd, scale)(torch.from_numpy(x[:2])).numpy()
@@ -133,7 +116,7 @@ def test_yolov9_engine_vs_oracle_and_batch_invariance(scale, impl):
 @pytest.mark.parametrize("scale", ["t", "m"])
 def test_yolov9_fused_detect_matches_reference_postprocessing(scale):
     """The device decode + candidate selection + NMS equals the reference's v8 host post-processing of the engine's own output."""
-    path, _ = v9_plan(scale)
+    path, _, _ = cached_plan("yolov9", scale=scale)
     eng = _capi.Engine(path, 0, max_batch=2)
     frames = np.stack([synth.frame(s) for s in (4, 5)])
     total = 0
@@ -156,9 +139,9 @@ def test_yolov9_fused_detect_matches_reference_postprocessing(scale):
 def test_yolov9_candidate_sets_follow_the_margin_rule(scale):
     """Candidates (max class probability > 0.4) agree with the fp32 oracle's wherever the oracle's score is more than 1e-3 from the
     threshold, and few of them sit inside that margin."""
-    path, sd = v9_plan(scale)
+    path, sd, _ = cached_plan("yolov9", scale=scale)
     eng = _capi.Engine(path, 0, max_batch=4)
-    x = _blob([synth.frame(s) for s in (4, 5, 6, 7)])
+    x = yolo_blob([synth.frame(s) for s in (4, 5, 6, 7)])
     raw = eng.infer(x)[0]
     eng.close()
     with torch.no_grad():
@@ -192,7 +175,7 @@ def test_yolo_detector_runs_a_yolov9_onnx_file(tmp_path):
     finally:
         os.environ.pop("ADAS_B200_PLAN_CACHE", None)
     assert det.engine.handle.model_kind == plan.MODEL_YOLOV8
-    out = det.engine.engine_inference(_blob([synth.frame(3)]))
+    out = det.engine.engine_inference(yolo_blob([synth.frame(3)]))
     assert out[0].shape == (1, 84, 8400)
     fr = [synth.frame(3), synth.frame(4)]
     det.DetectFrame(fr[0])

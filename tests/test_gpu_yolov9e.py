@@ -2,7 +2,6 @@
 to end against the fp32 oracle (tests/yolov9e_oracle.py), every op of the E plan against plan_interp's float64 references over
 consecutive batches, the fused detect against host post-processing, and YoloDetector on an exported E file."""
 import os
-import zlib
 
 import numpy as np
 import pytest
@@ -11,9 +10,9 @@ import torch
 import synth
 import adas_b200  # noqa: F401
 from adas_b200 import _capi, plan
-from gpu_util import from_padded, halo_is_zero
+from gpu_util import cached_plan, from_padded, halo_is_zero, yolo_blob
 from oracle import post
-import plan_interp_cbfuse as pi
+import plan_interp as pi
 import yolov9_oracle as o9
 import yolov9e_oracle as oe
 
@@ -142,28 +141,12 @@ def test_cblinear_cbfuse_block_matches_torch(tmp_path, impl):
     assert err.max() < 3e-3, (impl, float(err.max()))
 
 
-def v9e_plan(seed=0, in_h=640, in_w=640):
-    """Seeded synthetic YOLOv9-E plan, cached per operating point: (path, state_dict)."""
-    prof = zlib.crc32(repr((plan.SYNTH_PROFILES["yolov9"], plan.PLAN_VERSION)).encode()) & 0xffff
-    path = os.path.join(plan.cache_dir(), f"yolov9_e_{in_h}x{in_w}_s{seed}_{prof:04x}.b200w")
-    W = plan.synth_weights("yolov9", seed, variant="e")
-    pb = plan.build_yolov9(W, "e", in_h=in_h, in_w=in_w)
-    if not os.path.isfile(path):
-        pb.write(path + ".tmp")
-        os.replace(path + ".tmp", path)
-    return path, W.state_dict
-
-
-def _blob(frames, h=640, w=640):
-    return np.concatenate([post.yolo_prepare_input(f, h, w)[0] for f in frames])
-
-
 @pytest.mark.parametrize("impl", [0, 1])
 @pytest.mark.parametrize("h,w", [(640, 640), pytest.param(384, 640, marks=pytest.mark.slow)])
 def test_yolov9e_engine_vs_oracle_and_batch_invariance(h, w, impl):
-    path, sd = v9e_plan(in_h=h, in_w=w)
+    path, sd, _ = cached_plan("yolov9", scale="e", in_h=h, in_w=w)
     eng = _capi.Engine(path, 0, max_batch=3, conv_impl=impl)
-    x = _blob([synth.frame(s) for s in (0, 1, 2)], h, w)
+    x = yolo_blob([synth.frame(s) for s in (0, 1, 2)], h, w)
     raw = eng.infer(x)[0]
     with torch.no_grad():
         ref = oe.build(sd)(torch.from_numpy(x[:2])).numpy()
@@ -188,8 +171,7 @@ def test_every_op_of_the_e_plan_matches_float64(tmp_path):
     W = plan.synth_weights("yolov9", 0, variant="e")
     apart = plan.build_yolov9e(W, cbfuse_in_place=False)
     assert not pi.stale_reads(apart) and not pi.overwritten(apart)
-    with pi.extended():                                           # plan_interp with OP_CBFUSE for the A / B / A check
-        kinds, steps = gpc.run_aba(apart, "yolov9", {}, 2, 2, str(tmp_path / "e_apart.b200w"))
+    kinds, steps = gpc.run_aba(apart, "yolov9", {}, 2, 2, str(tmp_path / "e_apart.b200w"))
     gpc.check_steps(kinds, steps)
     assert kinds.count("cbfuse") == 5
     assert all(d.startswith("cbfuse ") for k, (_, d) in zip(kinds, steps) if k == "cbfuse")
@@ -197,7 +179,7 @@ def test_every_op_of_the_e_plan_matches_float64(tmp_path):
     eng = _capi.Engine(str(tmp_path / "e_apart.b200w"), 0, max_batch=2)
     a = eng.infer(x)[0]
     eng.close()
-    path, _ = v9e_plan()
+    path, _, _ = cached_plan("yolov9", scale="e")
     eng = _capi.Engine(path, 0, max_batch=2)
     b = eng.infer(x)[0]
     steps = [eng.time_step(2, i, 1)[2] for i in range(eng.num_steps(2))]
@@ -207,7 +189,7 @@ def test_every_op_of_the_e_plan_matches_float64(tmp_path):
 
 
 def test_yolov9e_fused_detect_matches_reference_postprocessing():
-    path, _ = v9e_plan()
+    path, _, _ = cached_plan("yolov9", scale="e")
     eng = _capi.Engine(path, 0, max_batch=2)
     frames = np.stack([synth.frame(s) for s in (4, 5)])
     total = 0
@@ -243,7 +225,7 @@ def test_yolo_detector_runs_a_yolov9e_onnx_file(tmp_path):
     finally:
         os.environ.pop("ADAS_B200_PLAN_CACHE", None)
     assert det.engine.handle.model_kind == plan.MODEL_YOLOV8
-    out = det.engine.engine_inference(_blob([synth.frame(0)]))
+    out = det.engine.engine_inference(yolo_blob([synth.frame(0)]))
     assert out[0].shape == (1, 84, 8400)
     fr = [synth.frame(0), synth.frame(2)]
     det.DetectFrame(fr[0])

@@ -191,3 +191,26 @@ def test_layernorm_bound_at_mean_over_std_200(two_pass, ok):
     got = _layernorm_emulate(x, g, bt, 4000, 1e-5, two_pass)
     assert (_violations(got, spec.ref, spec.bound) == 0) == ok
 
+
+def test_references_know_every_plan_op_and_activation():
+    """plan_interp and the bounds know Hardswish and every op type of the plan format with no setup; activation code 4 (which the
+    format leaves unused and the engine's validator refuses) and an unknown op type raise instead of passing as the identity."""
+    import plan_interp as pi
+    assert oc.act64(np.array([-1.0]), plan.ACT_HSWISH)[0] == -1.0 / 3.0
+    rng = np.random.default_rng(0)
+    pb = plan.PlanBuilder(plan.MODEL_YOLOV8, 3, 8, 8)
+    x = pb.new_padded(8, 8, 32)
+    pb.cbfuse(pb.sub(x, 0, 16), [(pb.sub(pb.new_padded(4, 4, 16), 0, 16), 1)])
+    pb.se(pb.sub(x, 16, 16), rng.standard_normal((4, 16)), rng.standard_normal(4), rng.standard_normal((16, 4)), rng.standard_normal(16))
+    pb.shuffle2(pb.sub(x, 0, 8), pb.sub(x, 8, 8))
+    assert [pi.op_kind(pb, i) for i in range(len(pb.ops))] == ["cbfuse", "se", "shuffle2"]
+    a = np.array([-1.0, 2.0])
+    for f in (lambda: pi._act(torch.from_numpy(a), 4), lambda: oc.act64(a, 4), lambda: oc.gemm_bound(a, a, 1, 4, a)):
+        with pytest.raises(ValueError, match="unknown activation code 4"):
+            f()
+    _, p, fl = pb.ops[0]
+    pb.ops[0] = (99, p, fl)
+    with pytest.raises(ValueError, match="unknown type 99"):
+        pi.op_regions(pb, 0)
+    with pytest.raises(ValueError, match="unknown type 99"):
+        pi.op_ref(pb, 0, pi.new_buffers(pb, 1, np.float64), 1)

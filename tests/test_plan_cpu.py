@@ -7,6 +7,7 @@ import torch
 
 import adas_b200  # noqa: F401
 from adas_b200 import plan
+import plan_footprint as fp
 
 
 def _params(W):
@@ -113,12 +114,6 @@ def test_ufld_v1_plan_geometry():
         assert not any(op[0] == plan.OP_LAYERNORM for op in pb.ops)
 
 
-def _corrupt(raw: bytes, off: int, fmt: str, value) -> bytes:
-    b = bytearray(raw)
-    struct.pack_into(fmt, b, off, value)
-    return bytes(b)
-
-
 def test_engine_rejects_inconsistent_plans(tmp_path):
     """Every index / offset / size of a plan is validated when it is loaded (before any device work, so this runs without a GPU):
     a corrupt or hostile plan must produce an error naming the plan, never an out-of-bounds access."""
@@ -134,13 +129,13 @@ def test_engine_rejects_inconsistent_plans(tmp_path):
     ten0 = op0 + n_ops * 112
     first_gemm = next(i for i, op in enumerate(pb.ops) if op[0] == plan.OP_GEMM)
     cases = {
-        "buffer index": _corrupt(raw, op0 + first_gemm * 112 + 4 + 4 * 11, "<i", n_buf + 7),          # out_buf of the first GEMM
-        "weight tensor index": _corrupt(raw, op0 + first_gemm * 112 + 4 + 4 * 4, "<i", 100000),
-        "channel slice": _corrupt(raw, op0 + first_gemm * 112 + 4 + 4 * 12, "<i", 1 << 20),            # out_coff
-        "tensor offset": _corrupt(raw, ten0, "<Q", 1 << 40),
-        "dataset id": _corrupt(raw, 8 + 4 * 2 + 4 * 3 + 4 * 4 + 4 * 6, "<I", 7),
-        "dataset geometry": _corrupt(raw, 8 + 4 * 2 + 4 * 3 + 4 * 4 + 4 * 6, "<I", 0),                 # TuSimple heads labelled CULane
-        "op type": _corrupt(raw, op0 + 112, "<I", 99),
+        "buffer index": fp.corrupt(raw, op0 + first_gemm * 112 + 4 + 4 * 11, "<i", n_buf + 7),          # out_buf of the first GEMM
+        "weight tensor index": fp.corrupt(raw, op0 + first_gemm * 112 + 4 + 4 * 4, "<i", 100000),
+        "channel slice": fp.corrupt(raw, op0 + first_gemm * 112 + 4 + 4 * 12, "<i", 1 << 20),            # out_coff
+        "tensor offset": fp.corrupt(raw, ten0, "<Q", 1 << 40),
+        "dataset id": fp.corrupt(raw, 8 + 4 * 2 + 4 * 3 + 4 * 4 + 4 * 6, "<I", 7),
+        "dataset geometry": fp.corrupt(raw, 8 + 4 * 2 + 4 * 3 + 4 * 4 + 4 * 6, "<I", 0),                 # TuSimple heads labelled CULane
+        "op type": fp.corrupt(raw, op0 + 112, "<I", 99),
         "truncated blob": raw[:len(raw) - 4096],
     }
     for name, data in cases.items():
@@ -173,3 +168,19 @@ def test_plan_cache_is_private(tmp_path, monkeypatch):
         assert "private" in str(e)
     else:
         raise AssertionError("a world-writable plan cache must be refused")
+
+
+def test_cached_plan_file_is_the_fresh_build(tmp_path, monkeypatch):
+    """gpu_util.cached_plan writes the plan it has just built even when the cache already holds a file of the same name from an older
+    builder: the engine must never load a plan other than the one whose weights and PlanBuilder the test compares against."""
+    from gpu_util import cached_plan
+    monkeypatch.setenv("ADAS_B200_PLAN_CACHE", str(tmp_path / "cache"))
+    path, _, _ = cached_plan("yolov5", scale="n", in_h=64, in_w=64)
+    old = open(path, "rb").read()
+    get = plan.Weights.get
+    monkeypatch.setattr(plan.Weights, "get", lambda self, name, shape, kind:
+                        get(self, name, shape, kind) * np.float32(2.0 if name == "model.0.conv.weight" else 1.0))
+    again, _, pb = cached_plan("yolov5", scale="n", in_h=64, in_w=64)
+    fresh = tmp_path / "fresh.b200w"
+    pb.write(str(fresh))
+    assert again == path and open(path, "rb").read() == fresh.read_bytes() != old

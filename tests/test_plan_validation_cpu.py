@@ -58,13 +58,6 @@ def _refused(path):
     return None
 
 
-def _corrupt(src, dst, off, fmt, value):
-    raw = bytearray(open(src, "rb").read())
-    struct.pack_into(fmt, raw, off, value)
-    open(dst, "wb").write(bytes(raw))
-    return dst
-
-
 def _values(v, neighbour, nb):
     vals = {0, -1, 1, v - 1, v + 1, v - 8, v + 8, INT32_MAX}
     if neighbour is not None:
@@ -176,11 +169,13 @@ def test_mutated_single_op_plans_are_refused_or_in_bounds(tmp_path_factory, fami
 
 # ---- the holes the loader had, each on the smallest plan that shows it ---------------------------------------------------------
 def _expect_refused(src, tmp_path, name, off, fmt, value, phrase):
-    bad = _corrupt(src, str(tmp_path / f"{name}.b200w"), off, fmt, value)
-    msg = _refused(bad)
+    raw = fp.corrupt(open(src, "rb").read(), off, fmt, value)
+    bad = tmp_path / f"{name}.b200w"
+    bad.write_bytes(raw)
+    msg = _refused(str(bad))
     assert msg is not None, f"{name}: the corrupted plan loads"
     assert msg.startswith("plan ") and phrase in msg, (name, msg)
-    return fp.parse(open(bad, "rb").read())
+    return fp.parse(raw)
 
 
 def test_yolov8_head_corruptions_are_refused(tmp_path_factory, tmp_path):

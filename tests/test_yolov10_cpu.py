@@ -10,7 +10,8 @@ import pytest
 import torch
 
 import adas_b200  # noqa: F401
-from adas_b200 import _capi, plan
+from adas_b200 import plan
+import plan_footprint as fp
 import yolov10_oracle as o10
 
 PUBLISHED = [("n", 2.299, 6.69), ("s", 7.249, 21.58), ("m", 15.359, 59.10), ("b", 19.066, 91.95), ("l", 24.371, 120.34),
@@ -124,25 +125,11 @@ def test_build_yolov10_refuses_bad_inputs():
     assert pb.meta[1] == 60 * 80 + 30 * 40 + 15 * 20
 
 
-def _engine_error(path):
-    try:
-        _capi.Engine(str(path))
-    except Exception as e:
-        return str(e)
-    return None
-
-
-def _corrupt(raw: bytes, off: int, fmt: str, value) -> bytes:
-    b = bytearray(raw)
-    struct.pack_into(fmt, b, off, value)
-    return bytes(b)
-
-
 def _check_cases(tmp_path, raw, cases):
     for name, data, msg in cases:
         bad = tmp_path / "bad.b200w"
         bad.write_bytes(data)
-        err = _engine_error(bad)
+        err = fp.engine_error(bad)
         assert err is not None and "plan" in err and msg in err, (name, err)
 
 
@@ -159,11 +146,11 @@ def test_plan_validator_rejects_bad_dwconv_ops(tmp_path):
     w7 = pb.tensor(np.zeros((49, 16), np.float16))
     good = tmp_path / "dw.b200w"
     pb.write(str(good))
-    assert "no CUDA device" in _engine_error(good)
+    assert "no CUDA device" in fp.engine_error(good)
     raw = good.read_bytes()
     op = struct.calcsize("<8sII3I4I16IQQ") + len(pb.buffers) * 24 + 4
     p = lambda i: op + 4 * i
-    c = lambda i, v, r=raw: _corrupt(r, p(i), "<i", v)
+    c = lambda i, v, r=raw: fp.corrupt(r, p(i), "<i", v)
     _check_cases(tmp_path, raw, [
         ("input index", c(0, 99), "index out of range"),
         ("output index", c(8, -1), "index out of range"),
@@ -199,12 +186,12 @@ def test_plan_validator_rejects_bad_attention_ops(tmp_path):
     pb.attention(qkv, 2, 32, 64, 32 ** -0.5, out=out)
     good = tmp_path / "at.b200w"
     pb.write(str(good))
-    assert "no CUDA device" in _engine_error(good)
+    assert "no CUDA device" in fp.engine_error(good)
     raw = good.read_bytes()
     op = struct.calcsize("<8sII3I4I16IQQ") + len(pb.buffers) * 24 + 4
     p = lambda i: op + 4 * i
     f0 = op + 4 * 23
-    c = lambda i, v, r=raw: _corrupt(r, p(i), "<i", v)
+    c = lambda i, v, r=raw: fp.corrupt(r, p(i), "<i", v)
     _check_cases(tmp_path, raw, [
         ("input index", c(0, 99), "index out of range"),
         ("output index", c(5, -1), "index out of range"),
@@ -218,8 +205,8 @@ def test_plan_validator_rejects_bad_attention_ops(tmp_path):
         ("qkv slice", c(2, 3), "exceeds"),
         ("output slice", c(6, 8), "exceeds"),
         ("in place", c(5, qkv.buf), "overlaps"),
-        ("scale", _corrupt(raw, f0, "<f", float("nan")), "scale"),
-        ("negative scale", _corrupt(raw, f0, "<f", -1.0), "scale"),
+        ("scale", fp.corrupt(raw, f0, "<f", float("nan")), "scale"),
+        ("negative scale", fp.corrupt(raw, f0, "<f", -1.0), "scale"),
     ])
 
 

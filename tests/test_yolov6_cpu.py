@@ -10,7 +10,8 @@ import pytest
 import torch
 
 import adas_b200  # noqa: F401
-from adas_b200 import _capi, plan
+from adas_b200 import plan
+import plan_footprint as fp
 import yolov6_oracle as o6
 
 
@@ -123,26 +124,12 @@ def test_deployed_checkpoint_packs_the_training_form_plan():
         assert a.shape == b.shape and np.abs(a.astype(np.float32) - b.astype(np.float32)).max() <= 2e-3 * max(1.0, float(np.abs(a).max()))
 
 
-def _engine_error(path):
-    try:
-        _capi.Engine(str(path))
-    except Exception as e:
-        return str(e)
-    return None
-
-
-def _corrupt(raw: bytes, off: int, fmt: str, value) -> bytes:
-    b = bytearray(raw)
-    struct.pack_into(fmt, b, off, value)
-    return bytes(b)
-
-
 @pytest.mark.skipif(torch.cuda.is_available(), reason="load-time validation is observed through the missing-device error")
 def test_plan_validator_rejects_bad_yolov6_fields(tmp_path):
     pb = plan.build_yolov6(plan.synth_weights("yolov6", 0), "m", in_h=320, in_w=320)
     good = tmp_path / "v6m.b200w"
     pb.write(str(good))
-    assert "no CUDA device" in _engine_error(good)
+    assert "no CUDA device" in fp.engine_error(good)
     raw = good.read_bytes()
     hdr = struct.calcsize("<8sII3I4I16IQQ")
     meta2 = 8 + 4 * 2 + 4 * 3 + 4 * 4 + 4 * 2
@@ -151,14 +138,14 @@ def test_plan_validator_rejects_bad_yolov6_fields(tmp_path):
     res = next(i for i, op in enumerate(pb.ops) if op[0] == plan.OP_GEMM and op[1][8] >= 0)
     out_rec = hdr + len(pb.buffers) * 24 + len(pb.ops) * 112 + len(pb.tensors) * 24
     cases = [
-        ("reg_max", _corrupt(raw, meta2, "<I", 8), "reg_max"),
-        ("narrow level", _corrupt(raw, out_rec + 8, "<I", 72 + 79), "columns wide"),
-        ("transposed Cout", _corrupt(raw, op0 + up * 112 + 4 + 6 * 4, "<i", pb.ops[up][1][6] - 16), "transposed conv"),
-        ("transposed geometry", _corrupt(raw, op0 + up * 112 + 4 + 11 * 4, "<i", pb.ops[up][1][0]), "transposed conv"),
-        ("residual scale", _corrupt(raw, op0 + res * 112 + 4 + 23 * 4, "<f", float("inf")), "residual scale"),
+        ("reg_max", fp.corrupt(raw, meta2, "<I", 8), "reg_max"),
+        ("narrow level", fp.corrupt(raw, out_rec + 8, "<I", 72 + 79), "columns wide"),
+        ("transposed Cout", fp.corrupt(raw, op0 + up * 112 + 4 + 6 * 4, "<i", pb.ops[up][1][6] - 16), "transposed conv"),
+        ("transposed geometry", fp.corrupt(raw, op0 + up * 112 + 4 + 11 * 4, "<i", pb.ops[up][1][0]), "transposed conv"),
+        ("residual scale", fp.corrupt(raw, op0 + res * 112 + 4 + 23 * 4, "<f", float("inf")), "residual scale"),
     ]
     for name, data, msg in cases:
         bad = tmp_path / "bad.b200w"
         bad.write_bytes(data)
-        err = _engine_error(bad)
+        err = fp.engine_error(bad)
         assert err is not None and "plan" in err and msg in err, (name, err)

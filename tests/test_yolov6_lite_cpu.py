@@ -14,8 +14,9 @@ import pytest
 import torch
 
 import adas_b200  # noqa: F401
-from adas_b200 import _capi, plan
-import plan_interp_lite as pl
+from adas_b200 import plan
+import plan_footprint as fp
+import plan_interp as pi
 import synth
 import yolov6_lite_oracle as ol
 from gpu_util import to_padded
@@ -140,7 +141,7 @@ def _decode(pb, bufs):
     """The device decode (yolo_post.cu, reg_max 0) of plan_interp's head buffers for image 0: [A, 4 + nc]."""
     outs = []
     for buf, _, _, stride in pb.outputs:
-        rows, C, _, H, W = pl.geom(pb, buf)
+        rows, C, _, H, W = pi.geom(pb, buf)
         v = bufs[buf][:rows].reshape(H + 2, W + 2, C)[1:-1, 1:-1]
         d = v[..., :4]
         yy, xx = np.meshgrid(np.arange(H), np.arange(W), indexing="ij")
@@ -155,12 +156,12 @@ def test_interpreter_reproduces_the_oracle(scale, h, w):
     """plan_interp (float64, every op of the plan) against the fp32 oracle, including the ceil(H / 64) x ceil(W / 64) P6 level of inputs
     that are not multiples of 64; rounded to the plan's dtypes (the device's storage) it stays inside the 1e-3 probability contract."""
     W, pb = _weights(scale, 0, in_h=h, in_w=w)
-    assert [(pl.geom(pb, b)[3], pl.geom(pb, b)[4]) for b, _, _, _ in pb.outputs] == [(-(-h // s), -(-w // s)) for s in (8, 16, 32, 64)]
+    assert [(pi.geom(pb, b)[3], pi.geom(pb, b)[4]) for b, _, _, _ in pb.outputs] == [(-(-h // s), -(-w // s)) for s in (8, 16, 32, 64)]
     blob = post.yolo_prepare_input(synth.frame(0), h, w)[0]
     with torch.no_grad():
         ref = ol.build(W.state_dict, scale)(torch.from_numpy(blob)).numpy()[0]
     for rnd, tol_p, tol_b in ((False, 3e-4, 0.02), (True, 1e-3, 0.1)):
-        got = _decode(pb, pl.interpret(pb, to_padded(blob, 4), 1, round_to_plan=rnd))
+        got = _decode(pb, pi.interpret(pb, to_padded(blob, 4), 1, round_to_plan=rnd))
         assert np.abs(got[:, 4:] - ref[:, 5:]).max() < tol_p, (rnd, np.abs(got[:, 4:] - ref[:, 5:]).max())
         assert np.abs(got[:, :4] - ref[:, :4]).max() < tol_b, (rnd, np.abs(got[:, :4] - ref[:, :4]).max())
 
@@ -170,21 +171,11 @@ def test_dataflow():
     overlaps are the SE ops writing the slice they read."""
     W = plan.synth_weights("yolov6lite", 0, variant="m")
     apart = plan.build_yolov6_lite(W, "m", se_in_place=False)
-    assert not pl.dataflow_violations(apart) and not pl.stale_reads(apart) and not pl.overwritten(apart)
+    assert not pi.dataflow_violations(apart) and not pi.stale_reads(apart) and not pi.overwritten(apart)
     inplace = plan.build_yolov6_lite(W, "m")
-    v = pl.dataflow_violations(inplace)
+    v = pi.dataflow_violations(inplace)
     assert v and all("(se) writes" in m for m in v)
-    assert all(inplace.ops[i][0] == plan.OP_SE for i in pl.stale_reads(inplace))
-
-
-def test_plan_interp_is_unchanged_outside_the_context():
-    import plan_interp
-    import op_conformance_cases as oc
-    assert plan.OP_SE not in plan_interp.OP_NAMES and oc.act64(np.array([-1.0]), plan.ACT_HSWISH)[0] == -1.0
-    with pl.extended():
-        assert plan_interp.OP_NAMES[plan.OP_SE] == "se"
-        assert oc.act64(np.array([-1.0]), plan.ACT_HSWISH)[0] == -1.0 / 3.0
-    assert plan.OP_SE not in plan_interp.OP_NAMES and oc.act64(np.array([-1.0]), plan.ACT_HSWISH)[0] == -1.0
+    assert all(inplace.ops[i][0] == plan.OP_SE for i in pi.stale_reads(inplace))
 
 
 def test_se_and_shuffle_references():
@@ -197,35 +188,23 @@ def test_se_and_shuffle_references():
     pb.se(x, sd["conv1.weight"], sd["conv1.bias"], sd["conv2.weight"], sd["conv2.bias"])
     a, b = pb.sub(pb.new_padded(5, 7, 16), 0, 16), pb.sub(x.__class__(x.buf, 16, 16, 5, 7), 0, 16)
     pb.shuffle2(a, b)
-    bufs = pl.new_buffers(pb, 1, np.float64)
+    bufs = pi.new_buffers(pb, 1, np.float64)
     xv = rng.standard_normal((1, 12, 5, 7))
     bufs[x.buf].reshape(7, 9, 32)[1:-1, 1:-1, 8:20] = xv[0].transpose(1, 2, 0)
     bufs[a.buf].reshape(7, 9, 16)[1:-1, 1:-1] = rng.standard_normal((5, 7, 16))
-    ref, bnd = pl.op_ref(pb, 0, bufs, 1)
+    ref, bnd = pi.op_ref(pb, 0, bufs, 1)
     with torch.no_grad():
         want = blk(torch.from_numpy(xv).float()).numpy()
     assert np.abs(ref[:, :12] - want).max() < 1e-5 and not ref[:, 12:].any() and np.all(bnd > 0)
-    sh, none = pl.op_ref(pb, 1, bufs, 1)
-    av = pl.pi.image_view(pb, bufs, a.buf, 0, 0, 16, "cpu")
-    bv = pl.pi.image_view(pb, bufs, b.buf, 0, b.coff, b.coff + 16, "cpu")
+    sh, none = pi.op_ref(pb, 1, bufs, 1)
+    av = pi.image_view(pb, bufs, a.buf, 0, 0, 16, "cpu")
+    bv = pi.image_view(pb, bufs, b.buf, 0, b.coff, b.coff + 16, "cpu")
     assert none is None and np.array_equal(sh, ol.channel_shuffle(torch.cat([av, bv], 1)).numpy())
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
 # the validators
 # ---------------------------------------------------------------------------------------------------------------------------
-def _engine_error(path):
-    try:
-        _capi.Engine(str(path))
-    except Exception as e:
-        return str(e)
-    return None
-
-
-def _put(raw: bytes, off: int, value) -> bytes:
-    b = bytearray(raw)
-    struct.pack_into("<i", b, off, value)
-    return bytes(b)
 
 
 def _op_field(pb, i, k):
@@ -236,7 +215,7 @@ def _check(tmp_path, raw, cases):
     for name, data, msg in cases:
         bad = tmp_path / "bad.b200w"
         bad.write_bytes(data)
-        err = _engine_error(bad)
+        err = fp.engine_error(bad)
         assert err is not None and "plan" in err and msg in err, (name, err)
 
 
@@ -255,29 +234,29 @@ def test_plan_validator_rejects_bad_se_ops(tmp_path):
     f16 = pb.tensor(np.zeros(24 * 5, np.float16))
     good = tmp_path / "se.b200w"
     pb.write(str(good))
-    assert "no CUDA device" in _engine_error(good)
+    assert "no CUDA device" in fp.engine_error(good)
     raw = good.read_bytes()
     p = lambda k: _op_field(pb, 0, k)
     _check(tmp_path, raw, [
-        ("input index", _put(raw, p(0), 99), "index out of range"),
-        ("output index", _put(raw, p(8), -1), "index out of range"),
-        ("fp32 input", _put(_put(raw, p(0), f32.buf), p(8), f32.buf), "fp16"),
-        ("geometry", _put(raw, p(8), other.buf), "H x W"),
-        ("channels", _put(raw, p(2), 12), "channels"),
-        ("too many channels", _put(raw, p(2), 1032), "channels"),
-        ("no hidden", _put(raw, p(3), 0), "hidden"),
-        ("hidden 257", _put(raw, p(3), 257), "hidden"),
-        ("offset", _put(_put(raw, p(1), 4), p(9), 4), "multiples of 8"),
-        ("w1 size", _put(raw, p(4), 1), "se tensor 0"),
-        ("w2 is b2", _put(raw, p(6), 3), "se tensor 2"),
-        ("fp16 tensor", _put(raw, p(5), f16), "se tensor 1"),
-        ("tensor index", _put(raw, p(7), 99), "se tensor 3"),
-        ("slice", _put(_put(raw, p(1), 24), p(9), 24), "exceeds"),
-        ("partial overlap", _put(raw, p(9), 16), "overlaps"),
+        ("input index", fp.corrupt(raw, p(0), "<i", 99), "index out of range"),
+        ("output index", fp.corrupt(raw, p(8), "<i", -1), "index out of range"),
+        ("fp32 input", fp.corrupt(fp.corrupt(raw, p(0), "<i", f32.buf), p(8), "<i", f32.buf), "fp16"),
+        ("geometry", fp.corrupt(raw, p(8), "<i", other.buf), "H x W"),
+        ("channels", fp.corrupt(raw, p(2), "<i", 12), "channels"),
+        ("too many channels", fp.corrupt(raw, p(2), "<i", 1032), "channels"),
+        ("no hidden", fp.corrupt(raw, p(3), "<i", 0), "hidden"),
+        ("hidden 257", fp.corrupt(raw, p(3), "<i", 257), "hidden"),
+        ("offset", fp.corrupt(fp.corrupt(raw, p(1), "<i", 4), p(9), "<i", 4), "multiples of 8"),
+        ("w1 size", fp.corrupt(raw, p(4), "<i", 1), "se tensor 0"),
+        ("w2 is b2", fp.corrupt(raw, p(6), "<i", 3), "se tensor 2"),
+        ("fp16 tensor", fp.corrupt(raw, p(5), "<i", f16), "se tensor 1"),
+        ("tensor index", fp.corrupt(raw, p(7), "<i", 99), "se tensor 3"),
+        ("slice", fp.corrupt(fp.corrupt(raw, p(1), "<i", 24), p(9), "<i", 24), "exceeds"),
+        ("partial overlap", fp.corrupt(raw, p(9), "<i", 16), "overlaps"),
     ])
     ok = tmp_path / "ok.b200w"
-    ok.write_bytes(_put(raw, p(8), out.buf))                                   # out of place
-    assert "no CUDA device" in _engine_error(ok)
+    ok.write_bytes(fp.corrupt(raw, p(8), "<i", out.buf))                                   # out of place
+    assert "no CUDA device" in fp.engine_error(ok)
 
 
 @no_gpu
@@ -289,21 +268,21 @@ def test_plan_validator_rejects_bad_shuffle2_ops(tmp_path):
     pb.shuffle2(pb.sub(src, 0, 16), pb.sub(src, 32, 16), out=pb.sub(pb.new_padded(8, 8, 40), 8, 32))
     good = tmp_path / "sh.b200w"
     pb.write(str(good))
-    assert "no CUDA device" in _engine_error(good)
+    assert "no CUDA device" in fp.engine_error(good)
     raw = good.read_bytes()
     p = lambda k: _op_field(pb, 0, k)
     _check(tmp_path, raw, [
-        ("a index", _put(raw, p(0), 99), "index out of range"),
-        ("b index", _put(raw, p(2), -1), "index out of range"),
-        ("out index", _put(raw, p(5), 99), "index out of range"),
-        ("fp32 source", _put(raw, p(2), f32.buf), "fp16"),
-        ("geometry", _put(raw, p(0), other.buf), "H x W"),
-        ("channels", _put(raw, p(4), 12), "multiples of 8"),
-        ("no channels", _put(raw, p(4), 0), "multiples of 8"),
-        ("offset", _put(raw, p(1), 4), "multiples of 8"),
-        ("source slice", _put(raw, p(3), 40), "exceeds"),
-        ("output slice", _put(raw, p(6), 16), "exceeds"),
-        ("output over a source", _put(_put(raw, p(5), src.buf), p(6), 16), "overlaps"),
+        ("a index", fp.corrupt(raw, p(0), "<i", 99), "index out of range"),
+        ("b index", fp.corrupt(raw, p(2), "<i", -1), "index out of range"),
+        ("out index", fp.corrupt(raw, p(5), "<i", 99), "index out of range"),
+        ("fp32 source", fp.corrupt(raw, p(2), "<i", f32.buf), "fp16"),
+        ("geometry", fp.corrupt(raw, p(0), "<i", other.buf), "H x W"),
+        ("channels", fp.corrupt(raw, p(4), "<i", 12), "multiples of 8"),
+        ("no channels", fp.corrupt(raw, p(4), "<i", 0), "multiples of 8"),
+        ("offset", fp.corrupt(raw, p(1), "<i", 4), "multiples of 8"),
+        ("source slice", fp.corrupt(raw, p(3), "<i", 40), "exceeds"),
+        ("output slice", fp.corrupt(raw, p(6), "<i", 16), "exceeds"),
+        ("output over a source", fp.corrupt(fp.corrupt(raw, p(5), "<i", src.buf), p(6), "<i", 16), "overlaps"),
     ])
 
 
@@ -326,14 +305,14 @@ def test_activation_codes(tmp_path, op):
     assert pb.ops[-1][0] == {"gemm": plan.OP_GEMM, "stem": plan.OP_STEMCONV, "dwconv": plan.OP_DWCONV}[op]
     good = tmp_path / f"{op}.b200w"
     pb.write(str(good))
-    assert "no CUDA device" in _engine_error(good)
+    assert "no CUDA device" in fp.engine_error(good)
     raw = good.read_bytes()
     f = _op_field(pb, len(pb.ops) - 1, k)
     msg = "dwconv act" if op == "dwconv" else "unknown activation"
-    _check(tmp_path, raw, [(f"act {a}", _put(raw, f, a), f"{msg} {a}") for a in (4, 6, -1)])
+    _check(tmp_path, raw, [(f"act {a}", fp.corrupt(raw, f, "<i", a), f"{msg} {a}") for a in (4, 6, -1)])
     if op == "dwconv":
-        _check(tmp_path, raw, [("k 5 stride 3", _put(raw, _op_field(pb, 0, 4), 3), "dwconv k 5 stride 3"),
-                               ("k 9", _put(raw, _op_field(pb, 0, 3), 9), "dwconv k 9")])
+        _check(tmp_path, raw, [("k 5 stride 3", fp.corrupt(raw, _op_field(pb, 0, 4), "<i", 3), "dwconv k 5 stride 3"),
+                               ("k 9", fp.corrupt(raw, _op_field(pb, 0, 3), "<i", 9), "dwconv k 9")])
 
 
 @no_gpu
@@ -343,14 +322,14 @@ def test_four_level_head_validation(tmp_path):
     _, pb = _weights("s", in_h=224, in_w=128)
     good = tmp_path / "lite.b200w"
     pb.write(str(good))
-    assert "no CUDA device" in _engine_error(good)
+    assert "no CUDA device" in fp.engine_error(good)
     raw = good.read_bytes()
     nb, no, nt = len(pb.buffers), len(pb.ops), len(pb.tensors)
     out = lambda i, k: HDR + nb * 24 + no * 112 + nt * 24 + i * 16 + 4 * k
     _check(tmp_path, raw, [
-        ("P6 grid of the P5 level", _put(raw, out(3, 0), pb.outputs[2][0]), "YOLOv6 head has 3 levels"),
-        ("P6 stride 32", _put(raw, out(3, 3), 32), "YOLOv6 head has 3 levels"),
-        ("P5 grid on level 2", _put(raw, out(2, 0), pb.outputs[1][0]), "YOLOv6 level 2"),
+        ("P6 grid of the P5 level", fp.corrupt(raw, out(3, 0), "<i", pb.outputs[2][0]), "YOLOv6 head has 3 levels"),
+        ("P6 stride 32", fp.corrupt(raw, out(3, 3), "<i", 32), "YOLOv6 head has 3 levels"),
+        ("P5 grid on level 2", fp.corrupt(raw, out(2, 0), "<i", pb.outputs[1][0]), "YOLOv6 level 2"),
     ])
 
 

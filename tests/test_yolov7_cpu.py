@@ -11,7 +11,8 @@ import pytest
 import torch
 
 import adas_b200  # noqa: F401
-from adas_b200 import _capi, onnx_import, plan
+from adas_b200 import onnx_import, plan
+import plan_footprint as fp
 import test_onnx_import as toi
 import yolov7_oracle as o7
 
@@ -139,25 +140,17 @@ def test_checkpoint_conversion(tmp_path):
     assert np.array_equal(pb.tensors[pb.meta[3] - 1], np.arange(1, 19, dtype=np.float32))
 
 
-def _engine_error(path):
-    try:
-        _capi.Engine(str(path))
-    except Exception as e:
-        return str(e)
-    return None
-
-
 @pytest.mark.skipif(torch.cuda.is_available(), reason="load-time validation is observed through the missing-device error")
 def test_anchor_table_and_activation_validation(tmp_path):
     # a plan without an anchor table (every YOLOv5 plan) validates and decodes with the YOLOv5 table
     v5 = tmp_path / "v5n.b200w"
     plan.build_yolov5(plan.synth_weights("yolov5", 0), "n").write(str(v5))
-    assert "no CUDA device" in _engine_error(v5)
+    assert "no CUDA device" in fp.engine_error(v5)
     assert np.array_equal(plan.read_anchors(str(v5)), np.asarray(plan.YOLOV5_ANCHORS, np.float32).reshape(3, 3, 2))
     v7 = tmp_path / "v7.b200w"
     pb = plan.build_yolov7(plan.synth_weights("yolov7", 0), "tiny", in_h=320, in_w=320, anchors=plan.YOLOV7_ANCHORS)
     pb.write(str(v7))
-    assert "no CUDA device" in _engine_error(v7)
+    assert "no CUDA device" in fp.engine_error(v7)
     assert np.array_equal(plan.read_anchors(str(v7)), np.asarray(plan.YOLOV7_ANCHORS, np.float32).reshape(3, 3, 2))
     # a non-positive anchor, an anchor index outside the tensors, an anchor table on a lite plan: rejected at load
     raw = v7.read_bytes()
@@ -166,13 +159,13 @@ def test_anchor_table_and_activation_validation(tmp_path):
     blob = struct.unpack_from("<Q", raw, hdr - 16)[0]
     off = struct.unpack_from("<Q", raw, t_rec)[0]
     meta3 = 8 + 4 * 2 + 4 * 3 + 4 * 4 + 4 * 3
-    for name, data in (("negative anchor", toi_corrupt(raw, blob + off + 8, "<f", -4.0)),
-                       ("nan anchor", toi_corrupt(raw, blob + off, "<f", float("nan"))),
-                       ("anchor index", toi_corrupt(raw, meta3, "<I", 100000)),
-                       ("lite flag", toi_corrupt(raw, meta3 - 4, "<I", 1))):
+    for name, data in (("negative anchor", fp.corrupt(raw, blob + off + 8, "<f", -4.0)),
+                       ("nan anchor", fp.corrupt(raw, blob + off, "<f", float("nan"))),
+                       ("anchor index", fp.corrupt(raw, meta3, "<I", 100000)),
+                       ("lite flag", fp.corrupt(raw, meta3 - 4, "<I", 1))):
         bad = tmp_path / "bad.b200w"
         bad.write_bytes(data)
-        err = _engine_error(bad)
+        err = fp.engine_error(bad)
         assert err is not None and "plan" in err and "anchor" in err, (name, err)
     # activation ids above 3 are rejected (GEMM and stem conv)
     for image in (False, True):
@@ -182,13 +175,7 @@ def test_anchor_table_and_activation_validation(tmp_path):
         p = tmp_path / f"act{int(image)}.b200w"
         b1.write(str(p))
         assert b1.ops[-1][0] == (plan.OP_STEMCONV if image else plan.OP_GEMM)
-        assert "unknown activation 4" in _engine_error(p)
+        assert "unknown activation 4" in fp.engine_error(p)
         b1.ops[-1][1][6 if image else 7] = plan.ACT_LEAKY
         b1.write(str(p))
-        assert "no CUDA device" in _engine_error(p)
-
-
-def toi_corrupt(raw: bytes, off: int, fmt: str, value) -> bytes:
-    b = bytearray(raw)
-    struct.pack_into(fmt, b, off, value)
-    return bytes(b)
+        assert "no CUDA device" in fp.engine_error(p)

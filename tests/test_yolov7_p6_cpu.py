@@ -9,7 +9,8 @@ import pytest
 import torch
 
 import adas_b200  # noqa: F401
-from adas_b200 import _capi, onnx_import, plan
+from adas_b200 import onnx_import, plan
+import plan_footprint as fp
 import test_onnx_import as toi
 import yolov7_p6_oracle as o6
 
@@ -115,14 +116,6 @@ def test_training_form_checkpoint_packs_its_main_path(tmp_path):
     assert plan.read_anchors(str(tmp_path / "w6.b200w")).shape == (4, 3, 2)
 
 
-def _engine_error(path):
-    try:
-        _capi.Engine(str(path))
-    except Exception as e:
-        return str(e)
-    return None
-
-
 def _write(pb, tmp_path, name):
     p = tmp_path / f"{name}.b200w"
     pb.write(str(p))
@@ -134,13 +127,13 @@ def test_four_level_plan_validation(tmp_path):
     W = plan.synth_weights("yolov7", 0)
     pb = plan.build_yolov7(W, "w6", in_h=256, in_w=256)
     ok = _write(pb, tmp_path, "w6")
-    assert "no CUDA device" in _engine_error(ok)
+    assert "no CUDA device" in fp.engine_error(ok)
     assert np.array_equal(plan.read_anchors(str(ok)), np.asarray(plan.YOLOV7_P6_ANCHORS, np.float32).reshape(4, 3, 2))
 
     def bad(name, edit, expect):
         b = plan.build_yolov7(plan.Weights(W.state_dict), "w6", in_h=256, in_w=256)
         edit(b)
-        err = _engine_error(_write(b, tmp_path, name))
+        err = fp.engine_error(_write(b, tmp_path, name))
         assert err is not None and expect in err, (name, err)
 
     bad("anchors18", lambda b: b.tensors.__setitem__(b.meta[3] - 1, np.ones(18, np.float32)), "anchor table")
@@ -153,17 +146,16 @@ def test_four_level_plan_validation(tmp_path):
     for name, b, expect in (("v8", plan.build_yolov8(plan.synth_weights("yolov8", 0), "n", in_h=256, in_w=256), "YOLOv8 head has 3 levels"),
                             ("v6", plan.build_yolov6(plan.synth_weights("yolov6", 0, variant="n"), "n", in_h=256, in_w=256), "YOLOv6 head has 3 levels"),
                             ("lite", plan.build_yolov5(plan.synth_weights("yolov5", 0), "n", in_h=256, in_w=256, lite=True), "4 without the lite flag")):
-        assert "no CUDA device" in _engine_error(_write(b, tmp_path, name + "_ok"))
+        assert "no CUDA device" in fp.engine_error(_write(b, tmp_path, name + "_ok"))
         b.outputs.append(b.outputs[-1][:3] + (64,))
-        err = _engine_error(_write(b, tmp_path, name))
+        err = fp.engine_error(_write(b, tmp_path, name))
         assert err is not None and expect in err, (name, err)
     # stem conv widths: 80 and 96 are supported, 40 is not
     for cout, expect in ((80, "no CUDA device"), (96, "no CUDA device"), (40, "bad stem conv")):
         b = plan.PlanBuilder(plan.MODEL_YOLOV5, 3, 64, 64)
         w = np.zeros((cout, 4, 6, 6), np.float32)
         b.stem_conv(b.image, w, np.zeros(cout, np.float32), 6, 2, 2, plan.ACT_SILU, b.new_padded(32, 32, (cout + 7) // 8 * 8))
-        assert expect in _engine_error(_write(b, tmp_path, f"stem{cout}"))
-
+        assert expect in fp.engine_error(_write(b, tmp_path, f"stem{cout}"))
 
 
 def _export_p6(tmp_path, scale, seed, anchors=None, size=256):

@@ -10,7 +10,8 @@ import torch
 import torch.nn.functional as F
 
 import adas_b200  # noqa: F401
-from adas_b200 import _capi, plan
+from adas_b200 import plan
+import plan_footprint as fp
 import yolov9_oracle as o9
 
 PUBLISHED = [("t", 2.002, 7.71), ("s", 7.106, 26.38), ("m", 19.979, 76.31), ("c", 25.289, 102.14)]
@@ -119,20 +120,6 @@ def test_yolov9m_aligned_layout_equals_the_oracle_weights():
     assert all(op[1][1] % 8 == 0 and op[1][12] % 8 == 0 for op in pb.ops if op[0] == plan.OP_GEMM)
 
 
-def _engine_error(path):
-    try:
-        _capi.Engine(str(path))
-    except Exception as e:
-        return str(e)
-    return None
-
-
-def _corrupt(raw: bytes, off: int, fmt: str, value) -> bytes:
-    b = bytearray(raw)
-    struct.pack_into(fmt, b, off, value)
-    return bytes(b)
-
-
 @pytest.mark.skipif(torch.cuda.is_available(), reason="load-time validation is observed through the missing-device error")
 def test_plan_validator_rejects_bad_avgpool2_ops(tmp_path):
     pb = plan.PlanBuilder(plan.MODEL_YOLOV8, 3, 16, 16)
@@ -143,25 +130,25 @@ def test_plan_validator_rejects_bad_avgpool2_ops(tmp_path):
     pb.avgpool2(pb.sub(xin, 8, 16), 1, out=pb.sub(out, 8, 16))
     good = tmp_path / "ap.b200w"
     pb.write(str(good))
-    assert "no CUDA device" in _engine_error(good)
+    assert "no CUDA device" in fp.engine_error(good)
     raw = good.read_bytes()
     op = struct.calcsize("<8sII3I4I16IQQ") + len(pb.buffers) * 24 + 4          # p[0] of the one op
     p = lambda i: op + 4 * i
     cases = [
-        ("input index", _corrupt(raw, p(0), "<i", 99), "index out of range"),
-        ("output index", _corrupt(raw, p(3), "<i", -1), "index out of range"),
-        ("fp32 output", _corrupt(raw, p(3), "<i", f32.buf), "fp16"),
-        ("geometry", _corrupt(raw, p(3), "<i", other.buf), "H x W"),
-        ("channels", _corrupt(raw, p(2), "<i", 12), "multiples of 8"),
-        ("input offset", _corrupt(raw, p(1), "<i", 4), "multiples of 8"),
-        ("output offset", _corrupt(raw, p(4), "<i", 12), "multiples of 8"),
-        ("input slice", _corrupt(raw, p(1), "<i", 56), "exceeds"),
-        ("output slice", _corrupt(raw, p(4), "<i", 24), "exceeds"),
-        ("in place", _corrupt(_corrupt(raw, p(3), "<i", xin.buf), p(4), "<i", 16), "overlaps"),
-        ("fill", _corrupt(raw, p(5), "<i", 2), "fill"),
+        ("input index", fp.corrupt(raw, p(0), "<i", 99), "index out of range"),
+        ("output index", fp.corrupt(raw, p(3), "<i", -1), "index out of range"),
+        ("fp32 output", fp.corrupt(raw, p(3), "<i", f32.buf), "fp16"),
+        ("geometry", fp.corrupt(raw, p(3), "<i", other.buf), "H x W"),
+        ("channels", fp.corrupt(raw, p(2), "<i", 12), "multiples of 8"),
+        ("input offset", fp.corrupt(raw, p(1), "<i", 4), "multiples of 8"),
+        ("output offset", fp.corrupt(raw, p(4), "<i", 12), "multiples of 8"),
+        ("input slice", fp.corrupt(raw, p(1), "<i", 56), "exceeds"),
+        ("output slice", fp.corrupt(raw, p(4), "<i", 24), "exceeds"),
+        ("in place", fp.corrupt(fp.corrupt(raw, p(3), "<i", xin.buf), p(4), "<i", 16), "overlaps"),
+        ("fill", fp.corrupt(raw, p(5), "<i", 2), "fill"),
     ]
     for name, data, msg in cases:
         bad = tmp_path / "bad.b200w"
         bad.write_bytes(data)
-        err = _engine_error(bad)
+        err = fp.engine_error(bad)
         assert err is not None and "plan" in err and msg in err, (name, err)

@@ -1,6 +1,6 @@
 """CPU: YOLOv9-E (GELAN-E) -- counts against the published figures, the oracle's fuse, the packer's folds, ONNX recognition and
 checkpoint conversion, the OP_CBFUSE validator, the float64 plan interpreter against the oracle, the plan's dataflow, and the teeth of
-the per-element CBFuse bound of plan_interp_cbfuse.
+the per-element CBFuse bound of plan_interp.
 
 The graph restates upstream's `models/detect/gelan-e.yaml` (v0.1); with no upstream file available, the published counts are its
 anchor: 57.3 M parameters and 189.0 GFLOP (YOLOv9-E, fused) and 58.1 M parameters (GELAN-E, training form)."""
@@ -11,8 +11,9 @@ import pytest
 import torch
 
 import adas_b200  # noqa: F401
-from adas_b200 import _capi, onnx_import, plan
-import plan_interp_cbfuse as pi
+from adas_b200 import onnx_import, plan
+import plan_footprint as fp
+import plan_interp as pi
 import post_conformance_cases as pc
 import synth
 import test_onnx_import as toi
@@ -163,18 +164,6 @@ def test_input_must_be_a_multiple_of_32():
 # ---------------------------------------------------------------------------------------------------------------------------
 # the OP_CBFUSE validator
 # ---------------------------------------------------------------------------------------------------------------------------
-def _engine_error(path):
-    try:
-        _capi.Engine(str(path))
-    except Exception as e:
-        return str(e)
-    return None
-
-
-def _corrupt(raw: bytes, off: int, value) -> bytes:
-    b = bytearray(raw)
-    struct.pack_into("<i", b, off, value)
-    return bytes(b)
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="load-time validation is observed through the missing-device error")
@@ -189,40 +178,40 @@ def test_plan_validator_rejects_bad_cbfuse_ops(tmp_path):
     pb.cbfuse(pb.sub(out, 8, 16), [(pb.sub(s0, 8, 16), 0), (pb.sub(s1, 0, 16), 1), (pb.sub(s2, 0, 16), 2)])
     good = tmp_path / "cbf.b200w"
     pb.write(str(good))
-    assert "no CUDA device" in _engine_error(good)
+    assert "no CUDA device" in fp.engine_error(good)
     raw = good.read_bytes()
     op = struct.calcsize("<8sII3I4I16IQQ") + len(pb.buffers) * 24 + 4          # p[0] of the one op
     p = lambda i: op + 4 * i
     cases = [
-        ("output index", _corrupt(raw, p(0), 99), "index out of range"),
-        ("base index", _corrupt(raw, p(3), -1), "index out of range"),
-        ("source index", _corrupt(raw, p(9), 99), "index out of range"),
-        ("fp32 source", _corrupt(raw, p(6), f32.buf), "fp16"),
-        ("fp32 output", _corrupt(_corrupt(raw, p(0), f32.buf), p(3), f32.buf), "fp16"),
-        ("no sources", _corrupt(raw, p(5), 0), "sources"),
-        ("six sources", _corrupt(raw, p(5), 6), "sources"),
-        ("shift 5", _corrupt(raw, p(11), 5), "shift"),
-        ("negative shift", _corrupt(raw, p(8), -1), "shift"),
-        ("shift + 1", _corrupt(raw, p(11), 2), "geometry"),
-        ("shift - 1", _corrupt(raw, p(14), 1), "geometry"),
-        ("base geometry", _corrupt(raw, p(3), other.buf), "output's H x W"),
-        ("channels", _corrupt(raw, p(2), 12), "multiples of 8"),
-        ("output offset", _corrupt(_corrupt(raw, p(1), 4), p(4), 4), "multiples of 8"),
-        ("source offset", _corrupt(raw, p(7), 4), "multiples of 8"),
-        ("output slice", _corrupt(_corrupt(raw, p(1), 40), p(4), 40), "exceeds"),
-        ("source slice", _corrupt(raw, p(7), 24), "exceeds"),
-        ("source is the output", _corrupt(_corrupt(raw, p(6), out.buf), p(7), 16), "overlaps"),
-        ("base overlaps the output", _corrupt(raw, p(4), 16), "overlaps"),
+        ("output index", fp.corrupt(raw, p(0), "<i", 99), "index out of range"),
+        ("base index", fp.corrupt(raw, p(3), "<i", -1), "index out of range"),
+        ("source index", fp.corrupt(raw, p(9), "<i", 99), "index out of range"),
+        ("fp32 source", fp.corrupt(raw, p(6), "<i", f32.buf), "fp16"),
+        ("fp32 output", fp.corrupt(fp.corrupt(raw, p(0), "<i", f32.buf), p(3), "<i", f32.buf), "fp16"),
+        ("no sources", fp.corrupt(raw, p(5), "<i", 0), "sources"),
+        ("six sources", fp.corrupt(raw, p(5), "<i", 6), "sources"),
+        ("shift 5", fp.corrupt(raw, p(11), "<i", 5), "shift"),
+        ("negative shift", fp.corrupt(raw, p(8), "<i", -1), "shift"),
+        ("shift + 1", fp.corrupt(raw, p(11), "<i", 2), "geometry"),
+        ("shift - 1", fp.corrupt(raw, p(14), "<i", 1), "geometry"),
+        ("base geometry", fp.corrupt(raw, p(3), "<i", other.buf), "output's H x W"),
+        ("channels", fp.corrupt(raw, p(2), "<i", 12), "multiples of 8"),
+        ("output offset", fp.corrupt(fp.corrupt(raw, p(1), "<i", 4), p(4), "<i", 4), "multiples of 8"),
+        ("source offset", fp.corrupt(raw, p(7), "<i", 4), "multiples of 8"),
+        ("output slice", fp.corrupt(fp.corrupt(raw, p(1), "<i", 40), p(4), "<i", 40), "exceeds"),
+        ("source slice", fp.corrupt(raw, p(7), "<i", 24), "exceeds"),
+        ("source is the output", fp.corrupt(fp.corrupt(raw, p(6), "<i", out.buf), p(7), "<i", 16), "overlaps"),
+        ("base overlaps the output", fp.corrupt(raw, p(4), "<i", 16), "overlaps"),
     ]
     for name, data, msg in cases:
         bad = tmp_path / "bad.b200w"
         bad.write_bytes(data)
-        err = _engine_error(bad)
+        err = fp.engine_error(bad)
         assert err is not None and "plan" in err and msg in err, (name, err)
     # out of place (base in another buffer) is valid
     ok = tmp_path / "ok.b200w"
-    ok.write_bytes(_corrupt(raw, p(3), s0.buf))
-    assert "no CUDA device" in _engine_error(ok)
+    ok.write_bytes(fp.corrupt(raw, p(3), "<i", s0.buf))
+    assert "no CUDA device" in fp.engine_error(ok)
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
@@ -323,16 +312,3 @@ def test_cbfuse_bound_accepts_fp32_and_rejects_faults():
     for name, kw in faults.items():
         assert _ratio(pb, bufs, _emulate(pb, bufs, **kw)) > 1.0, name
 
-
-def test_plan_interp_is_unchanged_outside_the_cbfuse_context():
-    """plan_interp_cbfuse extends plan_interp only inside extended(): afterwards OP_CBFUSE is unknown to it again, and the other ops'
-    regions are the same inside and outside."""
-    import plan_interp
-    pb, _ = _teeth_plan()
-    before = (plan_interp.op_regions, plan_interp.op_ref, dict(plan_interp.OP_NAMES))
-    assert pi.op_kind(pb, 0) == "cbfuse" and len(pi.op_regions(pb, 0)[1]) == 5
-    assert (plan_interp.op_regions, plan_interp.op_ref, dict(plan_interp.OP_NAMES)) == before
-    with pytest.raises(ValueError, match="unknown type"):
-        plan_interp.op_regions(pb, 0)
-    _, v9 = _weights(0)
-    assert all(pi.op_regions(v9, i) == plan_interp.op_regions(v9, i) for i in range(len(v9.ops)) if v9.ops[i][0] != plan.OP_CBFUSE)

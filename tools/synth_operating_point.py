@@ -3,7 +3,7 @@ Prints the probability / box error the device path will show, the candidates per
 of the threshold.  Test infrastructure (uses oracle/):  python tools/synth_operating_point.py yolov8 l 45,-9 40,-8.2
 (yolov9 t|s|m|c|e, yolov10 n|s|m|b|l|x: the scale's class bias; the head gains of plan.SYNTH_PROFILES[kind] are kept)
 (yolov6lite s|m|l: 320x320, gain = the class-logit gain, bias = the scale's class bias; the fp16 emulation is plan_interp's rounded run of
-the plan itself, tests/plan_interp_lite.py)
+the plan itself, tests/plan_interp.py)
 """
 import sys, os
 R = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, R); sys.path.insert(0, os.path.join(R, 'tests'))
@@ -20,14 +20,14 @@ x = torch.from_numpy(np.concatenate([post.yolo_prepare_input(synth.frame(s), siz
 for a in sys.argv[3:]:
     g,b = map(float,a.split(','))
     if kind=="yolov6lite":
-        import yolov6_lite_oracle, plan_interp_lite, test_yolov6_lite_cpu
+        import yolov6_lite_oracle, plan_interp, test_yolov6_lite_cpu
         from gpu_util import to_padded
         plan.SYNTH_PROFILES["yolov6lite"]={**plan.SYNTH_PROFILES["yolov6lite"], "gains":[(r"detect\.cls_preds\.\d\.weight", g)],
                                        "variants": {variant: {"fill": [(r"detect\.cls_preds\.\d\.bias", b)]}}}
         W = plan.synth_weights(kind, 0, variant=variant); pb = plan.build_yolov6_lite(W, variant)
         with torch.no_grad():
             ref = yolov6_lite_oracle.build(W.state_dict, variant)(x).numpy()
-        emu = np.stack([test_yolov6_lite_cpu._decode(pb, plan_interp_lite.interpret(pb, to_padded(x[i:i + 1].numpy(), 4), 1, round_to_plan=True))
+        emu = np.stack([test_yolov6_lite_cpu._decode(pb, plan_interp.interpret(pb, to_padded(x[i:i + 1].numpy(), 4), 1, round_to_plan=True))
                         for i in range(len(x))])
         ref = np.concatenate([ref[..., :4], ref[..., 5:]], -1)
         e=np.abs(ref[...,4:]-emu[...,4:]); mx=ref[...,4:].max(2); mg=emu[...,4:].max(2); eb=np.abs(ref[...,:4]-emu[...,:4]).max()

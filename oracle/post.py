@@ -311,14 +311,16 @@ def lapjv_extended(cost: np.ndarray, thresh: float):
     """lap.lapjv(cost, extend_cost=True, cost_limit=thresh) as used by matching.linear_assignment (matching.py:20-31).
     `lap` (requirements.txt:4, unpinned, not vendored) is absent; its documented behaviour is restated: pad to
     (T+D)x(T+D) with cost_limit/2 in the off blocks and 0 in the dummy block, solve exactly, drop dummy matches.
-    Exact for unique optima; tie-breaking of the real library is unpinned."""
+    Exact for unique optima; tie-breaking of the real library is unpinned.
+    A NaN cost (the IoU 0/0 of two zero-area boxes) never matches: `lap` documents nothing for NaN, so the pair is forbidden, as in
+    the device solver (csrc/track.cu), and the rest of the problem is solved as if it were absent."""
     from scipy.optimize import linear_sum_assignment
     cost = np.asarray(cost, float)
     nr, nc = cost.shape
     n = nr + nc
     ext = np.full((n, n), thresh / 2.0)
     ext[nr:, nc:] = 0
-    ext[:nr, :nc] = cost
+    ext[:nr, :nc] = np.where(np.isnan(cost), np.inf, cost)
     r, c = linear_sum_assignment(ext)
     x = np.full(n, -1)
     y = np.full(n, -1)

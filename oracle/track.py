@@ -89,13 +89,15 @@ def kf_update(mean, cov, z):
     return mean + np.dot(z - pm, k.T), cov - np.linalg.multi_dot((k, pc, k.T))
 
 
-def _assign(tracks, dets, thresh, fuse):
+def _assign(tracks, dets, thresh, fuse, solver=None):
+    """one association stage; `solver(cost, thresh) -> (x, y, ...)` is post.lapjv_extended unless given (a test may pass one that
+    follows another solver's tie-breaking)"""
     if not tracks or not dets:
         return [], list(range(len(tracks))), list(range(len(dets)))
     a = np.array([t.tlbr() for t in tracks])
     b = np.array([d.tlbr() for d in dets])
     cost = post.iou_cost(a, b, [d.score for d in dets] if fuse else None)
-    x, y, _ = post.lapjv_extended(cost, thresh)
+    x, y = (solver or post.lapjv_extended)(cost, thresh)[:2]
     return [(i, int(j)) for i, j in enumerate(x) if j >= 0], [i for i, j in enumerate(x) if j < 0], [j for j, i in enumerate(y) if i < 0]
 
 
@@ -116,9 +118,10 @@ def _sub(a, b):
 
 
 class Tracker:
-    def __init__(self, track_thresh=0.5, track_buffer=30, match_thresh=0.8, frame_rate=30):
+    def __init__(self, track_thresh=0.5, track_buffer=30, match_thresh=0.8, frame_rate=30, solver=None):
         self.tracked, self.lost, self.removed = [], [], []
         self.track_thresh, self.match_thresh = track_thresh, match_thresh
+        self.solver = solver
         self.det_thresh = track_thresh + 0.1
         self.max_lost = int(frame_rate / 30.0 * track_buffer)
         self.frame = 0
@@ -170,11 +173,11 @@ class Tracker:
             mm, cc = kf_multi_predict(mm, cc)
             for t, m, c in zip(pool, mm, cc):
                 t.mean, t.cov = m, c
-        m1, ut, ud = _assign(pool, dets, self.match_thresh, True)
+        m1, ut, ud = _assign(pool, dets, self.match_thresh, True, self.solver)
         for i, j in m1:
             self._hit(pool[i], dets[j], activated, refind)
         rem = [pool[i] for i in ut if pool[i].state == TRACKED]
-        m2, ut2, _ = _assign(rem, dets2, 0.5, False)
+        m2, ut2, _ = _assign(rem, dets2, 0.5, False, self.solver)
         for i, j in m2:
             self._hit(rem[i], dets2[j], activated, refind)
         for i in ut2:
@@ -182,7 +185,7 @@ class Tracker:
                 rem[i].state = LOST
                 lost.append(rem[i])
         dets = [dets[i] for i in ud]
-        m3, uu, ud3 = _assign(unconf, dets, 0.7, True)
+        m3, uu, ud3 = _assign(unconf, dets, 0.7, True, self.solver)
         for i, j in m3:
             self._hit(unconf[i], dets[j], activated, refind)
         for i in uu:

@@ -11,6 +11,13 @@
 // problem: T rows x (D real + T private dummy) columns, real cost c - thresh, own dummy cost 0.
 // One warp per problem; the column scan of each Dijkstra step is lane-parallel with a deterministic
 // (lowest column) argmin.
+// Ties (the real library's tie-breaking is unpinned): every entry point (lap, associate, the fused tracker stages) runs the same
+// lap_solve on the same float64 costs, so all of them return the same assignment.  Threshold rule: a pair whose cost equals
+// thresh exactly is matched when nothing else competes for it -- real columns precede the dummy ones, so the lowest-column argmin
+// prefers the match (a 1x1 problem at cost == thresh matches; one ulp above it does not).
+// NaN costs (IoU 0/0 of two zero-area boxes; the reference's behaviour is undefined): `cur < minv` is false for NaN, so the search
+// never relaxes a NaN edge and a NaN pair is never matched; the result is the optimum of the problem without those pairs.  Every
+// row still reaches its own finite dummy column, so the "no finite candidate" exit below is a guard, not a path.
 #include "common.h"
 
 namespace adas {

@@ -242,10 +242,21 @@ int adas_tracker_update(adas_tracker* t, int n, const double* boxes_xyxy, const 
  * of frame f (records beyond max_out are dropped from `out`, never from the tracker). */
 int adas_tracker_update_batch(adas_tracker* t, int n_frames, const int32_t* counts, const double* boxes_xyxy,
                               const double* scores, const int32_t* class_ids, int max_out, adas_track* out, int32_t* n_out);
+/* k trackers (one per camera of a rig; distinct, on one device) advanced n_frames frames each, with ONE association launch per frame
+ * for all of them (no reference counterpart).  counts[n_frames][k]; boxes / scores / class ids concatenated frame-major, then in
+ * tracker order; out holds n_frames * k * max_out records ([frame][tracker][max_out]), n_out[frame][tracker] the tracked-track
+ * counts.  Births take track ids (process-global) in tracker order within a frame, so the results equal driving the k trackers
+ * with adas_tracker_update interleaved: tracker 0 frame f, tracker 1 frame f, ..., then frame f + 1.  Refused, with every tracker
+ * unchanged: k < 1, a null or repeated tracker, trackers on different devices, a negative count.  The launch runs on trackers[0]'s
+ * stream and buffers. */
+int adas_tracker_update_multi(adas_tracker* const* trackers, int k, int n_frames, const int32_t* counts, const double* boxes_xyxy,
+                              const double* scores, const int32_t* class_ids, int max_out, adas_track* out, int32_t* n_out);
 int adas_tracker_get(adas_tracker* t, int which /* 0 tracked, 1 lost, 2 removed */, int max_out, adas_track* out, int* n_out);
 int adas_tracker_count(void);    /* BaseTrack._count */
-/* Wall-clock accounting of adas_tracker_update_batch since the tracker was created: out4 = {frames, total ms, ms spent between the
- * association launch and its result (the device round trip), association launches}.  Diagnostic; no reference counterpart. */
+/* Wall-clock accounting of adas_tracker_update_batch and adas_tracker_update_multi since the tracker was created: out4 = {frames,
+ * total ms of the calls that advanced it, ms spent between the association launches it took part in and their results (the device
+ * round trip), association launches it took part in (a launch for k trackers counts once for each)}.  Diagnostic; no reference
+ * counterpart. */
 int adas_tracker_stats(adas_tracker* t, double* out4);
 
 /* ---- test hooks (no reference counterpart): raw access to the plan's activation buffers so single kernels can be

@@ -1,1 +1,1 @@
-from .byteTrack.byteTracker import BYTETracker
+from .byteTrack.byteTracker import BYTETracker, update_trackers

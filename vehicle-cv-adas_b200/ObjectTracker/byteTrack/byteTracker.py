@@ -137,17 +137,22 @@ class BYTETracker(ObjectTrackBase):
     def update_batch_arrays(self, counts, xyxy, scores, class_ids):
         """update_batch on already concatenated arrays (the pipeline's hot path): counts [F] int, xyxy [sum, 4], scores [sum],
         class_ids [sum] integer labels.  Labels are mapped to the tracker's class slots in first-seen order like `update` does."""
+        return self._advanced(self._nt.update_batch(counts, xyxy, scores, self._class_slots(class_ids)))
+
+    def _class_slots(self, class_ids):
+        """class slots of a label array, registering unseen labels in order of first appearance"""
         cl = np.asarray(class_ids)
-        if cl.size:
-            uniq, first = np.unique(cl, return_index=True)
-            for u in uniq[np.argsort(first)].tolist():            # register unseen labels in order of first appearance
-                self._cid(u)
-            lut = np.array([self._labels[u] for u in uniq.tolist()], np.int32)
-            ids = lut[np.searchsorted(uniq, cl)]
-        else:
-            ids = np.zeros(0, np.int32)
-        recs = self._nt.update_batch(counts, xyxy, scores, ids)
-        self.frame_id += len(counts)
+        if not cl.size:
+            return np.zeros(0, np.int32)
+        uniq, first = np.unique(cl, return_index=True)
+        for u in uniq[np.argsort(first)].tolist():
+            self._cid(u)
+        lut = np.array([self._labels[u] for u in uniq.tolist()], np.int32)
+        return lut[np.searchsorted(uniq, cl)]
+
+    def _advanced(self, recs):
+        """bookkeeping after the native tracker advanced len(recs) frames"""
+        self.frame_id += len(recs)
         if recs:
             self.tracked_stracks = [self._view(r, None) for r in recs[-1]]
         return recs
@@ -185,3 +190,24 @@ class BYTETracker(ObjectTrackBase):
                 if show_traject:
                     self.plot_trajectories(frame, t.trajectories, t.class_id, t.track_id)
                     self.plot_directions(frame, t.xyah, t.filter_trajectories(frame, (10, 10)), t.class_id)
+
+
+def update_trackers(trackers, counts, xyxy, scores, class_ids):
+    """Advance K BYTETrackers (one per camera) over F frames in ONE library call, with one association launch per frame for all
+    cameras.  counts [F, K]; xyxy [sum, 4], scores [sum] and class_ids [sum] concatenated frame-major, then in camera order.  Each
+    tracker maps labels to its own class slots as update_batch_arrays does.  Returns, per camera, the list (per frame) of
+    TRACK_DTYPE record arrays: exactly what the K trackers' update_batch_arrays would return when driven one frame at a time in
+    camera order.  Each tracker's tracked_stracks afterwards reflects its last frame."""
+    from ... import _capi
+    K = len(trackers)
+    cnt = np.asarray(counts, np.int32).reshape(-1, K)
+    cl = np.asarray(class_ids)
+    cam = np.repeat(np.tile(np.arange(K), cnt.shape[0]), cnt.ravel())         # camera of each detection
+    ids = np.zeros(len(cl), np.int32)
+    for k, t in enumerate(trackers):
+        sel = cam == k
+        ids[sel] = t._class_slots(cl[sel])
+    recs = _capi.NativeTracker.update_multi([t._nt for t in trackers], cnt, xyxy, scores, ids)
+    for t, r in zip(trackers, recs):
+        t._advanced(r)
+    return recs

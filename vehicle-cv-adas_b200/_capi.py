@@ -25,7 +25,7 @@ SYMBOLS = [
     "adas_engine_stream", "adas_engine_num_buffers", "adas_engine_buffer_info", "adas_engine_write_buffer", "adas_engine_read_buffer",
     "adas_engine_run", "adas_plan_validate", "adas_engine_event_record", "adas_event_elapsed_ms", "adas_engine_time_ops", "adas_engine_num_steps", "adas_engine_time_step", "adas_detect_pair",
     "adas_comm_unique_id", "adas_comm_create", "adas_comm_destroy", "adas_comm_all_gather", "adas_comm_sync", "adas_comm_read", "adas_comm_info",
-    "adas_tracker_create", "adas_tracker_destroy", "adas_tracker_reset", "adas_tracker_update", "adas_tracker_update_batch", "adas_tracker_get", "adas_tracker_count", "adas_tracker_stats",
+    "adas_tracker_create", "adas_tracker_destroy", "adas_tracker_reset", "adas_tracker_update", "adas_tracker_update_batch", "adas_tracker_update_multi", "adas_tracker_get", "adas_tracker_count", "adas_tracker_stats",
 ]
 
 
@@ -151,6 +151,31 @@ class NativeTracker:
     @staticmethod
     def count() -> int:
         return int(lib().adas_tracker_count())
+
+    @staticmethod
+    def update_multi(trackers, counts, boxes_xyxy, scores, class_ids):
+        """Advance K trackers (one per camera) over F frames in one library call, with one association launch per frame for all of
+        them.  counts [F, K]; detections concatenated frame-major, then in tracker order.  Returns, per tracker, the list (per frame)
+        of TRACK_DTYPE record arrays -- exactly what K separate trackers updated one after another, frame by frame, return."""
+        ks = len(trackers)
+        if ks < 1:
+            raise Exception("adas_tracker_update_multi: no trackers")
+        cnt = as_c(np.asarray(counts, np.int32).reshape(-1, ks), np.int32)
+        nf = int(cnt.shape[0])
+        b = as_c(np.asarray(boxes_xyxy, np.float64).reshape(-1, 4), np.float64)
+        s = as_c(scores, np.float64)
+        c = as_c(class_ids, np.int32)
+        if not (b.shape[0] == s.shape[0] == c.shape[0] == int(cnt.sum())):
+            raise Exception(f"adas_tracker_update_multi: {int(cnt.sum())} detections counted, {b.shape[0]} boxes, {s.shape[0]} scores, "
+                            f"{c.shape[0]} class ids")
+        # rows per (frame, tracker): the tracks after frame f are at most those tracked before the call plus the detections of 0..f
+        max_out = max(1, max(t._count(0) + int(cnt[:, k].sum()) for k, t in enumerate(trackers)))
+        out = np.zeros((nf, ks, max_out), TRACK_DTYPE)
+        n_out = np.zeros((nf, ks), np.int32)
+        hs = (C.c_void_p * ks)(*[t._h.value for t in trackers])
+        check(lib().adas_tracker_update_multi(hs, ks, nf, _p(cnt, C.c_int32), _p(b, C.c_double), _p(s, C.c_double), _p(c, C.c_int32),
+                                              int(max_out), out.ctypes.data_as(C.c_void_p), _p(n_out, C.c_int32)))
+        return [[out[f, k, :int(n_out[f, k])] for f in range(nf)] for k in range(ks)]
 
 
 class Engine:

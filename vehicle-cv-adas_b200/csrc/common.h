@@ -204,4 +204,31 @@ int launch_ufld_post(const float* heads, int ld, int B, UfldDims d, int img_w, i
                      const double* col_anchor, int32_t* pts, int32_t* npts, uint8_t* status, double* coords,
                      int max_pts, cudaStream_t st);
 
+// ---- fused ByteTrack association (track.cu), driven by the native tracker (tracker.cu) ------------------------------------------
+// One problem (one camera's frame) of an assoc3 launch: where its slices start in the launch's buffers, in elements of each buffer.
+struct Assoc3Problem {
+    int64_t in_off, n_in;        // doubles of the input (mapped host buffer and its device copy)
+    int64_t out_off, n_out;      // int32 of the output (device buffer and mapped host buffer)
+    int64_t cost_off;            // doubles of the cost scratch
+    int64_t lists_off;           // int32 of the list scratch
+    int64_t ws_off, ws;          // column scratch: v / minv / u hold ws entries from ws_off, work_i 3 x ws from 3 x ws_off
+};
+static_assert(sizeof(Assoc3Problem) == 64, "one coalesced 64-byte read per problem");
+// The buffers of one launch.  `probs`, `in_host`, `out_host` and `done_host` are mapped pinned host memory (device-side addresses);
+// the rest is device memory.  `finished` counts the problems done so far and is 0 between launches.
+struct Assoc3Buffers {
+    const Assoc3Problem* probs;
+    const double* in_host;
+    int32_t* out_host;
+    int32_t* done_host;
+    double* in;
+    int32_t* out;
+    double* cost;
+    int32_t* lists;
+    double *v, *minv, *u;
+    int32_t* wi;
+    unsigned int* finished;
+};
+int launch_assoc3(int problems, const Assoc3Buffers& b, int32_t seq, cudaStream_t st);
+
 }  // namespace adas

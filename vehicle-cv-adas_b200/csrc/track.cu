@@ -164,11 +164,12 @@ __global__ void lap_kernel(const double* __restrict__ cost, const int64_t* __res
 // out (int32):   m1[P] det index or -1 | m2[P] det2 index or -1 (only for stage-2 rows) | m3[U] ORIGINAL det index or -1 |
 //                free3[D] 1 = high-score detection unmatched after stages 1 and 3 (a birth candidate)
 // Host round trip: `in_host` / `out_host` / `done_host` are MAPPED pinned host buffers.  The warp pulls the inputs over the link with
-// coalesced loads into device scratch, solves, pushes the results back and then publishes `seq` in *done_host behind a system-scope
-// fence -- the host spins on that word (tracker.cu) instead of paying two copy-engine transfers and a stream synchronisation per frame.
+// coalesced loads into device scratch, solves, pushes the results back and then (the last problem of the launch to finish) publishes
+// `seq` in *done_host behind a system-scope fence -- the host spins on that word (tracker.cu) instead of paying two copy-engine
+// transfers and a stream synchronisation per frame.
 // Row potentials live in shared memory only up to ASSOC_SMEM_ROWS rows (1 KB): next to a conv CTA that holds ~224 KB of an SM's shared
 // memory this block still fits, so it starts at once instead of waiting for a conv CTA to retire; larger problems use global scratch.
-// The column scratch (v, minv: ws doubles; p / way / used: 3 x ws int32) is sized by the host for the largest stage of the frame
+// The column scratch (v, minv: ws doubles; p / way / used: 3 x ws int32) is sized by the host for the largest stage of the problem
 // (ws > max(P + D, P + D2, U + D)), so the fused association has no size limit of its own -- like the reference.
 static constexpr int ASSOC_SMEM_ROWS = 120;
 
@@ -239,26 +240,38 @@ __device__ void assoc3_body(const double* __restrict__ in, int32_t* __restrict__
     }
 }
 
-__global__ void assoc3_kernel(const double* __restrict__ in_host, int n_in, double* __restrict__ in_dev, int32_t* __restrict__ out_host, int n_out,
-                              int32_t* __restrict__ out_dev, volatile int32_t* done_host, int32_t seq, double* __restrict__ cost,
-                              double* __restrict__ work_v, double* __restrict__ work_minv, int32_t* __restrict__ work_i, int ws,
-                              int32_t* __restrict__ lists, double* __restrict__ work_u) {
+// One block (one warp) per problem: the cameras of a multi-camera rig are independent trackers, so a time step solves all of them in
+// one launch.  Each problem has its own slices of every buffer (Assoc3Problem) and picks the shared-memory route on its own sizes, so
+// one crowded camera does not move the others to global memory.  The completion word is per launch: every block pushes its result,
+// fences and counts itself done; the last one publishes `seq`.
+__global__ void assoc3_kernel(Assoc3Buffers b, int problems, int32_t seq) {
     __shared__ double u_s[ASSOC_SMEM_ROWS + 1];
     const int lane = threadIdx.x;
-    for (int i = lane; i < n_in; i += 32) in_dev[i] = in_host[i];
+    const int64_t d = lane < 8 ? reinterpret_cast<const int64_t*>(b.probs + blockIdx.x)[lane] : 0;   // the descriptor: one 64-byte read
+    const int64_t in_off = __shfl_sync(0xffffffffu, d, 0), n_in = __shfl_sync(0xffffffffu, d, 1);
+    const int64_t out_off = __shfl_sync(0xffffffffu, d, 2), n_out = __shfl_sync(0xffffffffu, d, 3);
+    const int64_t cost_off = __shfl_sync(0xffffffffu, d, 4), lists_off = __shfl_sync(0xffffffffu, d, 5);
+    const int64_t ws_off = __shfl_sync(0xffffffffu, d, 6), ws = __shfl_sync(0xffffffffu, d, 7);
+    double* in = b.in + in_off;
+    for (int64_t i = lane; i < n_in; i += 32) in[i] = b.in_host[in_off + i];
     __syncwarp();
-    const int P = (int)in_dev[0], U = (int)in_dev[1];
-    assoc3_body(in_dev, out_dev, cost, work_v, work_minv, work_i, ws, lists, (P <= ASSOC_SMEM_ROWS && U <= ASSOC_SMEM_ROWS) ? u_s : work_u);
+    const int P = (int)in[0], U = (int)in[1];
+    int32_t* out = b.out + out_off;
+    assoc3_body(in, out, b.cost + cost_off, b.v + ws_off, b.minv + ws_off, b.wi + 3 * ws_off, (int)ws, b.lists + lists_off,
+                (P <= ASSOC_SMEM_ROWS && U <= ASSOC_SMEM_ROWS) ? u_s : b.u + ws_off);
     __syncwarp();
-    for (int i = lane; i < n_out; i += 32) out_host[i] = out_dev[i];
+    for (int64_t i = lane; i < n_out; i += 32) b.out_host[out_off + i] = out[i];
     __threadfence_system();
     __syncwarp();
-    if (lane == 0) *done_host = seq;
+    if (lane == 0 && atomicAdd(b.finished, 1u) == (unsigned)problems - 1) {
+        *b.finished = 0;                               // ready for the next launch (stream-ordered after this one)
+        __threadfence_system();
+        *(volatile int32_t*)b.done_host = seq;
+    }
 }
 
-int launch_assoc3(const double* in_host, int n_in, double* in_dev, int32_t* out_host, int n_out, int32_t* out_dev, int32_t* done_host, int32_t seq,
-                  double* cost, double* work_v, double* work_minv, int32_t* work_i, int ws, int32_t* lists, double* work_u, cudaStream_t st) {
-    assoc3_kernel<<<1, 32, 0, st>>>(in_host, n_in, in_dev, out_host, n_out, out_dev, done_host, seq, cost, work_v, work_minv, work_i, ws, lists, work_u);
+int launch_assoc3(int problems, const Assoc3Buffers& b, int32_t seq, cudaStream_t st) {
+    assoc3_kernel<<<problems, 32, 0, st>>>(b, problems, seq);
     count_launch();
     ADAS_CUDA(cudaGetLastError());
     return 0;

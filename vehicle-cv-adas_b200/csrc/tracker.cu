@@ -5,7 +5,10 @@
 // (constant-velocity filter, float64) and utils.py:9-69 (joint / sub / duplicate removal).  The IoU cost matrices and
 // the exact assignment of all three stages of a frame run on the device in ONE launch (track.cu assoc3_kernel: one upload, one
 // launch, one download, one synchronisation per frame); the 8x8 float64 Kalman algebra and the list bookkeeping are sequential
-// per stream and stay on the host.  adas_tracker_update_batch takes all frames of a pipeline step in one call.
+// per stream and stay on the host.  adas_tracker_update_batch takes all frames of a pipeline step in one call;
+// adas_tracker_update_multi advances several trackers (one per camera) a frame at a time with ONE association launch per frame for
+// all of them: each frame is split into prepare (detections, Kalman predict, packing the launch's input), the launch, and apply
+// (matches, births, ageing, list maintenance) in tracker order.
 #include "common.h"
 #include "../../include/adas_b200.h"
 #include <math.h>
@@ -17,14 +20,6 @@
 
 namespace adas {
 static inline uint64_t now_ns() { timespec ts; clock_gettime(CLOCK_MONOTONIC, &ts); return (uint64_t)ts.tv_sec * 1000000000ull + (uint64_t)ts.tv_nsec; }
-int launch_iou_cost(int problems, const double* a, const int32_t* a_off, const double* b, const int32_t* b_off,
-                    const double* det_scores, int fuse, double* cost, const int64_t* cost_off, cudaStream_t st);
-int launch_lap(int problems, const double* cost, const int64_t* cost_off, const int32_t* T, const int32_t* D,
-               const double* thresh, int32_t* x, const int32_t* x_off, int32_t* y, const int32_t* y_off, double* work_v,
-               double* work_minv, int32_t* work_i, cudaStream_t st);
-int lap_max_cols();
-int launch_assoc3(const double* in_host, int n_in, double* in_dev, int32_t* out_host, int n_out, int32_t* out_dev, int32_t* done_host, int32_t seq,
-                  double* cost, double* work_v, double* work_minv, int32_t* work_i, int ws, int32_t* lists, double* work_u, cudaStream_t st);
 
 enum { ST_NEW = 0, ST_TRACKED = 1, ST_LOST = 2, ST_REMOVED = 3 };
 static std::atomic<int> g_track_count{0};          // BaseTrack._count: process-global (base_track.py:12,33-36)
@@ -128,49 +123,74 @@ struct adas_tracker {
     double track_thresh = 0.5, match_thresh = 0.8, det_thresh = 0.6;
     int max_time_lost = 30, frame_id = 0;
     std::vector<TrackP> tracked, lost, removed;
-    // device scratch (persistent) for the association stages
+    // the frame between prepare and apply: its detections by score, the association's rows, and this tracker's problem in the launch
+    std::vector<TrackP> dets, dets2, unconfirmed, pool;
+    bool need_dev = false;
+    Assoc3Problem prob{};
+    // fused three-stage association of the calls this tracker leads (alone, or first of adas_tracker_update_multi): one launch and
+    // one synchronisation per frame for every tracker of the call.  Grown on demand, kept for reuse.
     cudaStream_t st = nullptr;
-    size_t cap_boxes = 0, cap_cost = 0;
-    double *d_a = nullptr, *d_b = nullptr, *d_s = nullptr, *d_c = nullptr, *d_th = nullptr, *d_v = nullptr, *d_mv = nullptr;
-    int32_t *d_meta = nullptr, *d_x = nullptr, *d_y = nullptr, *d_wi = nullptr;
-    int64_t* d_co = nullptr;
-    std::vector<double> ha, hb, hs;
-    std::vector<int32_t> hx, hy;
-    // fused three-stage association (one launch + one synchronisation per frame)
-    double* h3_in = nullptr; int32_t* h3_out = nullptr;      // pinned + mapped: the association kernel reads / writes them over the link
-    double* h3_in_dev = nullptr; int32_t* h3_out_dev = nullptr;   // their device-side addresses
-    int32_t* h_done = nullptr; int32_t* h_done_dev = nullptr; int32_t seq = 0;   // completion word the host spins on
-    double* d_u = nullptr;                                    // row potentials of problems beyond the kernel's shared-memory budget
-    size_t cap_ws = 0;                                        // entries of d_v / d_mv / d_u and of each third of d_wi (column scratch)
+    Assoc3Problem* h_probs = nullptr; double* h_in = nullptr; int32_t* h_out = nullptr;   // pinned + mapped: the kernel reads / writes
+    int32_t* h_done = nullptr; int32_t seq = 0;                                            // them over the link; h_done: completion word
+    Assoc3Buffers dev{};                                      // device-side addresses of the above, device copies and scratch
+    size_t cap_probs = 0, cap_in = 0, cap_out = 0, cap_cost = 0, cap_lists = 0, cap_ws = 0;
     // wall-clock accounting of the update path (adas_tracker_stats): frames, total ns, ns between launch and result, launches
     uint64_t st_frames = 0, st_total_ns = 0, st_wait_ns = 0, st_launches = 0;
-    double* d3_in = nullptr; int32_t* d3_out = nullptr; double* d3_cost = nullptr; int32_t* d3_lists = nullptr;
-    size_t cap3_in = 0, cap3_out = 0, cap3_cost = 0, cap3_lists = 0;
 };
 
 namespace adas {
 
-static int ensure_scratch(adas_tracker* t, size_t nb, size_t nc) {
+// mapped pinned host buffer (and, with `dev_copy`, a device buffer of the same size) of at least `need` elements
+template <typename T>
+static int grow_mapped(T** host, const T** host_dev, T** dev_copy, size_t* cap, size_t need, size_t min_cap) {
+    if (need <= *cap) return 0;
+    if (*host) cudaFreeHost(*host);
+    if (dev_copy) cudaFree(*dev_copy);
+    *host = nullptr; *cap = 0;
+    const size_t c = std::max(min_cap, need * 2);
+    ADAS_CUDA(cudaHostAlloc((void**)host, c * sizeof(T), cudaHostAllocMapped));
+    ADAS_CUDA(cudaHostGetDevicePointer((void**)host_dev, *host, 0));
+    if (dev_copy) ADAS_CUDA(cudaMalloc((void**)dev_copy, c * sizeof(T)));
+    *cap = c;
+    return 0;
+}
+
+// launch buffers of `problems` problems with the given total sizes; called before any tracker state is touched
+static int assoc3_reserve(adas_tracker* t, size_t problems, size_t n_in, size_t n_out, size_t n_cost, size_t n_lists, size_t n_ws) {
+    Assoc3Buffers& b = t->dev;
     if (t->st == nullptr) {
-        // the association kernels are tiny and on the host's critical path: highest priority, so they are scheduled as soon as any
+        // the association kernel is tiny and on the host's critical path: highest priority, so it is scheduled as soon as any
         // CTA slot frees up between the detectors' persistent conv kernels
         int prio_lo = 0, prio_hi = 0;
         cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
         ADAS_CUDA(cudaStreamCreateWithPriority(&t->st, cudaStreamNonBlocking, prio_hi));
-        const size_t wc = (size_t)lap_max_cols() + 1;
-        ADAS_CUDA(cudaMalloc(&t->d_th, 8)); ADAS_CUDA(cudaMalloc(&t->d_v, wc * 8)); ADAS_CUDA(cudaMalloc(&t->d_mv, wc * 8));
-        ADAS_CUDA(cudaMalloc(&t->d_wi, wc * 12)); ADAS_CUDA(cudaMalloc(&t->d_meta, 32)); ADAS_CUDA(cudaMalloc(&t->d_co, 16));
-        ADAS_CUDA(cudaMalloc(&t->d_u, wc * 8));
-        t->cap_ws = wc;
         ADAS_CUDA(cudaHostAlloc(&t->h_done, 64, cudaHostAllocMapped));
         *t->h_done = 0;
-        ADAS_CUDA(cudaHostGetDevicePointer(&t->h_done_dev, t->h_done, 0));
+        ADAS_CUDA(cudaHostGetDevicePointer((void**)&b.done_host, t->h_done, 0));
+        ADAS_CUDA(cudaMalloc(&b.finished, sizeof(unsigned int)));
+        ADAS_CUDA(cudaMemsetAsync(b.finished, 0, sizeof(unsigned int), t->st));
     }
-    if (nb > t->cap_boxes || nc > t->cap_cost) {
-        cudaFree(t->d_a); cudaFree(t->d_b); cudaFree(t->d_s); cudaFree(t->d_c); cudaFree(t->d_x); cudaFree(t->d_y);
-        t->cap_boxes = std::max<size_t>(256, nb * 2); t->cap_cost = std::max<size_t>(65536, nc * 2);
-        ADAS_CUDA(cudaMalloc(&t->d_a, t->cap_boxes * 32)); ADAS_CUDA(cudaMalloc(&t->d_b, t->cap_boxes * 32)); ADAS_CUDA(cudaMalloc(&t->d_s, t->cap_boxes * 8));
-        ADAS_CUDA(cudaMalloc(&t->d_c, t->cap_cost * 8)); ADAS_CUDA(cudaMalloc(&t->d_x, t->cap_boxes * 4)); ADAS_CUDA(cudaMalloc(&t->d_y, t->cap_boxes * 4));
+    if (grow_mapped(&t->h_probs, &b.probs, (Assoc3Problem**)nullptr, &t->cap_probs, problems, 16)) return 1;
+    if (grow_mapped(&t->h_in, &b.in_host, &b.in, &t->cap_in, n_in, 4096)) return 1;
+    if (grow_mapped(&t->h_out, (const int32_t**)&b.out_host, &b.out, &t->cap_out, n_out, 4096)) return 1;
+    if (n_cost > t->cap_cost) {
+        cudaFree(b.cost); b.cost = nullptr; t->cap_cost = 0;
+        const size_t c = std::max<size_t>(65536, n_cost * 2);
+        ADAS_CUDA(cudaMalloc(&b.cost, c * 8));
+        t->cap_cost = c;
+    }
+    if (n_lists > t->cap_lists) {
+        cudaFree(b.lists); b.lists = nullptr; t->cap_lists = 0;
+        const size_t c = std::max<size_t>(4096, n_lists * 2);
+        ADAS_CUDA(cudaMalloc(&b.lists, c * 4));
+        t->cap_lists = c;
+    }
+    if (n_ws > t->cap_ws) {
+        cudaFree(b.v); cudaFree(b.minv); cudaFree(b.u); cudaFree(b.wi);
+        b.v = b.minv = b.u = nullptr; b.wi = nullptr; t->cap_ws = 0;
+        const size_t wc = std::max<size_t>(4096, n_ws * 2);
+        ADAS_CUDA(cudaMalloc(&b.v, wc * 8)); ADAS_CUDA(cudaMalloc(&b.minv, wc * 8)); ADAS_CUDA(cudaMalloc(&b.u, wc * 8)); ADAS_CUDA(cudaMalloc(&b.wi, wc * 12));
+        t->cap_ws = wc;
     }
     return 0;
 }
@@ -223,131 +243,21 @@ static void fill_out(const Track& s, adas_track* o) {
 }  // namespace adas
 
 namespace adas {
-// scratch of the fused association, sized for this frame (called before any tracker state is touched)
-static int assoc3_prepare(adas_tracker* t, int P, int U, int D, int D2) {
-    if (ensure_scratch(t, 1, 1)) return 1;
-    // column scratch of the largest stage: stage 1 is P x (D + P), stage 2 R x (D2 + R) with R <= P, stage 3 U x (D + U)
-    const size_t ws = (size_t)std::max({P + D, P + D2, U + D}) + 1;
-    if (ws > t->cap_ws) {
-        cudaFree(t->d_v); cudaFree(t->d_mv); cudaFree(t->d_wi); cudaFree(t->d_u);
-        t->d_v = t->d_mv = t->d_u = nullptr; t->d_wi = nullptr; t->cap_ws = 0;
-        const size_t wc = ws * 2;
-        ADAS_CUDA(cudaMalloc(&t->d_v, wc * 8)); ADAS_CUDA(cudaMalloc(&t->d_mv, wc * 8));
-        ADAS_CUDA(cudaMalloc(&t->d_wi, wc * 12)); ADAS_CUDA(cudaMalloc(&t->d_u, wc * 8));
-        t->cap_ws = wc;
-    }
+// sizes of one problem of the fused association; the column scratch covers the largest stage: stage 1 is P x (D + P), stage 2
+// R x (D2 + R) with R <= P, stage 3 U x (D + U)
+static void assoc3_sizes(Assoc3Problem* p, int P, int U, int D, int D2, size_t* n_cost, size_t* n_lists) {
     const size_t mr = (size_t)std::max(P, U), mc = (size_t)std::max(D, D2);
-    const size_t n_in = 5 + (size_t)P * 5 + (size_t)U * 4 + (size_t)D * 5 + (size_t)D2 * 4, n_out = (size_t)2 * P + U + D + 4;
-    const size_t n_cost = mr * mc + (size_t)D * 5 + (size_t)P * 4 + 8, n_lists = (size_t)P + D + mr + mc + 8;
-    if (n_in > t->cap3_in) {
-        if (t->h3_in) cudaFreeHost(t->h3_in);
-        cudaFree(t->d3_in);
-        t->cap3_in = std::max<size_t>(4096, n_in * 2);
-        ADAS_CUDA(cudaHostAlloc(&t->h3_in, t->cap3_in * 8, cudaHostAllocMapped));
-        ADAS_CUDA(cudaHostGetDevicePointer(&t->h3_in_dev, t->h3_in, 0));
-        ADAS_CUDA(cudaMalloc(&t->d3_in, t->cap3_in * 8));
-    }
-    if (n_out > t->cap3_out) {
-        if (t->h3_out) cudaFreeHost(t->h3_out);
-        cudaFree(t->d3_out);
-        t->cap3_out = std::max<size_t>(4096, n_out * 2);
-        ADAS_CUDA(cudaHostAlloc(&t->h3_out, t->cap3_out * 4, cudaHostAllocMapped));
-        ADAS_CUDA(cudaHostGetDevicePointer(&t->h3_out_dev, t->h3_out, 0));
-        ADAS_CUDA(cudaMalloc(&t->d3_out, t->cap3_out * 4));
-    }
-    if (n_cost > t->cap3_cost) { cudaFree(t->d3_cost); t->cap3_cost = std::max<size_t>(65536, n_cost * 2); ADAS_CUDA(cudaMalloc(&t->d3_cost, t->cap3_cost * 8)); }
-    if (n_lists > t->cap3_lists) { cudaFree(t->d3_lists); t->cap3_lists = std::max<size_t>(4096, n_lists * 2); ADAS_CUDA(cudaMalloc(&t->d3_lists, t->cap3_lists * 4)); }
-    return 0;
+    p->n_in = 5 + (int64_t)P * 5 + (int64_t)U * 4 + (int64_t)D * 5 + (int64_t)D2 * 4;
+    p->n_out = (int64_t)2 * P + U + D;
+    p->ws = (int64_t)std::max({P + D, P + D2, U + D}) + 1;
+    *n_cost = mr * mc + (size_t)D * 5 + (size_t)P * 4 + 8;
+    *n_lists = (size_t)P + D + mr + mc + 8;
 }
 
-// the three association stages of one frame: one launch (track.cu assoc3_kernel) that reads and writes mapped host memory
-static int assoc3_run(adas_tracker* t, const std::vector<TrackP>& pool, const std::vector<TrackP>& unconf, const std::vector<TrackP>& dets,
-                      const std::vector<TrackP>& dets2, bool need_dev, std::vector<int32_t>* m1, std::vector<int32_t>* m2, std::vector<int32_t>* m3,
-                      std::vector<int32_t>* free3) {
-    const int P = (int)pool.size(), U = (int)unconf.size(), D = (int)dets.size(), D2 = (int)dets2.size();
-    m1->assign(P, -1); m2->assign(P, -2); m3->assign(U, -1); free3->assign(D, 1);
-    if (!need_dev) {
-        // nothing to match against (matching.py:21-22): every Tracked pool row goes through stage 2 unmatched, every detection stays free
-        for (int i = 0; i < P; ++i) if (pool[i]->state == ST_TRACKED) (*m2)[i] = -1;
-        return 0;
-    }
-    double* h = t->h3_in;
-    h[0] = P; h[1] = U; h[2] = D; h[3] = D2; h[4] = t->match_thresh;
-    double* q = h + 5;
-    for (int i = 0; i < P; ++i, q += 4) pool[i]->tlbr(q);
-    for (int i = 0; i < P; ++i) *q++ = pool[i]->state == ST_TRACKED ? 1.0 : 0.0;
-    for (int i = 0; i < U; ++i, q += 4) unconf[i]->tlbr(q);
-    for (int j = 0; j < D; ++j, q += 4) dets[j]->tlbr(q);
-    for (int j = 0; j < D; ++j) *q++ = dets[j]->score;
-    for (int j = 0; j < D2; ++j, q += 4) dets2[j]->tlbr(q);
-    const size_t n_in = (size_t)(q - h), n_out = (size_t)2 * P + U + D;
-    // one launch, no copies, no stream synchronisation: the kernel pulls `h` and pushes the result through mapped host memory and
-    // publishes this frame's sequence number last; the host spins on it (and asks the stream now and then, so that a failed launch
-    // or a device fault ends the wait with an error instead of a hang)
-    const int32_t seq = ++t->seq;
-    const uint64_t w0 = now_ns();
-    if (launch_assoc3(t->h3_in_dev, (int)n_in, t->d3_in, t->h3_out_dev, (int)n_out, t->d3_out, t->h_done_dev, seq, t->d3_cost, t->d_v, t->d_mv, t->d_wi,
-                      (int)t->cap_ws, t->d3_lists, t->d_u, t->st)) return 1;
-    {
-        volatile int32_t* done = t->h_done;
-        uint32_t spins = 0;
-        while (*done != seq) {
-            if ((++spins & 0xfffu) == 0) {
-                const cudaError_t q = cudaStreamQuery(t->st);
-                if (q == cudaSuccess) { ADAS_CHECK(*done == seq, "association kernel finished without publishing its result"); break; }
-                ADAS_CHECK(q == cudaErrorNotReady, "association kernel failed: %s", cudaGetErrorString(q));
-            }
-#if defined(__x86_64__) || defined(__i386__)
-            __builtin_ia32_pause();
-#endif
-        }
-        std::atomic_thread_fence(std::memory_order_acquire);
-    }
-    t->st_wait_ns += now_ns() - w0; t->st_launches += 1;
-    const int32_t* o = t->h3_out;
-    for (int i = 0; i < P; ++i) (*m1)[i] = o[i];
-    for (int i = 0; i < P; ++i) (*m2)[i] = o[P + i];
-    for (int k = 0; k < U; ++k) (*m3)[k] = o[2 * P + k];
-    for (int j = 0; j < D; ++j) (*free3)[j] = o[2 * P + U + j];
-    return 0;
-}
-}  // namespace adas
-
-extern "C" {
-
-int adas_tracker_create(int device, double track_thresh, int track_buffer, double match_thresh, int frame_rate, adas_tracker** out) {
-    ADAS_CHECK(out != nullptr, "adas_tracker_create: null argument");
-    adas_tracker* t = new adas_tracker();
-    t->device = device; t->track_thresh = track_thresh; t->match_thresh = match_thresh; t->det_thresh = track_thresh + 0.1;
-    t->max_time_lost = (int)((double)frame_rate / 30.0 * track_buffer);
-    *out = t;
-    return 0;
-}
-
-int adas_tracker_destroy(adas_tracker* t) {
-    if (!t) return 0;
-    cudaSetDevice(t->device);
-    cudaFree(t->d_a); cudaFree(t->d_b); cudaFree(t->d_s); cudaFree(t->d_c); cudaFree(t->d_x); cudaFree(t->d_y); cudaFree(t->d_th); cudaFree(t->d_v);
-    cudaFree(t->d_mv); cudaFree(t->d_wi); cudaFree(t->d_meta); cudaFree(t->d_co);
-    if (t->h3_in) cudaFreeHost(t->h3_in);
-    if (t->h3_out) cudaFreeHost(t->h3_out);
-    if (t->h_done) cudaFreeHost(t->h_done);
-    cudaFree(t->d_u);
-    cudaFree(t->d3_in); cudaFree(t->d3_out); cudaFree(t->d3_cost); cudaFree(t->d3_lists);
-    if (t->st) cudaStreamDestroy(t->st);
-    delete t;
-    return 0;
-}
-
-int adas_tracker_reset(adas_tracker* t) {          // BYTETracker.reset, byteTracker.py:187-200 (also BaseTrack.reset_counter)
-    t->frame_id = 0; t->tracked.clear(); t->lost.clear(); t->removed.clear();
-    g_track_count.store(0);
-    return 0;
-}
-
-static int update_one(adas_tracker* t, int n, const double* boxes_xyxy, const double* scores, const int32_t* class_ids, int max_out,
-                      adas_track* out, int* n_out) {
-    std::vector<TrackP> activated, refind, lost_now, removed_now, dets, dets2;
+// first half of a frame, without touching the tracker's state: the detections by score, the association's rows and whether the
+// frame needs the device (matching.py:21-22: no association when either side is empty)
+static void frame_classify(adas_tracker* t, int n, const double* boxes_xyxy, const double* scores, const int32_t* class_ids) {
+    t->dets.clear(); t->dets2.clear(); t->unconfirmed.clear(); t->pool.clear();
     for (int i = 0; i < n; ++i) {
         const double s = scores[i];
         const bool hi = s > t->track_thresh, lo = (s > 0.1) && (s < t->track_thresh);
@@ -356,20 +266,51 @@ static int update_one(adas_tracker* t, int n, const double* boxes_xyxy, const do
         d->tlwh0[0] = boxes_xyxy[i * 4]; d->tlwh0[1] = boxes_xyxy[i * 4 + 1];
         d->tlwh0[2] = boxes_xyxy[i * 4 + 2] - boxes_xyxy[i * 4]; d->tlwh0[3] = boxes_xyxy[i * 4 + 3] - boxes_xyxy[i * 4 + 1];
         d->score = s; d->cls = class_ids[i]; d->votes.push_back({class_ids[i], 1});
-        (hi ? dets : dets2).push_back(d);
+        (hi ? t->dets : t->dets2).push_back(d);
     }
-    std::vector<TrackP> unconfirmed, confirmed;
-    for (auto& x : t->tracked) (x->activated ? confirmed : unconfirmed).push_back(x);
-    std::vector<TrackP> pool = joint(confirmed, t->lost);
-    // the association has no size limit (its scratch grows with the frame, like the reference's); scratch is allocated BEFORE any
-    // state is touched, so a failed frame leaves the tracker exactly as it was
-    const int P = (int)pool.size(), U = (int)unconfirmed.size(), D = (int)dets.size(), D2 = (int)dets2.size();
-    std::vector<int32_t> m1, m2, m3, free3;
-    const bool need_dev = (P > 0 || U > 0) && (D > 0 || D2 > 0);
-    if (need_dev && assoc3_prepare(t, P, U, D, D2)) return 1;
+    std::vector<TrackP> confirmed;
+    for (auto& x : t->tracked) (x->activated ? confirmed : t->unconfirmed).push_back(x);
+    t->pool = joint(confirmed, t->lost);
+    t->need_dev = (!t->pool.empty() || !t->unconfirmed.empty()) && (!t->dets.empty() || !t->dets2.empty());
+}
+
+// prepare: the frame starts, the pool is predicted and, when the frame needs the device, its problem is packed at prob.in_off
+static void frame_prepare(adas_tracker* t, double* in) {
     t->frame_id += 1;
-    for (auto& x : pool) kf_predict(*x);
-    if (assoc3_run(t, pool, unconfirmed, dets, dets2, need_dev, &m1, &m2, &m3, &free3)) { t->frame_id -= 1; return 1; }
+    for (auto& x : t->pool) kf_predict(*x);
+    if (!t->need_dev) return;
+    const int P = (int)t->pool.size(), U = (int)t->unconfirmed.size(), D = (int)t->dets.size(), D2 = (int)t->dets2.size();
+    double* h = in + t->prob.in_off;
+    h[0] = P; h[1] = U; h[2] = D; h[3] = D2; h[4] = t->match_thresh;
+    double* q = h + 5;
+    for (int i = 0; i < P; ++i, q += 4) t->pool[i]->tlbr(q);
+    for (int i = 0; i < P; ++i) *q++ = t->pool[i]->state == ST_TRACKED ? 1.0 : 0.0;
+    for (int i = 0; i < U; ++i, q += 4) t->unconfirmed[i]->tlbr(q);
+    for (int j = 0; j < D; ++j, q += 4) t->dets[j]->tlbr(q);
+    for (int j = 0; j < D; ++j) *q++ = t->dets[j]->score;
+    for (int j = 0; j < D2; ++j, q += 4) t->dets2[j]->tlbr(q);
+}
+
+// apply: matches of the three stages (the kernel's output at prob.out_off), births, ageing and list maintenance
+// (byteTracker.py:100-185), then the tracked list into out[0, max_out)
+static void frame_apply(adas_tracker* t, const int32_t* out_all, int max_out, adas_track* out, int32_t* n_out) {
+    std::vector<TrackP>& pool = t->pool;
+    std::vector<TrackP>& unconfirmed = t->unconfirmed;
+    std::vector<TrackP>& dets = t->dets;
+    std::vector<TrackP>& dets2 = t->dets2;
+    const int P = (int)pool.size(), U = (int)unconfirmed.size(), D = (int)dets.size();
+    std::vector<int32_t> m1(P, -1), m2(P, -2), m3(U, -1), free3(D, 1);
+    if (t->need_dev) {
+        const int32_t* o = out_all + t->prob.out_off;
+        for (int i = 0; i < P; ++i) m1[i] = o[i];
+        for (int i = 0; i < P; ++i) m2[i] = o[P + i];
+        for (int k = 0; k < U; ++k) m3[k] = o[2 * P + k];
+        for (int j = 0; j < D; ++j) free3[j] = o[2 * P + U + j];
+    } else {
+        // nothing to match against (matching.py:21-22): every Tracked pool row goes through stage 2 unmatched, every detection stays free
+        for (int i = 0; i < P; ++i) if (pool[i]->state == ST_TRACKED) m2[i] = -1;
+    }
+    std::vector<TrackP> activated, refind, lost_now, removed_now;
     // stage 1: confirmed + lost vs high-score detections, fused cost
     for (int i = 0; i < P; ++i) if (m1[i] >= 0) hit(t, *pool[i], *dets[m1[i]], &activated, &refind, pool[i]);
     // stage 2: still-tracked leftovers vs low-score detections, plain IoU (m2 == -2: the row was not part of stage 2)
@@ -423,6 +364,110 @@ static int update_one(adas_tracker* t, int n, const double* boxes_xyxy, const do
     int k = 0;
     for (auto& x : t->tracked) { if (out && k < max_out) fill_out(*x, &out[k]); ++k; }
     if (n_out) *n_out = k;
+    t->dets.clear(); t->dets2.clear(); t->unconfirmed.clear(); t->pool.clear();
+}
+
+// one tracker's detections of one frame and where its records go
+struct CamFrame {
+    int n;
+    const double* boxes_xyxy;
+    const double* scores;
+    const int32_t* class_ids;
+    adas_track* out;
+    int32_t* n_out;
+};
+
+// spin on the launch's completion word (asking the stream now and then, so that a failed launch or a device fault ends the wait with an
+// error instead of a hang)
+static int assoc3_wait(adas_tracker* t, int32_t seq) {
+    volatile int32_t* done = t->h_done;
+    uint32_t spins = 0;
+    while (*done != seq) {
+        if ((++spins & 0xfffu) == 0) {
+            const cudaError_t q = cudaStreamQuery(t->st);
+            if (q == cudaSuccess) { ADAS_CHECK(*done == seq, "association kernel finished without publishing its result"); break; }
+            ADAS_CHECK(q == cudaErrorNotReady, "association kernel failed: %s", cudaGetErrorString(q));
+        }
+#if defined(__x86_64__) || defined(__i386__)
+        __builtin_ia32_pause();
+#endif
+    }
+    std::atomic_thread_fence(std::memory_order_acquire);
+    return 0;
+}
+
+// One frame of k distinct trackers on one device: prepare every tracker, ONE association launch (on ts[0]'s stream and buffers) for
+// all that need the device, one wait, then apply in tracker order -- births take track ids in that order, so the result is exactly
+// that of updating the trackers one after another.  The launch's buffers are sized before any tracker state is touched, so a frame
+// that fails there leaves every tracker exactly as it was.
+static int step_frame(adas_tracker* const* ts, int k, const CamFrame* cf, int max_out) {
+    adas_tracker* lead = ts[0];
+    int problems = 0;
+    size_t n_in = 0, n_out = 0, n_cost = 0, n_lists = 0, n_ws = 0;
+    for (int c = 0; c < k; ++c) {
+        adas_tracker* t = ts[c];
+        frame_classify(t, cf[c].n, cf[c].boxes_xyxy, cf[c].scores, cf[c].class_ids);
+        if (!t->need_dev) continue;
+        Assoc3Problem& p = t->prob;
+        size_t nc = 0, nl = 0;
+        assoc3_sizes(&p, (int)t->pool.size(), (int)t->unconfirmed.size(), (int)t->dets.size(), (int)t->dets2.size(), &nc, &nl);
+        p.in_off = (int64_t)n_in; p.out_off = (int64_t)n_out; p.cost_off = (int64_t)n_cost; p.lists_off = (int64_t)n_lists; p.ws_off = (int64_t)n_ws;
+        n_in += (size_t)p.n_in; n_out += (size_t)p.n_out; n_cost += nc; n_lists += nl; n_ws += (size_t)p.ws;
+        ++problems;
+    }
+    if (problems > 0 && assoc3_reserve(lead, (size_t)problems, n_in, n_out, n_cost, n_lists, n_ws)) return 1;
+    for (int c = 0, q = 0; c < k; ++c) {
+        frame_prepare(ts[c], lead->h_in);
+        if (ts[c]->need_dev) lead->h_probs[q++] = ts[c]->prob;
+    }
+    if (problems > 0) {
+        // one launch, no copies, no stream synchronisation: the kernel pulls the inputs and pushes the results through mapped host
+        // memory and publishes this frame's sequence number last
+        const int32_t seq = ++lead->seq;
+        const uint64_t w0 = now_ns();
+        if (launch_assoc3(problems, lead->dev, seq, lead->st) || assoc3_wait(lead, seq)) {
+            for (int c = 0; c < k; ++c) ts[c]->frame_id -= 1;
+            return 1;
+        }
+        const uint64_t w = now_ns() - w0;
+        for (int c = 0; c < k; ++c) if (ts[c]->need_dev) { ts[c]->st_wait_ns += w; ts[c]->st_launches += 1; }
+    }
+    for (int c = 0; c < k; ++c) frame_apply(ts[c], lead->h_out, max_out, cf[c].out, cf[c].n_out);
+    return 0;
+}
+}  // namespace adas
+
+extern "C" {
+
+int adas_tracker_create(int device, double track_thresh, int track_buffer, double match_thresh, int frame_rate, adas_tracker** out) {
+    ADAS_CHECK(out != nullptr, "adas_tracker_create: null argument");
+    adas_tracker* t = new adas_tracker();
+    t->device = device; t->track_thresh = track_thresh; t->match_thresh = match_thresh; t->det_thresh = track_thresh + 0.1;
+    t->max_time_lost = (int)((double)frame_rate / 30.0 * track_buffer);
+    *out = t;
+    return 0;
+}
+
+int adas_tracker_destroy(adas_tracker* t) {
+    if (!t) return 0;
+    if (t->st) {                                   // the stream is created first: a tracker without one holds no device resource
+        cudaSetDevice(t->device);
+        const Assoc3Buffers& b = t->dev;
+        cudaFree(b.in); cudaFree(b.out); cudaFree(b.cost); cudaFree(b.lists); cudaFree(b.v); cudaFree(b.minv); cudaFree(b.u); cudaFree(b.wi);
+        cudaFree(b.finished);
+        if (t->h_probs) cudaFreeHost(t->h_probs);
+        if (t->h_in) cudaFreeHost(t->h_in);
+        if (t->h_out) cudaFreeHost(t->h_out);
+        if (t->h_done) cudaFreeHost(t->h_done);
+        cudaStreamDestroy(t->st);
+    }
+    delete t;
+    return 0;
+}
+
+int adas_tracker_reset(adas_tracker* t) {          // BYTETracker.reset, byteTracker.py:187-200 (also BaseTrack.reset_counter)
+    t->frame_id = 0; t->tracked.clear(); t->lost.clear(); t->removed.clear();
+    g_track_count.store(0);
     return 0;
 }
 
@@ -430,7 +475,8 @@ int adas_tracker_update(adas_tracker* t, int n, const double* boxes_xyxy, const 
                         adas_track* out, int* n_out) {
     ADAS_CHECK(t != nullptr && n >= 0, "adas_tracker_update: bad arguments");
     ADAS_CUDA(cudaSetDevice(t->device));
-    return update_one(t, n, boxes_xyxy, scores, class_ids, max_out, out, n_out);
+    const adas::CamFrame cf{n, boxes_xyxy, scores, class_ids, out, n_out};
+    return adas::step_frame(&t, 1, &cf, max_out);
 }
 
 int adas_tracker_update_batch(adas_tracker* t, int n_frames, const int32_t* counts, const double* boxes_xyxy, const double* scores,
@@ -441,12 +487,46 @@ int adas_tracker_update_batch(adas_tracker* t, int n_frames, const int32_t* coun
     size_t off = 0;
     const uint64_t t0 = adas::now_ns();
     for (int f = 0; f < n_frames; ++f) {
-        int k = 0;
-        if (update_one(t, counts[f], boxes_xyxy + off * 4, scores + off, class_ids + off, max_out, out ? out + (size_t)f * max_out : nullptr, &k)) return 1;
-        n_out[f] = k;
+        const adas::CamFrame cf{counts[f], boxes_xyxy + off * 4, scores + off, class_ids + off, out ? out + (size_t)f * max_out : nullptr, &n_out[f]};
+        if (adas::step_frame(&t, 1, &cf, max_out)) return 1;
         off += (size_t)counts[f];
     }
     t->st_total_ns += adas::now_ns() - t0; t->st_frames += (uint64_t)n_frames;
+    return 0;
+}
+
+int adas_tracker_update_multi(adas_tracker* const* trackers, int k, int n_frames, const int32_t* counts, const double* boxes_xyxy,
+                              const double* scores, const int32_t* class_ids, int max_out, adas_track* out, int32_t* n_out) {
+    ADAS_CHECK(trackers != nullptr && k >= 1 && n_frames >= 0, "adas_tracker_update_multi: bad arguments (k = %d, n_frames = %d)", k, n_frames);
+    ADAS_CHECK(n_frames == 0 || (counts != nullptr && n_out != nullptr), "adas_tracker_update_multi: null counts or n_out");
+    for (int c = 0; c < k; ++c) {
+        ADAS_CHECK(trackers[c] != nullptr, "adas_tracker_update_multi: tracker %d is null", c);
+        for (int c2 = 0; c2 < c; ++c2)
+            ADAS_CHECK(trackers[c2] != trackers[c], "adas_tracker_update_multi: tracker %d is also tracker %d", c, c2);
+        ADAS_CHECK(trackers[c]->device == trackers[0]->device, "adas_tracker_update_multi: tracker %d is on device %d, tracker 0 on device %d", c,
+                   trackers[c]->device, trackers[0]->device);
+    }
+    size_t total = 0;
+    for (size_t i = 0; i < (size_t)n_frames * k; ++i) {
+        ADAS_CHECK(counts[i] >= 0, "adas_tracker_update_multi: negative detection count %d (frame %zu, tracker %zu)", counts[i], i / k, i % k);
+        total += (size_t)counts[i];
+    }
+    ADAS_CHECK(total == 0 || (boxes_xyxy != nullptr && scores != nullptr && class_ids != nullptr), "adas_tracker_update_multi: null detections");
+    ADAS_CUDA(cudaSetDevice(trackers[0]->device));
+    adas::NvtxRange nv("adas_tracker_update_multi");
+    std::vector<adas::CamFrame> cf(k);
+    size_t off = 0;
+    const uint64_t t0 = adas::now_ns();
+    for (int f = 0; f < n_frames; ++f) {
+        for (int c = 0; c < k; ++c) {
+            const size_t i = (size_t)f * k + c;
+            cf[c] = adas::CamFrame{counts[i], boxes_xyxy + off * 4, scores + off, class_ids + off, out ? out + i * max_out : nullptr, &n_out[i]};
+            off += (size_t)counts[i];
+        }
+        if (adas::step_frame(trackers, k, cf.data(), max_out)) return 1;
+    }
+    const uint64_t dt = adas::now_ns() - t0;
+    for (int c = 0; c < k; ++c) { trackers[c]->st_total_ns += dt; trackers[c]->st_frames += (uint64_t)n_frames; }
     return 0;
 }
 

@@ -9,6 +9,11 @@ instead was slower, the interpreter lock serialises the launches) -- while the h
 the PREVIOUS batch; consecutive batches alternate between two engine pairs so the device never waits for the host:
 the tracker is sequential in time per stream (SURVEY 8e), so it pipelines one batch behind the detectors.  Per-frame
 results are identical to calling the three detectors frame by frame.
+
+A rig of several cameras runs through ONE pipeline (`cameras=K`): the engines hold K * batch frames, each step makes one
+`adas_detect_pair` call for the frames of all cameras, and the K trackers (one per camera) advance in one library call with one
+association launch per frame for all of them (`adas_tracker_update_multi`).  Results equal K single-camera pipelines whose
+trackers are updated frame by frame in camera order.
 """
 from __future__ import annotations
 
@@ -21,7 +26,7 @@ from typing import List, Optional
 import numpy as np
 
 from . import _capi
-from .ObjectTracker import BYTETracker
+from .ObjectTracker import BYTETracker, update_trackers
 
 
 class StepResult:
@@ -35,25 +40,35 @@ class StepResult:
 
 class AdasPipeline:
     def __init__(self, yolo_plan: str, ufld_plan: str, device: int = 0, batch: int = 8, box_score: float = 0.4, box_nms_iou: float = 0.45,
-                 max_det: int = 1024, class_names: Optional[List[str]] = None, depth: int = 3, sets: int = 2, track_thresh: float = 0.5):
+                 max_det: int = 1024, class_names: Optional[List[str]] = None, depth: int = 3, sets: int = 2, track_thresh: float = 0.5,
+                 cameras: int = 1):
+        """`cameras` = K streams of one frame size through one pipeline: with K > 1, step / step_pipelined take [K, F, H, W, 3] frames
+        (F <= batch; a host array, a sequence of K [F, H, W, 3] host arrays, or a device pointer with shape (K, F, H, W)) and
+        return one StepResult per camera."""
+        if cameras < 1:
+            raise ValueError(f"cameras must be at least 1, got {cameras}")
         self.batch, self.box_score, self.box_nms_iou, self.max_det = batch, box_score, box_nms_iou, max_det
+        self.cameras = cameras
+        nb = cameras * batch
         # `sets` independent (object engine, lane engine) pairs: consecutive batches alternate between them so the next batch's
         # kernels are already queued on the device (own streams, own activation buffers) while the previous batch drains --
         # no idle gap between library calls, and four streams' worth of kernels to back-fill partial waves.
         self.sets = []
         for _ in range(max(1, sets)):
-            self.sets.append((_capi.Engine(yolo_plan, device, max_batch=batch), _capi.Engine(ufld_plan, device, max_batch=batch), threading.Lock()))
+            self.sets.append((_capi.Engine(yolo_plan, device, max_batch=nb), _capi.Engine(ufld_plan, device, max_batch=nb), threading.Lock()))
         self.yolo, self.ufld = self.sets[0][0], self.sets[0][1]
         # build every launch program here, one engine at a time: the per-layer tile autotune times candidates on the device and
         # must not run while another engine is busy (with two pairs the first two batches would otherwise tune concurrently);
         # the second pass captures the CUDA graphs.
         for y, u, _ in self.sets:
             for e in (y, u):
-                e.run(batch)
-                e.run(batch)
+                e.run(nb)
+                e.run(nb)
         self._next_set = 0
-        self.tracker = BYTETracker(track_thresh=track_thresh, names=class_names or [], device=device)
-        self.tracker.reset()
+        self.trackers = [BYTETracker(track_thresh=track_thresh, names=class_names or [], device=device) for _ in range(cameras)]
+        for t in self.trackers:
+            t.reset()
+        self.tracker = self.trackers[0]
         self.class_names = class_names
         self._pool = ThreadPoolExecutor(max_workers=len(self.sets))
         sys.setswitchinterval(2e-4)       # the detector thread only needs the interpreter between two library calls
@@ -98,28 +113,84 @@ class AdasPipeline:
         self.track_seconds = getattr(self, "track_seconds", 0.0) + (time.perf_counter() - t0)
         self.track_batches = getattr(self, "track_batches", 0) + 1
 
-    # -- public ---------------------------------------------------------------------------------------------
-    def step(self, frames, on_device: bool = False, shape=None) -> StepResult:
-        """Synchronous: detectors (concurrently), then the tracker for this batch."""
-        r = StepResult(*self._detect_both(frames, on_device, shape))
-        self._track(r)
-        return r
+    def _frames(self, frames, on_device: bool, shape):
+        """the frames of one step as adas_detect_pair takes them: with K > 1 cameras, camera-major [K * F, H, W, 3]"""
+        K = self.cameras
+        if K == 1:
+            return frames, on_device, shape
+        if on_device:
+            if shape is None or len(shape) != 4 or int(shape[0]) != K:
+                raise ValueError(f"device frames of {K} cameras need shape (cameras={K}, frames, H, W), got {shape}")
+            F, H, W = (int(v) for v in shape[1:])
+            if not 1 <= F <= self.batch:
+                raise ValueError(f"{F} frames per camera; this pipeline takes 1 to {self.batch}")
+            return frames, True, (K * F, H, W)
+        if not (isinstance(frames, np.ndarray) and frames.ndim == 5):
+            cams = [np.asarray(f) for f in frames]
+            if len(cams) != K:
+                raise ValueError(f"frames of {len(cams)} cameras for a pipeline of {K}")
+            for c, a in enumerate(cams):
+                if a.shape != cams[0].shape:
+                    raise ValueError(f"all cameras must send the same number of frames of one size: camera {c} sends {a.shape}, "
+                                     f"camera 0 {cams[0].shape}")
+            frames = np.stack(cams)
+        if frames.ndim != 5 or frames.shape[0] != K or frames.shape[4] != 3:
+            raise ValueError(f"frames of {K} cameras must be [cameras={K}, frames, H, W, 3], got {frames.shape}")
+        if not 1 <= frames.shape[1] <= self.batch:
+            raise ValueError(f"{frames.shape[1]} frames per camera; this pipeline takes 1 to {self.batch}")
+        return frames.reshape((-1,) + frames.shape[2:]), False, None
 
-    def step_pipelined(self, frames, on_device: bool = False, shape=None) -> Optional[StepResult]:
+    def _track_cameras(self, y, rs: List[StepResult]) -> None:
+        """ByteTrack for the frames of one batch of every camera in ONE library call (adas_tracker_update_multi): rs[c].tracks[i] is
+        the TRACK_DTYPE record array of camera c's frame i, as _track gives it for one camera."""
+        import time
+        t0 = time.perf_counter()
+        boxes, scores, cls, _, counts, _ = y                                     # [K * F, ...], camera-major
+        K = self.cameras
+        F = len(counts) // K
+        cnt = np.asarray(counts, np.int32).reshape(K, F).T                       # [F, K]
+        order = lambda a: a.reshape((K, F) + a.shape[1:]).swapaxes(0, 1)         # frame-major, then camera
+        keep = np.arange(boxes.shape[1])[None, None, :] < cnt[:, :, None]
+        bx = order(boxes)[keep]
+        xyxy = np.stack([bx[:, 0], bx[:, 1], bx[:, 0] + bx[:, 2], bx[:, 1] + bx[:, 3]], 1).astype(np.int64).astype(np.float64)
+        labels = order(cls)[keep]
+        if self.class_names is not None:
+            labels = np.asarray(self.class_names, dtype=object)[labels]
+        recs = update_trackers(self.trackers, cnt, xyxy, order(scores)[keep].astype(np.float64), labels)
+        for r, tr in zip(rs, recs):
+            r.tracks = tr
+        self.track_seconds = getattr(self, "track_seconds", 0.0) + (time.perf_counter() - t0)
+        self.track_batches = getattr(self, "track_batches", 0) + 1
+
+    def _result(self, yu):
+        y, u = yu
+        if self.cameras == 1:
+            r = StepResult(y, u)
+            self._track(r)
+            return r
+        F = len(y[4]) // self.cameras
+        cam = lambda t, c: tuple(None if a is None else a[c * F:(c + 1) * F] for a in t)
+        rs = [StepResult(cam(y, c), cam(u, c)) for c in range(self.cameras)]
+        self._track_cameras(y, rs)
+        return rs
+
+    # -- public ---------------------------------------------------------------------------------------------
+    def step(self, frames, on_device: bool = False, shape=None):
+        """Synchronous: detectors (concurrently), then the tracker for this batch.  One StepResult, or with K > 1 cameras a list of
+        K (one per camera)."""
+        return self._result(self._detect_both(*self._frames(frames, on_device, shape)))
+
+    def step_pipelined(self, frames, on_device: bool = False, shape=None):
         """Queue this batch for the detector thread (up to `depth` batches in flight, so the GPU never waits for Python) and
         return the oldest finished batch with its tracks (None while the pipeline fills); call flush() at the end.
         Frame buffers must stay valid until their batch has been returned."""
-        self._queue.append(self._detect(frames, on_device, shape))
+        self._queue.append(self._detect(*self._frames(frames, on_device, shape)))
         if len(self._queue) <= self.depth:
             return None
-        r = StepResult(*self._queue.popleft().result())
-        self._track(r)
-        return r
+        return self._result(self._queue.popleft().result())
 
-    def flush(self) -> List[StepResult]:
+    def flush(self) -> list:
         out = []
         while self._queue:
-            r = StepResult(*self._queue.popleft().result())
-            self._track(r)
-            out.append(r)
+            out.append(self._result(self._queue.popleft().result()))
         return out

@@ -512,25 +512,24 @@ def plan_route(spec: Spec) -> Optional[str]:
     types = [t for t, _, _ in ops]
     gemms = [p for t, p, _ in ops if t == plan.OP_GEMM]
     if plan.OP_IM2COL in types:
-        cin = [p for t, p, _ in ops if t == plan.OP_IM2COL][0][2]
+        cin = [p for t, p, _ in ops if t == plan.OP_IM2COL][0].Cin
         return "im2col4" if cin % 8 == 4 else "im2col8"
     if plan.OP_STEMCONV in types:
         return "stemconv"
     if plan.OP_STEMPACK in types:
-        return "stem7x7s2" if len(gemms) == 1 and gemms[0][3] == 4 else None
+        return "stem7x7s2" if len(gemms) == 1 and gemms[0].ntaps == 4 else None
     if len(gemms) == 1:
         p = gemms[0]
-        if p[14]:
-            return fc_route(p[2], p[6])
-        if p[19]:
+        if p.transposed:
+            return fc_route(p.Kc, p.N)
+        if p.up2:
             return "up2"
-        if p[16]:
+        if p.s2:
             return "s2"
-        if p[3] == 9:
-            return "tap" if p[18] else "slab"
-        if p[3] == 1:
+        if p.ntaps == 9:
+            return "tap" if p.no_slab else "slab"
+        if p.ntaps == 1:
             return "1x1"
         return None
-    names = {plan.OP_MAXPOOL: "maxpool", plan.OP_UPSAMPLE2X: "upsample", plan.OP_AVGPOOL2: "avgpool2", plan.OP_DWCONV: "dwconv",
-             plan.OP_ATTN: "attention", plan.OP_LAYERNORM: "layernorm"}
-    return names.get(types[0]) if len(types) == 1 else None
+    single = (plan.OP_MAXPOOL, plan.OP_UPSAMPLE2X, plan.OP_AVGPOOL2, plan.OP_DWCONV, plan.OP_ATTN, plan.OP_LAYERNORM)
+    return plan.OP_NAMES[types[0]] if len(types) == 1 and types[0] in single else None

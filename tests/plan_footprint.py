@@ -16,15 +16,11 @@ import struct
 from dataclasses import dataclass
 from typing import List, Optional, Tuple
 
-HDR_FMT = "<8sII3I4I16IQQ"
-HDR_SIZE = struct.calcsize(HDR_FMT)
-BUF_FMT, OP_FMT, TEN_FMT, OUT_FMT = "<6I", "<I23i4f", "<QQII", "<4I"
-BUF_SIZE, OP_SIZE, TEN_SIZE, OUT_SIZE = 24, 112, 24, 16
-assert (struct.calcsize(BUF_FMT), struct.calcsize(OP_FMT), struct.calcsize(TEN_FMT), struct.calcsize(OUT_FMT)) == (24, 112, 24, 16)
-
-OP_GEMM, OP_IM2COL, OP_MAXPOOL, OP_UPSAMPLE2X, OP_LAYERNORM, OP_STEMPACK, OP_STEMCONV = 1, 2, 3, 4, 5, 6, 7
-OP_AVGPOOL2, OP_DWCONV, OP_ATTN, OP_CBFUSE, OP_SE, OP_SHUFFLE2 = 8, 9, 10, 11, 12, 13
-MODEL_YOLOV8, MODEL_YOLOV5, MODEL_UFLDV2, MODEL_UFLDV1, MODEL_YOLOV6 = 0, 1, 2, 4, 5
+import adas_b200  # noqa: F401
+from adas_b200 import plan
+from adas_b200.plan import (BUF_FMT, BUF_SIZE, HDR_FMT, HDR_SIZE, MODEL_UFLDV1, MODEL_UFLDV2, MODEL_YOLOV6, MODEL_YOLOV8, OP_ATTN,
+                            OP_AVGPOOL2, OP_CBFUSE, OP_DWCONV, OP_FMT, OP_GEMM, OP_IM2COL, OP_LAYERNORM, OP_MAXPOOL, OP_NP, OP_SE,
+                            OP_SHUFFLE2, OP_SIZE, OP_STEMCONV, OP_STEMPACK, OP_UPSAMPLE2X, OUT_FMT, OUT_SIZE, TEN_FMT, TEN_SIZE)
 
 HEADER_FIELDS = ["version", "model_kind", "in_c", "in_h", "in_w", "n_buffers", "n_ops", "n_tensors", "n_outputs"] + \
                 [f"meta{i}" for i in range(16)]
@@ -34,7 +30,7 @@ HEADER_FIELDS = ["version", "model_kind", "in_c", "in_h", "in_w", "n_buffers", "
 class Plan:
     header: list            # unpacked HDR_FMT fields: magic, version, model_kind, in_c, in_h, in_w, n_buffers, n_ops, n_tensors, n_outputs, meta*16, blob_offset, blob_bytes
     bufs: List[list]        # rows_per_img, C, dtype, H, W, flags
-    ops: List[Tuple[int, list, list]]
+    ops: List[Tuple[int, plan.OpParams, list]]
     tensors: List[list]     # offset, bytes, dtype, pad
     outs: List[list]        # buffer, coff, C, stride
 
@@ -50,6 +46,19 @@ class Plan:
     def op_off(self, i): return HDR_SIZE + len(self.bufs) * BUF_SIZE + i * OP_SIZE
     def ten_off(self, i): return self.op_off(len(self.ops)) + i * TEN_SIZE
     def out_off(self, i): return self.ten_off(len(self.tensors)) + i * OUT_SIZE
+
+    def field_off(self, i, name):
+        """Byte offset of field `name` of op i: a field of plan.OP_FIELDS, "src<s>.<field>" of a CBFUSE source (plan.CBFUSE_SRC_FIELDS)
+        or a float of plan.OP_FLOATS."""
+        typ = self.ops[i][0]
+        if name in plan.OP_FLOATS.get(typ, ()):
+            slot = OP_NP + plan.OP_FLOATS[typ].index(name)
+        elif typ == OP_CBFUSE and name.startswith("src"):
+            s, field = name[3:].split(".")
+            slot = plan.cbfuse_src_slot(int(s)) + plan.CBFUSE_SRC_FIELDS.index(field)
+        else:
+            slot = plan.field_slot(typ, name)
+        return self.op_off(i) + 4 + 4 * slot
 
 
 def corrupt(raw: bytes, off: int, fmt: str, value) -> bytes:
@@ -79,7 +88,7 @@ def parse(raw: bytes) -> Plan:
     ops = []
     for i in range(no):
         r = struct.unpack_from(OP_FMT, raw, off + i * OP_SIZE)
-        ops.append((r[0], list(r[1:24]), list(r[24:])))
+        ops.append((r[0], plan.OpParams(r[0], r[1:1 + OP_NP]), list(r[1 + OP_NP:])))
     off += no * OP_SIZE
     tensors = [list(struct.unpack_from(TEN_FMT, raw, off + i * TEN_SIZE)) for i in range(nt)]
     off += nt * TEN_SIZE
@@ -136,106 +145,97 @@ class _Model:
         B, buf = self.B, self.buf
         w = f"op {oi}"
         if typ == OP_GEMM:
-            a, acoff, Kc, ntaps, wt, bt, N, act, rb, rcoff, rpre, ob, ocoff = p[:13]
-            transposed, s2, up2 = p[14], p[16], p[19]
-            self.tensor(wt, N * Kc * ntaps * 2, 0, w + " weights")
-            if bt >= 0:
-                self.tensor(bt, N * 4, 1, w + " bias")
+            self.tensor(p.w_tensor, p.N * p.Kc * p.ntaps * 2, 0, w + " weights")
+            if p.bias_tensor >= 0:
+                self.tensor(p.bias_tensor, p.N * 4, 1, w + " bias")
+            ob, N = p.out_buf, p.N
             oes = _esize(buf(ob)[2])
-            if transposed:
+            if p.transposed:
                 # one input vector per image: the whole per-image slab read flat (FC tensor-core and fc_stream routes alike)
-                self.region(a, False, B, buf(a)[0] * buf(a)[1], 0, Kc, 2, w + " FC input")
+                self.region(p.a_buf, False, B, buf(p.a_buf)[0] * buf(p.a_buf)[1], 0, p.Kc, 2, w + " FC input")
                 self.region(ob, True, B, buf(ob)[0] * buf(ob)[1], 0, N, oes, w + " FC output")
                 return
             # the operand tensor map spans the input's batch rows (taps past it read zeros); output rows follow the M walk
-            self.slice(a, False, self.padded_rows(a), acoff, Kc, w + " input")
-            if s2:
+            self.slice(p.a_buf, False, self.padded_rows(p.a_buf), p.a_coff, p.Kc, w + " input")
+            if p.s2:
                 out_rows = self.padded_rows(ob)
-            elif up2:
-                A_ = buf(a)
+            elif p.up2:
+                A_ = buf(p.a_buf)
                 out_rows = _rows(B, 2 * A_[3], 2 * A_[4])
             else:
-                out_rows = self.padded_rows(a)
-            self.slice(ob, True, out_rows, ocoff, N // 4 if up2 else N, w + " output", oes)
-            if rb >= 0:
+                out_rows = self.padded_rows(p.a_buf)
+            self.slice(ob, True, out_rows, p.out_coff, N // 4 if p.up2 else N, w + " output", oes)
+            if p.res_buf >= 0:
                 # the epilogue reads the residual at the output row index
-                self.slice(rb, False, out_rows, rcoff, N, w + " residual")
+                self.slice(p.res_buf, False, out_rows, p.res_coff, N, w + " residual")
         elif typ == OP_IM2COL:
-            i, icoff, Cin, kh, kw = p[:5]
-            o = p[7]
-            self.slice(i, False, self.padded_rows(i), icoff, Cin, w + " input")
-            self.region(o, True, _rows(B, buf(o)[3], buf(o)[4]), buf(o)[1], 0, kh * kw * Cin, 2, w + " patches")
+            o = p.out_buf
+            self.slice(p.in_buf, False, self.padded_rows(p.in_buf), p.in_coff, p.Cin, w + " input")
+            self.region(o, True, _rows(B, buf(o)[3], buf(o)[4]), buf(o)[1], 0, p.kh * p.kw * p.Cin, 2, w + " patches")
         elif typ == OP_MAXPOOL:
-            i, icoff, C = p[:3]
-            o, ocoff = p[6], p[7]
-            self.slice(i, False, self.padded_rows(i), icoff, C, w + " input")
-            self.slice(o, True, _rows(B, buf(o)[3], buf(o)[4]), ocoff, C, w + " output")
+            o = p.out_buf
+            self.slice(p.in_buf, False, self.padded_rows(p.in_buf), p.in_coff, p.C, w + " input")
+            self.slice(o, True, _rows(B, buf(o)[3], buf(o)[4]), p.out_coff, p.C, w + " output")
         elif typ == OP_UPSAMPLE2X:
-            i, icoff, C, o, ocoff = p[:5]
-            H, W = buf(i)[3], buf(i)[4]
-            self.slice(i, False, _rows(B, H, W), icoff, C, w + " input")
-            self.slice(o, True, _rows(B, 2 * H, 2 * W), ocoff, C, w + " output")
+            H, W = buf(p.in_buf)[3], buf(p.in_buf)[4]
+            self.slice(p.in_buf, False, _rows(B, H, W), p.in_coff, p.C, w + " input")
+            self.slice(p.out_buf, True, _rows(B, 2 * H, 2 * W), p.out_coff, p.C, w + " output")
         elif typ == OP_AVGPOOL2:
-            i, icoff, C, o, ocoff = p[:5]
-            rows = _rows(B, buf(i)[3], buf(i)[4])
-            self.slice(i, False, rows, icoff, C, w + " input")
-            self.slice(o, True, rows, ocoff, C, w + " output")
+            rows = _rows(B, buf(p.in_buf)[3], buf(p.in_buf)[4])
+            self.slice(p.in_buf, False, rows, p.in_coff, p.C, w + " input")
+            self.slice(p.out_buf, True, rows, p.out_coff, p.C, w + " output")
         elif typ == OP_DWCONV:
-            i, icoff, C, k, s, act, wt, bt, o, ocoff, rb, rcoff = p[:12]
-            self.tensor(wt, C * k * k * 2, 0, w + " weights")
-            self.tensor(bt, C * 4, 1, w + " bias")
-            self.slice(i, False, _rows(B, buf(i)[3], buf(i)[4]), icoff, C, w + " input")
-            orows = _rows(B, buf(o)[3], buf(o)[4])
-            self.slice(o, True, orows, ocoff, C, w + " output")
-            if rb >= 0:
-                self.slice(rb, False, orows, rcoff, C, w + " residual")
+            C, k = p.C, p.k
+            self.tensor(p.w_tensor, C * k * k * 2, 0, w + " weights")
+            self.tensor(p.bias_tensor, C * 4, 1, w + " bias")
+            self.slice(p.in_buf, False, _rows(B, buf(p.in_buf)[3], buf(p.in_buf)[4]), p.in_coff, C, w + " input")
+            orows = _rows(B, buf(p.out_buf)[3], buf(p.out_buf)[4])
+            self.slice(p.out_buf, True, orows, p.out_coff, C, w + " output")
+            if p.res_buf >= 0:
+                self.slice(p.res_buf, False, orows, p.res_coff, C, w + " residual")
         elif typ == OP_ATTN:
-            i, icoff, nh, kdp, hd, o, ocoff = p[:7]
-            rows = _rows(B, buf(i)[3], buf(i)[4])
-            self.slice(i, False, rows, icoff, nh * (2 * kdp + hd), w + " qkv")
-            self.slice(o, True, rows, ocoff, nh * hd, w + " output")
+            nh, kdp, hd = p.nh, p.kdp, p.hd
+            rows = _rows(B, buf(p.in_buf)[3], buf(p.in_buf)[4])
+            self.slice(p.in_buf, False, rows, p.in_coff, nh * (2 * kdp + hd), w + " qkv")
+            self.slice(p.out_buf, True, rows, p.out_coff, nh * hd, w + " output")
         elif typ == OP_CBFUSE:
-            o, ocoff, C, bb, bcoff, n_src = p[:6]
-            H, W = buf(o)[3], buf(o)[4]
-            self.slice(o, True, _rows(B, H, W), ocoff, C, w + " output")
-            self.slice(bb, False, _rows(B, H, W), bcoff, C, w + " base")
-            for s in range(n_src):
-                sb, scoff, sh = p[6 + 3 * s:9 + 3 * s]
+            C = p.C
+            H, W = buf(p.out_buf)[3], buf(p.out_buf)[4]
+            self.slice(p.out_buf, True, _rows(B, H, W), p.out_coff, C, w + " output")
+            self.slice(p.base_buf, False, _rows(B, H, W), p.base_coff, C, w + " base")
+            for s, (sb, scoff, sh) in enumerate(plan.cbfuse_sources(p)):
                 self.slice(sb, False, _rows(B, H >> sh, W >> sh), scoff, C, w + f" source {s}")
         elif typ == OP_SE:
-            i, icoff, C, hid = p[:4]
-            o, ocoff = p[8], p[9]
-            for t, n in zip(p[4:8], (hid * C, hid, C * hid, C)):
+            C, hid = p.C, p.hid
+            for t, n in zip((p.w1, p.b1, p.w2, p.b2), (hid * C, hid, C * hid, C)):
                 self.tensor(t, n * 4, 1, w + " se tensor")
-            rows = _rows(B, buf(i)[3], buf(i)[4])
-            self.slice(i, False, rows, icoff, C, w + " input")
-            self.slice(o, True, rows, ocoff, C, w + " output")
+            rows = _rows(B, buf(p.in_buf)[3], buf(p.in_buf)[4])
+            self.slice(p.in_buf, False, rows, p.in_coff, C, w + " input")
+            self.slice(p.out_buf, True, rows, p.out_coff, C, w + " output")
         elif typ == OP_SHUFFLE2:
-            a, acoff, b, bcoff, n, o, ocoff = p[:7]
-            rows = _rows(B, buf(o)[3], buf(o)[4])
-            self.slice(a, False, rows, acoff, n, w + " a")
-            self.slice(b, False, rows, bcoff, n, w + " b")
-            self.slice(o, True, rows, ocoff, 2 * n, w + " output")
+            n = p.n
+            rows = _rows(B, buf(p.out_buf)[3], buf(p.out_buf)[4])
+            self.slice(p.a_buf, False, rows, p.a_coff, n, w + " a")
+            self.slice(p.b_buf, False, rows, p.b_coff, n, w + " b")
+            self.slice(p.out_buf, True, rows, p.out_coff, 2 * n, w + " output")
         elif typ == OP_STEMPACK:
-            i, o = p[:2]
-            H, W = buf(i)[3], buf(i)[4]
-            self.region(i, False, _rows(B, H, W), 4, 0, 4, 2, w + " image")       # the kernel's image row stride is 4 channels
-            self.region(o, True, _rows(B, H >> 1, W >> 1), 64, 0, 64, 2, w + " packed")
+            H, W = buf(p.in_buf)[3], buf(p.in_buf)[4]
+            self.region(p.in_buf, False, _rows(B, H, W), 4, 0, 4, 2, w + " image")       # the kernel's image row stride is 4 channels
+            self.region(p.out_buf, True, _rows(B, H >> 1, W >> 1), 64, 0, 64, 2, w + " packed")
         elif typ == OP_STEMCONV:
-            i, wt, bt, Cout, k = p[:5]
-            o, ocoff = p[7], p[8]
-            self.tensor(wt, Cout * k * ((4 * k + 15) // 16 * 16) * 2, None, w + " weights")
-            if bt >= 0:
-                self.tensor(bt, Cout * 4, None, w + " bias")
-            H, W = buf(i)[3], buf(i)[4]
-            self.region(i, False, _rows(B, H, W), 4, 0, 4, 2, w + " image")
-            self.slice(o, True, _rows(B, buf(o)[3], buf(o)[4]), ocoff, Cout, w + " output")
+            Cout, k = p.Cout, p.k
+            self.tensor(p.w_tensor, Cout * k * ((4 * k + 15) // 16 * 16) * 2, None, w + " weights")
+            if p.bias_tensor >= 0:
+                self.tensor(p.bias_tensor, Cout * 4, None, w + " bias")
+            H, W = buf(p.in_buf)[3], buf(p.in_buf)[4]
+            self.region(p.in_buf, False, _rows(B, H, W), 4, 0, 4, 2, w + " image")
+            self.slice(p.out_buf, True, _rows(B, buf(p.out_buf)[3], buf(p.out_buf)[4]), p.out_coff, Cout, w + " output")
         elif typ == OP_LAYERNORM:
-            i, d_len, gt, bt, o = p[:5]
-            self.tensor(gt, d_len * 4, None, w + " gamma")
-            self.tensor(bt, d_len * 4, None, w + " beta")
-            self.region(i, False, B, buf(i)[0] * buf(i)[1], 0, d_len, 2, w + " input")
-            self.region(o, True, B, buf(o)[0] * buf(o)[1], 0, d_len, 2, w + " output")
+            d_len = p.d_len
+            self.tensor(p.gamma_tensor, d_len * 4, None, w + " gamma")
+            self.tensor(p.beta_tensor, d_len * 4, None, w + " beta")
+            self.region(p.in_buf, False, B, buf(p.in_buf)[0] * buf(p.in_buf)[1], 0, d_len, 2, w + " input")
+            self.region(p.out_buf, True, B, buf(p.out_buf)[0] * buf(p.out_buf)[1], 0, d_len, 2, w + " output")
         else:
             self.faults.append(f"{w}: unknown op type {typ}")
 

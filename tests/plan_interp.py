@@ -29,11 +29,6 @@ class Region(NamedTuple):
     hi: int
 
 
-OP_NAMES = {plan.OP_GEMM: "gemm", plan.OP_IM2COL: "im2col", plan.OP_MAXPOOL: "maxpool", plan.OP_UPSAMPLE2X: "upsample",
-            plan.OP_LAYERNORM: "layernorm", plan.OP_STEMPACK: "stempack", plan.OP_STEMCONV: "stemconv", plan.OP_AVGPOOL2: "avgpool2",
-            plan.OP_DWCONV: "dwconv", plan.OP_ATTN: "attention", plan.OP_CBFUSE: "cbfuse", plan.OP_SE: "se", plan.OP_SHUFFLE2: "shuffle2"}
-
-
 def geom(pb, buf):
     rows, C, dtype, H, W, _ = pb.buffers[buf]
     return rows, C, dtype, H, W
@@ -48,15 +43,15 @@ def _flat(pb, buf, lo, hi) -> Region:
 
 def gemm_route(p) -> str:
     """The GEMM route of a packed op (the names of op_conformance_cases.plan_route)."""
-    if p[14]:
-        return oc.fc_route(p[2], p[6])
-    if p[19]:
+    if p.transposed:
+        return oc.fc_route(p.Kc, p.N)
+    if p.up2:
         return "up2"
-    if p[16]:
+    if p.s2:
         return "s2"
-    if p[3] == 9:
+    if p.ntaps == 9:
         return "9tap"
-    if p[3] == 4:
+    if p.ntaps == 4:
         return "stem7x7s2"
     return "1x1"
 
@@ -66,49 +61,44 @@ def op_kind(pb, i) -> str:
     t, p, _ = pb.ops[i]
     if t == plan.OP_GEMM:
         return "gemm-" + gemm_route(p)
-    return OP_NAMES[t]
-
-
-def cbfuse_sources(p) -> List[Tuple[int, int, int]]:
-    """(buffer, channel offset, shift) of each source of an OP_CBFUSE op, in summation order."""
-    return [tuple(p[6 + 3 * s:9 + 3 * s]) for s in range(p[5])]
+    return plan.OP_NAMES[t]
 
 
 def op_regions(pb, i) -> Tuple[List[Region], List[Region]]:
     """(writes, reads) of op i.  An in-place CBFuse or SE reads its own write region."""
     t, p, _ = pb.ops[i]
     if t == plan.OP_GEMM:
-        a, acoff, Kc, N, out, ocoff = p[0], p[1], p[2], p[6], p[11], p[12]
-        if p[14]:
+        a, acoff, Kc, N, out, ocoff = p.a_buf, p.a_coff, p.Kc, p.N, p.out_buf, p.out_coff
+        if p.transposed:
             return [Region(out, ocoff, ocoff + N)], [_flat(pb, a, 0, Kc)]
-        reads = [Region(a, acoff, acoff + Kc)] + ([Region(p[8], p[9], p[9] + N)] if p[8] >= 0 else [])
-        return [Region(out, ocoff, ocoff + (N // 4 if p[19] else N))], reads
+        reads = [Region(a, acoff, acoff + Kc)] + ([Region(p.res_buf, p.res_coff, p.res_coff + N)] if p.res_buf >= 0 else [])
+        return [Region(out, ocoff, ocoff + (N // 4 if p.up2 else N))], reads
     if t == plan.OP_IM2COL:      # owns its whole patch buffer: columns past kh * kw * Cin stay zero, and meet zero weights
-        return [Region(p[7], 0, geom(pb, p[7])[1])], [Region(p[0], p[1], p[1] + p[2])]
-    if t == plan.OP_MAXPOOL:
-        return [Region(p[6], p[7], p[7] + p[2])], [Region(p[0], p[1], p[1] + p[2])]
-    if t in (plan.OP_UPSAMPLE2X, plan.OP_AVGPOOL2):
-        return [Region(p[3], p[4], p[4] + p[2])], [Region(p[0], p[1], p[1] + p[2])]
+        return [Region(p.out_buf, 0, geom(pb, p.out_buf)[1])], [Region(p.in_buf, p.in_coff, p.in_coff + p.Cin)]
+    if t in (plan.OP_MAXPOOL, plan.OP_UPSAMPLE2X, plan.OP_AVGPOOL2):
+        return [Region(p.out_buf, p.out_coff, p.out_coff + p.C)], [Region(p.in_buf, p.in_coff, p.in_coff + p.C)]
     if t == plan.OP_STEMPACK:
-        return [Region(p[1], 0, 64)], [Region(p[0], 0, 4)]
+        return [Region(p.out_buf, 0, 64)], [Region(p.in_buf, 0, 4)]
     if t == plan.OP_STEMCONV:
-        return [Region(p[7], p[8], p[8] + p[3])], [Region(p[0], 0, 4)]
+        return [Region(p.out_buf, p.out_coff, p.out_coff + p.Cout)], [Region(p.in_buf, 0, 4)]
     if t == plan.OP_LAYERNORM:
-        return [Region(p[4], 0, p[1])], [_flat(pb, p[0], 0, p[1])]
+        return [Region(p.out_buf, 0, p.d_len)], [_flat(pb, p.in_buf, 0, p.d_len)]
     if t == plan.OP_DWCONV:
-        C = p[2]
-        return [Region(p[8], p[9], p[9] + C)], [Region(p[0], p[1], p[1] + C)] + ([Region(p[10], p[11], p[11] + C)] if p[10] >= 0 else [])
+        C = p.C
+        return ([Region(p.out_buf, p.out_coff, p.out_coff + C)],
+                [Region(p.in_buf, p.in_coff, p.in_coff + C)] + ([Region(p.res_buf, p.res_coff, p.res_coff + C)] if p.res_buf >= 0 else []))
     if t == plan.OP_ATTN:
-        nh, kdp, hd = p[2], p[3], p[4]
-        return [Region(p[5], p[6], p[6] + nh * hd)], [Region(p[0], p[1], p[1] + nh * (2 * kdp + hd))]
+        nh, kdp, hd = p.nh, p.kdp, p.hd
+        return [Region(p.out_buf, p.out_coff, p.out_coff + nh * hd)], [Region(p.in_buf, p.in_coff, p.in_coff + nh * (2 * kdp + hd))]
     if t == plan.OP_CBFUSE:
-        C = p[2]
-        return [Region(p[0], p[1], p[1] + C)], [Region(p[3], p[4], p[4] + C)] + [Region(q[0], q[1], q[1] + C) for q in cbfuse_sources(p)]
+        C = p.C
+        return ([Region(p.out_buf, p.out_coff, p.out_coff + C)],
+                [Region(p.base_buf, p.base_coff, p.base_coff + C)] + [Region(q[0], q[1], q[1] + C) for q in plan.cbfuse_sources(p)])
     if t == plan.OP_SE:
-        return [Region(p[8], p[9], p[9] + p[2])], [Region(p[0], p[1], p[1] + p[2])]
+        return [Region(p.out_buf, p.out_coff, p.out_coff + p.C)], [Region(p.in_buf, p.in_coff, p.in_coff + p.C)]
     if t == plan.OP_SHUFFLE2:
-        n = p[4]
-        return [Region(p[5], p[6], p[6] + 2 * n)], [Region(p[0], p[1], p[1] + n), Region(p[2], p[3], p[3] + n)]
+        n = p.n
+        return [Region(p.out_buf, p.out_coff, p.out_coff + 2 * n)], [Region(p.a_buf, p.a_coff, p.a_coff + n), Region(p.b_buf, p.b_coff, p.b_coff + n)]
     raise ValueError(f"op {i}: unknown type {t}")
 
 
@@ -250,11 +240,11 @@ def _np(t: torch.Tensor) -> np.ndarray:
 
 def _gemm_conv(pb, p, bufs, b, dev, absval=False):
     """Accumulator [1, N, Ho, Wo] of a non-FC GEMM for image b (the kernel's operand addressing), or of |x| |w| with absval."""
-    a, acoff, Kc, ntaps, N = p[0], p[1], p[2], p[3], p[6]
-    w = torch.from_numpy(pb.tensors[p[4]].astype(np.float64)).to(dev)
+    a, acoff, Kc, ntaps, N = p.a_buf, p.a_coff, p.Kc, p.ntaps, p.N
+    w = torch.from_numpy(pb.tensors[p.w_tensor].astype(np.float64)).to(dev)
     f = (lambda t: t.abs()) if absval else (lambda t: t)
     w = f(w)
-    if p[19]:                                                     # 2x2 transposed conv: a 1x1 GEMM with columns (dy, dx, c)
+    if p.up2:                                                     # 2x2 transposed conv: a 1x1 GEMM with columns (dy, dx, c)
         x = f(image_view(pb, bufs, a, b, acoff, acoff + Kc, dev))
         acc = torch.einsum("nk,bkhw->bnhw", w, x)
         co = N // 4
@@ -270,7 +260,7 @@ def _gemm_conv(pb, p, bufs, b, dev, absval=False):
         return F.conv2d(x, wk)
     k = 3 if ntaps == 9 else 1
     wk = w.reshape(N, k, k, Kc).permute(0, 3, 1, 2)
-    s = 2 if p[16] else 1
+    s = 2 if p.s2 else 1
     if k == 3:                                                    # the halo supplies the padding
         return F.conv2d(f(image_view(pb, bufs, a, b, acoff, acoff + Kc, dev, halo=True)), wk, stride=s)
     return F.conv2d(f(image_view(pb, bufs, a, b, acoff, acoff + Kc, dev)), wk, stride=s)
@@ -278,50 +268,50 @@ def _gemm_conv(pb, p, bufs, b, dev, absval=False):
 
 def _gemm_ref(pb, i, bufs, B, dev, want_bound):
     t, p, fl = pb.ops[i]
-    N, act = p[6], p[7]
-    out_f32 = geom(pb, p[11])[2] == 1
-    bias = torch.from_numpy(pb.tensors[p[5]].astype(np.float64)).to(dev) if p[5] >= 0 else None
-    if p[14]:                                                     # FC: one K-vector per image, the whole per-image slab
-        rows, C, _, _, _ = geom(pb, p[0])
-        x = _t(bufs[p[0]][:B * rows].reshape(B, rows * C)[:, :p[2]], dev)
-        w = torch.from_numpy(pb.tensors[p[4]].astype(np.float64)).to(dev)
+    N, act = p.N, p.act
+    out_f32 = geom(pb, p.out_buf)[2] == 1
+    bias = torch.from_numpy(pb.tensors[p.bias_tensor].astype(np.float64)).to(dev) if p.bias_tensor >= 0 else None
+    if p.transposed:                                              # FC: one K-vector per image, the whole per-image slab
+        rows, C, _, _, _ = geom(pb, p.a_buf)
+        x = _t(bufs[p.a_buf][:B * rows].reshape(B, rows * C)[:, :p.Kc], dev)
+        w = torch.from_numpy(pb.tensors[p.w_tensor].astype(np.float64)).to(dev)
         a = x @ w.T + (bias if bias is not None else 0.0)
         ref = _act(a, act)
         if not want_bound:
             return _np(ref), None
         S = x.abs() @ w.abs().T + (bias.abs() if bias is not None else 0.0)
-        return _np(ref), oc.gemm_bound(_np(ref), _np(S), p[2], act, _np(a), None, out_f32)
+        return _np(ref), oc.gemm_bound(_np(ref), _np(S), p.Kc, act, _np(a), None, out_f32)
     refs, bnds = [], []
-    alpha = float(np.float32(fl[0])) if fl[0] != 0.0 else 1.0
-    K = p[3] * p[2]
+    alpha = float(np.float32(fl[0])) if fl[0] != 0.0 else 1.0       # f[0] = res_scale
+    K = p.ntaps * p.Kc
     for b in range(B):
         acc = _gemm_conv(pb, p, bufs, b, dev)
         bb = bias[None, :, None, None] if bias is not None else 0.0
-        if p[19] and bias is not None:
+        if p.up2 and bias is not None:
             bb = bias[:N // 4][None, :, None, None]
         a = acc + bb
         r = None
-        if p[8] >= 0:
-            r = image_view(pb, bufs, p[8], b, p[9], p[9] + N, dev)
-            if p[10]:
+        if p.res_buf >= 0:
+            r = image_view(pb, bufs, p.res_buf, b, p.res_coff, p.res_coff + N, dev)
+            if p.res_pre_act:
                 a = a + r
         y = _act(a, act)
         rp = None
-        if r is not None and not p[10]:
+        if r is not None and not p.res_pre_act:
             rp = alpha * r
             y = y + rp
         refs.append(_np(y))
         if want_bound:
             S = _gemm_conv(pb, p, bufs, b, dev, absval=True) + (bb.abs() if bias is not None else 0.0)
-            if r is not None and p[10]:
+            if r is not None and p.res_pre_act:
                 S = S + r.abs()
-            bnds.append(oc.gemm_bound(refs[-1], _np(S), p[2] if p[19] else K, act, _np(a), None if rp is None else _np(rp), out_f32))
+            bnds.append(oc.gemm_bound(refs[-1], _np(S), p.Kc if p.up2 else K, act, _np(a), None if rp is None else _np(rp), out_f32))
     return np.concatenate(refs), (np.concatenate(bnds) if want_bound else None)
 
 
 def _im2col_ref(pb, p, bufs, B, dev):
-    in_buf, coff, Cin, kh, kw, s, pad, out = p[:8]
-    _, Kpad, _, Ho, Wo = geom(pb, out)
+    in_buf, coff, Cin, kh, kw, s, pad = p.in_buf, p.in_coff, p.Cin, p.kh, p.kw, p.stride, p.pad
+    _, Kpad, _, Ho, Wo = geom(pb, p.out_buf)
     res = []
     for b in range(B):
         x = F.pad(image_view(pb, bufs, in_buf, b, coff, coff + Cin, dev), (pad, pad + kw, pad, pad + kh))
@@ -332,7 +322,7 @@ def _im2col_ref(pb, p, bufs, B, dev):
 
 
 def _stempack_ref(pb, p, bufs, B, dev):
-    img, q = p[0], p[1]
+    img = p.in_buf
     _, _, _, H, W = geom(pb, img)
     Ho, Wo = H // 2, W // 2
     res = []
@@ -348,8 +338,8 @@ def _stempack_ref(pb, p, bufs, B, dev):
 
 
 def _stemconv_ref(pb, p, bufs, B, dev, want_bound):
-    img, wt, bt, cout, k, pad, act, out, ocoff = p[:9]
-    s = 2 if p[9] == 0 else p[9]
+    img, wt, bt, cout, k, pad, act = p.in_buf, p.w_tensor, p.bias_tensor, p.Cout, p.k, p.pad, p.act
+    s = 2 if p.stride == 0 else p.stride
     KR = (4 * k + 15) // 16 * 16
     wq = pb.tensors[wt].astype(np.float64).reshape(cout, k, KR)[:, :, :4 * k].reshape(cout, k, k, 4)
     w = torch.from_numpy(wq).permute(0, 3, 1, 2).contiguous().to(dev)
@@ -366,7 +356,7 @@ def _stemconv_ref(pb, p, bufs, B, dev, want_bound):
 
 
 def _dwconv_ref(pb, p, bufs, B, dev, want_bound):
-    in_buf, coff, C, k, s, act, wt, bt, out, ocoff, rb, rcoff = p[:12]
+    in_buf, coff, C, k, s, act, wt, bt, rb, rcoff = p.in_buf, p.in_coff, p.C, p.k, p.stride, p.act, p.w_tensor, p.bias_tensor, p.res_buf, p.res_coff
     w = torch.from_numpy(pb.tensors[wt].astype(np.float64).T.reshape(C, 1, k, k).copy()).to(dev)
     bias = torch.from_numpy(pb.tensors[bt].astype(np.float64)).to(dev)
     refs, bnds = [], []
@@ -387,7 +377,7 @@ def _dwconv_ref(pb, p, bufs, B, dev, want_bound):
 def _layernorm_ref(pb, p, fl, bufs, B, want_bound):
     """Statistics over the d_norm entries the plan gives a nonzero gamma or beta (the rest are structural zeros, as the kernel counts
     them: mean = sum / d_norm, variance = (sum of (x - mean)^2 - (d_len - d_norm) mean^2) / d_norm)."""
-    in_buf, d_len, gt, bt, out, d_norm = p[:6]
+    in_buf, d_len, gt, bt, d_norm = p.in_buf, p.d_len, p.gamma_tensor, p.beta_tensor, p.d_norm
     rows, C, _, _, _ = geom(pb, in_buf)
     x = bufs[in_buf][:B * rows].reshape(B, rows * C)[:, :d_len].astype(np.float64)
     g = pb.tensors[gt].astype(np.float64)[:d_len]
@@ -398,7 +388,7 @@ def _layernorm_ref(pb, p, fl, bufs, B, want_bound):
     order = np.concatenate([np.nonzero(real)[0], np.nonzero(~real)[0]])
     mu = x.sum(1, keepdims=True) / d_norm
     var = (((x - mu) ** 2).sum(1, keepdims=True) - (d_len - d_norm) * mu ** 2) / d_norm
-    ref = (x - mu) / np.sqrt(var + float(np.float32(fl[0]))) * g + be
+    ref = (x - mu) / np.sqrt(var + float(np.float32(fl[0]))) * g + be          # f[0] = eps
     if not want_bound:
         return ref, None
     inv = np.argsort(order)
@@ -409,18 +399,18 @@ def _layernorm_ref(pb, p, fl, bufs, B, want_bound):
 def _cbfuse_ref(pb, p, bufs, B, dev, want_bound):
     """base + sum of the sources, each repeated 2^shift times along H and W.  The kernel sums in fp32 (base first, then the sources
     in order) and rounds once: within n_src * 2^-24 * (|base| + sum |src|) of the exact sum, then half an fp16 ulp."""
-    C = p[2]
+    C = p.C
     refs, bnds = [], []
     for b in range(B):
-        acc = image_view(pb, bufs, p[3], b, p[4], p[4] + C, dev)
+        acc = image_view(pb, bufs, p.base_buf, b, p.base_coff, p.base_coff + C, dev)
         S = acc.abs()
-        for buf, coff, s in cbfuse_sources(p):
+        for buf, coff, s in plan.cbfuse_sources(p):
             v = image_view(pb, bufs, buf, b, coff, coff + C, dev).repeat_interleave(1 << s, 2).repeat_interleave(1 << s, 3)
             acc = acc + v
             S = S + v.abs()
         refs.append(_np(acc))
         if want_bound:
-            e32 = p[5] * 2.0 ** -24 * _np(S)
+            e32 = p.n_src * 2.0 ** -24 * _np(S)
             bnds.append(e32 + 0.5 * np.spacing((np.abs(refs[-1]) + e32).astype(np.float16)).astype(np.float64))
     return np.concatenate(refs), (np.concatenate(bnds) if want_bound else None)
 
@@ -430,8 +420,8 @@ def _se_ref(pb, p, bufs, B, dev, want_bound):
     terms and a division, within (HW + 1) 2^-24 mean|x|; each FC is an fp32 dot product with a bias, within n 2^-24 (|b| + sum |w| |v|)
     of its fp32 inputs plus the propagated input error (ReLU: Lipschitz 1); hardsigmoid (Lipschitz 1/6, then + 3 and / 6 in fp32) adds
     2^-23; the product x * g adds 2^-24 |x g|; the fp16 store 2^-11 |ref| + 2^-24.  Each 2^-24 is doubled below for margin."""
-    in_buf, coff, C, hid = p[:4]
-    w1, b1, w2, b2 = (pb.tensors[t].astype(np.float64) for t in p[4:8])
+    in_buf, coff, C, hid = p.in_buf, p.in_coff, p.C, p.hid
+    w1, b1, w2, b2 = (pb.tensors[t].astype(np.float64) for t in (p.w1, p.b1, p.w2, p.b2))
     w1, w2 = w1.reshape(hid, C), w2.reshape(C, hid)
     refs, bnds = [], []
     for b in range(B):
@@ -456,11 +446,11 @@ def _se_ref(pb, p, bufs, B, dev, want_bound):
 
 def _shuffle2_ref(pb, p, bufs, B, dev):
     """cat(a, b) with the channels interleaved (a0, b0, a1, b1, ...): ShuffleNetV2's channel_shuffle of two groups."""
-    n = p[4]
+    n = p.n
     res = []
     for b in range(B):
-        a = image_view(pb, bufs, p[0], b, p[1], p[1] + n, dev)
-        c = image_view(pb, bufs, p[2], b, p[3], p[3] + n, dev)
+        a = image_view(pb, bufs, p.a_buf, b, p.a_coff, p.a_coff + n, dev)
+        c = image_view(pb, bufs, p.b_buf, b, p.b_coff, p.b_coff + n, dev)
         res.append(_np(torch.stack([a, c], 2).reshape(1, 2 * n, a.shape[2], a.shape[3])))
     return np.concatenate(res)
 
@@ -483,14 +473,14 @@ def op_ref(pb, i, bufs, B, device="cpu", want_bound=True) -> Tuple[np.ndarray, O
         if t == plan.OP_LAYERNORM:
             return _layernorm_ref(pb, p, fl, bufs, B, want_bound)
         if t == plan.OP_MAXPOOL:
-            in_buf, coff, C, k, s, pad = p[:6]
+            in_buf, coff, C, k, s, pad = p.in_buf, p.in_coff, p.C, p.k, p.stride, p.pad
             return np.concatenate([_np(F.max_pool2d(image_view(pb, bufs, in_buf, b, coff, coff + C, dev), k, s, pad)) for b in range(B)]), None
         if t == plan.OP_UPSAMPLE2X:
-            in_buf, coff, C = p[:3]
+            in_buf, coff, C = p.in_buf, p.in_coff, p.C
             return np.concatenate([_np(image_view(pb, bufs, in_buf, b, coff, coff + C, dev).repeat_interleave(2, 2).repeat_interleave(2, 3))
                                    for b in range(B)]), None
         if t == plan.OP_AVGPOOL2:
-            in_buf, coff, C, _, _, fill = p[:6]
+            in_buf, coff, C, fill = p.in_buf, p.in_coff, p.C, p.fill
             res = []
             for b in range(B):
                 x = _np(image_view(pb, bufs, in_buf, b, coff, coff + C, dev)).astype(np.float32)    # the kernel's fp32 order, one rounding
@@ -500,11 +490,11 @@ def op_ref(pb, i, bufs, B, device="cpu", want_bound=True) -> Tuple[np.ndarray, O
                 res.append(r)
             return np.concatenate(res), None
         if t == plan.OP_ATTN:
-            in_buf, coff, nh, kdp, hd = p[:5]
+            in_buf, coff, nh, kdp, hd = p.in_buf, p.in_coff, p.nh, p.kdp, p.hd
             refs, bnds = [], []
             for b in range(B):
                 qkv = _np(image_view(pb, bufs, in_buf, b, coff, coff + nh * (2 * kdp + hd), dev))
-                r, bd = oc.attention_ref(qkv, nh, kdp, hd, float(np.float32(fl[0])))
+                r, bd = oc.attention_ref(qkv, nh, kdp, hd, float(np.float32(fl[0])))     # f[0] = softmax scale
                 refs.append(r)
                 bnds.append(bd)
             return np.concatenate(refs), (np.concatenate(bnds) if want_bound else None)

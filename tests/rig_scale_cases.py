@@ -34,7 +34,7 @@ def halo_is_zero(pb, i: int, a: np.ndarray, B: int) -> bool:
     if H == 0:
         return True
     v = a[:B * (H + 2) * (W + 2)].reshape(B, H + 2, W + 2, C)
-    stem = any(t == plan.OP_STEMPACK and p[1] == i for t, p, _ in pb.ops)
+    stem = any(t == plan.OP_STEMPACK and p.out_buf == i for t, p, _ in pb.ops)
     edges = [v[:, -1], v[:, :, 0], v[:, :, -1]] + ([] if stem else [v[:, 0]])
     return not any(np.any(e != 0) for e in edges)
 

@@ -73,7 +73,7 @@ def read_all(eng, pb, mb):
 
 
 def halo_errors(pb, bufs, mb):
-    stem_q = {p[1] for t, p, _ in pb.ops if t == plan.OP_STEMPACK}
+    stem_q = {p.out_buf for t, p, _ in pb.ops if t == plan.OP_STEMPACK}
     bad = []
     for i, (rows, C, _, H, W, _) in enumerate(pb.buffers):
         if H == 0:

@@ -244,19 +244,19 @@ def test_network_every_candidate(tmp_path, family, scale, kw, mb, B):
     # every GEMM the autotuner chooses for: its timed candidates, or the one configuration it ran without timing
     tuned = {}
     for i, (t, p, _) in enumerate(pb.ops):
-        if t != plan.OP_GEMM or p[14] or p[15] > 0:
+        if t != plan.OP_GEMM or p.transposed or p.BN > 0:
             continue
         if i in cands:
             tuned[i] = cands[i]
         else:
             BN, MT, slab, _ = _ran(descs[i])
-            tuned[i] = [(BN, MT, p[18])]
+            tuned[i] = [(BN, MT, p.no_slab)]
     assert set(cands) <= set(tuned), sorted(set(cands) - set(tuned))
     V = max(len(c) for c in tuned.values())
     fails = []
     for v in range(V):
         pv = copy.copy(pb)
-        pv.ops = [(t, list(p), list(f)) for t, p, f in pb.ops]
+        pv.ops = [(t, p.copy(), list(f)) for t, p, f in pb.ops]
         for i, cl in tuned.items():
             ts.force_tile(pv, i, *cl[v % len(cl)])
         path = str(tmp_path / f"variant{v}.b200w")
@@ -272,7 +272,7 @@ def test_network_every_candidate(tmp_path, family, scale, kw, mb, B):
         os.remove(path)
         if bad or bad0:
             forced = {i: cl[v % len(cl)] for i, cl in tuned.items()}
-            suspects = sorted({i for i, (t, p, _) in enumerate(pb.ops) if t == plan.OP_GEMM and p[11] in bad})
+            suspects = sorted({i for i, (t, p, _) in enumerate(pb.ops) if t == plan.OP_GEMM and p.out_buf in bad})
             fails.append(f"variant {v}: buffers {bad} differ from the autotuned run, image 0 of run(1) differs in {bad0}; "
                          f"GEMMs writing them ran (BN, MT, no_slab) {[(i, forced.get(i)) for i in suspects]}")
     kinds = {}

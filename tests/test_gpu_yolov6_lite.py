@@ -40,14 +40,14 @@ def _up2_hs(sweep_case, case, seed=0):
     sw = sweep_case(case, seed)
     a = sw.ref
     for i, _, _ in sw.ops:
-        sw.pb.ops[i][1][7] = HS
+        sw.pb.ops[i][1].act = HS
     name, _, B, H, W, cin, in_off, cout = case[:8]
     x = sw.ins[0][2]
-    w = sw.pb.tensors[sw.pb.ops[sw.ops[0][0]][1][4]].astype(np.float64)     # [4 Cout, Cin] in (dy, dx, c) order
+    w = sw.pb.tensors[sw.pb.ops[sw.ops[0][0]][1].w_tensor].astype(np.float64)     # [4 Cout, Cin] in (dy, dx, c) order
     S = np.zeros_like(a)
     for q in range(4):
         S[:, :, q // 2::2, q % 2::2] = np.einsum("nk,bkhw->bnhw", np.abs(w[q * cout:(q + 1) * cout]), np.abs(x))
-    S += np.abs(sw.pb.tensors[sw.pb.ops[sw.ops[0][0]][1][5]][:cout].astype(np.float64))[None, :, None, None]
+    S += np.abs(sw.pb.tensors[sw.pb.ops[sw.ops[0][0]][1].bias_tensor][:cout].astype(np.float64))[None, :, None, None]
     sw.ref = oc.act64(a, HS)
     sw.bound = oc.gemm_bound(sw.ref, S, oc.r8(cin), HS, a)
     return sw

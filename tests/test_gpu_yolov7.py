@@ -112,7 +112,7 @@ def test_stem_conv_direct_stride1(tmp_path, cout, act):
         w = (rng.standard_normal((cout, 3, 3, 3)) * np.sqrt(2.0 / 27)).astype(np.float32)
         b = (rng.standard_normal(cout) * 0.1).astype(np.float32)
         out = pb.conv(pb.image, w, b, 3, 1, act)
-        assert [op[0] for op in pb.ops] == [plan.OP_STEMCONV] and pb.ops[0][1][9] == 1
+        assert [op[0] for op in pb.ops] == [plan.OP_STEMCONV] and pb.ops[0][1].stride == 1
         path = str(tmp_path / f"stem1_{cout}_{act}_{H}.b200w")
         pb.write(path)
         eng = _capi.Engine(path, 0, max_batch=B)

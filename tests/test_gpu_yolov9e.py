@@ -52,8 +52,8 @@ def _fill(pb, out, B, mb, seed):
         inner = v[:, 1:-1, 1:-1]
         inner[:] = SENTINEL if i == out.buf else np.float16(np.nan)
         lo = 16 if i == out.buf else 8
-        if i != out.buf or p[3] == p[0]:                          # the output slice holds the base when in place
-            inner[:B, :, :, lo:lo + p[2]] = (rng.standard_normal((B, H, W, p[2])) * 3).astype(np.float16)
+        if i != out.buf or p.base_buf == p.out_buf:               # the output slice holds the base when in place
+            inner[:B, :, :, lo:lo + p.C] = (rng.standard_normal((B, H, W, p.C)) * 3).astype(np.float16)
         bufs[i] = v.reshape(mb * rows, Cb)
     return bufs
 

@@ -186,8 +186,8 @@ def _layernorm_emulate(x, gamma, beta, d_norm, eps, two_pass):
 def test_layernorm_bound_at_mean_over_std_200(two_pass, ok):
     spec = oc.layernorm_spec((4, 4992, 4000, 200.0))
     x = spec.ins[0][2]
-    g = spec.pb.tensors[spec.pb.ops[0][1][2]]
-    bt = spec.pb.tensors[spec.pb.ops[0][1][3]]
+    g = spec.pb.tensors[spec.pb.ops[0][1].gamma_tensor]
+    bt = spec.pb.tensors[spec.pb.ops[0][1].beta_tensor]
     got = _layernorm_emulate(x, g, bt, 4000, 1e-5, two_pass)
     assert (_violations(got, spec.ref, spec.bound) == 0) == ok
 

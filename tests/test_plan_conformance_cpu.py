@@ -48,8 +48,8 @@ def psa_in_place(pb, msg):
     t, p, _ = pb.ops[i]
     j = int(msg.split(" over op ")[1].split("'")[0])
     tj, pj, _ = pb.ops[j]
-    return (t == tj == plan.OP_GEMM and p[8] >= 0 and p[3] == pj[3] == 1
-            and p[11] == pj[11] and p[12] == pj[12] + p[6] and pj[6] == 2 * p[6])
+    return (t == tj == plan.OP_GEMM and p.res_buf >= 0 and p.ntaps == pj.ntaps == 1
+            and p.out_buf == pj.out_buf and p.out_coff == pj.out_coff + p.N and pj.N == 2 * p.N)
 
 
 @pytest.mark.parametrize("family,scale,kw", DATAFLOW, ids=[f"{f}-{s}" + ("-" + kw["cfg"] if "cfg" in kw else "") for f, s, kw in DATAFLOW])
@@ -175,23 +175,23 @@ def _emulate(pb, i, bufs, rng):
     """Op i as an fp32 kernel with a shuffled accumulation order: exact fp16 products, fp32 sums in a random K order, fp32 bias and
     activation, stored in the buffer's dtype."""
     t, p, _ = pb.ops[i]
-    w = pb.tensors[p[4]].astype(np.float32)
-    bias = pb.tensors[p[5]].astype(np.float32)
-    if p[14]:
-        rows, C = pb.buffers[p[0]][:2]
-        x = bufs[p[0]][:B * rows].reshape(B, rows * C)[:, :p[2]].astype(np.float32)
-        cols = [x[:, k:k + 1] * w[:, k][None, :] for k in range(p[2])]                # [B, N] per k
+    w = pb.tensors[p.w_tensor].astype(np.float32)
+    bias = pb.tensors[p.bias_tensor].astype(np.float32)
+    if p.transposed:
+        rows, C = pb.buffers[p.a_buf][:2]
+        x = bufs[p.a_buf][:B * rows].reshape(B, rows * C)[:, :p.Kc].astype(np.float32)
+        cols = [x[:, k:k + 1] * w[:, k][None, :] for k in range(p.Kc)]                # [B, N] per k
     else:
-        rows, C, _, Hh, Ww = pb.buffers[p[0]][:5]
-        xp = bufs[p[0]][:B * rows].reshape(B, Hh + 2, Ww + 2, C)[..., p[1]:p[1] + p[2]].astype(np.float32)
-        wk = w.reshape(p[6], 3, 3, p[2])
-        cols = [xp[:, dy:dy + Hh, dx:dx + Ww, c:c + 1] * wk[:, dy, dx, c] for dy in range(3) for dx in range(3) for c in range(p[2])]
+        rows, C, _, Hh, Ww = pb.buffers[p.a_buf][:5]
+        xp = bufs[p.a_buf][:B * rows].reshape(B, Hh + 2, Ww + 2, C)[..., p.a_coff:p.a_coff + p.Kc].astype(np.float32)
+        wk = w.reshape(p.N, 3, 3, p.Kc)
+        cols = [xp[:, dy:dy + Hh, dx:dx + Ww, c:c + 1] * wk[:, dy, dx, c] for dy in range(3) for dx in range(3) for c in range(p.Kc)]
     acc = np.zeros_like(cols[0])
     for k in rng.permutation(len(cols)):
         acc = acc + cols[k]
     a = acc + bias
-    y = a / (np.float32(1) + np.exp(-a)) if p[7] == 1 else a
-    if p[14]:
+    y = a / (np.float32(1) + np.exp(-a)) if p.act == 1 else a
+    if p.transposed:
         return y.astype(np.float64)
     return y.transpose(0, 3, 1, 2).astype(np.float16).astype(np.float64)
 
@@ -235,33 +235,34 @@ def test_teeth_accepts_shuffled_fp32(teeth):
 def test_teeth_rejects_fc_prefetch_from_previous_batch(teeth):
     pb, (A, Bb) = teeth
     t, p, _ = pb.ops[1]
-    rows, C = pb.buffers[p[0]][:2]
-    x = Bb[p[0]][:B * rows].reshape(B, rows * C).astype(np.float64).copy()
-    x[:, :384] = A[p[0]][:B * rows].reshape(B, rows * C)[:, :384]
-    assert (x != Bb[p[0]][:B * rows].reshape(B, rows * C)).any()
-    w = pb.tensors[p[4]].astype(np.float64)
-    got = x @ w.T + pb.tensors[p[5]]
+    rows, C = pb.buffers[p.a_buf][:2]
+    x = Bb[p.a_buf][:B * rows].reshape(B, rows * C).astype(np.float64).copy()
+    x[:, :384] = A[p.a_buf][:B * rows].reshape(B, rows * C)[:, :384]
+    assert (x != Bb[p.a_buf][:B * rows].reshape(B, rows * C)).any()
+    w = pb.tensors[p.w_tensor].astype(np.float64)
+    got = x @ w.T + pb.tensors[p.bias_tensor]
     ref, bnd = pi.op_ref(pb, 1, Bb, B)
     assert pi.excess(got, ref, bnd)[0] > 1.0
 
 
 def _tile_fault(pb, A, Bb, from_a_inputs):
     """The conv's padded-row M tile [128, 256) of batch B: computed from batch A's input, or left at batch A's output."""
-    out = Bb[pb.ops[0][1][11]].copy()
+    conv = pb.ops[0][1]
+    out = Bb[conv.out_buf].copy()
     if from_a_inputs:
         redo = {k: v.copy() for k, v in Bb.items()}
-        redo[pb.ops[0][1][0]] = A[pb.ops[0][1][0]]
+        redo[conv.a_buf] = A[conv.a_buf]
         pi.write_out(pb, 0, redo, B, pi.op_ref(pb, 0, redo, B, want_bound=False)[0])
-        src = redo[pb.ops[0][1][11]]
+        src = redo[conv.out_buf]
     else:
-        src = A[pb.ops[0][1][11]]
+        src = A[conv.out_buf]
     rows = np.arange(out.shape[0])
     hp = (rows % ((H + 2) * (W_ + 2))) // (W_ + 2)
     wp = rows % (W_ + 2)
     sel = (rows >= 128) & (rows < 256) & (hp >= 1) & (hp <= H) & (wp >= 1) & (wp <= W_)
     out[sel] = src[sel].astype(out.dtype)
     bufs = dict(Bb)
-    bufs[pb.ops[0][1][11]] = out
+    bufs[conv.out_buf] = out
     ref, bnd = pi.op_ref(pb, 0, bufs, B)
     return pi.excess(pi.read_out(pb, 0, bufs, B), ref, bnd)
 
@@ -284,7 +285,9 @@ def test_teeth_rejects_neighbour_slice(teeth):
     t, p, f = pb.ops[0]
     pb2 = plan.PlanBuilder(pb.model_kind, 3, H, W_)
     pb2.buffers, pb2.tensors = pb.buffers, pb.tensors
-    pb2.ops = [(t, p[:1] + [p[1] + 64] + p[2:], f)] + pb.ops[1:]     # the conv reads channels [128, 192)
+    q = p.copy()
+    q.a_coff += 64                                                   # the conv reads channels [128, 192)
+    pb2.ops = [(t, q, f)] + pb.ops[1:]
     pi.write_out(pb, 0, moved, B, pi.op_ref(pb2, 0, Bb, B, want_bound=False)[0].astype(np.float16).astype(np.float64))
     ref, bnd = pi.op_ref(pb, 0, Bb, B)
     assert pi.excess(pi.read_out(pb, 0, moved, B), ref, bnd)[0] > 1.0

@@ -1,5 +1,7 @@
 """CPU: host logic of the packer (adas_b200.plan): graph restatements reproduce the published FLOP / parameter counts,
 BN folding and weight layout are right, the UFLD FC1 scatter matches view(-1, input_dim), the .b200w header parses."""
+import os
+import re
 import struct
 
 import numpy as np
@@ -59,8 +61,8 @@ def test_ufld_fc1_scatter_equals_flatten():
     W = plan.synth_weights("ufldv2", 1)
     pb = plan.build_ufldv2(W, "18")
     assert abs(pb.flops_per_img / 1e9 - (75.15 - 2 * (37.58 - 0.195 - 18.9))) < 60   # res18 is lighter; sanity only
-    fc1 = [op for op in pb.ops if op[0] == plan.OP_GEMM and op[1][14] == 1][0]
-    w1p = pb.tensors[fc1[1][4]].astype(np.float32)            # [2048, slab]
+    fc1 = [op for op in pb.ops if op[0] == plan.OP_GEMM and op[1].transposed == 1][0]
+    w1p = pb.tensors[fc1[1].w_tensor].astype(np.float32)            # [2048, slab]
     fh, fw = 10, 50
     fea = np.random.default_rng(0).standard_normal((8, fh, fw)).astype(np.float32)
     slab = np.zeros(((fh + 2), (fw + 2), 8), np.float32)
@@ -69,7 +71,7 @@ def test_ufld_fc1_scatter_equals_flatten():
     ref = W.state_dict["cls.1.weight"].astype(np.float16).astype(np.float32) @ fea.ravel()
     assert np.allclose(got, ref, atol=1e-3)
     ln = [op for op in pb.ops if op[0] == plan.OP_LAYERNORM][0]
-    assert ln[1][1] == (fh + 2) * (fw + 2) * 8 and ln[1][5] == 4000
+    assert ln[1].d_len == (fh + 2) * (fw + 2) * 8 and ln[1].d_norm == 4000
 
 
 def test_plan_file_header(tmp_path):
@@ -78,15 +80,14 @@ def test_plan_file_header(tmp_path):
     path = tmp_path / "v5n.b200w"
     pb.write(str(path))
     raw = path.read_bytes()
-    fmt = "<8sII3I4I16IQQ"
-    h = struct.unpack_from(fmt, raw)
+    h = struct.unpack_from(plan.HDR_FMT, raw)
     assert h[0] == b"B200PLAN" and h[1] == plan.PLAN_VERSION and h[2] == plan.MODEL_YOLOV5
     assert h[3:6] == (3, 640, 640)
     n_buf, n_ops, n_t, n_out = h[6:10]
     assert (n_buf, n_ops, n_t, n_out) == (len(pb.buffers), len(pb.ops), len(pb.tensors), 3)
     blob_off, blob_bytes = h[-2:]
     assert blob_off % 256 == 0 and blob_off + blob_bytes == len(raw)
-    assert struct.calcsize(fmt) + n_buf * 24 + n_ops * 112 + n_t * 24 + n_out * 16 <= blob_off
+    assert plan.HDR_SIZE + n_buf * plan.BUF_SIZE + n_ops * plan.OP_SIZE + n_t * plan.TEN_SIZE + n_out * plan.OUT_SIZE <= blob_off
 
 
 def test_tusimple_plan_geometry():
@@ -97,8 +98,8 @@ def test_tusimple_plan_geometry():
     assert (pb.in_h, pb.in_w) == (320, 800)
     assert not any(op[0] == plan.OP_LAYERNORM for op in pb.ops)                 # fc_norm = False: cls.0 is Identity
     assert "cls.0.weight" not in W.state_dict
-    fc1 = [op for op in pb.ops if op[0] == plan.OP_GEMM and op[1][14] == 1][0]
-    assert fc1[1][2] == (10 + 2) * (25 + 2) * 8                                  # reads the padded 10x25x8 pool slab directly
+    fc1 = [op for op in pb.ops if op[0] == plan.OP_GEMM and op[1].transposed == 1][0]
+    assert fc1[1].Kc == (10 + 2) * (25 + 2) * 8                                  # reads the padded 10x25x8 pool slab directly
     assert plan.build_ufldv2(plan.synth_weights("ufldv2", 0), "34").meta[6] == 0  # CULane
 
 
@@ -123,19 +124,17 @@ def test_engine_rejects_inconsistent_plans(tmp_path):
     good = tmp_path / "good.b200w"
     pb.write(str(good))
     raw = good.read_bytes()
-    hdr = struct.calcsize("<8sII3I4I16IQQ")
-    n_buf, n_ops = len(pb.buffers), len(pb.ops)
-    op0 = hdr + n_buf * 24
-    ten0 = op0 + n_ops * 112
+    pl = fp.parse(raw)
+    n_buf = len(pb.buffers)
     first_gemm = next(i for i, op in enumerate(pb.ops) if op[0] == plan.OP_GEMM)
     cases = {
-        "buffer index": fp.corrupt(raw, op0 + first_gemm * 112 + 4 + 4 * 11, "<i", n_buf + 7),          # out_buf of the first GEMM
-        "weight tensor index": fp.corrupt(raw, op0 + first_gemm * 112 + 4 + 4 * 4, "<i", 100000),
-        "channel slice": fp.corrupt(raw, op0 + first_gemm * 112 + 4 + 4 * 12, "<i", 1 << 20),            # out_coff
-        "tensor offset": fp.corrupt(raw, ten0, "<Q", 1 << 40),
+        "buffer index": fp.corrupt(raw, pl.field_off(first_gemm, "out_buf"), "<i", n_buf + 7),
+        "weight tensor index": fp.corrupt(raw, pl.field_off(first_gemm, "w_tensor"), "<i", 100000),
+        "channel slice": fp.corrupt(raw, pl.field_off(first_gemm, "out_coff"), "<i", 1 << 20),
+        "tensor offset": fp.corrupt(raw, pl.ten_off(0), "<Q", 1 << 40),
         "dataset id": fp.corrupt(raw, 8 + 4 * 2 + 4 * 3 + 4 * 4 + 4 * 6, "<I", 7),
         "dataset geometry": fp.corrupt(raw, 8 + 4 * 2 + 4 * 3 + 4 * 4 + 4 * 6, "<I", 0),                 # TuSimple heads labelled CULane
-        "op type": fp.corrupt(raw, op0 + 112, "<I", 99),
+        "op type": fp.corrupt(raw, pl.op_off(1), "<I", 99),
         "truncated blob": raw[:len(raw) - 4096],
     }
     for name, data in cases.items():
@@ -154,6 +153,59 @@ def test_engine_rejects_inconsistent_plans(tmp_path):
             _capi.Engine(str(good))
         except Exception as e:
             assert "no CUDA device" in str(e), str(e)
+
+
+def _plan_h_op_layout():
+    """PlanOpType's enumerators {name: value} and the op structs {name: (int32 fields, nested arrays [(name, fields, count)])} of
+    csrc/plan.h, in declaration order."""
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    src = re.sub(r"//[^\n]*", "", open(os.path.join(root, "vehicle-cv-adas_b200", "csrc", "plan.h")).read())
+    src = src[src.index("enum PlanOpType"):]                  # the op structs follow the enum (PlanOp itself precedes it)
+    enum = re.search(r"enum PlanOpType : uint32_t \{(.*?)\};", src, re.S).group(1)
+    values = {n: int(v) for n, v in re.findall(r"(OP_\w+)\s*=\s*(\d+)", enum)}
+    fields = lambda body: [n.strip() for decl in re.findall(r"int32_t ([^;]+);", body) for n in decl.split(",")]
+    structs = {}
+    for name, body in re.findall(r"struct (\w+Op) \{(.*?)\};", src, re.S):
+        nested = [(m[2], fields(m[1]), int(m[3])) for m in re.findall(r"struct (\w+) \{([^}]*)\} (\w+)\[(\d+)\];", body)]
+        structs[name] = (fields(re.sub(r"struct \w+ \{[^}]*\}[^;]*;", "", body)), nested)
+    return values, structs
+
+
+def test_plan_h_op_structs_match_op_fields():
+    """plan.h's op structs (what the loader reads) and plan.OP_FIELDS (what the packer and the tests write and read) name the same
+    fields in the same order; the op codes and record sizes agree."""
+    values, structs = _plan_h_op_layout()
+    assert len(values) == len(plan.OP_FIELDS) == len(plan.OP_NAMES) == 13
+    assert {getattr(plan, n) for n in values} == set(plan.OP_FIELDS) == set(plan.OP_NAMES)
+    assert sorted(structs) == sorted(n[3:].capitalize() + "Op" for n in values)          # OP_GEMM: GemmOp, OP_IM2COL: Im2colOp, ...
+    for n, v in values.items():
+        assert getattr(plan, n) == v, n
+        flat, nested = structs[n[3:].capitalize() + "Op"]
+        assert tuple(flat) == plan.OP_FIELDS[v], n
+        assert nested == ([("src", list(plan.CBFUSE_SRC_FIELDS), plan.CBFUSE_MAX_SRC)] if v == plan.OP_CBFUSE else []), n
+        assert len(flat) + sum(len(f) * c for _, f, c in nested) <= plan.OP_NP, n
+    assert (plan.HDR_SIZE, plan.BUF_SIZE, plan.OP_SIZE, plan.TEN_SIZE, plan.OUT_SIZE) == (124, 24, 112, 24, 16)
+
+
+def test_op_params_read_and_write_by_name():
+    p = plan.OpParams(plan.OP_SHUFFLE2, [1, 2, 3, 4, 8, 5, 16])
+    assert p == [1, 2, 3, 4, 8, 5, 16] + [0] * 16 and (p.b_buf, p.n, p.out_coff) == (3, 8, 16)
+    p.out_coff = 24
+    assert p == [1, 2, 3, 4, 8, 5, 24] + [0] * 16 and p.copy() == p and p.copy().typ == plan.OP_SHUFFLE2
+    for bad in (lambda: p.BN, lambda: setattr(p, "BN", 64)):
+        try:
+            bad()
+        except AttributeError as e:
+            assert "shuffle2 op has no field 'BN'" in str(e)
+        else:
+            raise AssertionError("a field of another op type was accepted")
+    pb = plan.PlanBuilder(plan.MODEL_YOLOV8, 3, 8, 8)
+    try:
+        pb._op(plan.OP_MAXPOOL, in_buf=0, out_coff=8, fill=1)
+    except AttributeError as e:
+        assert "maxpool op has no field 'fill'" in str(e)
+    else:
+        raise AssertionError("_op accepted a field the op does not have")
 
 
 def test_plan_cache_is_private(tmp_path, monkeypatch):

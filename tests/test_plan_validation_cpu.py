@@ -15,9 +15,6 @@ import plan_footprint as fp
 
 INT32_MAX = 2 ** 31 - 1
 REFUSALS = ("plan ", "truncated ", "Parameters must be a .b200w plan file")
-# parameters each op type reads (plan.h); CBFUSE adds 3 per source
-OP_FIELDS = {fp.OP_GEMM: 20, fp.OP_IM2COL: 8, fp.OP_MAXPOOL: 8, fp.OP_UPSAMPLE2X: 5, fp.OP_LAYERNORM: 6, fp.OP_STEMPACK: 2,
-             fp.OP_STEMCONV: 10, fp.OP_AVGPOOL2: 6, fp.OP_DWCONV: 12, fp.OP_ATTN: 7, fp.OP_CBFUSE: 6, fp.OP_SE: 10, fp.OP_SHUFFLE2: 7}
 
 FAMILIES = [
     ("v5n", lambda: plan.build_yolov5(plan.synth_weights("yolov5", 0, variant="n"), "n", in_h=256, in_w=256)),
@@ -67,6 +64,14 @@ def _values(v, neighbour, nb):
     return sorted(x for x in vals if x != v)
 
 
+def _op_fields(typ, p):
+    """Names of the fields the loader reads of an op, in slot order: its plan.OP_FIELDS, then the sources of a CBFUSE"""
+    names = plan.OP_FIELDS[typ]
+    if typ == plan.OP_CBFUSE:
+        names += tuple(f"src{s}.{n}" for s in range(max(0, min(p.n_src, plan.CBFUSE_MAX_SRC))) for n in plan.CBFUSE_SRC_FIELDS)
+    return names
+
+
 def _mutations(pl):
     """(description, byte offset, value) of every single-field corruption of the sweep"""
     nb = len(pl.bufs)
@@ -102,18 +107,17 @@ def _mutations(pl):
     # ops: the first of each (type, route) in the plan, every field it reads
     picked, routes = [], set()
     for oi, (typ, p, _) in enumerate(pl.ops):
-        route = (typ, p[3], p[8] >= 0, p[14], p[16], p[19]) if typ == fp.OP_GEMM else (typ,)
+        route = (typ, p.ntaps, p.res_buf >= 0, p.transposed, p.s2, p.up2) if typ == plan.OP_GEMM else (typ,)
         if route not in routes:
             routes.add(route)
             picked.append(oi)
     for oi in picked:
         typ, p, _ = pl.ops[oi]
-        n = OP_FIELDS.get(typ, 23) + (3 * max(0, min(p[5], 5)) if typ == fp.OP_CBFUSE else 0)
-        for f in range(n):
+        for f, name in enumerate(_op_fields(typ, p)):
             nbr = pl.ops[oi - 1][1][f] if oi else None
             for x in _values(p[f], nbr, nb):
                 if -2 ** 31 <= x <= INT32_MAX:
-                    out.append((f"op {oi} (type {typ}) p[{f}] {p[f]} -> {x}", pl.op_off(oi) + 4 + 4 * f, "<i", x))
+                    out.append((f"op {oi} (type {typ}) p[{f}] {name} {p[f]} -> {x}", pl.op_off(oi) + 4 + 4 * f, "<i", x))
     return out
 
 
@@ -250,10 +254,10 @@ def test_gemm_residual_must_have_the_output_geometry(tmp_path_factory, tmp_path)
     path = _write(tmp_path_factory, "v8n", dict(FAMILIES)["v8n"])
     pl = fp.parse(open(path, "rb").read())
     oi = next(i for i, (t, p, _) in enumerate(pl.ops)
-              if t == fp.OP_GEMM and p[8] >= 0 and pl.bufs[p[11]][3] == 64 and pl.bufs[p[11]][4] == 64)
+              if t == plan.OP_GEMM and p.res_buf >= 0 and pl.bufs[p.out_buf][3] == 64 and pl.bufs[p.out_buf][4] == 64)
     p = pl.ops[oi][1]
-    small = next(i for i, b in enumerate(pl.bufs) if b[3] == 16 and b[4] == 16 and b[2] == 0 and b[1] >= p[9] + p[6])
-    bad = _expect_refused(path, tmp_path, "v8-residual", pl.op_off(oi) + 4 + 4 * 8, "<i", small, "residual")
+    small = next(i for i, b in enumerate(pl.bufs) if b[3] == 16 and b[4] == 16 and b[2] == 0 and b[1] >= p.res_coff + p.N)
+    bad = _expect_refused(path, tmp_path, "v8-residual", pl.field_off(oi, "res_buf"), "<i", small, "residual")
     assert fp.out_of_bounds(bad, 1)
 
 

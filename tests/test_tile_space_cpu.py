@@ -41,7 +41,7 @@ def test_sweep_reaches_every_stage_count():
 @pytest.mark.parametrize("case", ts.SWEEP_CASES, ids=[c[0] for c in ts.SWEEP_CASES])
 def test_sweep_case_packs_onto_its_route(case):
     sw = ts.sweep_case(case)
-    N = sw.pb.ops[sw.ops[0][0]][1][6]
+    N = sw.pb.ops[sw.ops[0][0]][1].N
     assert [c for _, c, _ in sw.ops] == ts.tile_space(sw.route, N)
     want = {"slab": ("slab", "tap"), "im2col": ("im2col8", "im2col4")}.get(sw.route, (sw.route,))
     outs = set()
@@ -49,8 +49,8 @@ def test_sweep_case_packs_onto_its_route(case):
         p = sw.pb.ops[i][1]
         route = ts.op_route(sw.pb, i)
         assert route in want and (route == "tap") == bool(c.no_slab), (sw.name, i, route)
-        assert (p[15], p[17], p[18]) == (c.BN, c.MT, c.no_slab)
-        assert (p[11], p[12]) == (ob, coff) and coff == ts.OUT_OFF
+        assert (p.BN, p.MT, p.no_slab) == (c.BN, c.MT, c.no_slab)
+        assert (p.out_buf, p.out_coff) == (ob, coff) and coff == ts.OUT_OFF
         outs.add(ob)
     assert len(outs) == len(sw.ops)
     assert sw.bound.shape == sw.ref.shape and (sw.bound > 0).all() and np.isfinite(sw.ref).all()
@@ -60,8 +60,8 @@ def test_force_tile_on_fc_sets_only_the_mt_hint():
     pb, ops, _, _, _ = ts.fc_sweep(64, 40, 2, [1, 3])
     for i, mt, out in ops:
         p = pb.ops[i][1]
-        assert p[14] == 1 and p[15] == 0 and p[17] == mt and p[11] == out
-    assert pb.ops[0][1][4] == pb.ops[1][1][4]             # one weight tensor
+        assert p.transposed == 1 and p.BN == 0 and p.MT == mt and p.out_buf == out
+    assert pb.ops[0][1].w_tensor == pb.ops[1][1].w_tensor     # one weight tensor
 
 
 # ---- the bounds have teeth -----------------------------------------------------------------------------------------------------

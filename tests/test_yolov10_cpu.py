@@ -3,7 +3,6 @@ validation of the depthwise-conv and attention ops.
 
 The graphs restate ultralytics 8.2.41's yolov10{n,s,m,b,l,x}.yaml with the one-to-one head; the published counts are their anchor:
 parameters of the fused graph (the 16 fixed DFL weights included) and 2 * MAC of the convolutions at 640x640."""
-import struct
 
 import numpy as np
 import pytest
@@ -29,10 +28,10 @@ def test_yolov10_counts_match_the_published_figures(scale, mparams, gflop):
     assert pb.model_kind == plan.MODEL_YOLOV8 and pb.meta[:2] == [80, 8400] and len(pb.outputs) == 3
     assert sum(1 for op in pb.ops if op[0] == plan.OP_ATTN) == 1
     dw = [op for op in pb.ops if op[0] == plan.OP_DWCONV]
-    n_lk = sum(1 for op in dw if op[1][3] == 7)
+    n_lk = sum(1 for op in dw if op[1].k == 7)
     lk_blocks = [li for li, lk in plan.YOLOV10_CIB[scale].items() if lk]
     assert n_lk == len(lk_blocks) * plan._v8_n(3, plan.YOLOV10_SCALES[scale][0])
-    assert sum(1 for op in dw if op[1][4] == 2) == 3                          # the three SCDowns
+    assert sum(1 for op in dw if op[1].stride == 2) == 3                          # the three SCDowns
     assert 0 < pb.dw_flops_per_img < pb.flops_per_img
 
 
@@ -49,10 +48,10 @@ def test_packer_folds_equal_oracle_fuse(scale):
             c = m.conv
             v = g.repvggdw(plan.View(0, 0, (c.out_channels + 7) // 8 * 8, 8, 8), name, c.out_channels)
             op = pb.ops[-1]
-            wk = pb.tensors[op[1][6]].astype(np.float32)[:, :c.out_channels]
+            wk = pb.tensors[op[1].w_tensor].astype(np.float32)[:, :c.out_channels]
             ref = c.weight.detach().numpy().reshape(c.out_channels, 49).T
             assert np.abs(wk - ref).max() <= 1e-3 * max(1.0, float(np.abs(ref).max())) and v.C % 8 == 0
-            assert np.abs(pb.tensors[op[1][7]][:c.out_channels] - c.bias.detach().numpy()).max() < 1e-5
+            assert np.abs(pb.tensors[op[1].bias_tensor][:c.out_channels] - c.bias.detach().numpy()).max() < 1e-5
             n_rep += 1
         elif isinstance(m, o10.Conv):
             c = m.conv
@@ -148,31 +147,30 @@ def test_plan_validator_rejects_bad_dwconv_ops(tmp_path):
     pb.write(str(good))
     assert "no CUDA device" in fp.engine_error(good)
     raw = good.read_bytes()
-    op = struct.calcsize("<8sII3I4I16IQQ") + len(pb.buffers) * 24 + 4
-    p = lambda i: op + 4 * i
-    c = lambda i, v, r=raw: fp.corrupt(r, p(i), "<i", v)
+    off = lambda name: fp.parse(raw).field_off(0, name)
+    c = lambda name, v, r=raw: fp.corrupt(r, off(name), "<i", v)
     _check_cases(tmp_path, raw, [
-        ("input index", c(0, 99), "index out of range"),
-        ("output index", c(8, -1), "index out of range"),
-        ("residual index", c(10, 77), "index out of range"),
-        ("fp32 output", c(8, f32.buf), "fp16"),
-        ("fp32 residual", c(10, f32.buf), "fp16"),
-        ("kernel", c(3, 5), "dwconv k"),
-        ("stride", c(4, 3), "dwconv k"),
-        ("7x7 stride 2", c(4, 2, c(3, 7, c(6, w7))), "dwconv k"),
-        ("act", c(5, 2), "act"),
-        ("geometry", c(8, half.buf), "output geometry"),
-        ("channels", c(2, 12), "multiples of 8"),
-        ("input offset", c(1, 4), "multiples of 8"),
-        ("output offset", c(9, 12), "multiples of 8"),
-        ("residual offset", c(11, 4), "multiples of 8"),
-        ("weight size", c(3, 7), "weight tensor"),
-        ("bias tensor", c(7, 0), "bias tensor"),
-        ("residual geometry", c(10, half.buf), "residual"),
-        ("residual slice", c(11, 24), "residual"),
-        ("input slice", c(1, 56), "exceeds"),
-        ("output slice", c(9, 24), "exceeds"),
-        ("in place", c(9, 16, c(8, xin.buf)), "overlaps"),
+        ("input index", c("in_buf", 99), "index out of range"),
+        ("output index", c("out_buf", -1), "index out of range"),
+        ("residual index", c("res_buf", 77), "index out of range"),
+        ("fp32 output", c("out_buf", f32.buf), "fp16"),
+        ("fp32 residual", c("res_buf", f32.buf), "fp16"),
+        ("kernel", c("k", 5), "dwconv k"),
+        ("stride", c("stride", 3), "dwconv k"),
+        ("7x7 stride 2", c("stride", 2, c("k", 7, c("w_tensor", w7))), "dwconv k"),
+        ("act", c("act", 2), "act"),
+        ("geometry", c("out_buf", half.buf), "output geometry"),
+        ("channels", c("C", 12), "multiples of 8"),
+        ("input offset", c("in_coff", 4), "multiples of 8"),
+        ("output offset", c("out_coff", 12), "multiples of 8"),
+        ("residual offset", c("res_coff", 4), "multiples of 8"),
+        ("weight size", c("k", 7), "weight tensor"),
+        ("bias tensor", c("bias_tensor", 0), "bias tensor"),
+        ("residual geometry", c("res_buf", half.buf), "residual"),
+        ("residual slice", c("res_coff", 24), "residual"),
+        ("input slice", c("in_coff", 56), "exceeds"),
+        ("output slice", c("out_coff", 24), "exceeds"),
+        ("in place", c("out_coff", 16, c("out_buf", xin.buf)), "overlaps"),
     ])
 
 
@@ -188,25 +186,23 @@ def test_plan_validator_rejects_bad_attention_ops(tmp_path):
     pb.write(str(good))
     assert "no CUDA device" in fp.engine_error(good)
     raw = good.read_bytes()
-    op = struct.calcsize("<8sII3I4I16IQQ") + len(pb.buffers) * 24 + 4
-    p = lambda i: op + 4 * i
-    f0 = op + 4 * 23
-    c = lambda i, v, r=raw: fp.corrupt(r, p(i), "<i", v)
+    off = lambda name: fp.parse(raw).field_off(0, name)
+    c = lambda name, v, r=raw: fp.corrupt(r, off(name), "<i", v)
     _check_cases(tmp_path, raw, [
-        ("input index", c(0, 99), "index out of range"),
-        ("output index", c(5, -1), "index out of range"),
-        ("fp32 output", c(5, f32.buf), "fp16"),
-        ("geometry", c(5, half.buf), "H x W"),
-        ("heads", c(2, 0), "attention heads"),
-        ("kdp", c(3, 24), "attention heads"),
-        ("hd", c(4, 60), "attention heads"),
-        ("input offset", c(1, 4), "multiples of 8"),
-        ("output offset", c(6, 12), "multiples of 8"),
-        ("qkv slice", c(2, 3), "exceeds"),
-        ("output slice", c(6, 8), "exceeds"),
-        ("in place", c(5, qkv.buf), "overlaps"),
-        ("scale", fp.corrupt(raw, f0, "<f", float("nan")), "scale"),
-        ("negative scale", fp.corrupt(raw, f0, "<f", -1.0), "scale"),
+        ("input index", c("in_buf", 99), "index out of range"),
+        ("output index", c("out_buf", -1), "index out of range"),
+        ("fp32 output", c("out_buf", f32.buf), "fp16"),
+        ("geometry", c("out_buf", half.buf), "H x W"),
+        ("heads", c("nh", 0), "attention heads"),
+        ("kdp", c("kdp", 24), "attention heads"),
+        ("hd", c("hd", 60), "attention heads"),
+        ("input offset", c("in_coff", 4), "multiples of 8"),
+        ("output offset", c("out_coff", 12), "multiples of 8"),
+        ("qkv slice", c("nh", 3), "exceeds"),
+        ("output slice", c("out_coff", 8), "exceeds"),
+        ("in place", c("out_buf", qkv.buf), "overlaps"),
+        ("scale", fp.corrupt(raw, off("scale"), "<f", float("nan")), "scale"),
+        ("negative scale", fp.corrupt(raw, off("scale"), "<f", -1.0), "scale"),
     ])
 
 

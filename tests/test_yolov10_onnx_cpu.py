@@ -131,10 +131,10 @@ def test_class_branch_wider_than_its_input_and_not_a_multiple_of_8():
     W = plan.synth_weights("yolov10", 0, variant="n")
     pb = plan.build_yolov10(W, "n", nc=70, in_h=320, in_w=320)
     assert pb.meta[:2] == [70, 2100] and all(o[2] == 64 + 72 for o in pb.outputs)
-    dw72 = [p for t, p, _ in pb.ops if t == plan.OP_DWCONV and p[2] == 72]
+    dw72 = [p for t, p, _ in pb.ops if t == plan.OP_DWCONV and p.C == 72]
     assert len(dw72) == 3                                                  # one2one_cv3.i.1.0 per level
     for p in dw72:
-        assert not pb.tensors[p[6]][:, 70:].astype(np.float32).any() and not pb.tensors[p[7]][70:].any()
+        assert not pb.tensors[p.w_tensor][:, 70:].astype(np.float32).any() and not pb.tensors[p.bias_tensor][70:].any()
     # per level the 1x1 c3 -> c3 and c3 -> nc convs: 72 x 72 packed, zero past 70 rows and input channels
-    gemms = [pb.tensors[p[4]] for t, p, _ in pb.ops if t == plan.OP_GEMM and pb.tensors[p[4]].shape == (72, 72)]
+    gemms = [pb.tensors[p.w_tensor] for t, p, _ in pb.ops if t == plan.OP_GEMM and pb.tensors[p.w_tensor].shape == (72, 72)]
     assert len(gemms) == 6 and all(not g[70:].astype(np.float32).any() and not g[:, 70:].astype(np.float32).any() for g in gemms)

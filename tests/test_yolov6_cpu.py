@@ -3,7 +3,6 @@
 The graphs restate meituan/YOLOv6 0.4.0 (configs/yolov6{n,s,m,l}.py); with no upstream file available, the published deployed-model counts
 are their anchor.  The published GFLOP figures (thop, 2 * MAC at 640x640) count a ConvTranspose2d(k=2, s=2) at output elements x Cin x 4
 MACs, four times its algorithmic MACs; the plan counts algorithmic FLOP, so the check adds the difference back."""
-import struct
 
 import numpy as np
 import pytest
@@ -28,8 +27,8 @@ def _fused_params(W):
 
 
 def _transpose_flops(pb):
-    return sum(2 * pb.buffers[op[1][0]][3] * pb.buffers[op[1][0]][4] * op[1][2] * op[1][6] for op in pb.ops
-               if op[0] == plan.OP_GEMM and op[1][19] == 1)
+    return sum(2 * pb.buffers[p.a_buf][3] * pb.buffers[p.a_buf][4] * p.Kc * p.N for t, p, _ in pb.ops
+               if t == plan.OP_GEMM and p.up2 == 1)
 
 
 PUBLISHED = [("n", 11.4, 4.7), ("s", 45.3, 18.5), ("m", 85.8, 34.9), ("l", 150.7, 59.6)]
@@ -43,11 +42,11 @@ def test_yolov6_flops_match_published_counts(scale, gflop, mparams):
     assert abs(thop / 1e9 - gflop) < 0.05, thop / 1e9
     reg_max = 16 if scale in "ml" else 0
     assert pb.model_kind == plan.MODEL_YOLOV6 and pb.meta[:3] == [80, 8400, reg_max] and len(pb.outputs) == 3
-    gemm_acts = {op[1][7] for op in pb.ops if op[0] == plan.OP_GEMM and not pb.buffers[op[1][11]][2] and op[1][19] == 0}
+    gemm_acts = {p.act for t, p, _ in pb.ops if t == plan.OP_GEMM and not pb.buffers[p.out_buf][2] and p.up2 == 0}
     assert gemm_acts == ({plan.ACT_SILU, plan.ACT_RELU})
     stem = pb.ops[0]
-    assert stem[0] == plan.OP_STEMCONV and stem[1][6] == (plan.ACT_SILU if scale == "l" else plan.ACT_RELU)
-    assert sum(1 for op in pb.ops if op[0] == plan.OP_GEMM and op[1][19] == 1) == 2          # the two BiFusion transposed convs
+    assert stem[0] == plan.OP_STEMCONV and stem[1].act == (plan.ACT_SILU if scale == "l" else plan.ACT_RELU)
+    assert sum(1 for t, p, _ in pb.ops if t == plan.OP_GEMM and p.up2 == 1) == 2          # the two BiFusion transposed convs
     n_scaled = sum(1 for op in pb.ops if op[0] == plan.OP_GEMM and op[2][0] != 0.0)
     assert n_scaled == ({"m": 2 + 3 + 5 + 2 + 4 * 3, "l": 3 + 6 + 9 + 3 + 4 * 6}.get(scale, 0))   # BottleReps with their alpha
 
@@ -65,9 +64,9 @@ def test_yolov6_params_match_published_counts(scale, gflop, mparams):
 
 def test_activation_arguments_choose_the_epilogues():
     pb = plan.build_yolov6(plan.synth_weights("yolov6", 0), "s", act_body="silu", act_neck="silu", act_head="relu", in_h=320, in_w=320)
-    assert {op[1][7] for op in pb.ops if op[0] == plan.OP_GEMM and not pb.buffers[op[1][11]][2] and op[1][19] == 0} == {plan.ACT_SILU, plan.ACT_RELU}
+    assert {p.act for t, p, _ in pb.ops if t == plan.OP_GEMM and not pb.buffers[p.out_buf][2] and p.up2 == 0} == {plan.ACT_SILU, plan.ACT_RELU}
     pb = plan.build_yolov6(plan.synth_weights("yolov6", 0), "s", act_body="silu", act_neck="silu", act_head="silu", in_h=320, in_w=320)
-    assert {op[1][7] for op in pb.ops if op[0] == plan.OP_GEMM and not pb.buffers[op[1][11]][2] and op[1][19] == 0} == {plan.ACT_SILU}
+    assert {p.act for t, p, _ in pb.ops if t == plan.OP_GEMM and not pb.buffers[p.out_buf][2] and p.up2 == 0} == {plan.ACT_SILU}
 
 
 @pytest.mark.parametrize("scale", ["s", "m"])
@@ -131,18 +130,16 @@ def test_plan_validator_rejects_bad_yolov6_fields(tmp_path):
     pb.write(str(good))
     assert "no CUDA device" in fp.engine_error(good)
     raw = good.read_bytes()
-    hdr = struct.calcsize("<8sII3I4I16IQQ")
-    meta2 = 8 + 4 * 2 + 4 * 3 + 4 * 4 + 4 * 2
-    op0 = hdr + len(pb.buffers) * 24
-    up = next(i for i, op in enumerate(pb.ops) if op[0] == plan.OP_GEMM and op[1][19] == 1)
-    res = next(i for i, op in enumerate(pb.ops) if op[0] == plan.OP_GEMM and op[1][8] >= 0)
-    out_rec = hdr + len(pb.buffers) * 24 + len(pb.ops) * 112 + len(pb.tensors) * 24
+    pl = fp.parse(raw)
+    meta2 = 8 + 4 * fp.HEADER_FIELDS.index("meta2")
+    up = next(i for i, (t, p, _) in enumerate(pb.ops) if t == plan.OP_GEMM and p.up2 == 1)
+    res = next(i for i, (t, p, _) in enumerate(pb.ops) if t == plan.OP_GEMM and p.res_buf >= 0)
     cases = [
         ("reg_max", fp.corrupt(raw, meta2, "<I", 8), "reg_max"),
-        ("narrow level", fp.corrupt(raw, out_rec + 8, "<I", 72 + 79), "columns wide"),
-        ("transposed Cout", fp.corrupt(raw, op0 + up * 112 + 4 + 6 * 4, "<i", pb.ops[up][1][6] - 16), "transposed conv"),
-        ("transposed geometry", fp.corrupt(raw, op0 + up * 112 + 4 + 11 * 4, "<i", pb.ops[up][1][0]), "transposed conv"),
-        ("residual scale", fp.corrupt(raw, op0 + res * 112 + 4 + 23 * 4, "<f", float("inf")), "residual scale"),
+        ("narrow level", fp.corrupt(raw, pl.out_off(0) + 8, "<I", 72 + 79), "columns wide"),
+        ("transposed Cout", fp.corrupt(raw, pl.field_off(up, "N"), "<i", pb.ops[up][1].N - 16), "transposed conv"),
+        ("transposed geometry", fp.corrupt(raw, pl.field_off(up, "out_buf"), "<i", pb.ops[up][1].a_buf), "transposed conv"),
+        ("residual scale", fp.corrupt(raw, pl.field_off(res, "res_scale"), "<f", float("inf")), "residual scale"),
     ]
     for name, data, msg in cases:
         bad = tmp_path / "bad.b200w"

@@ -7,7 +7,6 @@ The graph restates upstream's configs (release 0.4.0); with no upstream file ava
 0.55 / 0.79 / 1.09 M for S / M / L.  The restatement has 0.558 / 0.791 / 1.099 M (DPBlock's convs carry a bias, as nn.Conv2d does by
 default); the published figures are these truncated to two decimals (without the DPBlock biases M would have 0.788 M)."""
 import hashlib
-import struct
 
 import numpy as np
 import pytest
@@ -21,9 +20,6 @@ import synth
 import yolov6_lite_oracle as ol
 from gpu_util import to_padded
 from oracle import post
-
-HDR = struct.calcsize("<8sII3I4I16IQQ")
-
 
 def _weights(scale, seed=0, **kw):
     W = plan.synth_weights("yolov6lite", seed, variant=scale)
@@ -53,12 +49,12 @@ def test_plan_shape():
     kinds = [t for t, _, _ in pb.ops]
     n_s1 = sum(n - 1 for n in plan.YOLOV6_LITE_BLOCKS)
     assert kinds.count(plan.OP_SE) == n_s1 + 4 and kinds.count(plan.OP_SHUFFLE2) == n_s1
-    assert kinds[0] == plan.OP_STEMCONV and pb.ops[0][1][3] == 24 and pb.ops[0][1][6] == plan.ACT_HSWISH
+    assert kinds[0] == plan.OP_STEMCONV and pb.ops[0][1].Cout == 24 and pb.ops[0][1].act == plan.ACT_HSWISH
     dws = [p for t, p, _ in pb.ops if t == plan.OP_DWCONV]
-    assert {(p[3], p[4]) for p in dws} == {(3, 1), (3, 2), (5, 1), (5, 2)}
+    assert {(p.k, p.stride) for p in dws} == {(3, 1), (3, 2), (5, 1), (5, 2)}
     assert plan.OP_IM2COL not in kinds                                          # every conv is a 1x1 GEMM, a depthwise or the stem
     # SE hidden widths: C // 4 of the real (unpadded) widths, C padded to 8
-    assert sorted({(p[2], p[3]) for t, p, _ in pb.ops if t == plan.OP_SE}) == [(8, 2), (16, 3), (24, 6), (48, 11), (48, 12), (88, 22)]
+    assert sorted({(p.C, p.hid) for t, p, _ in pb.ops if t == plan.OP_SE}) == [(8, 2), (16, 3), (24, 6), (48, 11), (48, 12), (88, 22)]
 
 
 def test_oracle_fused_equals_training_form():
@@ -81,13 +77,13 @@ def test_packer_folds_equal_oracle_fuse():
     packed = []
     for t, p, _ in pb.ops:
         if t == plan.OP_DWCONV:
-            C, k = p[2], p[3]
-            packed.append(("dw", pb.tensors[p[6]].astype(np.float64).T.reshape(C, k, k), pb.tensors[p[7]]))
+            C, k = p.C, p.k
+            packed.append(("dw", pb.tensors[p.w_tensor].astype(np.float64).T.reshape(C, k, k), pb.tensors[p.bias_tensor]))
         elif t == plan.OP_STEMCONV:
-            packed.append(("stem", pb.tensors[p[1]][:, :, :12].astype(np.float64).reshape(24, 3, 3, 4)[..., :3].transpose(0, 3, 1, 2),
-                           pb.tensors[p[2]]))
+            packed.append(("stem", pb.tensors[p.w_tensor][:, :, :12].astype(np.float64).reshape(24, 3, 3, 4)[..., :3].transpose(0, 3, 1, 2),
+                           pb.tensors[p.bias_tensor]))
         elif t == plan.OP_GEMM:
-            packed.append(("gemm", pb.tensors[p[4]].astype(np.float64), pb.tensors[p[5]]))
+            packed.append(("gemm", pb.tensors[p.w_tensor].astype(np.float64), pb.tensors[p.bias_tensor]))
     se = [m for m in fused.modules() if isinstance(m, ol.SEBlock)]
     assert len(packed) + 2 * len(se) == len(convs)
     # match each packed conv to the oracle conv of its bias (the head's box / class convs share a filled bias: then also by weights)
@@ -207,8 +203,8 @@ def test_se_and_shuffle_references():
 # ---------------------------------------------------------------------------------------------------------------------------
 
 
-def _op_field(pb, i, k):
-    return HDR + len(pb.buffers) * 24 + i * 112 + 4 + 4 * k
+def _op_field(raw, i, name):
+    return fp.parse(raw).field_off(i, name)
 
 
 def _check(tmp_path, raw, cases):
@@ -236,26 +232,26 @@ def test_plan_validator_rejects_bad_se_ops(tmp_path):
     pb.write(str(good))
     assert "no CUDA device" in fp.engine_error(good)
     raw = good.read_bytes()
-    p = lambda k: _op_field(pb, 0, k)
+    p = lambda name: _op_field(raw, 0, name)
     _check(tmp_path, raw, [
-        ("input index", fp.corrupt(raw, p(0), "<i", 99), "index out of range"),
-        ("output index", fp.corrupt(raw, p(8), "<i", -1), "index out of range"),
-        ("fp32 input", fp.corrupt(fp.corrupt(raw, p(0), "<i", f32.buf), p(8), "<i", f32.buf), "fp16"),
-        ("geometry", fp.corrupt(raw, p(8), "<i", other.buf), "H x W"),
-        ("channels", fp.corrupt(raw, p(2), "<i", 12), "channels"),
-        ("too many channels", fp.corrupt(raw, p(2), "<i", 1032), "channels"),
-        ("no hidden", fp.corrupt(raw, p(3), "<i", 0), "hidden"),
-        ("hidden 257", fp.corrupt(raw, p(3), "<i", 257), "hidden"),
-        ("offset", fp.corrupt(fp.corrupt(raw, p(1), "<i", 4), p(9), "<i", 4), "multiples of 8"),
-        ("w1 size", fp.corrupt(raw, p(4), "<i", 1), "se tensor 0"),
-        ("w2 is b2", fp.corrupt(raw, p(6), "<i", 3), "se tensor 2"),
-        ("fp16 tensor", fp.corrupt(raw, p(5), "<i", f16), "se tensor 1"),
-        ("tensor index", fp.corrupt(raw, p(7), "<i", 99), "se tensor 3"),
-        ("slice", fp.corrupt(fp.corrupt(raw, p(1), "<i", 24), p(9), "<i", 24), "exceeds"),
-        ("partial overlap", fp.corrupt(raw, p(9), "<i", 16), "overlaps"),
+        ("input index", fp.corrupt(raw, p("in_buf"), "<i", 99), "index out of range"),
+        ("output index", fp.corrupt(raw, p("out_buf"), "<i", -1), "index out of range"),
+        ("fp32 input", fp.corrupt(fp.corrupt(raw, p("in_buf"), "<i", f32.buf), p("out_buf"), "<i", f32.buf), "fp16"),
+        ("geometry", fp.corrupt(raw, p("out_buf"), "<i", other.buf), "H x W"),
+        ("channels", fp.corrupt(raw, p("C"), "<i", 12), "channels"),
+        ("too many channels", fp.corrupt(raw, p("C"), "<i", 1032), "channels"),
+        ("no hidden", fp.corrupt(raw, p("hid"), "<i", 0), "hidden"),
+        ("hidden 257", fp.corrupt(raw, p("hid"), "<i", 257), "hidden"),
+        ("offset", fp.corrupt(fp.corrupt(raw, p("in_coff"), "<i", 4), p("out_coff"), "<i", 4), "multiples of 8"),
+        ("w1 size", fp.corrupt(raw, p("w1"), "<i", 1), "se tensor 0"),
+        ("w2 is b2", fp.corrupt(raw, p("w2"), "<i", 3), "se tensor 2"),
+        ("fp16 tensor", fp.corrupt(raw, p("b1"), "<i", f16), "se tensor 1"),
+        ("tensor index", fp.corrupt(raw, p("b2"), "<i", 99), "se tensor 3"),
+        ("slice", fp.corrupt(fp.corrupt(raw, p("in_coff"), "<i", 24), p("out_coff"), "<i", 24), "exceeds"),
+        ("partial overlap", fp.corrupt(raw, p("out_coff"), "<i", 16), "overlaps"),
     ])
     ok = tmp_path / "ok.b200w"
-    ok.write_bytes(fp.corrupt(raw, p(8), "<i", out.buf))                                   # out of place
+    ok.write_bytes(fp.corrupt(raw, p("out_buf"), "<i", out.buf))                                   # out of place
     assert "no CUDA device" in fp.engine_error(ok)
 
 
@@ -270,19 +266,19 @@ def test_plan_validator_rejects_bad_shuffle2_ops(tmp_path):
     pb.write(str(good))
     assert "no CUDA device" in fp.engine_error(good)
     raw = good.read_bytes()
-    p = lambda k: _op_field(pb, 0, k)
+    p = lambda name: _op_field(raw, 0, name)
     _check(tmp_path, raw, [
-        ("a index", fp.corrupt(raw, p(0), "<i", 99), "index out of range"),
-        ("b index", fp.corrupt(raw, p(2), "<i", -1), "index out of range"),
-        ("out index", fp.corrupt(raw, p(5), "<i", 99), "index out of range"),
-        ("fp32 source", fp.corrupt(raw, p(2), "<i", f32.buf), "fp16"),
-        ("geometry", fp.corrupt(raw, p(0), "<i", other.buf), "H x W"),
-        ("channels", fp.corrupt(raw, p(4), "<i", 12), "multiples of 8"),
-        ("no channels", fp.corrupt(raw, p(4), "<i", 0), "multiples of 8"),
-        ("offset", fp.corrupt(raw, p(1), "<i", 4), "multiples of 8"),
-        ("source slice", fp.corrupt(raw, p(3), "<i", 40), "exceeds"),
-        ("output slice", fp.corrupt(raw, p(6), "<i", 16), "exceeds"),
-        ("output over a source", fp.corrupt(fp.corrupt(raw, p(5), "<i", src.buf), p(6), "<i", 16), "overlaps"),
+        ("a index", fp.corrupt(raw, p("a_buf"), "<i", 99), "index out of range"),
+        ("b index", fp.corrupt(raw, p("b_buf"), "<i", -1), "index out of range"),
+        ("out index", fp.corrupt(raw, p("out_buf"), "<i", 99), "index out of range"),
+        ("fp32 source", fp.corrupt(raw, p("b_buf"), "<i", f32.buf), "fp16"),
+        ("geometry", fp.corrupt(raw, p("a_buf"), "<i", other.buf), "H x W"),
+        ("channels", fp.corrupt(raw, p("n"), "<i", 12), "multiples of 8"),
+        ("no channels", fp.corrupt(raw, p("n"), "<i", 0), "multiples of 8"),
+        ("offset", fp.corrupt(raw, p("a_coff"), "<i", 4), "multiples of 8"),
+        ("source slice", fp.corrupt(raw, p("b_coff"), "<i", 40), "exceeds"),
+        ("output slice", fp.corrupt(raw, p("out_coff"), "<i", 16), "exceeds"),
+        ("output over a source", fp.corrupt(fp.corrupt(raw, p("out_buf"), "<i", src.buf), p("out_coff"), "<i", 16), "overlaps"),
     ])
 
 
@@ -295,24 +291,21 @@ def test_activation_codes(tmp_path, op):
     x = pb.new_padded(16, 16, 32)
     if op == "gemm":
         pb.conv(x, rng.standard_normal((32, 32, 1, 1)).astype(np.float32), np.zeros(32, np.float32), 1, 1, plan.ACT_HSWISH)
-        k = 7
     elif op == "stem":
         pb.conv(pb.image, rng.standard_normal((24, 3, 3, 3)).astype(np.float32), np.zeros(24, np.float32), 3, 2, plan.ACT_HSWISH)
-        k = 6
     else:
         pb.dwconv(x, rng.standard_normal((32, 1, 5, 5)).astype(np.float32), np.zeros(32, np.float32), 5, 2, plan.ACT_HSWISH)
-        k = 5
     assert pb.ops[-1][0] == {"gemm": plan.OP_GEMM, "stem": plan.OP_STEMCONV, "dwconv": plan.OP_DWCONV}[op]
     good = tmp_path / f"{op}.b200w"
     pb.write(str(good))
     assert "no CUDA device" in fp.engine_error(good)
     raw = good.read_bytes()
-    f = _op_field(pb, len(pb.ops) - 1, k)
+    f = _op_field(raw, len(pb.ops) - 1, "act")
     msg = "dwconv act" if op == "dwconv" else "unknown activation"
     _check(tmp_path, raw, [(f"act {a}", fp.corrupt(raw, f, "<i", a), f"{msg} {a}") for a in (4, 6, -1)])
     if op == "dwconv":
-        _check(tmp_path, raw, [("k 5 stride 3", fp.corrupt(raw, _op_field(pb, 0, 4), "<i", 3), "dwconv k 5 stride 3"),
-                               ("k 9", fp.corrupt(raw, _op_field(pb, 0, 3), "<i", 9), "dwconv k 9")])
+        _check(tmp_path, raw, [("k 5 stride 3", fp.corrupt(raw, _op_field(raw, 0, "stride"), "<i", 3), "dwconv k 5 stride 3"),
+                               ("k 9", fp.corrupt(raw, _op_field(raw, 0, "k"), "<i", 9), "dwconv k 9")])
 
 
 @no_gpu
@@ -324,8 +317,7 @@ def test_four_level_head_validation(tmp_path):
     pb.write(str(good))
     assert "no CUDA device" in fp.engine_error(good)
     raw = good.read_bytes()
-    nb, no, nt = len(pb.buffers), len(pb.ops), len(pb.tensors)
-    out = lambda i, k: HDR + nb * 24 + no * 112 + nt * 24 + i * 16 + 4 * k
+    out = lambda i, k: fp.parse(raw).out_off(i) + 4 * k
     _check(tmp_path, raw, [
         ("P6 grid of the P5 level", fp.corrupt(raw, out(3, 0), "<i", pb.outputs[2][0]), "YOLOv6 head has 3 levels"),
         ("P6 stride 32", fp.corrupt(raw, out(3, 3), "<i", 32), "YOLOv6 head has 3 levels"),

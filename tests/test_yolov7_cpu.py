@@ -4,7 +4,6 @@ The graphs restate cfg/training/yolov7.yaml and yolov7-tiny.yaml; with no upstre
 anchor (FLOP = 2 * MAC of the fused graph at 640x640).  ONNX files are written by torch's exporter from the oracle (tests/yolov7_oracle.py)
 after the upstream-style fuse(), at 320x320 to keep CPU time short."""
 import os
-import struct
 
 import numpy as np
 import pytest
@@ -31,15 +30,15 @@ def test_yolov7_graph_matches_published_counts(scale, gflop, mparams):
     assert pb.model_kind == plan.MODEL_YOLOV5 and pb.meta[:3] == [80, 25200, 0] and len(pb.outputs) == 3
     anc = plan.YOLOV7_ANCHORS if scale == "base" else plan.YOLOV5_ANCHORS
     assert np.array_equal(pb.tensors[pb.meta[3] - 1], np.asarray(anc, np.float32).reshape(18))
-    acts = {op[1][7] for op in pb.ops if op[0] == plan.OP_GEMM and not pb.buffers[op[1][11]][2]}
+    acts = {op[1].act for op in pb.ops if op[0] == plan.OP_GEMM and not pb.buffers[op[1].out_buf][2]}
     assert acts == {plan.ACT_LEAKY if scale == "tiny" else plan.ACT_SILU}
-    stem = pb.ops[0]                               # the image conv runs in stem_conv.cu: stride 1 (base, p[9] = 1) or 2 (tiny, p[9] = 0)
-    assert stem[0] == plan.OP_STEMCONV and stem[1][3] == 32 and stem[1][9] == (1 if scale == "base" else 0)
+    stem = pb.ops[0]                               # the image conv runs in stem_conv.cu: stride 1 (base, field 1) or 2 (tiny, field 0)
+    assert stem[0] == plan.OP_STEMCONV and stem[1].Cout == 32 and stem[1].stride == (1 if scale == "base" else 0)
 
 
 def test_tiny_silu_variant():
     pb = plan.build_yolov7(plan.synth_weights("yolov7", 0), "tiny", act="silu")
-    assert {op[1][7] for op in pb.ops if op[0] == plan.OP_GEMM and op[1][7] != plan.ACT_NONE} == {plan.ACT_SILU}
+    assert {p.act for t, p, _ in pb.ops if t == plan.OP_GEMM and p.act != plan.ACT_NONE} == {plan.ACT_SILU}
 
 
 def test_packer_folds_equal_oracle_fuse():
@@ -154,10 +153,9 @@ def test_anchor_table_and_activation_validation(tmp_path):
     assert np.array_equal(plan.read_anchors(str(v7)), np.asarray(plan.YOLOV7_ANCHORS, np.float32).reshape(3, 3, 2))
     # a non-positive anchor, an anchor index outside the tensors, an anchor table on a lite plan: rejected at load
     raw = v7.read_bytes()
-    hdr = struct.calcsize("<8sII3I4I16IQQ")
-    t_rec = hdr + len(pb.buffers) * 24 + len(pb.ops) * 112 + (pb.meta[3] - 1) * 24
-    blob = struct.unpack_from("<Q", raw, hdr - 16)[0]
-    off = struct.unpack_from("<Q", raw, t_rec)[0]
+    pl = fp.parse(raw)
+    blob = pl.header[-2]
+    off = pl.tensors[pb.meta[3] - 1][0]
     meta3 = 8 + 4 * 2 + 4 * 3 + 4 * 4 + 4 * 3
     for name, data in (("negative anchor", fp.corrupt(raw, blob + off + 8, "<f", -4.0)),
                        ("nan anchor", fp.corrupt(raw, blob + off, "<f", float("nan"))),
@@ -176,6 +174,6 @@ def test_anchor_table_and_activation_validation(tmp_path):
         b1.write(str(p))
         assert b1.ops[-1][0] == (plan.OP_STEMCONV if image else plan.OP_GEMM)
         assert "unknown activation 4" in fp.engine_error(p)
-        b1.ops[-1][1][6 if image else 7] = plan.ACT_LEAKY
+        b1.ops[-1][1].act = plan.ACT_LEAKY
         b1.write(str(p))
         assert "no CUDA device" in fp.engine_error(p)

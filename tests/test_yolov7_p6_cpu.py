@@ -40,7 +40,7 @@ def test_p6_graph_matches_published_counts(scale, gflop, mparams):
     assert pb.model_kind == plan.MODEL_YOLOV5 and pb.meta[:3] == [80, 102000, 0] and [o[3] for o in pb.outputs] == [8, 16, 32, 64]
     assert np.array_equal(pb.tensors[pb.meta[3] - 1], np.asarray(plan.YOLOV7_P6_ANCHORS, np.float32).reshape(24))
     stem = pb.ops[0]                      # ReOrg + 3x3 as one 6x6 stride-2 pad-2 conv in stem_conv.cu
-    assert stem[0] == plan.OP_STEMCONV and stem[1][3:6] == [{"w6": 64, "d6": 96}.get(scale, 80), 6, 2] and stem[1][9] == 0
+    assert stem[0] == plan.OP_STEMCONV and (stem[1].Cout, stem[1].k, stem[1].pad) == ({"w6": 64, "d6": 96}.get(scale, 80), 6, 2) and stem[1].stride == 0
     assert 0 <= gflop - pb.flops_per_img / 1e9 < 0.002 * gflop
     assert abs(_fused_params(W) / 1e6 - mparams) < 0.05
 
@@ -74,7 +74,7 @@ def test_packer_folds_equal_oracle_fuse(scale):
     w6 = np.zeros((stem.out_channels, 4, 6, 6), np.float32)
     w6[:, :3] = plan.reorg_stem_weights(stem.weight.detach().numpy())
     KR = 32
-    packed = pb.tensors[pb.ops[0][1][1]].astype(np.float32).reshape(stem.out_channels, 6, KR)[:, :, :24]
+    packed = pb.tensors[pb.ops[0][1].w_tensor].astype(np.float32).reshape(stem.out_channels, 6, KR)[:, :, :24]
     assert np.array_equal(packed, np.transpose(w6, (0, 2, 3, 1)).reshape(stem.out_channels, 6, 24).astype(np.float16).astype(np.float32))
 
 

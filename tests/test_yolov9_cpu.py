@@ -2,7 +2,6 @@
 
 The graphs restate WongKinYiu/yolov9 v0.1's converted (GELAN) models; with no upstream file available, the published counts are their
 anchor: parameters of the fused graph (grouped convs at their grouped size, the 16 fixed DFL weights included) and 2 * MAC at 640x640."""
-import struct
 
 import numpy as np
 import pytest
@@ -28,7 +27,7 @@ def test_yolov9_counts_match_the_published_figures(scale, mparams, gflop):
     assert pb.model_kind == plan.MODEL_YOLOV8 and pb.meta[:2] == [80, 8400] and len(pb.outputs) == 3
     n_pool = sum(1 for op in pb.ops if op[0] == plan.OP_AVGPOOL2)
     assert n_pool == (10 if scale == "c" else 5)                     # ADown: one per half; AConv: one
-    assert sum(1 for op in pb.ops if op[0] == plan.OP_AVGPOOL2 and op[1][5] == 1) == (5 if scale == "c" else 0)
+    assert sum(1 for op in pb.ops if op[0] == plan.OP_AVGPOOL2 and op[1].fill == 1) == (5 if scale == "c" else 0)
 
 
 def test_grouped_conv_packs_as_block_diagonal():
@@ -91,7 +90,7 @@ def test_fused_checkpoint_packs_the_training_form_plan():
 
 
 def _gemm_weights(pb, shape):
-    return [pb.tensors[op[1][4]].astype(np.float32) for op in pb.ops if op[0] == plan.OP_GEMM and pb.tensors[op[1][4]].shape == shape]
+    return [pb.tensors[op[1].w_tensor].astype(np.float32) for op in pb.ops if op[0] == plan.OP_GEMM and pb.tensors[op[1].w_tensor].shape == shape]
 
 
 def test_yolov9m_aligned_layout_equals_the_oracle_weights():
@@ -117,7 +116,7 @@ def test_yolov9m_aligned_layout_equals_the_oracle_weights():
     assert np.array_equal(w[:180, :90], ref[:, :90]) and np.array_equal(w[:180, 96:186], ref[:, 90:])
     assert not w[:, 90:96].any() and not w[:, 186:].any() and not w[180:].any()
     # every GEMM reads and writes at multiples of 8 channels
-    assert all(op[1][1] % 8 == 0 and op[1][12] % 8 == 0 for op in pb.ops if op[0] == plan.OP_GEMM)
+    assert all(op[1].a_coff % 8 == 0 and op[1].out_coff % 8 == 0 for op in pb.ops if op[0] == plan.OP_GEMM)
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="load-time validation is observed through the missing-device error")
@@ -132,20 +131,19 @@ def test_plan_validator_rejects_bad_avgpool2_ops(tmp_path):
     pb.write(str(good))
     assert "no CUDA device" in fp.engine_error(good)
     raw = good.read_bytes()
-    op = struct.calcsize("<8sII3I4I16IQQ") + len(pb.buffers) * 24 + 4          # p[0] of the one op
-    p = lambda i: op + 4 * i
+    p = lambda name: fp.parse(raw).field_off(0, name)
     cases = [
-        ("input index", fp.corrupt(raw, p(0), "<i", 99), "index out of range"),
-        ("output index", fp.corrupt(raw, p(3), "<i", -1), "index out of range"),
-        ("fp32 output", fp.corrupt(raw, p(3), "<i", f32.buf), "fp16"),
-        ("geometry", fp.corrupt(raw, p(3), "<i", other.buf), "H x W"),
-        ("channels", fp.corrupt(raw, p(2), "<i", 12), "multiples of 8"),
-        ("input offset", fp.corrupt(raw, p(1), "<i", 4), "multiples of 8"),
-        ("output offset", fp.corrupt(raw, p(4), "<i", 12), "multiples of 8"),
-        ("input slice", fp.corrupt(raw, p(1), "<i", 56), "exceeds"),
-        ("output slice", fp.corrupt(raw, p(4), "<i", 24), "exceeds"),
-        ("in place", fp.corrupt(fp.corrupt(raw, p(3), "<i", xin.buf), p(4), "<i", 16), "overlaps"),
-        ("fill", fp.corrupt(raw, p(5), "<i", 2), "fill"),
+        ("input index", fp.corrupt(raw, p("in_buf"), "<i", 99), "index out of range"),
+        ("output index", fp.corrupt(raw, p("out_buf"), "<i", -1), "index out of range"),
+        ("fp32 output", fp.corrupt(raw, p("out_buf"), "<i", f32.buf), "fp16"),
+        ("geometry", fp.corrupt(raw, p("out_buf"), "<i", other.buf), "H x W"),
+        ("channels", fp.corrupt(raw, p("C"), "<i", 12), "multiples of 8"),
+        ("input offset", fp.corrupt(raw, p("in_coff"), "<i", 4), "multiples of 8"),
+        ("output offset", fp.corrupt(raw, p("out_coff"), "<i", 12), "multiples of 8"),
+        ("input slice", fp.corrupt(raw, p("in_coff"), "<i", 56), "exceeds"),
+        ("output slice", fp.corrupt(raw, p("out_coff"), "<i", 24), "exceeds"),
+        ("in place", fp.corrupt(fp.corrupt(raw, p("out_buf"), "<i", xin.buf), p("out_coff"), "<i", 16), "overlaps"),
+        ("fill", fp.corrupt(raw, p("fill"), "<i", 2), "fill"),
     ]
     for name, data, msg in cases:
         bad = tmp_path / "bad.b200w"

@@ -4,7 +4,6 @@ the per-element CBFuse bound of plan_interp.
 
 The graph restates upstream's `models/detect/gelan-e.yaml` (v0.1); with no upstream file available, the published counts are its
 anchor: 57.3 M parameters and 189.0 GFLOP (YOLOv9-E, fused) and 58.1 M parameters (GELAN-E, training form)."""
-import struct
 
 import numpy as np
 import pytest
@@ -42,11 +41,11 @@ def test_yolov9e_counts_match_the_published_figures():
     assert (n_fused, n_train) == (261, 309) == (plan.yolov9_conv_count("e"), 261 + plan.yolov9_repconvn_count("e"))
     assert pb.model_kind == plan.MODEL_YOLOV8 and pb.meta[:2] == [80, 8400] and len(pb.outputs) == 3
     fuses = [op for op in pb.ops if op[0] == plan.OP_CBFUSE]
-    assert [p[5] for _, p, _ in fuses] == [5, 4, 3, 2, 1]
-    assert all(p[0] == p[3] and p[1] == p[4] for _, p, _ in fuses)                         # in place
-    assert [p[2] for _, p, _ in fuses] == [64, 128, 256, 512, 1024]
+    assert [p.n_src for _, p, _ in fuses] == [5, 4, 3, 2, 1]
+    assert all(p.out_buf == p.base_buf and p.out_coff == p.base_coff for _, p, _ in fuses)    # in place
+    assert [p.C for _, p, _ in fuses] == [64, 128, 256, 512, 1024]
     # the two image convs run in stem_conv.cu
-    assert sum(1 for t, p, _ in pb.ops if t == plan.OP_STEMCONV and p[3] == 64) == 2
+    assert sum(1 for t, p, _ in pb.ops if t == plan.OP_STEMCONV and p.Cout == 64) == 2
 
 
 def test_oracle_fused_equals_training_form():
@@ -79,14 +78,14 @@ def test_packer_folds_equal_oracle_fuse():
             continue
         assert np.abs(w - c.weight.detach().numpy()).max() < 1e-5 and np.abs(b - c.bias.detach().numpy()).max() < 1e-5, name
     assert n_rep == 48 and n_conv > 0
-    gemms = {pb.tensors[p[4]].shape: p for t, p, _ in pb.ops                   # the head's final 1x1 convs store fp32
-             if t == plan.OP_GEMM and p[7] == plan.ACT_NONE and pb.buffers[p[11]][2] == 0}
+    gemms = {pb.tensors[p.w_tensor].shape: p for t, p, _ in pb.ops             # the head's final 1x1 convs store fp32
+             if t == plan.OP_GEMM and p.act == plan.ACT_NONE and pb.buffers[p.out_buf][2] == 0}
     assert len(gemms) == 5
     for i, (cin, cout) in enumerate(((64, 64), (256, 192), (512, 448), (1024, 960), (1024, 1984))):
         p = gemms[(cout, cin)]
         w = fused.model[10 + i].conv.weight.detach().numpy()[:, :, 0, 0]
-        assert np.array_equal(pb.tensors[p[4]], w.astype(np.float16))
-        assert np.array_equal(pb.tensors[p[5]], fused.model[10 + i].conv.bias.detach().numpy())
+        assert np.array_equal(pb.tensors[p.w_tensor], w.astype(np.float16))
+        assert np.array_equal(pb.tensors[p.bias_tensor], fused.model[10 + i].conv.bias.detach().numpy())
 
 
 def test_fused_checkpoint_packs_the_training_form_plan():
@@ -180,28 +179,27 @@ def test_plan_validator_rejects_bad_cbfuse_ops(tmp_path):
     pb.write(str(good))
     assert "no CUDA device" in fp.engine_error(good)
     raw = good.read_bytes()
-    op = struct.calcsize("<8sII3I4I16IQQ") + len(pb.buffers) * 24 + 4          # p[0] of the one op
-    p = lambda i: op + 4 * i
+    p = lambda name: fp.parse(raw).field_off(0, name)
     cases = [
-        ("output index", fp.corrupt(raw, p(0), "<i", 99), "index out of range"),
-        ("base index", fp.corrupt(raw, p(3), "<i", -1), "index out of range"),
-        ("source index", fp.corrupt(raw, p(9), "<i", 99), "index out of range"),
-        ("fp32 source", fp.corrupt(raw, p(6), "<i", f32.buf), "fp16"),
-        ("fp32 output", fp.corrupt(fp.corrupt(raw, p(0), "<i", f32.buf), p(3), "<i", f32.buf), "fp16"),
-        ("no sources", fp.corrupt(raw, p(5), "<i", 0), "sources"),
-        ("six sources", fp.corrupt(raw, p(5), "<i", 6), "sources"),
-        ("shift 5", fp.corrupt(raw, p(11), "<i", 5), "shift"),
-        ("negative shift", fp.corrupt(raw, p(8), "<i", -1), "shift"),
-        ("shift + 1", fp.corrupt(raw, p(11), "<i", 2), "geometry"),
-        ("shift - 1", fp.corrupt(raw, p(14), "<i", 1), "geometry"),
-        ("base geometry", fp.corrupt(raw, p(3), "<i", other.buf), "output's H x W"),
-        ("channels", fp.corrupt(raw, p(2), "<i", 12), "multiples of 8"),
-        ("output offset", fp.corrupt(fp.corrupt(raw, p(1), "<i", 4), p(4), "<i", 4), "multiples of 8"),
-        ("source offset", fp.corrupt(raw, p(7), "<i", 4), "multiples of 8"),
-        ("output slice", fp.corrupt(fp.corrupt(raw, p(1), "<i", 40), p(4), "<i", 40), "exceeds"),
-        ("source slice", fp.corrupt(raw, p(7), "<i", 24), "exceeds"),
-        ("source is the output", fp.corrupt(fp.corrupt(raw, p(6), "<i", out.buf), p(7), "<i", 16), "overlaps"),
-        ("base overlaps the output", fp.corrupt(raw, p(4), "<i", 16), "overlaps"),
+        ("output index", fp.corrupt(raw, p("out_buf"), "<i", 99), "index out of range"),
+        ("base index", fp.corrupt(raw, p("base_buf"), "<i", -1), "index out of range"),
+        ("source index", fp.corrupt(raw, p("src1.buf"), "<i", 99), "index out of range"),
+        ("fp32 source", fp.corrupt(raw, p("src0.buf"), "<i", f32.buf), "fp16"),
+        ("fp32 output", fp.corrupt(fp.corrupt(raw, p("out_buf"), "<i", f32.buf), p("base_buf"), "<i", f32.buf), "fp16"),
+        ("no sources", fp.corrupt(raw, p("n_src"), "<i", 0), "sources"),
+        ("six sources", fp.corrupt(raw, p("n_src"), "<i", 6), "sources"),
+        ("shift 5", fp.corrupt(raw, p("src1.shift"), "<i", 5), "shift"),
+        ("negative shift", fp.corrupt(raw, p("src0.shift"), "<i", -1), "shift"),
+        ("shift + 1", fp.corrupt(raw, p("src1.shift"), "<i", 2), "geometry"),
+        ("shift - 1", fp.corrupt(raw, p("src2.shift"), "<i", 1), "geometry"),
+        ("base geometry", fp.corrupt(raw, p("base_buf"), "<i", other.buf), "output's H x W"),
+        ("channels", fp.corrupt(raw, p("C"), "<i", 12), "multiples of 8"),
+        ("output offset", fp.corrupt(fp.corrupt(raw, p("out_coff"), "<i", 4), p("base_coff"), "<i", 4), "multiples of 8"),
+        ("source offset", fp.corrupt(raw, p("src0.coff"), "<i", 4), "multiples of 8"),
+        ("output slice", fp.corrupt(fp.corrupt(raw, p("out_coff"), "<i", 40), p("base_coff"), "<i", 40), "exceeds"),
+        ("source slice", fp.corrupt(raw, p("src0.coff"), "<i", 24), "exceeds"),
+        ("source is the output", fp.corrupt(fp.corrupt(raw, p("src0.buf"), "<i", out.buf), p("src0.coff"), "<i", 16), "overlaps"),
+        ("base overlaps the output", fp.corrupt(raw, p("base_coff"), "<i", 16), "overlaps"),
     ]
     for name, data, msg in cases:
         bad = tmp_path / "bad.b200w"
@@ -210,7 +208,7 @@ def test_plan_validator_rejects_bad_cbfuse_ops(tmp_path):
         assert err is not None and "plan" in err and msg in err, (name, err)
     # out of place (base in another buffer) is valid
     ok = tmp_path / "ok.b200w"
-    ok.write_bytes(fp.corrupt(raw, p(3), "<i", s0.buf))
+    ok.write_bytes(fp.corrupt(raw, p("base_buf"), "<i", s0.buf))
     assert "no CUDA device" in fp.engine_error(ok)
 
 
@@ -286,9 +284,9 @@ def _emulate(pb, bufs, drop=None, shift_delta=(None, 0), coff_delta=(None, 0), b
         ys, xs = np.minimum(np.arange(HT) >> s, H - 1), np.minimum(np.arange(WT) >> s, W - 1)
         return v[:, ys][:, :, xs]
     dt = np.float16 if f16_acc else np.float32
-    base = view(p[3], p[4], 0).astype(dt)
+    base = view(p.base_buf, p.base_coff, 0).astype(dt)
     acc = base + base if base_twice else base
-    for k, (buf, coff, s) in enumerate(pi.cbfuse_sources(p)):
+    for k, (buf, coff, s) in enumerate(plan.cbfuse_sources(p)):
         if k == drop:
             continue
         s = s + (shift_delta[1] if shift_delta[0] == k else 0)

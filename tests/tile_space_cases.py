@@ -60,7 +60,7 @@ def stages(BN: int, MT: int, slab: bool) -> int:
 class Config:
     BN: int
     MT: int
-    no_slab: int = 0          # the plan field p[18]
+    no_slab: int = 0          # the GEMM plan field no_slab
     slab: int = 0             # what the kernel runs: slab mode only for 3x3 stride-1 convs that fit
     stages: int = 0
 
@@ -97,14 +97,14 @@ def tile_space(route: str, N: int) -> List[Config]:
 
 
 def force_tile(pb, op_index: int, BN: int, MT: int, no_slab: int = 0) -> None:
-    """Write the tile fields of a packed GEMM op: p[15] BN, p[17] MT hint, p[18] per-tap loads.  The swap-AB FC takes only p[17]: its
-    BN follows the batch."""
+    """Write the tile fields of a packed GEMM op: BN, the MT hint and no_slab (per-tap loads).  The swap-AB FC takes only MT: its BN
+    follows the batch."""
     t, p, _ = pb.ops[op_index]
     assert t == plan.OP_GEMM, t
-    if not p[14]:
-        p[15] = BN
-        p[18] = no_slab
-    p[17] = MT
+    if not p.transposed:
+        p.BN = BN
+        p.no_slab = no_slab
+    p.MT = MT
 
 
 def clone_gemm(pb, op_index: int, out) -> int:
@@ -112,8 +112,8 @@ def clone_gemm(pb, op_index: int, out) -> int:
     shared."""
     t, p, f = pb.ops[op_index]
     assert t == plan.OP_GEMM
-    q = list(p)
-    q[11], q[12] = out.buf, out.coff
+    q = p.copy()
+    q.out_buf, q.out_coff = out.buf, out.coff
     pb.ops.append((t, q, list(f)))
     return len(pb.ops) - 1
 
@@ -121,7 +121,7 @@ def clone_gemm(pb, op_index: int, out) -> int:
 def op_route(pb, i: int) -> Optional[str]:
     """oc.plan_route of GEMM op i alone, with the op that feeds it (IM2COL / STEMPACK) when there is one."""
     t, p, _ = pb.ops[i]
-    pre = [op for op in pb.ops if op[0] in (plan.OP_IM2COL, plan.OP_STEMPACK) and op[1][{plan.OP_IM2COL: 7, plan.OP_STEMPACK: 1}[op[0]]] == p[0]]
+    pre = [op for op in pb.ops if op[0] in (plan.OP_IM2COL, plan.OP_STEMPACK) and op[1].out_buf == p.a_buf]
     return oc.plan_route(SimpleNamespace(pb=SimpleNamespace(ops=pre[:1] + [pb.ops[i]])))
 
 
@@ -189,7 +189,7 @@ def _fan_out(sw, new_out, configs):
         i = first if j == 0 else clone_gemm(sw.pb, first, new_out())
         force_tile(sw.pb, i, c.BN, c.MT, c.no_slab)
         p = sw.pb.ops[i][1]
-        sw.ops.append((i, c, (p[11], p[12])))
+        sw.ops.append((i, c, (p.out_buf, p.out_coff)))
 
 
 def _up2_sweep(name, B, H, W, cin, in_off, cout, rng) -> Sweep:
@@ -219,7 +219,7 @@ def _stem_sweep(name, B, H, W, cout, act, rng) -> Sweep:
     # the builder's output is a buffer of its own: move every op (the first included) to a slice of a wider buffer
     first = max(i for i, (t, _, _) in enumerate(pb.ops) if t == plan.OP_GEMM)
     ov = oc.view(pb, o.H, o.W, cout, OUT_OFF)
-    pb.ops[first][1][11], pb.ops[first][1][12] = ov.buf, ov.coff
+    pb.ops[first][1].out_buf, pb.ops[first][1].out_coff = ov.buf, ov.coff
     _fan_out(sw, lambda: oc.view(pb, o.H, o.W, cout, OUT_OFF), tile_space("stem7x7s2", cout))
     return sw
 

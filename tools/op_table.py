@@ -33,8 +33,7 @@ else:
 eng = _capi.Engine(path, 0, max_batch=B)
 eng.run(B)
 n = eng.num_steps(B)
-names = {1: "gemm", 2: "im2col", 3: "maxpool", 4: "upsample", 5: "layernorm", 6: "stempack", 7: "stemconv", 8: "avgpool2", 9: "dwconv", 10: "attention",
-         11: "cbfuse", 12: "se", 13: "shuffle2", 31: "(folded)"}
+names = {**plan.OP_NAMES, 31: "(folded)"}
 tot = 0.0; tot_g = 0.0; rows = []
 for i in range(n):
     ms, t, d = eng.time_step(B, i, iters)
@@ -55,7 +54,7 @@ ms_g, ng = eng.time_ops(B, 1 << 1, 10)
 print(f"back-to-back: all {ms_all * 1e3:.1f} us ({nl} launches), gemm only {ms_g * 1e3:.1f} us ({ng}) -> {flops / ms_g / 1e9:.1f} TFLOP/s, "
       f"plan only {B / ms_all * 1e3:.0f} images/s")
 ms_ap = sum(r[0] for r in rows if r[2] == "avgpool2")
-ms_ic = sum(r[0] for r in rows if r[2] == "im2col" and pb.ops[r[1]][1][2] < 64)        # one launch per plan op; im2col p[2] = Cin
+ms_ic = sum(r[0] for r in rows if r[2] == "im2col" and pb.ops[r[1]][1].Cin < 64)        # one launch per plan op
 print(f"share of the sum of isolated launches: avgpool2 {100 * ms_ap / tot:.1f} %, im2col of convs with < 64 input channels {100 * ms_ic / tot:.1f} %")
 dw_rows = [r for r in rows if r[2] == "dwconv"]
 if dw_rows:
@@ -64,9 +63,9 @@ if dw_rows:
     dw_bytes = 0                              # fp16 input + output (+ residual) of every depthwise launch, weights once: computed from shapes
     for r in dw_rows:
         p = pb.ops[r[1]][1]
-        bi, bo = pb.buffers[p[0]], pb.buffers[p[8]]
-        C, k = p[2], p[3]
-        dw_bytes += 2 * B * C * (bi[3] * bi[4] + bo[3] * bo[4] * (2 if p[10] >= 0 else 1)) + C * (2 * k * k + 4)
+        bi, bo = pb.buffers[p.in_buf], pb.buffers[p.out_buf]
+        C, k = p.C, p.k
+        dw_bytes += 2 * B * C * (bi[3] * bi[4] + bo[3] * bo[4] * (2 if p.res_buf >= 0 else 1)) + C * (2 * k * k + 4)
     print(f"share of the sum of isolated launches: dwconv {100 * ms_dw / tot:.1f} %, attention {100 * ms_at / tot:.1f} %; "
           f"dwconv {dw_bytes / 1e6:.1f} MB in {ms_dw * 1e3:.1f} us -> {dw_bytes / ms_dw / 1e6:.0f} GB/s (HBM3 data sheet: 3350 GB/s)")
 cb_rows = [r for r in rows if r[2] == "cbfuse"]
@@ -75,8 +74,8 @@ if cb_rows:
     cb_bytes = 0                              # fp16: the target read and written once, each source read once at its own resolution
     for r in cb_rows:
         p = pb.ops[r[1]][1]
-        ob = pb.buffers[p[0]]
-        cb_bytes += 2 * B * p[2] * ob[3] * ob[4] * 2 + sum(2 * B * p[2] * pb.buffers[p[6 + 3 * s]][3] * pb.buffers[p[6 + 3 * s]][4] for s in range(p[5]))
+        ob = pb.buffers[p.out_buf]
+        cb_bytes += 2 * B * p.C * ob[3] * ob[4] * 2 + sum(2 * B * p.C * pb.buffers[sb][3] * pb.buffers[sb][4] for sb, _, _ in plan.cbfuse_sources(p))
     print(f"share of the sum of isolated launches: cbfuse {100 * ms_cb / tot:.1f} %; cbfuse {cb_bytes / 1e6:.1f} MB in {ms_cb * 1e3:.1f} us -> "
           f"{cb_bytes / ms_cb / 1e6:.0f} GB/s (HBM3 data sheet: 3350 GB/s)")
 se_rows = [r for r in rows if r[2] in ("se", "shuffle2")]
@@ -87,8 +86,12 @@ if se_rows:
         nbytes = 0                            # its fp32 FC weights once per image; SHUFFLE2 reads two n-channel slices and writes 2n channels
         for r in (r for r in rows if r[2] == k):
             p = pb.ops[r[1]][1]
-            b = pb.buffers[p[0]]
-            nbytes += 2 * B * b[3] * b[4] * 3 * p[2] + B * 4 * (2 * p[2] * p[3] + p[2] + p[3]) if k == "se" else 2 * B * b[3] * b[4] * 4 * p[4]
+            if k == "se":
+                b = pb.buffers[p.in_buf]
+                nbytes += 2 * B * b[3] * b[4] * 3 * p.C + B * 4 * (2 * p.C * p.hid + p.C + p.hid)
+            else:
+                b = pb.buffers[p.a_buf]
+                nbytes += 2 * B * b[3] * b[4] * 4 * p.n
         print(f"{k}: {nbytes / 1e6:.2f} MB in {share[k] * 1e3:.1f} us -> {nbytes / share[k] / 1e6:.0f} GB/s (HBM3 data sheet: 3350 GB/s)")
     act = sum(B * rows_ * C * (4 if f32 else 2) for rows_, C, f32, _, _, _ in pb.buffers)
     wts = sum(t.nbytes for t in pb.tensors)

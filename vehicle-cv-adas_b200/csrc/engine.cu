@@ -124,47 +124,42 @@ static const void* tensor_ptr(const adas_engine* e, int idx) {
 static int build_program(adas_engine* e, int batch, Program* prog) {
     for (size_t oi = 0; oi < e->ops.size(); ++oi) {
         const PlanOp& op = e->ops[oi];
-        const int32_t* p = op.p;
         prog->step_type.push_back(op.type);
         switch (op.type) {
             case OP_GEMM: {
-                const int a_buf = p[0], a_coff = p[1], Kc = p[2], ntaps = p[3], w_t = p[4], bias_t = p[5], N = p[6], act = p[7];
-                const int res_buf = p[8], res_coff = p[9], res_pre = p[10], out_buf = p[11], out_coff = p[12], masked = p[13];
-                const int transposed = p[14];
-                int BN = p[15];
-                const int s2 = p[16];
-                const int up2 = p[19];
-                const PlanBuffer& ab = e->bufs[a_buf];
-                const PlanBuffer& ob = e->bufs[out_buf];
+                const GemmOp o = op_fields<GemmOp>(op);
+                int BN = o.BN;
+                const PlanBuffer& ab = e->bufs[o.a_buf];
+                const PlanBuffer& ob = e->bufs[o.out_buf];
                 ADAS_CHECK(ab.dtype == 0, "op %zu: GEMM input buffer must be fp16", oi);
-                ADAS_CHECK(Kc % 8 == 0 && a_coff % 8 == 0 && ab.C % 8 == 0, "op %zu: K alignment", oi);
-                ADAS_CHECK(ntaps == 1 || ((ntaps == 9 || ntaps == 4) && Kc % 64 == 0 && ab.W > 0), "op %zu: tap mode needs Cin %% 64 == 0", oi);
-                ADAS_CHECK(!s2 || (Kc % 64 == 0 && ab.W > 0 && ob.W > 0 && !transposed), "op %zu: stride-2 mode needs Cin %% 64 == 0 on padded grids", oi);
+                ADAS_CHECK(o.Kc % 8 == 0 && o.a_coff % 8 == 0 && ab.C % 8 == 0, "op %zu: K alignment", oi);
+                ADAS_CHECK(o.ntaps == 1 || ((o.ntaps == 9 || o.ntaps == 4) && o.Kc % 64 == 0 && ab.W > 0), "op %zu: tap mode needs Cin %% 64 == 0", oi);
+                ADAS_CHECK(!o.s2 || (o.Kc % 64 == 0 && ab.W > 0 && ob.W > 0 && !o.transposed), "op %zu: stride-2 mode needs Cin %% 64 == 0 on padded grids", oi);
                 GemmParams g;
                 memset(&g, 0, sizeof(g));
-                const int Ktot = ntaps * Kc;
-                const __half* wptr = static_cast<const __half*>(tensor_ptr(e, w_t));
-                ADAS_CHECK((size_t)e->tensors[w_t].bytes >= (size_t)(transposed ? N : N) * Ktot * 2, "op %zu: weight tensor too small", oi);
-                const __half* aptr = static_cast<const __half*>(e->dbufs[a_buf].ptr) + a_coff;
+                const int Ktot = o.ntaps * o.Kc;
+                const __half* wptr = static_cast<const __half*>(tensor_ptr(e, o.w_tensor));
+                ADAS_CHECK((size_t)e->tensors[o.w_tensor].bytes >= (size_t)o.N * Ktot * 2, "op %zu: weight tensor too small", oi);
+                const __half* aptr = static_cast<const __half*>(e->dbufs[o.a_buf].ptr) + o.a_coff;
                 const int a_rows = batch * (int)ab.rows_per_img;
                 const void *opA, *opB;
                 uint64_t a_inner, a_rows_u, a_stride, b_inner, b_rows_u, b_stride;
-                if (!transposed) {
+                if (!o.transposed) {
                     g.M = a_rows;
-                    g.N = N;
-                    if (BN <= 0 && !s2) {           // a starting point only: the v3 path ranks / times its own tile candidates below
-                        if (N <= 256) BN = (N + 15) / 16 * 16;
-                        else if (N % 256 == 0) BN = 256;
-                        else if (N % 160 == 0) BN = 160;
-                        else if (N % 128 == 0) BN = 128;
+                    g.N = o.N;
+                    if (BN <= 0 && !o.s2) {         // a starting point only: the v3 path ranks / times its own tile candidates below
+                        if (o.N <= 256) BN = (o.N + 15) / 16 * 16;
+                        else if (o.N % 256 == 0) BN = 256;
+                        else if (o.N % 160 == 0) BN = 160;
+                        else if (o.N % 128 == 0) BN = 128;
                         else BN = 256;
                     }
-                    opA = aptr; a_inner = (uint64_t)Kc; a_rows_u = (uint64_t)a_rows; a_stride = (uint64_t)ab.C * 2;
-                    opB = wptr; b_inner = (uint64_t)Ktot; b_rows_u = (uint64_t)N; b_stride = (uint64_t)Ktot * 2;
+                    opA = aptr; a_inner = (uint64_t)o.Kc; a_rows_u = (uint64_t)a_rows; a_stride = (uint64_t)ab.C * 2;
+                    opB = wptr; b_inner = (uint64_t)Ktot; b_rows_u = (uint64_t)o.N; b_stride = (uint64_t)Ktot * 2;
                     g.A = aptr; g.a_ld = (int)ab.C; g.Wt = wptr; g.w_ld = Ktot;
                     g.out_ld = (int)ob.C;
-                    ADAS_CHECK(s2 || up2 || (int)ob.rows_per_img == (int)ab.rows_per_img, "op %zu: GEMM in/out row geometry differs", oi);
-                    if (s2) {
+                    ADAS_CHECK(o.s2 || o.up2 || (int)ob.rows_per_img == (int)ab.rows_per_img, "op %zu: GEMM in/out row geometry differs", oi);
+                    if (o.s2) {
                         // output-pixel patch (bw x bh <= 128) that wastes the fewest rows of the 128-row MMA tile
                         const int Ho = (int)ob.H, Wo = (int)ob.W;
                         int best_bw = 8, best_bh = 16; double best_eff = -1.0;
@@ -183,66 +178,66 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
                         g.s2_Ho = Ho; g.s2_Wo = Wo; g.s2_Hp_in = (int)ab.H + 2;
                         if (e->conv_impl == 1) g.M = batch * (int)ob.rows_per_img;        // SIMT kernel walks output rows
                         else g.M = batch * g.s2_tw * g.s2_th * 128;                         // wgmma kernel walks patches
-                        if (p[15] <= 0) BN = N <= 256 ? (N + 15) / 16 * 16 : (N % 256 == 0 ? 256 : 128);
+                        if (o.BN <= 0) BN = o.N <= 256 ? (o.N + 15) / 16 * 16 : (o.N % 256 == 0 ? 256 : 128);
                     }
                 } else {
                     // swap-AB: rows = output features (weights stream once through the A operand), cols = batch rows
                     // FC semantics: ONE input vector per image -- the whole per-image slab of the input buffer (a dense [1, K] row, or a
                     // padded feature map read flat: its halo entries are zeros that meet zero weight columns)
                     const uint64_t x_ld = (uint64_t)ab.rows_per_img * ab.C;
-                    g.M = N;
+                    g.M = o.N;
                     g.N = batch;
                     BN = (batch + 15) / 16 * 16;
                     ADAS_CHECK(BN <= 256, "op %zu: transposed GEMM supports at most 256 images per batch", oi);
-                    ADAS_CHECK((uint64_t)Kc <= x_ld && a_coff == 0 && (x_ld * 2) % 16 == 0, "op %zu: FC input vector exceeds its buffer", oi);
-                    opA = wptr; a_inner = (uint64_t)Ktot; a_rows_u = (uint64_t)N; a_stride = (uint64_t)Ktot * 2;
-                    opB = aptr; b_inner = (uint64_t)Kc; b_rows_u = (uint64_t)batch; b_stride = x_ld * 2;
+                    ADAS_CHECK((uint64_t)o.Kc <= x_ld && o.a_coff == 0 && (x_ld * 2) % 16 == 0, "op %zu: FC input vector exceeds its buffer", oi);
+                    opA = wptr; a_inner = (uint64_t)Ktot; a_rows_u = (uint64_t)o.N; a_stride = (uint64_t)Ktot * 2;
+                    opB = aptr; b_inner = (uint64_t)o.Kc; b_rows_u = (uint64_t)batch; b_stride = x_ld * 2;
                     g.A = wptr; g.a_ld = Ktot; g.Wt = aptr; g.w_ld = (int)x_ld;
                     g.out_ld = (int)(ob.rows_per_img * ob.C);
                 }
-                if (p[17] > 0) g.mt_hint = p[17];       // plan-forced sub-tile count (test hook of plan.py)
-                g.no_slab = p[18];                      // plan-forced per-tap operand loads (test hook of plan.py)
+                if (o.MT > 0) g.mt_hint = o.MT;         // plan-forced sub-tile count (test hook of plan.py)
+                g.no_slab = o.no_slab;                  // plan-forced per-tap operand loads (test hook of plan.py)
                 // Fully connected layers whose weight matrix stays in L2 (FC1 of the UFLD head: 20 MB; up to half of the H100's 50 MB) run
                 // as a weight stream on the CUDA cores: the swap-AB tensor-core GEMM has only N/256 CTAs for them.
                 static const bool fc_stream_on = !(getenv("ADAS_B200_FC_STREAM") && getenv("ADAS_B200_FC_STREAM")[0] == '0');
-                if (transposed && e->conv_impl == 0 && fc_stream_on && ntaps == 1 && (size_t)N * Kc * 2 <= ((size_t)25 << 20) && Kc % 8 == 0 && ab.C % 8 == 0) {
-                    const float* bias_p = static_cast<const float*>(tensor_ptr(e, bias_t));
-                    void* out_p = static_cast<uint8_t*>(e->dbufs[out_buf].ptr) + (size_t)out_coff * elem_size(ob.dtype);
+                if (o.transposed && e->conv_impl == 0 && fc_stream_on && o.ntaps == 1 && (size_t)o.N * o.Kc * 2 <= ((size_t)25 << 20) && o.Kc % 8 == 0 && ab.C % 8 == 0) {
+                    const float* bias_p = static_cast<const float*>(tensor_ptr(e, o.bias_tensor));
+                    void* out_p = static_cast<uint8_t*>(e->dbufs[o.out_buf].ptr) + (size_t)o.out_coff * elem_size(ob.dtype);
                     const int x_ld = (int)(ab.rows_per_img * ab.C), o_ld = (int)(ob.rows_per_img * ob.C), of32 = ob.dtype == 1 ? 1 : 0;
                     char d[128];
-                    snprintf(d, sizeof(d), "M=%d N=%d K=%d fc_stream", batch, N, Kc);
+                    snprintf(d, sizeof(d), "M=%d N=%d K=%d fc_stream", batch, o.N, o.Kc);
                     prog->step_desc.resize(prog->step_type.size());
                     prog->step_desc.back() = d;
-                    prog->steps.push_back([=](cudaStream_t st) { return launch_fc_stream(aptr, x_ld, batch, wptr, Kc, N, bias_p, act, out_p, o_ld, of32, st); });
+                    prog->steps.push_back([=](cudaStream_t st) { return launch_fc_stream(aptr, x_ld, batch, wptr, o.Kc, o.N, bias_p, o.act, out_p, o_ld, of32, st); });
                     break;
                 }
-                g.Kc = Kc; g.ntaps = ntaps; g.Wp = (int)ab.W + 2; g.kpt = (Kc + 63) / 64; g.BN = BN;
-                g.act = act; g.out_f32 = ob.dtype == 1 ? 1 : 0;
-                g.transposed = transposed;
-                g.up2 = up2;
-                g.res_scale = op.f[0] == 0.f ? 1.f : op.f[0];     // f[0] = 0 (plans without the field): plain residual add
-                g.bias = static_cast<const float*>(tensor_ptr(e, bias_t));
-                if (res_buf >= 0) {
-                    const PlanBuffer& rb = e->bufs[res_buf];
-                    g.res = static_cast<const __half*>(e->dbufs[res_buf].ptr) + res_coff;
-                    g.res_ld = res_pre ? -(int)rb.C : (int)rb.C;
+                g.Kc = o.Kc; g.ntaps = o.ntaps; g.Wp = (int)ab.W + 2; g.kpt = (o.Kc + 63) / 64; g.BN = BN;
+                g.act = o.act; g.out_f32 = ob.dtype == 1 ? 1 : 0;
+                g.transposed = o.transposed;
+                g.up2 = o.up2;
+                g.res_scale = op.f[0] == 0.f ? 1.f : op.f[0];     // f[0] = res_scale; 0 (plans without the field): plain residual add
+                g.bias = static_cast<const float*>(tensor_ptr(e, o.bias_tensor));
+                if (o.res_buf >= 0) {
+                    const PlanBuffer& rb = e->bufs[o.res_buf];
+                    g.res = static_cast<const __half*>(e->dbufs[o.res_buf].ptr) + o.res_coff;
+                    g.res_ld = o.res_pre_act ? -(int)rb.C : (int)rb.C;
                 }
-                g.out = static_cast<uint8_t*>(e->dbufs[out_buf].ptr) + (size_t)out_coff * elem_size(ob.dtype);
-                if (masked) { g.mask_H = (int)ob.H; g.mask_W = (int)ob.W; ADAS_CHECK(ob.H > 0, "op %zu: masked store into a dense buffer", oi); }
-                if (up2) { g.mask_H = (int)ab.H; g.mask_W = (int)ab.W; }     // the mask walks the INPUT grid; stores go to the 2H x 2W output
+                g.out = static_cast<uint8_t*>(e->dbufs[o.out_buf].ptr) + (size_t)o.out_coff * elem_size(ob.dtype);
+                if (o.masked) { g.mask_H = (int)ob.H; g.mask_W = (int)ob.W; ADAS_CHECK(ob.H > 0, "op %zu: masked store into a dense buffer", oi); }
+                if (o.up2) { g.mask_H = (int)ab.H; g.mask_W = (int)ab.W; }     // the mask walks the INPUT grid; stores go to the 2H x 2W output
                 if (e->conv_impl == 0) {
                     // ---- product path: gemm_v3.cu ----
                     void* opaque = nullptr;
                     const uint64_t a_Wp = (uint64_t)ab.W + 2, a_Hp = (uint64_t)ab.H + 2, a_ldC = (uint64_t)ab.C;
                     std::function<int(const GemmParams&, void**)> prep = [=](const GemmParams& gc, void** out) -> int {
-                        if (s2) return gemm_v3_prepare_s2(gc, aptr, (uint64_t)Kc, a_Wp, a_Hp, (uint64_t)batch, a_ldC, opB, b_inner, b_rows_u, b_stride, out);
+                        if (o.s2) return gemm_v3_prepare_s2(gc, aptr, (uint64_t)o.Kc, a_Wp, a_Hp, (uint64_t)batch, a_ldC, opB, b_inner, b_rows_u, b_stride, out);
                         return gemm_v3_prepare(gc, opA, a_inner, a_rows_u, a_stride, opB, b_inner, b_rows_u, b_stride, out);
                     };
-                    if (!transposed && p[15] <= 0) {
+                    if (!o.transposed && o.BN <= 0) {
                         // tile candidates ranked by the cost model; with autotuning the best few are timed on the device once per
                         // (op, batch).  Every candidate accumulates in the same K order, so the choice never changes results.
                         int cBN[16], cMT[16], cNS[16];
-                        const int nc = gemm_v3_candidates(g, e->autotune ? (ntaps == 9 && !s2 ? 16 : 10) : 1, cBN, cMT, cNS);
+                        const int nc = gemm_v3_candidates(g, e->autotune ? (o.ntaps == 9 && !o.s2 ? 16 : 10) : 1, cBN, cMT, cNS);
                         float best_ms = 1e30f;
                         cudaEvent_t ev0 = nullptr, ev1 = nullptr;
                         if (nc > 1) { ADAS_CUDA(cudaEventCreate(&ev0)); ADAS_CUDA(cudaEventCreate(&ev1)); }
@@ -262,7 +257,7 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
                             float ms = 1e30f;
                             if (!rc) cudaEventElapsedTime(&ms, ev0, ev1);
                             static const bool at_log = getenv("ADAS_B200_AT_LOG") != nullptr;
-                            if (at_log) fprintf(stderr, "[autotune] op %zu M=%d N=%d K=%d taps=%d s2=%d BN=%d mt=%d no_slab=%d : %.1f us\n", oi, g.M, g.N, Kc * ntaps, ntaps, s2,
+                            if (at_log) fprintf(stderr, "[autotune] op %zu M=%d N=%d K=%d taps=%d s2=%d BN=%d mt=%d no_slab=%d : %.1f us\n", oi, g.M, g.N, o.Kc * o.ntaps, o.ntaps, o.s2,
                                                 gc.BN, gc.mt_hint, gc.no_slab, rc ? -1.0 : ms * 1000.0 / 4.0);
                             if (!rc && ms < best_ms) { best_ms = ms; if (opaque) gemm_v3_free(opaque); opaque = cand; }
                             else gemm_v3_free(cand);
@@ -286,11 +281,12 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
                 break;
             }
             case OP_IM2COL: {
-                const PlanBuffer& ib = e->bufs[p[0]];
-                const PlanBuffer& ob = e->bufs[p[7]];
-                const __half* in = static_cast<const __half*>(e->dbufs[p[0]].ptr);
-                __half* out = static_cast<__half*>(e->dbufs[p[7]].ptr);
-                const int in_ld = (int)ib.C, in_coff = p[1], H = (int)ib.H, W = (int)ib.W, Cin = p[2], kh = p[3], kw = p[4], s = p[5], pad = p[6];
+                const Im2colOp o = op_fields<Im2colOp>(op);
+                const PlanBuffer& ib = e->bufs[o.in_buf];
+                const PlanBuffer& ob = e->bufs[o.out_buf];
+                const __half* in = static_cast<const __half*>(e->dbufs[o.in_buf].ptr);
+                __half* out = static_cast<__half*>(e->dbufs[o.out_buf].ptr);
+                const int in_ld = (int)ib.C, in_coff = o.in_coff, H = (int)ib.H, W = (int)ib.W, Cin = o.Cin, kh = o.kh, kw = o.kw, s = o.stride, pad = o.pad;
                 const int Ho = (int)ob.H, Wo = (int)ob.W, Kpad = (int)ob.C;
                 ADAS_CHECK(kh * kw * Cin <= Kpad, "op %zu: im2col K exceeds the patch buffer width", oi);
                 prog->steps.push_back([=](cudaStream_t st) {
@@ -299,34 +295,37 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
                 break;
             }
             case OP_MAXPOOL: {
-                const PlanBuffer& ib = e->bufs[p[0]];
-                const PlanBuffer& ob = e->bufs[p[6]];
-                const __half* in = static_cast<const __half*>(e->dbufs[p[0]].ptr) + p[1];
-                __half* out = static_cast<__half*>(e->dbufs[p[6]].ptr) + p[7];
-                const int in_ld = (int)ib.C, H = (int)ib.H, W = (int)ib.W, C = p[2], k = p[3], s = p[4], pad = p[5];
+                const MaxpoolOp o = op_fields<MaxpoolOp>(op);
+                const PlanBuffer& ib = e->bufs[o.in_buf];
+                const PlanBuffer& ob = e->bufs[o.out_buf];
+                const __half* in = static_cast<const __half*>(e->dbufs[o.in_buf].ptr) + o.in_coff;
+                __half* out = static_cast<__half*>(e->dbufs[o.out_buf].ptr) + o.out_coff;
+                const int in_ld = (int)ib.C, H = (int)ib.H, W = (int)ib.W, C = o.C, k = o.k, s = o.stride, pad = o.pad;
                 const int out_ld = (int)ob.C, Ho = (int)ob.H, Wo = (int)ob.W;
                 prog->steps.push_back([=](cudaStream_t st) { return launch_maxpool(in, in_ld, batch, H, W, C, k, s, pad, out, out_ld, Ho, Wo, st); });
                 break;
             }
             case OP_AVGPOOL2: {
-                const PlanBuffer& ib = e->bufs[p[0]];
-                const PlanBuffer& ob = e->bufs[p[3]];
-                const __half* in = static_cast<const __half*>(e->dbufs[p[0]].ptr) + p[1];
-                __half* out = static_cast<__half*>(e->dbufs[p[3]].ptr) + p[4];
-                const int in_ld = (int)ib.C, H = (int)ib.H, W = (int)ib.W, C = p[2], out_ld = (int)ob.C, fill = p[5];
+                const Avgpool2Op o = op_fields<Avgpool2Op>(op);
+                const PlanBuffer& ib = e->bufs[o.in_buf];
+                const PlanBuffer& ob = e->bufs[o.out_buf];
+                const __half* in = static_cast<const __half*>(e->dbufs[o.in_buf].ptr) + o.in_coff;
+                __half* out = static_cast<__half*>(e->dbufs[o.out_buf].ptr) + o.out_coff;
+                const int in_ld = (int)ib.C, H = (int)ib.H, W = (int)ib.W, C = o.C, out_ld = (int)ob.C, fill = o.fill;
                 prog->steps.push_back([=](cudaStream_t st) { return launch_avgpool2(in, in_ld, batch, H, W, C, out, out_ld, fill, st); });
                 break;
             }
             case OP_DWCONV: {
-                const PlanBuffer& ib = e->bufs[p[0]];
-                const PlanBuffer& ob = e->bufs[p[8]];
-                const __half* in = static_cast<const __half*>(e->dbufs[p[0]].ptr) + p[1];
-                __half* out = static_cast<__half*>(e->dbufs[p[8]].ptr) + p[9];
-                const __half* res = p[10] >= 0 ? static_cast<const __half*>(e->dbufs[p[10]].ptr) + p[11] : nullptr;
-                const int res_ld = p[10] >= 0 ? (int)e->bufs[p[10]].C : 0;
-                const __half* w = static_cast<const __half*>(tensor_ptr(e, p[6]));
-                const float* bias = static_cast<const float*>(tensor_ptr(e, p[7]));
-                const int in_ld = (int)ib.C, H = (int)ib.H, W = (int)ib.W, C = p[2], k = p[3], s = p[4], act = p[5];
+                const DwconvOp o = op_fields<DwconvOp>(op);
+                const PlanBuffer& ib = e->bufs[o.in_buf];
+                const PlanBuffer& ob = e->bufs[o.out_buf];
+                const __half* in = static_cast<const __half*>(e->dbufs[o.in_buf].ptr) + o.in_coff;
+                __half* out = static_cast<__half*>(e->dbufs[o.out_buf].ptr) + o.out_coff;
+                const __half* res = o.res_buf >= 0 ? static_cast<const __half*>(e->dbufs[o.res_buf].ptr) + o.res_coff : nullptr;
+                const int res_ld = o.res_buf >= 0 ? (int)e->bufs[o.res_buf].C : 0;
+                const __half* w = static_cast<const __half*>(tensor_ptr(e, o.w_tensor));
+                const float* bias = static_cast<const float*>(tensor_ptr(e, o.bias_tensor));
+                const int in_ld = (int)ib.C, H = (int)ib.H, W = (int)ib.W, C = o.C, k = o.k, s = o.stride, act = o.act;
                 const int out_ld = (int)ob.C, Ho = (int)ob.H, Wo = (int)ob.W;
                 char d[128];
                 snprintf(d, sizeof(d), "dwconv %dx%d s%d C=%d, %dx%d -> %dx%d%s%s", k, k, s, C, H, W, Ho, Wo, act == 5 ? " hardswish" : act ? " silu" : "", res ? " +res" : "");
@@ -338,12 +337,13 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
                 break;
             }
             case OP_ATTN: {
-                const PlanBuffer& ib = e->bufs[p[0]];
-                const PlanBuffer& ob = e->bufs[p[5]];
-                const __half* in = static_cast<const __half*>(e->dbufs[p[0]].ptr) + p[1];
-                __half* out = static_cast<__half*>(e->dbufs[p[5]].ptr) + p[6];
-                const int in_ld = (int)ib.C, H = (int)ib.H, W = (int)ib.W, nh = p[2], kdp = p[3], hd = p[4], out_ld = (int)ob.C;
-                const float scale = op.f[0];
+                const AttnOp o = op_fields<AttnOp>(op);
+                const PlanBuffer& ib = e->bufs[o.in_buf];
+                const PlanBuffer& ob = e->bufs[o.out_buf];
+                const __half* in = static_cast<const __half*>(e->dbufs[o.in_buf].ptr) + o.in_coff;
+                __half* out = static_cast<__half*>(e->dbufs[o.out_buf].ptr) + o.out_coff;
+                const int in_ld = (int)ib.C, H = (int)ib.H, W = (int)ib.W, nh = o.nh, kdp = o.kdp, hd = o.hd, out_ld = (int)ob.C;
+                const float scale = op.f[0];            // f[0] = softmax scale
                 char d[128];
                 snprintf(d, sizeof(d), "attention N=%d heads=%d kdp=%d hd=%d", H * W, nh, kdp, hd);
                 prog->step_desc.resize(prog->step_type.size());
@@ -352,60 +352,63 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
                 break;
             }
             case OP_UPSAMPLE2X: {
-                const PlanBuffer& ib = e->bufs[p[0]];
-                const PlanBuffer& ob = e->bufs[p[3]];
-                const __half* in = static_cast<const __half*>(e->dbufs[p[0]].ptr) + p[1];
-                __half* out = static_cast<__half*>(e->dbufs[p[3]].ptr) + p[4];
-                const int in_ld = (int)ib.C, H = (int)ib.H, W = (int)ib.W, C = p[2], out_ld = (int)ob.C;
+                const Upsample2xOp o = op_fields<Upsample2xOp>(op);
+                const PlanBuffer& ib = e->bufs[o.in_buf];
+                const PlanBuffer& ob = e->bufs[o.out_buf];
+                const __half* in = static_cast<const __half*>(e->dbufs[o.in_buf].ptr) + o.in_coff;
+                __half* out = static_cast<__half*>(e->dbufs[o.out_buf].ptr) + o.out_coff;
+                const int in_ld = (int)ib.C, H = (int)ib.H, W = (int)ib.W, C = o.C, out_ld = (int)ob.C;
                 ADAS_CHECK((int)ob.H == 2 * H && (int)ob.W == 2 * W, "op %zu: upsample geometry", oi);
                 prog->steps.push_back([=](cudaStream_t st) { return launch_upsample2x(in, in_ld, batch, H, W, C, out, out_ld, st); });
                 break;
             }
             case OP_CBFUSE: {
-                const PlanBuffer& ob = e->bufs[p[0]];
-                const PlanBuffer& bb = e->bufs[p[3]];
+                const CbfuseOp o = op_fields<CbfuseOp>(op);
+                const PlanBuffer& ob = e->bufs[o.out_buf];
+                const PlanBuffer& bb = e->bufs[o.base_buf];
                 CbfuseParams cp;
                 memset(&cp, 0, sizeof(cp));
-                cp.out = static_cast<__half*>(e->dbufs[p[0]].ptr) + p[1];
+                cp.out = static_cast<__half*>(e->dbufs[o.out_buf].ptr) + o.out_coff;
                 cp.out_ld = (int)ob.C;
-                cp.base = static_cast<const __half*>(e->dbufs[p[3]].ptr) + p[4];
+                cp.base = static_cast<const __half*>(e->dbufs[o.base_buf].ptr) + o.base_coff;
                 cp.base_ld = (int)bb.C;
-                cp.B = batch; cp.H = (int)ob.H; cp.W = (int)ob.W; cp.C = p[2]; cp.n_src = p[5];
+                cp.B = batch; cp.H = (int)ob.H; cp.W = (int)ob.W; cp.C = o.C; cp.n_src = o.n_src;
                 for (int s = 0; s < cp.n_src; ++s) {
-                    const int* q = p + 6 + 3 * s;
-                    cp.src[s].ptr = static_cast<const __half*>(e->dbufs[q[0]].ptr) + q[1];
-                    cp.src[s].ld = (int)e->bufs[q[0]].C;
-                    cp.src[s].shift = q[2];
+                    cp.src[s].ptr = static_cast<const __half*>(e->dbufs[o.src[s].buf].ptr) + o.src[s].coff;
+                    cp.src[s].ld = (int)e->bufs[o.src[s].buf].C;
+                    cp.src[s].shift = o.src[s].shift;
                 }
                 char d[128];
-                snprintf(d, sizeof(d), "cbfuse C=%d %dx%d sources=%d%s", cp.C, cp.H, cp.W, cp.n_src, (p[0] == p[3] && p[1] == p[4]) ? " in place" : "");
+                snprintf(d, sizeof(d), "cbfuse C=%d %dx%d sources=%d%s", cp.C, cp.H, cp.W, cp.n_src, (o.out_buf == o.base_buf && o.out_coff == o.base_coff) ? " in place" : "");
                 prog->step_desc.resize(prog->step_type.size());
                 prog->step_desc.back() = d;
                 prog->steps.push_back([=](cudaStream_t st) { return launch_cbfuse(cp, st); });
                 break;
             }
             case OP_SE: {
-                const PlanBuffer& ib = e->bufs[p[0]];
-                const PlanBuffer& ob = e->bufs[p[8]];
+                const SeOp o = op_fields<SeOp>(op);
+                const PlanBuffer& ib = e->bufs[o.in_buf];
+                const PlanBuffer& ob = e->bufs[o.out_buf];
                 SeParams sp;
-                sp.in = static_cast<const __half*>(e->dbufs[p[0]].ptr) + p[1]; sp.in_ld = (int)ib.C;
-                sp.out = static_cast<__half*>(e->dbufs[p[8]].ptr) + p[9]; sp.out_ld = (int)ob.C;
-                sp.w1 = static_cast<const float*>(tensor_ptr(e, p[4])); sp.b1 = static_cast<const float*>(tensor_ptr(e, p[5]));
-                sp.w2 = static_cast<const float*>(tensor_ptr(e, p[6])); sp.b2 = static_cast<const float*>(tensor_ptr(e, p[7]));
-                sp.B = batch; sp.H = (int)ib.H; sp.W = (int)ib.W; sp.C = p[2]; sp.hid = p[3];
+                sp.in = static_cast<const __half*>(e->dbufs[o.in_buf].ptr) + o.in_coff; sp.in_ld = (int)ib.C;
+                sp.out = static_cast<__half*>(e->dbufs[o.out_buf].ptr) + o.out_coff; sp.out_ld = (int)ob.C;
+                sp.w1 = static_cast<const float*>(tensor_ptr(e, o.w1)); sp.b1 = static_cast<const float*>(tensor_ptr(e, o.b1));
+                sp.w2 = static_cast<const float*>(tensor_ptr(e, o.w2)); sp.b2 = static_cast<const float*>(tensor_ptr(e, o.b2));
+                sp.B = batch; sp.H = (int)ib.H; sp.W = (int)ib.W; sp.C = o.C; sp.hid = o.hid;
                 char d[128];
-                snprintf(d, sizeof(d), "se C=%d hidden=%d %dx%d%s", sp.C, sp.hid, sp.H, sp.W, (p[0] == p[8] && p[1] == p[9]) ? " in place" : "");
+                snprintf(d, sizeof(d), "se C=%d hidden=%d %dx%d%s", sp.C, sp.hid, sp.H, sp.W, (o.in_buf == o.out_buf && o.in_coff == o.out_coff) ? " in place" : "");
                 prog->step_desc.resize(prog->step_type.size());
                 prog->step_desc.back() = d;
                 prog->steps.push_back([=](cudaStream_t st) { return launch_se(sp, st); });
                 break;
             }
             case OP_SHUFFLE2: {
-                const PlanBuffer& ob = e->bufs[p[5]];
-                const __half* a = static_cast<const __half*>(e->dbufs[p[0]].ptr) + p[1];
-                const __half* b = static_cast<const __half*>(e->dbufs[p[2]].ptr) + p[3];
-                __half* out = static_cast<__half*>(e->dbufs[p[5]].ptr) + p[6];
-                const int a_ld = (int)e->bufs[p[0]].C, b_ld = (int)e->bufs[p[2]].C, out_ld = (int)ob.C, H = (int)ob.H, W = (int)ob.W, n = p[4];
+                const Shuffle2Op o = op_fields<Shuffle2Op>(op);
+                const PlanBuffer& ob = e->bufs[o.out_buf];
+                const __half* a = static_cast<const __half*>(e->dbufs[o.a_buf].ptr) + o.a_coff;
+                const __half* b = static_cast<const __half*>(e->dbufs[o.b_buf].ptr) + o.b_coff;
+                __half* out = static_cast<__half*>(e->dbufs[o.out_buf].ptr) + o.out_coff;
+                const int a_ld = (int)e->bufs[o.a_buf].C, b_ld = (int)e->bufs[o.b_buf].C, out_ld = (int)ob.C, H = (int)ob.H, W = (int)ob.W, n = o.n;
                 char d[128];
                 snprintf(d, sizeof(d), "shuffle2 2x%d channels %dx%d", n, H, W);
                 prog->step_desc.resize(prog->step_type.size());
@@ -414,24 +417,26 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
                 break;
             }
             case OP_STEMPACK: {
-                const PlanBuffer& ib = e->bufs[p[0]];
-                const PlanBuffer& ob = e->bufs[p[1]];
+                const StempackOp o = op_fields<StempackOp>(op);
+                const PlanBuffer& ib = e->bufs[o.in_buf];
+                const PlanBuffer& ob = e->bufs[o.out_buf];
                 ADAS_CHECK(ib.C == 4 && ob.C == 64 && ob.H * 2 == ib.H && ob.W * 2 == ib.W, "op %zu: stem pack geometry", oi);
-                const __half* in = static_cast<const __half*>(e->dbufs[p[0]].ptr);
-                __half* out = static_cast<__half*>(e->dbufs[p[1]].ptr);
+                const __half* in = static_cast<const __half*>(e->dbufs[o.in_buf].ptr);
+                __half* out = static_cast<__half*>(e->dbufs[o.out_buf].ptr);
                 const int H = (int)ib.H, W = (int)ib.W;
                 prog->steps.push_back([=](cudaStream_t st) { return launch_stempack(in, batch, H, W, out, st); });
                 break;
             }
             case OP_STEMCONV: {
-                const PlanBuffer& ib = e->bufs[p[0]];
-                const PlanBuffer& ob = e->bufs[p[7]];
-                const int Cout = p[3], k = p[4], pad = p[5], act = p[6], out_coff = p[8], stride = p[9] == 0 ? 2 : p[9];
-                ADAS_CHECK(ib.C == 4 && ib.dtype == 0 && ob.dtype == 0 && stem_conv_supported(Cout, k, pad) && out_coff % 8 == 0 && ob.C % 8 == 0, "op %zu: stem conv geometry", oi);
-                const __half* in = static_cast<const __half*>(e->dbufs[p[0]].ptr);
-                const __half* wq = static_cast<const __half*>(tensor_ptr(e, p[1]));
-                const float* bias = static_cast<const float*>(tensor_ptr(e, p[2]));
-                __half* out = static_cast<__half*>(e->dbufs[p[7]].ptr) + out_coff;
+                const StemconvOp o = op_fields<StemconvOp>(op);
+                const PlanBuffer& ib = e->bufs[o.in_buf];
+                const PlanBuffer& ob = e->bufs[o.out_buf];
+                const int Cout = o.Cout, k = o.k, pad = o.pad, act = o.act, stride = o.stride == 0 ? 2 : o.stride;
+                ADAS_CHECK(ib.C == 4 && ib.dtype == 0 && ob.dtype == 0 && stem_conv_supported(Cout, k, pad) && o.out_coff % 8 == 0 && ob.C % 8 == 0, "op %zu: stem conv geometry", oi);
+                const __half* in = static_cast<const __half*>(e->dbufs[o.in_buf].ptr);
+                const __half* wq = static_cast<const __half*>(tensor_ptr(e, o.w_tensor));
+                const float* bias = static_cast<const float*>(tensor_ptr(e, o.bias_tensor));
+                __half* out = static_cast<__half*>(e->dbufs[o.out_buf].ptr) + o.out_coff;
                 const int H = (int)ib.H, W = (int)ib.W, Ho = (int)ob.H, Wo = (int)ob.W, out_ld = (int)ob.C;
                 char d[128];
                 snprintf(d, sizeof(d), "stem %dx%d s%d p%d 3->%d, %dx%d -> %dx%d, warp MMA from the image", k, k, stride, pad, Cout, H, W, Ho, Wo);
@@ -442,15 +447,16 @@ static int build_program(adas_engine* e, int batch, Program* prog) {
             }
             case OP_LAYERNORM: {
                 // each image's whole slab (rows_per_img * C elements) is one LayerNorm row
-                const PlanBuffer& ib = e->bufs[p[0]];
-                const PlanBuffer& ob = e->bufs[p[4]];
-                const __half* in = static_cast<const __half*>(e->dbufs[p[0]].ptr);
-                __half* out = static_cast<__half*>(e->dbufs[p[4]].ptr);
-                const int in_ld = (int)(ib.rows_per_img * ib.C), d_len = p[1], d_norm = p[5], out_ld = (int)(ob.rows_per_img * ob.C);
+                const LayernormOp o = op_fields<LayernormOp>(op);
+                const PlanBuffer& ib = e->bufs[o.in_buf];
+                const PlanBuffer& ob = e->bufs[o.out_buf];
+                const __half* in = static_cast<const __half*>(e->dbufs[o.in_buf].ptr);
+                __half* out = static_cast<__half*>(e->dbufs[o.out_buf].ptr);
+                const int in_ld = (int)(ib.rows_per_img * ib.C), d_len = o.d_len, d_norm = o.d_norm, out_ld = (int)(ob.rows_per_img * ob.C);
                 ADAS_CHECK(d_len <= in_ld && d_len <= out_ld && d_norm > 0, "op %zu: layernorm extent", oi);
-                const float* gamma = static_cast<const float*>(tensor_ptr(e, p[2]));
-                const float* beta = static_cast<const float*>(tensor_ptr(e, p[3]));
-                const float eps = op.f[0];
+                const float* gamma = static_cast<const float*>(tensor_ptr(e, o.gamma_tensor));
+                const float* beta = static_cast<const float*>(tensor_ptr(e, o.beta_tensor));
+                const float eps = op.f[0];              // f[0] = eps
                 prog->steps.push_back([=](cudaStream_t st) { return launch_layernorm(in, in_ld, batch, d_len, d_norm, gamma, beta, eps, out, out_ld, st); });
                 break;
             }
@@ -667,196 +673,221 @@ static int validate_plan(const adas_engine* e, uint64_t file_bytes, const char* 
     auto tensor_ok = [&](int t, uint64_t min_bytes) { return t >= 0 && t < nt && e->tensors[t].bytes >= min_bytes; };
     for (size_t oi = 0; oi < e->ops.size(); ++oi) {
         const PlanOp& op = e->ops[oi];
-        const int32_t* p = op.p;
         switch (op.type) {
             case OP_GEMM: {
-                const int Kc = p[2], ntaps = p[3], N = p[6], transposed = p[14], up2 = p[19];
+                const GemmOp o = op_fields<GemmOp>(op);
+                const int Kc = o.Kc, ntaps = o.ntaps, N = o.N, transposed = o.transposed, up2 = o.up2;
                 ADAS_CHECK(Kc >= 8 && Kc <= (1 << 20) && N >= 1 && N <= (1 << 20) && (ntaps == 1 || ntaps == 4 || ntaps == 9), "plan %s: op %zu: bad GEMM shape", path, oi);
-                ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[11]) && p[1] >= 0 && p[12] >= 0, "plan %s: op %zu: GEMM buffer index out of range", path, oi);
+                ADAS_CHECK(buf_ok(o.a_buf) && buf_ok(o.out_buf) && o.a_coff >= 0 && o.out_coff >= 0, "plan %s: op %zu: GEMM buffer index out of range", path, oi);
                 ADAS_CHECK(up2 == 0 || up2 == 1, "plan %s: op %zu: bad transposed-conv flag %d", path, oi, up2);
                 ADAS_CHECK(isfinite(op.f[0]), "plan %s: op %zu: residual scale is not finite", path, oi);
                 if (up2) {
                     // 2x2 stride-2 transposed conv: a 1x1 GEMM with N = 4 * Cout (Cout % 8 == 0) from an H x W grid into a 2H x 2W one
-                    const PlanBuffer &ab = e->bufs[p[0]], &ob = e->bufs[p[11]];
-                    ADAS_CHECK(N % 32 == 0 && ntaps == 1 && !transposed && !p[16] && p[8] < 0 && (p[15] == 0 || p[15] == 64 || p[15] == 128 || p[15] == 256) && ab.H > 0 && ob.H == 2 * ab.H && ob.W == 2 * ab.W &&
-                                   view_ok(p[0], p[1], Kc) && view_ok(p[11], p[12], N / 4),
+                    const PlanBuffer &ab = e->bufs[o.a_buf], &ob = e->bufs[o.out_buf];
+                    ADAS_CHECK(N % 32 == 0 && ntaps == 1 && !transposed && !o.s2 && o.res_buf < 0 && (o.BN == 0 || o.BN == 64 || o.BN == 128 || o.BN == 256) && ab.H > 0 && ob.H == 2 * ab.H && ob.W == 2 * ab.W &&
+                                   view_ok(o.a_buf, o.a_coff, Kc) && view_ok(o.out_buf, o.out_coff, N / 4),
                                "plan %s: op %zu: transposed conv needs Cout %% 8 == 0, a 2H x 2W output of its H x W input and BN 64 / 128 / 256 if forced (Cout %d, %ux%u -> %ux%u)",
                                path, oi, N / 4, ab.H, ab.W, ob.H, ob.W);
                 } else if (!transposed) {
-                    ADAS_CHECK(view_ok(p[0], p[1], Kc) && view_ok(p[11], p[12], N), "plan %s: op %zu: GEMM channel slice exceeds its buffer", path, oi);
+                    ADAS_CHECK(view_ok(o.a_buf, o.a_coff, Kc) && view_ok(o.out_buf, o.out_coff, N), "plan %s: op %zu: GEMM channel slice exceeds its buffer", path, oi);
                 } else {
-                    const PlanBuffer &ab = e->bufs[p[0]], &ob = e->bufs[p[11]];
-                    ADAS_CHECK(p[1] == 0 && p[12] == 0 && (uint64_t)Kc <= (uint64_t)ab.rows_per_img * ab.C && (uint64_t)N <= (uint64_t)ob.rows_per_img * ob.C,
+                    const PlanBuffer &ab = e->bufs[o.a_buf], &ob = e->bufs[o.out_buf];
+                    ADAS_CHECK(o.a_coff == 0 && o.out_coff == 0 && (uint64_t)Kc <= (uint64_t)ab.rows_per_img * ab.C && (uint64_t)N <= (uint64_t)ob.rows_per_img * ob.C,
                                "plan %s: op %zu: FC vector exceeds its buffer", path, oi);
                 }
-                ADAS_CHECK(tensor_ok(p[4], (uint64_t)N * Kc * ntaps * 2) && e->tensors[p[4]].dtype == 0, "plan %s: op %zu: weight tensor missing or too small", path, oi);
-                ADAS_CHECK(p[5] < 0 || (tensor_ok(p[5], (uint64_t)N * 4) && e->tensors[p[5]].dtype == 1), "plan %s: op %zu: bias tensor missing or too small", path, oi);
-                ADAS_CHECK(p[8] < 0 || (!transposed && view_ok(p[8], p[9], N) && e->bufs[p[8]].dtype == 0), "plan %s: op %zu: residual slice exceeds its buffer", path, oi);
-                ADAS_CHECK(p[15] >= 0 && p[15] <= 256 && p[17] >= 0 && p[17] <= 4 && (p[18] == 0 || p[18] == 1), "plan %s: op %zu: bad forced tile shape", path, oi);
-                ADAS_CHECK(act_code_ok(p[7]), "plan %s: op %zu: unknown activation %d", path, oi, p[7]);
+                ADAS_CHECK(tensor_ok(o.w_tensor, (uint64_t)N * Kc * ntaps * 2) && e->tensors[o.w_tensor].dtype == 0, "plan %s: op %zu: weight tensor missing or too small", path, oi);
+                ADAS_CHECK(o.bias_tensor < 0 || (tensor_ok(o.bias_tensor, (uint64_t)N * 4) && e->tensors[o.bias_tensor].dtype == 1), "plan %s: op %zu: bias tensor missing or too small", path, oi);
+                ADAS_CHECK(o.res_buf < 0 || (!transposed && view_ok(o.res_buf, o.res_coff, N) && e->bufs[o.res_buf].dtype == 0), "plan %s: op %zu: residual slice exceeds its buffer", path, oi);
+                ADAS_CHECK(o.BN >= 0 && o.BN <= 256 && o.MT >= 0 && o.MT <= 4 && (o.no_slab == 0 || o.no_slab == 1), "plan %s: op %zu: bad forced tile shape", path, oi);
+                ADAS_CHECK(act_code_ok(o.act), "plan %s: op %zu: unknown activation %d", path, oi, o.act);
                 // the launch-time preconditions of build_program, checked here too so that a plan accepted at load runs in bounds
-                const PlanBuffer &ab = e->bufs[p[0]], &ob = e->bufs[p[11]];
+                const PlanBuffer &ab = e->bufs[o.a_buf], &ob = e->bufs[o.out_buf];
                 ADAS_CHECK(ab.dtype == 0, "plan %s: op %zu: GEMM input buffer must be fp16", path, oi);
-                ADAS_CHECK(Kc % 8 == 0 && p[1] % 8 == 0 && ab.C % 8 == 0, "plan %s: op %zu: GEMM K, input offset and row stride must be multiples of 8", path, oi);
+                ADAS_CHECK(Kc % 8 == 0 && o.a_coff % 8 == 0 && ab.C % 8 == 0, "plan %s: op %zu: GEMM K, input offset and row stride must be multiples of 8", path, oi);
                 ADAS_CHECK(ntaps == 1 || (Kc % 64 == 0 && ab.W > 0), "plan %s: op %zu: tap mode needs Cin %% 64 == 0 on a padded grid", path, oi);
-                ADAS_CHECK(!p[16] || (Kc % 64 == 0 && ab.W > 0 && ob.W > 0 && !transposed), "plan %s: op %zu: stride-2 mode needs Cin %% 64 == 0 on padded grids", path, oi);
-                ADAS_CHECK(transposed || p[16] || up2 || ob.rows_per_img == ab.rows_per_img, "plan %s: op %zu: GEMM in/out row geometry differs", path, oi);
-                ADAS_CHECK(!p[13] || ob.H > 0, "plan %s: op %zu: masked store into a dense buffer", path, oi);
+                ADAS_CHECK(!o.s2 || (Kc % 64 == 0 && ab.W > 0 && ob.W > 0 && !transposed), "plan %s: op %zu: stride-2 mode needs Cin %% 64 == 0 on padded grids", path, oi);
+                ADAS_CHECK(transposed || o.s2 || up2 || ob.rows_per_img == ab.rows_per_img, "plan %s: op %zu: GEMM in/out row geometry differs", path, oi);
+                ADAS_CHECK(!o.masked || ob.H > 0, "plan %s: op %zu: masked store into a dense buffer", path, oi);
                 ADAS_CHECK(!transposed || ((uint64_t)ab.rows_per_img * ab.C) % 8 == 0, "plan %s: op %zu: FC input slab must be a multiple of 8 elements", path, oi);
                 // the epilogue reads the residual at the output's row index
-                ADAS_CHECK(p[8] < 0 || (e->bufs[p[8]].rows_per_img == ob.rows_per_img && e->bufs[p[8]].H == ob.H && e->bufs[p[8]].W == ob.W),
+                ADAS_CHECK(o.res_buf < 0 || (e->bufs[o.res_buf].rows_per_img == ob.rows_per_img && e->bufs[o.res_buf].H == ob.H && e->bufs[o.res_buf].W == ob.W),
                            "plan %s: op %zu: GEMM residual slice must have the output's geometry", path, oi);
                 break;
             }
-            case OP_IM2COL:
-                ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[7]) && view_ok(p[0], p[1], p[2]) && e->bufs[p[0]].H > 0 && e->bufs[p[7]].H > 0 && p[3] >= 1 && p[3] <= 7 && p[4] >= 1 && p[4] <= 7 &&
-                           p[5] >= 1 && p[5] <= 4 && p[6] >= 0 && p[6] <= 3 && (uint64_t)p[2] * p[3] * p[4] <= e->bufs[p[7]].C &&
-                           e->bufs[p[0]].dtype == 0 && e->bufs[p[7]].dtype == 0,
+            case OP_IM2COL: {
+                const Im2colOp o = op_fields<Im2colOp>(op);
+                ADAS_CHECK(buf_ok(o.in_buf) && buf_ok(o.out_buf) && view_ok(o.in_buf, o.in_coff, o.Cin) && e->bufs[o.in_buf].H > 0 && e->bufs[o.out_buf].H > 0 &&
+                           o.kh >= 1 && o.kh <= 7 && o.kw >= 1 && o.kw <= 7 && o.stride >= 1 && o.stride <= 4 && o.pad >= 0 && o.pad <= 3 &&
+                           (uint64_t)o.Cin * o.kh * o.kw <= e->bufs[o.out_buf].C && e->bufs[o.in_buf].dtype == 0 && e->bufs[o.out_buf].dtype == 0,
                            "plan %s: op %zu: bad im2col", path, oi);
                 break;
-            case OP_MAXPOOL:
-                ADAS_CHECK(view_ok(p[0], p[1], p[2]) && view_ok(p[6], p[7], p[2]) && e->bufs[p[0]].H > 0 && e->bufs[p[6]].H > 0 && p[3] >= 1 && p[3] <= 7 && p[4] >= 1 && p[4] <= 4 && p[5] >= 0 && p[5] <= 3 &&
-                           e->bufs[p[0]].dtype == 0 && e->bufs[p[6]].dtype == 0,
+            }
+            case OP_MAXPOOL: {
+                const MaxpoolOp o = op_fields<MaxpoolOp>(op);
+                ADAS_CHECK(view_ok(o.in_buf, o.in_coff, o.C) && view_ok(o.out_buf, o.out_coff, o.C) && e->bufs[o.in_buf].H > 0 && e->bufs[o.out_buf].H > 0 &&
+                           o.k >= 1 && o.k <= 7 && o.stride >= 1 && o.stride <= 4 && o.pad >= 0 && o.pad <= 3 &&
+                           e->bufs[o.in_buf].dtype == 0 && e->bufs[o.out_buf].dtype == 0,
                            "plan %s: op %zu: bad maxpool", path, oi);
                 break;
+            }
             case OP_AVGPOOL2: {
-                ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[3]), "plan %s: op %zu: avgpool2 buffer index out of range", path, oi);
-                const PlanBuffer &ib = e->bufs[p[0]], &ob = e->bufs[p[3]];
+                const Avgpool2Op o = op_fields<Avgpool2Op>(op);
+                ADAS_CHECK(buf_ok(o.in_buf) && buf_ok(o.out_buf), "plan %s: op %zu: avgpool2 buffer index out of range", path, oi);
+                const PlanBuffer &ib = e->bufs[o.in_buf], &ob = e->bufs[o.out_buf];
                 ADAS_CHECK(ib.dtype == 0 && ob.dtype == 0, "plan %s: op %zu: avgpool2 buffers must be fp16", path, oi);
                 ADAS_CHECK(ib.H > 0 && ob.H == ib.H && ob.W == ib.W, "plan %s: op %zu: avgpool2 output must have its input's H x W (%ux%u -> %ux%u)", path, oi,
                            ib.H, ib.W, ob.H, ob.W);
-                ADAS_CHECK(p[2] >= 8 && p[2] % 8 == 0 && p[1] % 8 == 0 && p[4] % 8 == 0 && ib.C % 8 == 0 && ob.C % 8 == 0,
+                ADAS_CHECK(o.C >= 8 && o.C % 8 == 0 && o.in_coff % 8 == 0 && o.out_coff % 8 == 0 && ib.C % 8 == 0 && ob.C % 8 == 0,
                            "plan %s: op %zu: avgpool2 channels and offsets must be multiples of 8", path, oi);
-                ADAS_CHECK(view_ok(p[0], p[1], p[2]) && view_ok(p[3], p[4], p[2]) && (p[0] != p[3] || p[4] >= p[1] + p[2] || p[1] >= p[4] + p[2]),
+                ADAS_CHECK(view_ok(o.in_buf, o.in_coff, o.C) && view_ok(o.out_buf, o.out_coff, o.C) &&
+                               (o.in_buf != o.out_buf || o.out_coff >= o.in_coff + o.C || o.in_coff >= o.out_coff + o.C),
                            "plan %s: op %zu: avgpool2 channel slice exceeds its buffer or overlaps its input", path, oi);
-                ADAS_CHECK(p[5] == 0 || p[5] == 1, "plan %s: op %zu: avgpool2 fill %d (0: zero, 1: -inf)", path, oi, p[5]);
+                ADAS_CHECK(o.fill == 0 || o.fill == 1, "plan %s: op %zu: avgpool2 fill %d (0: zero, 1: -inf)", path, oi, o.fill);
                 break;
             }
             case OP_DWCONV: {
-                const int C = p[2], k = p[3], s = p[4], act = p[5], rb = p[10];
-                ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[8]) && (rb == -1 || buf_ok(rb)), "plan %s: op %zu: dwconv buffer index out of range", path, oi);
-                const PlanBuffer &ib = e->bufs[p[0]], &ob = e->bufs[p[8]];
+                const DwconvOp o = op_fields<DwconvOp>(op);
+                const int C = o.C, k = o.k, s = o.stride, rb = o.res_buf;
+                ADAS_CHECK(buf_ok(o.in_buf) && buf_ok(o.out_buf) && (rb == -1 || buf_ok(rb)), "plan %s: op %zu: dwconv buffer index out of range", path, oi);
+                const PlanBuffer &ib = e->bufs[o.in_buf], &ob = e->bufs[o.out_buf];
                 ADAS_CHECK(ib.dtype == 0 && ob.dtype == 0 && (rb < 0 || e->bufs[rb].dtype == 0), "plan %s: op %zu: dwconv buffers must be fp16", path, oi);
                 ADAS_CHECK(((k == 3 || k == 5) && (s == 1 || s == 2)) || (k == 7 && s == 1), "plan %s: op %zu: dwconv k %d stride %d (3 / 5 s1 / s2, 7 s1)", path, oi, k, s);
-                ADAS_CHECK(act == 0 || act == 1 || act == 5, "plan %s: op %zu: dwconv act %d (0 none, 1 SiLU, 5 Hardswish)", path, oi, act);
+                ADAS_CHECK(o.act == 0 || o.act == 1 || o.act == 5, "plan %s: op %zu: dwconv act %d (0 none, 1 SiLU, 5 Hardswish)", path, oi, o.act);
                 ADAS_CHECK(ib.H > 0 && ob.H > 0 && (int)ob.H == ((int)ib.H + 2 * (k / 2) - k) / s + 1 && (int)ob.W == ((int)ib.W + 2 * (k / 2) - k) / s + 1,
                            "plan %s: op %zu: dwconv output geometry %ux%u does not match a %dx%d stride-%d conv of %ux%u", path, oi, ob.H, ob.W, k, k, s, ib.H, ib.W);
-                ADAS_CHECK(C >= 8 && C % 8 == 0 && p[1] % 8 == 0 && p[9] % 8 == 0 && (rb < 0 || (p[11] % 8 == 0 && e->bufs[rb].C % 8 == 0)) &&
+                ADAS_CHECK(C >= 8 && C % 8 == 0 && o.in_coff % 8 == 0 && o.out_coff % 8 == 0 && (rb < 0 || (o.res_coff % 8 == 0 && e->bufs[rb].C % 8 == 0)) &&
                            ib.C % 8 == 0 && ob.C % 8 == 0, "plan %s: op %zu: dwconv channels and offsets must be multiples of 8", path, oi);
-                ADAS_CHECK(tensor_ok(p[6], 0) && e->tensors[p[6]].dtype == 0 && e->tensors[p[6]].bytes == (uint64_t)C * k * k * 2,
+                ADAS_CHECK(tensor_ok(o.w_tensor, 0) && e->tensors[o.w_tensor].dtype == 0 && e->tensors[o.w_tensor].bytes == (uint64_t)C * k * k * 2,
                            "plan %s: op %zu: dwconv k %d: the weight tensor must be fp16 [k*k][C] (%llu bytes)", path, oi, k, (unsigned long long)C * k * k * 2);
-                ADAS_CHECK(tensor_ok(p[7], 0) && e->tensors[p[7]].dtype == 1 && e->tensors[p[7]].bytes == (uint64_t)C * 4,
+                ADAS_CHECK(tensor_ok(o.bias_tensor, 0) && e->tensors[o.bias_tensor].dtype == 1 && e->tensors[o.bias_tensor].bytes == (uint64_t)C * 4,
                            "plan %s: op %zu: dwconv bias tensor must be fp32 [C]", path, oi);
-                ADAS_CHECK(rb < 0 || (e->bufs[rb].H == ob.H && e->bufs[rb].W == ob.W && view_ok(rb, p[11], C)),
+                ADAS_CHECK(rb < 0 || (e->bufs[rb].H == ob.H && e->bufs[rb].W == ob.W && view_ok(rb, o.res_coff, C)),
                            "plan %s: op %zu: dwconv residual slice must have the output's geometry and fit its buffer", path, oi);
-                ADAS_CHECK(view_ok(p[0], p[1], C) && view_ok(p[8], p[9], C) && (p[0] != p[8] || p[9] >= p[1] + C || p[1] >= p[9] + C) &&
-                           (rb != p[8] || p[11] == p[9] || p[11] >= p[9] + C || p[9] >= p[11] + C),
+                ADAS_CHECK(view_ok(o.in_buf, o.in_coff, C) && view_ok(o.out_buf, o.out_coff, C) && (o.in_buf != o.out_buf || o.out_coff >= o.in_coff + C || o.in_coff >= o.out_coff + C) &&
+                               (rb != o.out_buf || o.res_coff == o.out_coff || o.res_coff >= o.out_coff + C || o.out_coff >= o.res_coff + C),
                            "plan %s: op %zu: dwconv channel slice exceeds its buffer or overlaps its input", path, oi);
                 break;
             }
             case OP_ATTN: {
-                const int nh = p[2], kdp = p[3], hd = p[4];
-                ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[5]), "plan %s: op %zu: attention buffer index out of range", path, oi);
-                const PlanBuffer &ib = e->bufs[p[0]], &ob = e->bufs[p[5]];
+                const AttnOp o = op_fields<AttnOp>(op);
+                const int nh = o.nh, kdp = o.kdp, hd = o.hd;
+                ADAS_CHECK(buf_ok(o.in_buf) && buf_ok(o.out_buf), "plan %s: op %zu: attention buffer index out of range", path, oi);
+                const PlanBuffer &ib = e->bufs[o.in_buf], &ob = e->bufs[o.out_buf];
                 ADAS_CHECK(ib.dtype == 0 && ob.dtype == 0, "plan %s: op %zu: attention buffers must be fp16", path, oi);
                 ADAS_CHECK(ib.H > 0 && ob.H == ib.H && ob.W == ib.W, "plan %s: op %zu: attention output must have its input's H x W", path, oi);
                 ADAS_CHECK(attention_supported(nh, kdp, hd), "plan %s: op %zu: attention heads %d, kdp %d (multiple of 16, <= 64), hd %d (multiple of 8, <= 128)",
                            path, oi, nh, kdp, hd);
-                ADAS_CHECK(p[1] % 8 == 0 && p[6] % 8 == 0 && ib.C % 8 == 0 && ob.C % 8 == 0, "plan %s: op %zu: attention channels and offsets must be multiples of 8", path, oi);
+                ADAS_CHECK(o.in_coff % 8 == 0 && o.out_coff % 8 == 0 && ib.C % 8 == 0 && ob.C % 8 == 0, "plan %s: op %zu: attention channels and offsets must be multiples of 8", path, oi);
                 const int cin = nh * (2 * kdp + hd), cout = nh * hd;
-                ADAS_CHECK(view_ok(p[0], p[1], cin) && view_ok(p[5], p[6], cout) && (p[0] != p[5] || p[6] >= p[1] + cin || p[1] >= p[6] + cout),
+                ADAS_CHECK(view_ok(o.in_buf, o.in_coff, cin) && view_ok(o.out_buf, o.out_coff, cout) &&
+                               (o.in_buf != o.out_buf || o.out_coff >= o.in_coff + cin || o.in_coff >= o.out_coff + cout),
                            "plan %s: op %zu: attention channel slice exceeds its buffer or overlaps its input", path, oi);
                 ADAS_CHECK(std::isfinite(op.f[0]) && op.f[0] > 0.f, "plan %s: op %zu: attention scale %g", path, oi, (double)op.f[0]);
                 break;
             }
-            case OP_UPSAMPLE2X:
-                ADAS_CHECK(view_ok(p[0], p[1], p[2]) && view_ok(p[3], p[4], p[2]) && e->bufs[p[0]].H > 0 && e->bufs[p[3]].H == 2 * e->bufs[p[0]].H && e->bufs[p[3]].W == 2 * e->bufs[p[0]].W &&
-                           e->bufs[p[0]].dtype == 0 && e->bufs[p[3]].dtype == 0,
+            case OP_UPSAMPLE2X: {
+                const Upsample2xOp o = op_fields<Upsample2xOp>(op);
+                ADAS_CHECK(view_ok(o.in_buf, o.in_coff, o.C) && view_ok(o.out_buf, o.out_coff, o.C) && e->bufs[o.in_buf].H > 0 &&
+                           e->bufs[o.out_buf].H == 2 * e->bufs[o.in_buf].H && e->bufs[o.out_buf].W == 2 * e->bufs[o.in_buf].W &&
+                           e->bufs[o.in_buf].dtype == 0 && e->bufs[o.out_buf].dtype == 0,
                            "plan %s: op %zu: bad upsample", path, oi);
                 break;
+            }
             case OP_CBFUSE: {
-                const int C = p[2], n_src = p[5];
+                const CbfuseOp o = op_fields<CbfuseOp>(op);
+                const int C = o.C, n_src = o.n_src;
                 ADAS_CHECK(n_src >= 1 && n_src <= kCbfuseMaxSrc, "plan %s: op %zu: cbfuse with %d sources (1 to %d)", path, oi, n_src, kCbfuseMaxSrc);
-                ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[3]), "plan %s: op %zu: cbfuse buffer index out of range", path, oi);
+                ADAS_CHECK(buf_ok(o.out_buf) && buf_ok(o.base_buf), "plan %s: op %zu: cbfuse buffer index out of range", path, oi);
                 for (int s = 0; s < n_src; ++s)
-                    ADAS_CHECK(buf_ok(p[6 + 3 * s]), "plan %s: op %zu: cbfuse buffer index out of range", path, oi);
-                const PlanBuffer &ob = e->bufs[p[0]], &bb = e->bufs[p[3]];
+                    ADAS_CHECK(buf_ok(o.src[s].buf), "plan %s: op %zu: cbfuse buffer index out of range", path, oi);
+                const PlanBuffer &ob = e->bufs[o.out_buf], &bb = e->bufs[o.base_buf];
                 bool f16 = ob.dtype == 0 && bb.dtype == 0;
-                for (int s = 0; s < n_src; ++s) f16 = f16 && e->bufs[p[6 + 3 * s]].dtype == 0;
+                for (int s = 0; s < n_src; ++s) f16 = f16 && e->bufs[o.src[s].buf].dtype == 0;
                 ADAS_CHECK(f16, "plan %s: op %zu: cbfuse buffers must be fp16", path, oi);
                 ADAS_CHECK(ob.H > 0 && bb.H == ob.H && bb.W == ob.W, "plan %s: op %zu: cbfuse base must have the output's H x W", path, oi);
                 for (int s = 0; s < n_src; ++s) {
-                    const int* q = p + 6 + 3 * s;
-                    const PlanBuffer& sb = e->bufs[q[0]];
-                    ADAS_CHECK(q[2] >= 0 && q[2] <= 4, "plan %s: op %zu: cbfuse source %d shift %d (0 to 4)", path, oi, s, q[2]);
-                    ADAS_CHECK(sb.H > 0 && ((uint64_t)sb.H << q[2]) == ob.H && ((uint64_t)sb.W << q[2]) == ob.W,
-                               "plan %s: op %zu: cbfuse source %d geometry %ux%u << %d is not the output's %ux%u", path, oi, s, sb.H, sb.W, q[2], ob.H, ob.W);
+                    const int shift = o.src[s].shift;
+                    const PlanBuffer& sb = e->bufs[o.src[s].buf];
+                    ADAS_CHECK(shift >= 0 && shift <= 4, "plan %s: op %zu: cbfuse source %d shift %d (0 to 4)", path, oi, s, shift);
+                    ADAS_CHECK(sb.H > 0 && ((uint64_t)sb.H << shift) == ob.H && ((uint64_t)sb.W << shift) == ob.W,
+                               "plan %s: op %zu: cbfuse source %d geometry %ux%u << %d is not the output's %ux%u", path, oi, s, sb.H, sb.W, shift, ob.H, ob.W);
                 }
-                bool al = C >= 8 && C % 8 == 0 && p[1] % 8 == 0 && p[4] % 8 == 0 && ob.C % 8 == 0 && bb.C % 8 == 0;
-                for (int s = 0; s < n_src; ++s) al = al && p[7 + 3 * s] % 8 == 0 && e->bufs[p[6 + 3 * s]].C % 8 == 0;
+                bool al = C >= 8 && C % 8 == 0 && o.out_coff % 8 == 0 && o.base_coff % 8 == 0 && ob.C % 8 == 0 && bb.C % 8 == 0;
+                for (int s = 0; s < n_src; ++s) al = al && o.src[s].coff % 8 == 0 && e->bufs[o.src[s].buf].C % 8 == 0;
                 ADAS_CHECK(al, "plan %s: op %zu: cbfuse channels and offsets must be multiples of 8", path, oi);
-                bool fits = view_ok(p[0], p[1], C) && view_ok(p[3], p[4], C);
-                for (int s = 0; s < n_src; ++s) fits = fits && view_ok(p[6 + 3 * s], p[7 + 3 * s], C);
+                bool fits = view_ok(o.out_buf, o.out_coff, C) && view_ok(o.base_buf, o.base_coff, C);
+                for (int s = 0; s < n_src; ++s) fits = fits && view_ok(o.src[s].buf, o.src[s].coff, C);
                 ADAS_CHECK(fits, "plan %s: op %zu: cbfuse channel slice exceeds its buffer", path, oi);
-                auto apart = [&](int b, int coff) { return b != p[0] || coff >= p[1] + C || p[1] >= coff + C; };
-                bool sep = apart(p[3], p[4]) || p[4] == p[1];
-                for (int s = 0; s < n_src; ++s) sep = sep && apart(p[6 + 3 * s], p[7 + 3 * s]);
+                auto apart = [&](int b, int coff) { return b != o.out_buf || coff >= o.out_coff + C || o.out_coff >= coff + C; };
+                bool sep = apart(o.base_buf, o.base_coff) || o.base_coff == o.out_coff;
+                for (int s = 0; s < n_src; ++s) sep = sep && apart(o.src[s].buf, o.src[s].coff);
                 ADAS_CHECK(sep, "plan %s: op %zu: cbfuse source slice overlaps the output (only the base may be the output slice itself)", path, oi);
                 break;
             }
             case OP_SE: {
-                const int C = p[2], hid = p[3];
-                ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[8]), "plan %s: op %zu: se buffer index out of range", path, oi);
-                const PlanBuffer &ib = e->bufs[p[0]], &ob = e->bufs[p[8]];
+                const SeOp o = op_fields<SeOp>(op);
+                const int C = o.C, hid = o.hid;
+                ADAS_CHECK(buf_ok(o.in_buf) && buf_ok(o.out_buf), "plan %s: op %zu: se buffer index out of range", path, oi);
+                const PlanBuffer &ib = e->bufs[o.in_buf], &ob = e->bufs[o.out_buf];
                 ADAS_CHECK(ib.dtype == 0 && ob.dtype == 0, "plan %s: op %zu: se buffers must be fp16", path, oi);
                 ADAS_CHECK(ib.H > 0 && ob.H == ib.H && ob.W == ib.W, "plan %s: op %zu: se output must have its input's H x W", path, oi);
                 ADAS_CHECK(se_supported(C, hid), "plan %s: op %zu: se with %d channels and %d hidden (C a multiple of 8 up to %d, 1 to %d hidden)", path, oi, C, hid,
                            kSeMaxC, kSeMaxC / 4);
-                ADAS_CHECK(p[1] % 8 == 0 && p[9] % 8 == 0 && ib.C % 8 == 0 && ob.C % 8 == 0, "plan %s: op %zu: se channels and offsets must be multiples of 8", path, oi);
+                ADAS_CHECK(o.in_coff % 8 == 0 && o.out_coff % 8 == 0 && ib.C % 8 == 0 && ob.C % 8 == 0, "plan %s: op %zu: se channels and offsets must be multiples of 8", path, oi);
+                const int tensors[4] = {o.w1, o.b1, o.w2, o.b2};
                 const uint64_t sz[4] = {(uint64_t)hid * C * 4, (uint64_t)hid * 4, (uint64_t)C * hid * 4, (uint64_t)C * 4};
                 for (int t = 0; t < 4; ++t)
-                    ADAS_CHECK(tensor_ok(p[4 + t], 0) && e->tensors[p[4 + t]].dtype == 1 && e->tensors[p[4 + t]].bytes == sz[t],
+                    ADAS_CHECK(tensor_ok(tensors[t], 0) && e->tensors[tensors[t]].dtype == 1 && e->tensors[tensors[t]].bytes == sz[t],
                                "plan %s: op %zu: se tensor %d must be fp32 of %llu bytes (w1 [hid][C], b1 [hid], w2 [C][hid], b2 [C])", path, oi, t,
                                (unsigned long long)sz[t]);
-                ADAS_CHECK(view_ok(p[0], p[1], C) && view_ok(p[8], p[9], C) && (p[0] != p[8] || p[1] == p[9] || p[9] >= p[1] + C || p[1] >= p[9] + C),
+                ADAS_CHECK(view_ok(o.in_buf, o.in_coff, C) && view_ok(o.out_buf, o.out_coff, C) &&
+                               (o.in_buf != o.out_buf || o.in_coff == o.out_coff || o.out_coff >= o.in_coff + C || o.in_coff >= o.out_coff + C),
                            "plan %s: op %zu: se channel slice exceeds its buffer or partly overlaps its input (in place or apart)", path, oi);
                 break;
             }
             case OP_SHUFFLE2: {
-                const int n = p[4];
-                ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[2]) && buf_ok(p[5]), "plan %s: op %zu: shuffle2 buffer index out of range", path, oi);
-                const PlanBuffer &ab = e->bufs[p[0]], &bb = e->bufs[p[2]], &ob = e->bufs[p[5]];
+                const Shuffle2Op o = op_fields<Shuffle2Op>(op);
+                const int n = o.n;
+                ADAS_CHECK(buf_ok(o.a_buf) && buf_ok(o.b_buf) && buf_ok(o.out_buf), "plan %s: op %zu: shuffle2 buffer index out of range", path, oi);
+                const PlanBuffer &ab = e->bufs[o.a_buf], &bb = e->bufs[o.b_buf], &ob = e->bufs[o.out_buf];
                 ADAS_CHECK(ab.dtype == 0 && bb.dtype == 0 && ob.dtype == 0, "plan %s: op %zu: shuffle2 buffers must be fp16", path, oi);
                 ADAS_CHECK(ob.H > 0 && ab.H == ob.H && ab.W == ob.W && bb.H == ob.H && bb.W == ob.W, "plan %s: op %zu: shuffle2 sources must have the output's H x W", path, oi);
-                ADAS_CHECK(n >= 8 && n % 8 == 0 && p[1] % 8 == 0 && p[3] % 8 == 0 && p[6] % 8 == 0 && ab.C % 8 == 0 && bb.C % 8 == 0 && ob.C % 8 == 0,
+                ADAS_CHECK(n >= 8 && n % 8 == 0 && o.a_coff % 8 == 0 && o.b_coff % 8 == 0 && o.out_coff % 8 == 0 && ab.C % 8 == 0 && bb.C % 8 == 0 && ob.C % 8 == 0,
                            "plan %s: op %zu: shuffle2 channels and offsets must be multiples of 8", path, oi);
-                ADAS_CHECK(view_ok(p[0], p[1], n) && view_ok(p[2], p[3], n) && (uint64_t)n * 2 <= (1u << 20) && view_ok(p[5], p[6], 2 * n),
+                ADAS_CHECK(view_ok(o.a_buf, o.a_coff, n) && view_ok(o.b_buf, o.b_coff, n) && (uint64_t)n * 2 <= (1u << 20) && view_ok(o.out_buf, o.out_coff, 2 * n),
                            "plan %s: op %zu: shuffle2 channel slice exceeds its buffer", path, oi);
-                auto apart = [&](int b, int coff) { return b != p[5] || coff >= p[6] + 2 * n || p[6] >= coff + n; };
-                ADAS_CHECK(apart(p[0], p[1]) && apart(p[2], p[3]), "plan %s: op %zu: shuffle2 output overlaps a source", path, oi);
+                auto apart = [&](int b, int coff) { return b != o.out_buf || coff >= o.out_coff + 2 * n || o.out_coff >= coff + n; };
+                ADAS_CHECK(apart(o.a_buf, o.a_coff) && apart(o.b_buf, o.b_coff), "plan %s: op %zu: shuffle2 output overlaps a source", path, oi);
                 break;
             }
-            case OP_STEMPACK:
-                ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[1]) && e->bufs[p[0]].H > 0 && e->bufs[p[1]].H > 0 && e->bufs[p[0]].C == 4 && e->bufs[p[1]].C == 64 &&
-                           e->bufs[p[0]].dtype == 0 && e->bufs[p[1]].dtype == 0 && e->bufs[p[1]].H * 2 == e->bufs[p[0]].H && e->bufs[p[1]].W * 2 == e->bufs[p[0]].W,
+            case OP_STEMPACK: {
+                const StempackOp o = op_fields<StempackOp>(op);
+                ADAS_CHECK(buf_ok(o.in_buf) && buf_ok(o.out_buf) && e->bufs[o.in_buf].H > 0 && e->bufs[o.out_buf].H > 0 && e->bufs[o.in_buf].C == 4 && e->bufs[o.out_buf].C == 64 &&
+                           e->bufs[o.in_buf].dtype == 0 && e->bufs[o.out_buf].dtype == 0 && e->bufs[o.out_buf].H * 2 == e->bufs[o.in_buf].H &&
+                           e->bufs[o.out_buf].W * 2 == e->bufs[o.in_buf].W,
                            "plan %s: op %zu: bad stem re-layout", path, oi);
                 break;
+            }
             case OP_STEMCONV: {
-                const int Cout = p[3], k = p[4], s = p[9] == 0 ? 2 : p[9];          // p[9] = 0: stride 2 (plans without the field)
-                ADAS_CHECK(act_code_ok(p[6]), "plan %s: op %zu: unknown activation %d", path, oi, p[6]);
-                ADAS_CHECK((s == 1 || s == 2) && buf_ok(p[0]) && e->bufs[p[0]].H > 0 && e->bufs[p[0]].C == 4 && e->bufs[p[0]].dtype == 0 && stem_conv_supported(Cout, k, p[5]) &&
-                           buf_ok(p[7]) && e->bufs[p[7]].dtype == 0 && p[8] % 8 == 0 && e->bufs[p[7]].C % 8 == 0 &&
-                           view_ok(p[7], p[8], Cout) && e->bufs[p[7]].H > 0 && tensor_ok(p[1], (uint64_t)Cout * k * ((4 * k + 15) / 16 * 16) * 2) &&
-                           (p[2] < 0 || tensor_ok(p[2], (uint64_t)Cout * 4)) &&
-                           e->bufs[p[7]].H == (e->bufs[p[0]].H + 2 * p[5] - k) / s + 1 && e->bufs[p[7]].W == (e->bufs[p[0]].W + 2 * p[5] - k) / s + 1,
+                const StemconvOp o = op_fields<StemconvOp>(op);
+                const int Cout = o.Cout, k = o.k, s = o.stride == 0 ? 2 : o.stride;      // stride 0: 2 (plans without the field)
+                ADAS_CHECK(act_code_ok(o.act), "plan %s: op %zu: unknown activation %d", path, oi, o.act);
+                ADAS_CHECK((s == 1 || s == 2) && buf_ok(o.in_buf) && e->bufs[o.in_buf].H > 0 && e->bufs[o.in_buf].C == 4 && e->bufs[o.in_buf].dtype == 0 &&
+                           stem_conv_supported(Cout, k, o.pad) && buf_ok(o.out_buf) && e->bufs[o.out_buf].dtype == 0 && o.out_coff % 8 == 0 && e->bufs[o.out_buf].C % 8 == 0 &&
+                           view_ok(o.out_buf, o.out_coff, Cout) && e->bufs[o.out_buf].H > 0 && tensor_ok(o.w_tensor, (uint64_t)Cout * k * ((4 * k + 15) / 16 * 16) * 2) &&
+                           (o.bias_tensor < 0 || tensor_ok(o.bias_tensor, (uint64_t)Cout * 4)) &&
+                           e->bufs[o.out_buf].H == (e->bufs[o.in_buf].H + 2 * o.pad - k) / s + 1 && e->bufs[o.out_buf].W == (e->bufs[o.in_buf].W + 2 * o.pad - k) / s + 1,
                            "plan %s: op %zu: bad stem conv", path, oi);
                 break;
             }
             case OP_LAYERNORM: {
-                ADAS_CHECK(buf_ok(p[0]) && buf_ok(p[4]) && p[1] >= 1 && p[5] >= 1 && p[5] <= p[1] && e->bufs[p[0]].dtype == 0 && e->bufs[p[4]].dtype == 0,
+                const LayernormOp o = op_fields<LayernormOp>(op);
+                ADAS_CHECK(buf_ok(o.in_buf) && buf_ok(o.out_buf) && o.d_len >= 1 && o.d_norm >= 1 && o.d_norm <= o.d_len && e->bufs[o.in_buf].dtype == 0 &&
+                           e->bufs[o.out_buf].dtype == 0,
                            "plan %s: op %zu: bad layernorm", path, oi);
-                const PlanBuffer &ib = e->bufs[p[0]], &ob = e->bufs[p[4]];
-                ADAS_CHECK((uint64_t)p[1] <= (uint64_t)ib.rows_per_img * ib.C && (uint64_t)p[1] <= (uint64_t)ob.rows_per_img * ob.C && tensor_ok(p[2], (uint64_t)p[1] * 4) && tensor_ok(p[3], (uint64_t)p[1] * 4),
+                const PlanBuffer &ib = e->bufs[o.in_buf], &ob = e->bufs[o.out_buf];
+                ADAS_CHECK((uint64_t)o.d_len <= (uint64_t)ib.rows_per_img * ib.C && (uint64_t)o.d_len <= (uint64_t)ob.rows_per_img * ob.C &&
+                           tensor_ok(o.gamma_tensor, (uint64_t)o.d_len * 4) && tensor_ok(o.beta_tensor, (uint64_t)o.d_len * 4),
                            "plan %s: op %zu: layernorm vector exceeds its buffers", path, oi);
                 break;
             }

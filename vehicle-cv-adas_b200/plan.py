@@ -32,14 +32,85 @@ import numpy as np
 
 MODEL_YOLOV8, MODEL_YOLOV5, MODEL_UFLDV2, MODEL_UFLDV1 = 0, 1, 2, 4      # 3 = ADAS_MODEL_YOLOV5_LITE (post-processing kind only)
 MODEL_YOLOV6 = 5                                                         # anchor-free head, [B, 8400, 5 + nc] output; meta[2] = reg_max
-OP_GEMM, OP_IM2COL, OP_MAXPOOL, OP_UPSAMPLE2X, OP_LAYERNORM, OP_STEMPACK, OP_STEMCONV = 1, 2, 3, 4, 5, 6, 7
-OP_AVGPOOL2 = 8
-OP_DWCONV, OP_ATTN = 9, 10
-OP_CBFUSE = 11
-OP_SE, OP_SHUFFLE2 = 12, 13
 ACT_NONE, ACT_SILU, ACT_RELU, ACT_LEAKY = 0, 1, 2, 3          # ACT_LEAKY: LeakyReLU(0.1)
 ACT_HSWISH = 5                                                # Hardswish x * clamp(x + 3, 0, 6) / 6; code 4 is unused
 PLAN_VERSION = 1
+
+# ---------------------------------------------------------------------------------------------
+# record layout (csrc/plan.h)
+# ---------------------------------------------------------------------------------------------
+HDR_FMT, BUF_FMT, OP_FMT, TEN_FMT, OUT_FMT = "<8sII3I4I16IQQ", "<6I", "<I23i4f", "<QQII", "<4I"
+HDR_SIZE, BUF_SIZE, OP_SIZE, TEN_SIZE, OUT_SIZE = (struct.calcsize(f) for f in (HDR_FMT, BUF_FMT, OP_FMT, TEN_FMT, OUT_FMT))
+OP_NP, OP_NF = 23, 4                                          # PlanOp: type, int32 p[23], float f[4]
+
+OP_GEMM, OP_IM2COL, OP_MAXPOOL, OP_UPSAMPLE2X, OP_LAYERNORM, OP_STEMPACK, OP_STEMCONV = 1, 2, 3, 4, 5, 6, 7
+OP_AVGPOOL2, OP_DWCONV, OP_ATTN, OP_CBFUSE, OP_SE, OP_SHUFFLE2 = 8, 9, 10, 11, 12, 13
+OP_NAMES = {OP_GEMM: "gemm", OP_IM2COL: "im2col", OP_MAXPOOL: "maxpool", OP_UPSAMPLE2X: "upsample", OP_LAYERNORM: "layernorm",
+            OP_STEMPACK: "stempack", OP_STEMCONV: "stemconv", OP_AVGPOOL2: "avgpool2", OP_DWCONV: "dwconv", OP_ATTN: "attention",
+            OP_CBFUSE: "cbfuse", OP_SE: "se", OP_SHUFFLE2: "shuffle2"}
+# The fields of PlanOp.p per op type, in slot order: the members of plan.h's op structs (OP_GEMM: GemmOp, ...).  What each field
+# means is documented there.
+OP_FIELDS = {
+    OP_GEMM: ("a_buf", "a_coff", "Kc", "ntaps", "w_tensor", "bias_tensor", "N", "act", "res_buf", "res_coff", "res_pre_act", "out_buf",
+              "out_coff", "masked", "transposed", "BN", "s2", "MT", "no_slab", "up2"),
+    OP_IM2COL: ("in_buf", "in_coff", "Cin", "kh", "kw", "stride", "pad", "out_buf"),
+    OP_MAXPOOL: ("in_buf", "in_coff", "C", "k", "stride", "pad", "out_buf", "out_coff"),
+    OP_UPSAMPLE2X: ("in_buf", "in_coff", "C", "out_buf", "out_coff"),
+    OP_LAYERNORM: ("in_buf", "d_len", "gamma_tensor", "beta_tensor", "out_buf", "d_norm"),
+    OP_STEMPACK: ("in_buf", "out_buf"),
+    OP_STEMCONV: ("in_buf", "w_tensor", "bias_tensor", "Cout", "k", "pad", "act", "out_buf", "out_coff", "stride"),
+    OP_AVGPOOL2: ("in_buf", "in_coff", "C", "out_buf", "out_coff", "fill"),
+    OP_DWCONV: ("in_buf", "in_coff", "C", "k", "stride", "act", "w_tensor", "bias_tensor", "out_buf", "out_coff", "res_buf", "res_coff"),
+    OP_ATTN: ("in_buf", "in_coff", "nh", "kdp", "hd", "out_buf", "out_coff"),
+    OP_CBFUSE: ("out_buf", "out_coff", "C", "base_buf", "base_coff", "n_src"),     # then CBFUSE_MAX_SRC x CBFUSE_SRC_FIELDS
+    OP_SE: ("in_buf", "in_coff", "C", "hid", "w1", "b1", "w2", "b2", "out_buf", "out_coff"),
+    OP_SHUFFLE2: ("a_buf", "a_coff", "b_buf", "b_coff", "n", "out_buf", "out_coff"),
+}
+CBFUSE_SRC_FIELDS, CBFUSE_MAX_SRC = ("buf", "coff", "shift"), 5
+OP_FLOATS = {OP_GEMM: ("res_scale",), OP_LAYERNORM: ("eps",), OP_ATTN: ("scale",)}      # the named entries of PlanOp.f
+_FIELD_SLOT = {t: {n: i for i, n in enumerate(names)} for t, names in OP_FIELDS.items()}
+
+
+class OpParams(list):
+    """PlanOp.p of one op: the 23 int32 slots as a list (so it packs, indexes and compares as one), whose fields of OP_FIELDS[typ]
+    also read and write by name (`p.out_buf`, `p.BN = 64`).  A name the op type does not have is an error."""
+    __slots__ = ("typ",)
+
+    def __init__(self, typ: int, values=()):
+        values = list(values)
+        assert len(values) <= OP_NP, (typ, values)
+        super().__init__(values + [0] * (OP_NP - len(values)))
+        object.__setattr__(self, "typ", typ)
+
+    def __getattr__(self, name: str) -> int:
+        return self[field_slot(self.typ, name)]
+
+    def __setattr__(self, name: str, value: int) -> None:
+        self[field_slot(self.typ, name)] = value
+
+    def copy(self) -> "OpParams":
+        return OpParams(self.typ, self)
+
+    def __reduce__(self):                                     # copy.copy / deepcopy / pickle rebuild through __init__
+        return OpParams, (self.typ, list(self))
+
+
+def field_slot(typ: int, name: str) -> int:
+    """Slot of field `name` of op type `typ` in PlanOp.p."""
+    try:
+        return _FIELD_SLOT[typ][name]
+    except KeyError:
+        raise AttributeError(f"{OP_NAMES.get(typ, typ)} op has no field {name!r}") from None
+
+
+def cbfuse_src_slot(s: int) -> int:
+    """Slot of the first field of source s of an OP_CBFUSE op in PlanOp.p."""
+    return len(OP_FIELDS[OP_CBFUSE]) + len(CBFUSE_SRC_FIELDS) * s
+
+
+def cbfuse_sources(p: OpParams) -> List[Tuple[int, int, int]]:
+    """(buffer, channel offset, shift) of each source of an OP_CBFUSE op, in summation order."""
+    return [tuple(p[cbfuse_src_slot(s):cbfuse_src_slot(s + 1)]) for s in range(p.n_src)]
 
 
 def cache_dir() -> str:
@@ -337,7 +408,7 @@ class PlanBuilder:
     def __init__(self, model_kind: int, in_c: int, in_h: int, in_w: int):
         self.model_kind, self.in_c, self.in_h, self.in_w = model_kind, in_c, in_h, in_w
         self.buffers: List[Tuple[int, int, int, int, int, int]] = []   # rows_per_img, C, dtype, H, W, flags
-        self.ops: List[Tuple[int, List[int], List[float]]] = []
+        self.ops: List[Tuple[int, OpParams, List[float]]] = []
         self.tensors: List[np.ndarray] = []
         self.outputs: List[Tuple[int, int, int, int]] = []
         self.meta = [0] * 16
@@ -370,10 +441,13 @@ class PlanBuilder:
         return View(v.buf, v.coff + coff, C, v.H, v.W)
 
     # -- ops ----------------------------------------------------------------------------------
-    def _op(self, typ: int, p: List[int], f: Optional[List[float]] = None) -> None:
-        p = list(p) + [0] * (23 - len(p))
-        f = list(f or []) + [0.0] * (4 - len(f or []))
-        self.ops.append((typ, p, f))
+    def _op(self, typ: int, f: Optional[List[float]] = None, **fields: int) -> OpParams:
+        """Append an op of type `typ` with the named fields of OP_FIELDS[typ] (the others 0) and floats f (the others 0.0)."""
+        p = OpParams(typ)
+        for name, v in fields.items():
+            setattr(p, name, v)
+        self.ops.append((typ, p, list(f or []) + [0.0] * (OP_NF - len(f or []))))
+        return p
 
     def conv(self, x: View, w: np.ndarray, b: Optional[np.ndarray], k: int, s: int, act: int, out: Optional[View] = None,
              res: Optional[View] = None, res_pre_act: bool = False, out_f32: bool = False, pad: Optional[int] = None,
@@ -431,14 +505,15 @@ class PlanBuilder:
             Kpad = (k * k * cin + 7) // 8 * 8
             self.buffers.append(((Ho + 2) * (Wo + 2), Kpad, 0, Ho, Wo, 0))
             pb = len(self.buffers) - 1
-            self._op(OP_IM2COL, [x.buf, x.coff, cin, k, k, s, pad, pb])
+            self._op(OP_IM2COL, in_buf=x.buf, in_coff=x.coff, Cin=cin, kh=k, kw=k, stride=s, pad=pad, out_buf=pb)
             a, ntaps, Kc = View(pb, 0, Kpad, Ho, Wo), 1, Kpad
             if Kpad != wk.shape[1]:
                 wk = np.concatenate([wk, np.zeros((wk.shape[0], Kpad - wk.shape[1]), np.float32)], 1)
         w_t = self.tensor(wk.astype(np.float16))
         bn, mt = tile if tile is not None else (0, 0)          # (BN, MT) forced by tests; 0 = cost model + autotune
-        self._op(OP_GEMM, [a.buf, a.coff, Kc, ntaps, w_t, bias_t, n_store, act, res_buf, res_coff, 1 if res_pre_act else 0,
-                           out.buf, out.coff, 1, 0, bn, s2, mt, 1 if no_slab else 0], [res_scale] if res_scale is not None else None)
+        self._op(OP_GEMM, [res_scale] if res_scale is not None else None, a_buf=a.buf, a_coff=a.coff, Kc=Kc, ntaps=ntaps, w_tensor=w_t,
+                 bias_tensor=bias_t, N=n_store, act=act, res_buf=res_buf, res_coff=res_coff, res_pre_act=1 if res_pre_act else 0,
+                 out_buf=out.buf, out_coff=out.coff, masked=1, BN=bn, s2=s2, MT=mt, no_slab=1 if no_slab else 0)
         return View(out.buf, out.coff, cout, Ho, Wo)
 
     def conv_transpose2x2(self, x: View, w: np.ndarray, b: Optional[np.ndarray], out: View, tile: Optional[Tuple[int, int]] = None) -> View:
@@ -452,8 +527,8 @@ class PlanBuilder:
         wk = np.transpose(w, (2, 3, 1, 0)).reshape(4 * cout, cin)             # [dy, dx, Cout, Cin]
         bias_t = self.tensor(np.tile(b.astype(np.float32), 4)) if b is not None else -1
         bn, mt = tile if tile is not None else (0, 0)
-        self._op(OP_GEMM, [x.buf, x.coff, cin, 1, self.tensor(wk.astype(np.float16)), bias_t, 4 * cout, ACT_NONE, -1, 0, 0,
-                           out.buf, out.coff, 1, 0, bn, 0, mt, 0, 1])
+        self._op(OP_GEMM, a_buf=x.buf, a_coff=x.coff, Kc=cin, ntaps=1, w_tensor=self.tensor(wk.astype(np.float16)), bias_tensor=bias_t,
+                 N=4 * cout, act=ACT_NONE, res_buf=-1, out_buf=out.buf, out_coff=out.coff, masked=1, BN=bn, MT=mt, up2=1)
         return View(out.buf, out.coff, cout, out.H, out.W)
 
     def stem_conv(self, x: View, w: np.ndarray, b: Optional[np.ndarray], k: int, s: int, pad: int, act: int, out: View) -> View:
@@ -467,7 +542,8 @@ class PlanBuilder:
         w_t = self.tensor(wq.astype(np.float16))
         bias_t = self.tensor(b.astype(np.float32)) if b is not None else -1
         self.stem_flops_per_img += 2 * out.H * out.W * cout * 3 * k * k
-        self._op(OP_STEMCONV, [x.buf, w_t, bias_t, cout, k, pad, act, out.buf, out.coff, 0 if s == 2 else s])   # 0 = stride 2
+        self._op(OP_STEMCONV, in_buf=x.buf, w_tensor=w_t, bias_tensor=bias_t, Cout=cout, k=k, pad=pad, act=act, out_buf=out.buf,
+                 out_coff=out.coff, stride=0 if s == 2 else s)   # 0 = stride 2
         return View(out.buf, out.coff, cout, out.H, out.W)
 
     def stem7x7s2(self, x: View, w: np.ndarray, b: np.ndarray, act: int) -> View:
@@ -479,7 +555,7 @@ class PlanBuilder:
         Ho, Wo = x.H // 2, x.W // 2
         self.flops_per_img += 2 * Ho * Wo * cout * cin_real * 49
         q = self.new_padded(Ho, Wo, 64)
-        self._op(OP_STEMPACK, [x.buf, q.buf])
+        self._op(OP_STEMPACK, in_buf=x.buf, out_buf=q.buf)
         wq = np.zeros((cout, 4, 2, 8, 4), np.float32)             # [n][t][p][kx(7 used of 8)][c]
         for t in range(4):
             for pp in range(2):
@@ -490,7 +566,8 @@ class PlanBuilder:
         w_t = self.tensor(wq.reshape(cout, 256).astype(np.float16))
         bias_t = self.tensor(b.astype(np.float32))
         # ntaps = 4 selects the vertical tap table (row shifts -2, -1, 0, +1 padded rows)
-        self._op(OP_GEMM, [q.buf, 0, 64, 4, w_t, bias_t, cout, act, -1, 0, 0, out.buf, 0, 1, 0, 0, 0])
+        self._op(OP_GEMM, a_buf=q.buf, Kc=64, ntaps=4, w_tensor=w_t, bias_tensor=bias_t, N=cout, act=act, res_buf=-1, out_buf=out.buf,
+                 masked=1)
         return View(out.buf, 0, cout, Ho, Wo)
 
     def maxpool(self, x: View, k: int, s: int, p: int, out: Optional[View] = None) -> View:
@@ -499,7 +576,7 @@ class PlanBuilder:
         if out is None:
             out = self.new_padded(Ho, Wo, x.C)
         assert out.H == Ho and out.W == Wo and x.C % 8 == 0
-        self._op(OP_MAXPOOL, [x.buf, x.coff, x.C, k, s, p, out.buf, out.coff])
+        self._op(OP_MAXPOOL, in_buf=x.buf, in_coff=x.coff, C=x.C, k=k, stride=s, pad=p, out_buf=out.buf, out_coff=out.coff)
         return View(out.buf, out.coff, x.C, Ho, Wo)
 
     def avgpool2(self, x: View, fill: int, out: Optional[View] = None) -> View:
@@ -509,7 +586,7 @@ class PlanBuilder:
         if out is None:
             out = self.new_padded(x.H, x.W, x.C)
         assert out.H == x.H and out.W == x.W and x.C % 8 == 0 and x.coff % 8 == 0 and out.coff % 8 == 0 and fill in (0, 1)
-        self._op(OP_AVGPOOL2, [x.buf, x.coff, x.C, out.buf, out.coff, fill])
+        self._op(OP_AVGPOOL2, in_buf=x.buf, in_coff=x.coff, C=x.C, out_buf=out.buf, out_coff=out.coff, fill=fill)
         return View(out.buf, out.coff, x.C, x.H, x.W)
 
     def dwconv(self, x: View, w: np.ndarray, b: np.ndarray, k: int, s: int, act: int, out: Optional[View] = None,
@@ -534,8 +611,9 @@ class PlanBuilder:
         f = 2 * Ho * Wo * c_real * k * k
         self.flops_per_img += f
         self.dw_flops_per_img += f
-        self._op(OP_DWCONV, [x.buf, x.coff, x.C, k, s, act, self.tensor(wk.astype(np.float16)), self.tensor(bk), out.buf, out.coff,
-                             res.buf if res is not None else -1, res.coff if res is not None else 0])
+        self._op(OP_DWCONV, in_buf=x.buf, in_coff=x.coff, C=x.C, k=k, stride=s, act=act, w_tensor=self.tensor(wk.astype(np.float16)),
+                 bias_tensor=self.tensor(bk), out_buf=out.buf, out_coff=out.coff, res_buf=res.buf if res is not None else -1,
+                 res_coff=res.coff if res is not None else 0)
         return View(out.buf, out.coff, x.C, Ho, Wo)
 
     def attention(self, qkv: View, nh: int, kdp: int, hd: int, scale: float, out: Optional[View] = None) -> View:
@@ -545,12 +623,12 @@ class PlanBuilder:
         if out is None:
             out = self.new_padded(qkv.H, qkv.W, nh * hd)
         assert out.H == qkv.H and out.W == qkv.W and out.coff % 8 == 0, out
-        self._op(OP_ATTN, [qkv.buf, qkv.coff, nh, kdp, hd, out.buf, out.coff], [scale])
+        self._op(OP_ATTN, [scale], in_buf=qkv.buf, in_coff=qkv.coff, nh=nh, kdp=kdp, hd=hd, out_buf=out.buf, out_coff=out.coff)
         return View(out.buf, out.coff, nh * hd, qkv.H, qkv.W)
 
     def upsample2x(self, x: View, out: View) -> View:
         assert out.H == 2 * x.H and out.W == 2 * x.W and x.C % 8 == 0
-        self._op(OP_UPSAMPLE2X, [x.buf, x.coff, x.C, out.buf, out.coff])
+        self._op(OP_UPSAMPLE2X, in_buf=x.buf, in_coff=x.coff, C=x.C, out_buf=out.buf, out_coff=out.coff)
         return View(out.buf, out.coff, x.C, out.H, out.W)
 
     def cbfuse(self, base: View, srcs: Sequence[Tuple[View, int]], out: Optional[View] = None) -> View:
@@ -559,12 +637,12 @@ class PlanBuilder:
         out = base if out is None else out
         assert 1 <= len(srcs) <= 5 and base.C == out.C and base.C % 8 == 0 and base.coff % 8 == 0 and out.coff % 8 == 0, (base, out)
         assert (base.H, base.W) == (out.H, out.W), (base, out)
-        p = [out.buf, out.coff, out.C, base.buf, base.coff, len(srcs)]
         for v, shift in srcs:
             assert v.C == out.C and v.coff % 8 == 0 and 0 <= shift <= 4 and (v.H << shift, v.W << shift) == (out.H, out.W), (v, shift, out)
             assert v.buf != out.buf or v.coff >= out.coff + out.C or out.coff >= v.coff + v.C, (v, out)
-            p += [v.buf, v.coff, shift]
-        self._op(OP_CBFUSE, p)
+        p = self._op(OP_CBFUSE, out_buf=out.buf, out_coff=out.coff, C=out.C, base_buf=base.buf, base_coff=base.coff, n_src=len(srcs))
+        for s, (v, shift) in enumerate(srcs):
+            p[cbfuse_src_slot(s):cbfuse_src_slot(s + 1)] = [v.buf, v.coff, shift]
         return View(out.buf, out.coff, out.C, out.H, out.W)
 
     def se(self, x: View, w1: np.ndarray, b1: np.ndarray, w2: np.ndarray, b2: np.ndarray, out: Optional[View] = None) -> View:
@@ -581,8 +659,8 @@ class PlanBuilder:
         w2p[:c_real] = w2.reshape(c_real, hid)
         b2p = np.zeros(x.C, np.float32)
         b2p[:c_real] = b2
-        self._op(OP_SE, [x.buf, x.coff, x.C, hid, self.tensor(w1p), self.tensor(np.asarray(b1, np.float32).reshape(hid)),
-                         self.tensor(w2p), self.tensor(b2p), out.buf, out.coff])
+        self._op(OP_SE, in_buf=x.buf, in_coff=x.coff, C=x.C, hid=hid, w1=self.tensor(w1p), b1=self.tensor(np.asarray(b1, np.float32).reshape(hid)),
+                 w2=self.tensor(w2p), b2=self.tensor(b2p), out_buf=out.buf, out_coff=out.coff)
         return View(out.buf, out.coff, x.C, x.H, x.W)
 
     def shuffle2(self, a: View, b: View, out: Optional[View] = None) -> View:
@@ -594,45 +672,43 @@ class PlanBuilder:
         assert out.C == 2 * n and (out.H, out.W) == (a.H, a.W) and out.coff % 8 == 0, out
         for v in (a, b):
             assert v.buf != out.buf or v.coff >= out.coff + 2 * n or out.coff >= v.coff + n, (v, out)
-        self._op(OP_SHUFFLE2, [a.buf, a.coff, b.buf, b.coff, n, out.buf, out.coff])
+        self._op(OP_SHUFFLE2, a_buf=a.buf, a_coff=a.coff, b_buf=b.buf, b_coff=b.coff, n=n, out_buf=out.buf, out_coff=out.coff)
         return View(out.buf, out.coff, 2 * n, a.H, a.W)
 
     def layernorm(self, in_buf: int, d_len: int, d_norm: int, gamma: np.ndarray, beta: np.ndarray, eps: float, out_buf: int) -> None:
-        self._op(OP_LAYERNORM, [in_buf, d_len, self.tensor(gamma.astype(np.float32)), self.tensor(beta.astype(np.float32)), out_buf, d_norm],
-                 [eps])
+        self._op(OP_LAYERNORM, [eps], in_buf=in_buf, d_len=d_len, gamma_tensor=self.tensor(gamma.astype(np.float32)),
+                 beta_tensor=self.tensor(beta.astype(np.float32)), out_buf=out_buf, d_norm=d_norm)
 
     def fc(self, in_buf: int, K: int, w: np.ndarray, b: np.ndarray, act: int, out_buf: int) -> None:
         """swap-AB GEMM: weights [Nout, K] stream through the A operand once per batch."""
         nout = int(w.shape[0])
         assert w.shape[1] == K and K % 8 == 0
-        self._op(OP_GEMM, [in_buf, 0, K, 1, self.tensor(w.astype(np.float16)), self.tensor(b.astype(np.float32)), nout, act, -1, 0, 0,
-                           out_buf, 0, 0, 1, 0])
+        self._op(OP_GEMM, a_buf=in_buf, Kc=K, ntaps=1, w_tensor=self.tensor(w.astype(np.float16)), bias_tensor=self.tensor(b.astype(np.float32)),
+                 N=nout, act=act, res_buf=-1, out_buf=out_buf, transposed=1)
 
     # -- serialisation ---------------------------------------------------------------------------
     def write(self, path: str) -> None:
-        hdr_fmt = "<8sII3I4I16IQQ"
-        hdr_size = struct.calcsize(hdr_fmt)
         rec = bytearray()
         for b in self.buffers:
-            rec += struct.pack("<6I", *b)
+            rec += struct.pack(BUF_FMT, *b)
         for typ, p, f in self.ops:
-            rec += struct.pack("<I23i4f", typ, *p, *f)
+            rec += struct.pack(OP_FMT, typ, *p, *f)
         offs = []
         off = 0
         for t in self.tensors:
             offs.append(off)
             off += (t.nbytes + 255) // 256 * 256
         for t, o in zip(self.tensors, offs):
-            rec += struct.pack("<QQII", o, t.nbytes, 1 if t.dtype == np.float32 else 0, 0)
+            rec += struct.pack(TEN_FMT, o, t.nbytes, 1 if t.dtype == np.float32 else 0, 0)
         for o in self.outputs:
-            rec += struct.pack("<4I", *o)
-        blob_offset = (hdr_size + len(rec) + 255) // 256 * 256
-        hdr = struct.pack(hdr_fmt, b"B200PLAN", PLAN_VERSION, self.model_kind, self.in_c, self.in_h, self.in_w, len(self.buffers),
+            rec += struct.pack(OUT_FMT, *o)
+        blob_offset = (HDR_SIZE + len(rec) + 255) // 256 * 256
+        hdr = struct.pack(HDR_FMT, b"B200PLAN", PLAN_VERSION, self.model_kind, self.in_c, self.in_h, self.in_w, len(self.buffers),
                           len(self.ops), len(self.tensors), len(self.outputs), *self.meta, blob_offset, off)
         with open(path, "wb") as f:
             f.write(hdr)
             f.write(rec)
-            f.write(b"\0" * (blob_offset - hdr_size - len(rec)))
+            f.write(b"\0" * (blob_offset - HDR_SIZE - len(rec)))
             for t in self.tensors:
                 f.write(t.tobytes())
                 padn = (-t.nbytes) % 256
@@ -1105,12 +1181,12 @@ def read_anchors(path: str) -> np.ndarray:
     YOLOv5 table (L = 3)."""
     with open(path, "rb") as f:
         raw = f.read()
-    h = struct.unpack_from("<8sII3I4I16IQQ", raw)
+    h = struct.unpack_from(HDR_FMT, raw)
     n_buf, n_ops, n_t, n_out, meta, blob = h[6], h[7], h[8], h[9], h[10:26], h[26]
     if meta[3] == 0:
         return np.asarray(YOLOV5_ANCHORS, np.float32).reshape(3, 3, 2)
-    rec = struct.calcsize("<8sII3I4I16IQQ") + n_buf * 24 + n_ops * 112 + (meta[3] - 1) * 24
-    off, nbytes, _, _ = struct.unpack_from("<QQII", raw, rec)
+    rec = HDR_SIZE + n_buf * BUF_SIZE + n_ops * OP_SIZE + (meta[3] - 1) * TEN_SIZE
+    off, nbytes, _, _ = struct.unpack_from(TEN_FMT, raw, rec)
     assert meta[3] <= n_t and nbytes == 24 * n_out
     return np.frombuffer(raw, np.float32, 6 * n_out, blob + off).reshape(n_out, 3, 2).copy()
 

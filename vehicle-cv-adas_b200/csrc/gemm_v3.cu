@@ -19,6 +19,8 @@
 // 128/64/32/16 columns) and runs the epilogue of those rows straight from its accumulator registers: +bias -> activation ->
 // (+residual) -> fp16/fp32 stores of interior rows (the zero halo of padded outputs is never written).  Persistent: grid =
 // min(tiles, SMs); the producer runs ahead into the next tile while the consumers finish the epilogue of the current one.
+// The consumers' tile loop is compiled once per (sub-tile count, taps per stage) and picked once per CTA, so a stage's wgmmas
+// are issued as one unbroken chain with compile-time operand offsets (v3_mainloop).
 //
 // Function attributes and the SM count are per device (a process may hold engines on several GPUs).
 #include "common.h"
@@ -41,10 +43,203 @@ __device__ __forceinline__ float v3_act(float x, int act) {
     else return act_apply_base(x, act);
 }
 
+// Layout of one pipeline stage, as gemm_v3_config computes it: MT activation tiles (slab mode: SLAB_BYTES each, else
+// A_STAGE_BYTES), then the weight tiles of its taps, each padded to 1024 bytes.
+__host__ __device__ constexpr int v3_b_bytes(int BN) { return ((BN * BK * 2) + 1023) & ~1023; }
+__host__ __device__ constexpr int v3_mt_max(int BN) { return V3_ACC_COLS / BN < 4 ? V3_ACC_COLS / BN : 4; }
+__host__ __device__ constexpr int v3_slab_stage_bytes(int BN, int MT) { return MT * SLAB_BYTES + 3 * v3_b_bytes(BN); }
+// slab mode needs two stages in shared memory
+__host__ __device__ constexpr bool v3_slab_fits(int BN, int MT) { return 2 * v3_slab_stage_bytes(BN, MT) <= V3_DYN_SMEM_MAX - 1024; }
+
+// Consumer mainloop of one tile: nsteps pipeline stages of TPS taps each (3 in slab mode, else 1).  A stage is one wgmma chain:
+// one fence, then all TPS x MT x BK/16 x pieces(BN) wgmmas of this warpgroup's 64 rows back to back, then one commit, so the
+// tensor pipe does not drain between taps or sub-tiles.  Nothing else touches the accumulators inside the loop: the wgmmas'
+// "+f" operands order them, and reg_fence after the last wait keeps the epilogue's reads behind it.  Per sub-tile the K order is
+// (dy, k-block, dx, k16) in both modes -- slab tap t reads the slab from row t on and its own weight tile -- so every tile shape
+// and mode gives the same bits.
+template <int BN, int MT, int TPS>
+__device__ __forceinline__ void v3_mainloop(float (&acc)[MT][BN / 2], uint32_t smem_base, uint32_t a_row_off, int nsteps, int stages,
+                                            uint32_t& s, uint32_t& ph, uint64_t* full_bar, uint64_t* empty_bar, int lane) {
+    constexpr uint32_t A_SUB = TPS == 3 ? SLAB_BYTES : A_STAGE_BYTES;
+    constexpr uint32_t B_BYTES = v3_b_bytes(BN);
+    constexpr uint32_t STAGE = MT * A_SUB + TPS * B_BYTES;
+    uint32_t prev = 0;
+    for (int ks = 0; ks < nsteps; ++ks) {
+        mbar_wait(smem_u32(&full_bar[s]), ph);
+        const uint32_t st = smem_base + s * STAGE;
+        const uint64_t adesc = make_smem_desc(st + a_row_off);
+        const uint64_t bdesc = make_smem_desc(st + MT * A_SUB);
+        const uint32_t scale = ks != 0;                     // the first k-step of a tile overwrites the accumulators
+        wgmma_fence();
+#pragma unroll
+        for (int t = 0; t < TPS; ++t)
+#pragma unroll
+            for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+                for (int k = 0; k < BK / 16; ++k)           // descriptors count 16-byte units
+                    WgmmaCols<0, BN>::run(acc[mt], adesc + (mt * A_SUB + t * 128) / 16 + 2 * k, bdesc + t * B_BYTES / 16 + 2 * k,
+                                          (t | k) != 0 ? 1u : scale);
+        wgmma_commit();
+        wgmma_wait<1>();                                    // the wgmmas of the previous step are done: its stage can be refilled
+        if (ks > 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
+        prev = s;
+        if (++s == (uint32_t)stages) { s = 0; ph ^= 1u; }
+    }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) reg_fence(acc[mt][i]);
+    if (lane == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
+}
+
+// The tiles of one consumer warpgroup (rows cw*64 .. cw*64+63 of every sub-tile): mainloop, then the epilogue straight from the
+// accumulator registers.
+template <int BN, bool UP2, bool HS, int MT, int TPS>
+__device__ __forceinline__ void v3_tiles(const GemmV3& g, uint32_t smem_base, uint64_t* full_bar, uint64_t* empty_bar, int warp_idx, int lane) {
+    const GemmParams& p = g.p;
+    const int cw = (warp_idx - 4) >> 2;                 // consumer warpgroup
+    const int wq = warp_idx & 3;                        // warp of the group: 16 of those rows
+    const int nsteps = p.ntaps * p.kpt / TPS;           // pipeline stages per tile
+    const int per_img = p.s2_tw * p.s2_th;
+    const size_t res_ld = (size_t)(p.res_ld < 0 ? -p.res_ld : p.res_ld);
+    float acc[MT][BN / 2];
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[mt][i] = 0.f;
+    uint32_t s = 0, ph = 0;
+    for (int w = blockIdx.x; w < g.total_tiles; w += gridDim.x) {
+        v3_mainloop<BN, MT, TPS>(acc, smem_base, (uint32_t)cw * (64u * 128u), nsteps, g.stages, s, ph, full_bar, empty_bar, lane);
+
+        // ---- epilogue: thread holds rows r0 and r0 + 8 of each sub-tile, columns 8j + 2(lane%4) + {0,1} ----
+        const int n_t = w % g.n_tiles, m_t = w / g.n_tiles;
+        const int n0 = n_t * BN;
+        const int m0 = m_t * (BM * MT);
+        const int c0 = 2 * (lane & 3);
+        const float neg_slope = p.act == 3 ? 0.1f : 0.f;     // ReLU and LeakyReLU(0.1) share one instruction sequence
+#pragma unroll
+        for (int mt = 0; mt < MT; ++mt) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = cw * 64 + wq * 16 + (lane >> 2) + 8 * h;      // row inside the sub-tile
+                int row = m0 + mt * BM + r;
+                bool ok = row < p.M;
+                if (p.s2) {
+                    const int pi = m_t * MT + mt;
+                    const int b = fast_div(pi, g.fd_per_img);
+                    const int rem = pi - b * per_img;
+                    const int ty = fast_div(rem, g.fd_tw), tx = rem - ty * p.s2_tw;
+                    const int j = fast_div(r, g.fd_bw), i = r - j * p.s2_bw;
+                    const int yo = ty * p.s2_bh + j, xo = tx * p.s2_bw + i;
+                    ok = (pi < g.n_patches) && (r < p.s2_bw * p.s2_bh) && (yo < p.s2_Ho) && (xo < p.s2_Wo);
+                    row = (b * (p.s2_Ho + 2) + yo + 1) * (p.s2_Wo + 2) + xo + 1;
+                } else if (p.mask_H > 0 && ok) {
+                    const int Wp = p.mask_W + 2;
+                    const int pp = row - fast_div(row, g.fd_img) * g.fd_img.d;
+                    const int yy = fast_div(pp, g.fd_wp);
+                    const int xx = pp - yy * Wp;
+                    ok = (yy >= 1) && (yy <= p.mask_H) && (xx >= 1) && (xx <= p.mask_W);
+                }
+                if (!ok) continue;
+                if (p.transposed) {
+                    // swap-AB FC: rows are output features, columns are batch entries
+                    const float row_bias = p.bias != nullptr ? __ldg(p.bias + row) : 0.f;
+#pragma unroll
+                    for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int col = n0 + 8 * j + c0 + e;
+                            if (col < p.N) {
+                                const float x = v3_act<HS>(acc[mt][4 * j + 2 * h + e] + row_bias, p.act);
+                                if (p.out_f32) reinterpret_cast<float*>(p.out)[(size_t)col * (size_t)p.out_ld + row] = x;
+                                else reinterpret_cast<__half*>(p.out)[(size_t)col * (size_t)p.out_ld + row] = __float2half_rn(x);
+                            }
+                        }
+                    }
+                    continue;
+                }
+                if constexpr (UP2) {
+                    // 2x2 stride-2 transposed conv (no residual): column n = (2 dy + dx) * Cout + c of input pixel (yy, xx) goes to
+                    // output pixel (2 yy - 1 + dy, 2 xx - 1 + dx) of the (2H+2) x (2W+2) grid.  Cout % 8 == 0, so an 8-column
+                    // group lies in one (dy, dx).
+                    const int bi = fast_div(row, g.fd_img);
+                    const int pp = row - bi * g.fd_img.d;
+                    const int yy = fast_div(pp, g.fd_wp), xx = pp - yy * (p.mask_W + 2);
+                    const int Wo2 = 2 * p.mask_W + 2, co = p.N >> 2;
+                    const int up_row = (bi * (2 * p.mask_H + 2) + 2 * yy - 1) * Wo2 + 2 * xx - 1;
+#pragma unroll
+                    for (int j = 0; j < BN / 8; ++j) {
+                        const int n = n0 + 8 * j + c0;
+                        if (n0 + 8 * j >= p.N) break;
+                        float x0 = acc[mt][4 * j + 2 * h], x1 = acc[mt][4 * j + 2 * h + 1];
+                        if (p.bias != nullptr) { x0 += __ldg(p.bias + n); x1 += __ldg(p.bias + n + 1); }
+                        x0 = v3_act<HS>(x0, p.act); x1 = v3_act<HS>(x1, p.act);
+                        const int q = (n >= co) + (n >= 2 * co) + (n >= 3 * co);
+                        const size_t o = (size_t)(up_row + (q >> 1) * Wo2 + (q & 1)) * (size_t)p.out_ld + (n - q * co);
+                        if (p.out_f32) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + o) = make_float2(x0, x1);
+                        else *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.out) + o) = __floats2half2_rn(x0, x1);
+                    }
+                    continue;
+                }
+                const __half* rp = p.res != nullptr ? p.res + (size_t)row * res_ld : nullptr;
+                // Bias and residual loads go out RB column groups at a time, ahead of their stores.  The stores may alias them as far
+                // as the compiler knows, so a load inside the store loop waits for the previous store and each one pays its full
+                // L1 / L2 / HBM latency in turn.
+                constexpr int RB = BN / 8 < 8 ? BN / 8 : 8;
+#pragma unroll
+                for (int j0 = 0; j0 < BN / 8; j0 += RB) {
+                    if (n0 + 8 * j0 >= p.N) break;
+                    __half2 rq[RB];
+                    float2 bq[RB];
+#pragma unroll
+                    for (int jj = 0; jj < RB; ++jj) {
+                        const int j = j0 + jj;
+                        const bool in = j < BN / 8 && n0 + 8 * j < p.N;
+                        rq[jj] = __float2half2_rn(0.f);
+                        bq[jj] = make_float2(0.f, 0.f);
+                        if (rp != nullptr && in) rq[jj] = *reinterpret_cast<const __half2*>(rp + n0 + 8 * j + c0);
+                        if (p.bias != nullptr && in) bq[jj] = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + 8 * j + c0));
+                    }
+#pragma unroll
+                    for (int jj = 0; jj < RB; ++jj) {
+                        const int j = j0 + jj;
+                        if (j >= BN / 8) break;
+                        const int n = n0 + 8 * j + c0;
+                        if (n0 + 8 * j >= p.N) break;                  // N % 8 == 0: an 8-column group is all in or all out
+                        float x0 = acc[mt][4 * j + 2 * h], x1 = acc[mt][4 * j + 2 * h + 1];
+                        if (p.bias != nullptr) { x0 += bq[jj].x; x1 += bq[jj].y; }
+                        const float2 rv = __half22float2(rq[jj]);
+                        if (p.res_ld < 0) { x0 += rv.x; x1 += rv.y; }
+                        if constexpr (HS) { x0 = hardswish(x0); x1 = hardswish(x1); }
+                        else if (p.act == 1) silu2(x0, x1);
+                        else if (p.act >= 2) { x0 = relu_leaky(x0, neg_slope); x1 = relu_leaky(x1, neg_slope); }
+                        if (p.res_ld > 0) { x0 += p.res_scale * rv.x; x1 += p.res_scale * rv.y; }   // scale 1: the bits of a plain add
+                        if (p.out_f32) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + (size_t)row * (size_t)p.out_ld + n) = make_float2(x0, x1);
+                        else *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.out) + (size_t)row * (size_t)p.out_ld + n) = __floats2half2_rn(x0, x1);
+                    }
+                }
+            }
+        }
+    }
+}
+
+// Picks the consumers' tile loop once per CTA: one instantiation per sub-tile count that fits the accumulator registers, each
+// with a slab-mode twin where two slab stages fit.
+template <int BN, bool UP2, bool HS, int MT>
+__device__ __forceinline__ void v3_consumers(const GemmV3& g, uint32_t smem_base, uint64_t* full_bar, uint64_t* empty_bar, int warp_idx, int lane) {
+    if constexpr (MT < v3_mt_max(BN)) {
+        if (g.MT != MT) { v3_consumers<BN, UP2, HS, MT + 1>(g, smem_base, full_bar, empty_bar, warp_idx, lane); return; }
+    }
+    if constexpr (!UP2 && v3_slab_fits(BN, MT)) {          // the transposed-conv store runs 1x1 GEMMs only
+        if (g.slab) { v3_tiles<BN, UP2, HS, MT, 3>(g, smem_base, full_bar, empty_bar, warp_idx, lane); return; }
+    }
+    v3_tiles<BN, UP2, HS, MT, 1>(g, smem_base, full_bar, empty_bar, warp_idx, lane);
+}
+
 template <int BN, bool UP2, bool HS>
 __global__ void __launch_bounds__(V3_THREADS, 1)
 conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmV3 g) {
-    constexpr int MTX = V3_ACC_COLS / BN >= 4 ? 4 : V3_ACC_COLS / BN >= 1 ? V3_ACC_COLS / BN : 1;   // sub-tiles held in registers
     extern __shared__ uint8_t smem_raw[];
     __shared__ __align__(8) uint64_t full_bar[8];
     __shared__ __align__(8) uint64_t empty_bar[8];
@@ -156,145 +351,7 @@ conv_gemm_v3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     } else {
         asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
         // ================= consumers (MMA + epilogue) =================
-        const int cw = (warp_idx - 4) >> 2;                 // consumer warpgroup: rows cw*64 .. cw*64+63 of every sub-tile
-        const int wq = warp_idx & 3;                        // warp of the group: 16 of those rows
-        const int nsteps = p.ntaps * p.kpt / tps;           // pipeline stages per tile
-        const size_t res_ld = (size_t)(p.res_ld < 0 ? -p.res_ld : p.res_ld);
-        float acc[MTX][BN / 2];
-#pragma unroll
-        for (int mt = 0; mt < MTX; ++mt)
-#pragma unroll
-            for (int i = 0; i < BN / 2; ++i) acc[mt][i] = 0.f;
-        uint32_t s = 0, ph = 0;
-        for (int w = blockIdx.x; w < g.total_tiles; w += gridDim.x) {
-            uint32_t prev = 0;
-            for (int ks = 0; ks < nsteps; ++ks) {
-                mbar_wait(smem_u32(&full_bar[s]), ph);
-                const uint32_t a_base = smem_base + s * g.stage_bytes + (uint32_t)cw * (64u * 128u);
-                const uint32_t b_base = smem_base + s * g.stage_bytes + g.MT * g.a_sub_bytes;
-#pragma unroll
-                for (int mt = 0; mt < MTX; ++mt)
-#pragma unroll
-                    for (int i = 0; i < BN / 2; ++i) reg_fence(acc[mt][i]);
-                wgmma_fence();
-                // slab mode: tap dx reads the slab from row dx on and its own weight tile.  Per sub-tile the K order stays
-                // (dy, k-block, dx, k16), the per-tap order, so both modes give the same bits.
-                for (int t = 0; t < tps; ++t) {
-                    const uint64_t bdesc = make_smem_desc(b_base + t * g.b_bytes);
-#pragma unroll
-                    for (int mt = 0; mt < MTX; ++mt) {
-                        if (mt < g.MT) {
-                            const uint64_t adesc = make_smem_desc(a_base + (uint32_t)(mt * g.a_sub_bytes + t * 128));
-#pragma unroll
-                            for (int k = 0; k < BK / 16; ++k)
-                                WgmmaCols<0, BN>::run(acc[mt], adesc + 2u * k, bdesc + 2u * k, (uint32_t)((ks | t | k) != 0));
-                        }
-                    }
-                }
-                wgmma_commit();
-                wgmma_wait<1>();                            // the wgmmas of the previous step are done: its stage can be refilled
-                if (ks > 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
-                prev = s;
-                if (++s == (uint32_t)stages) { s = 0; ph ^= 1u; }
-            }
-            wgmma_wait<0>();
-#pragma unroll
-            for (int mt = 0; mt < MTX; ++mt)
-#pragma unroll
-                for (int i = 0; i < BN / 2; ++i) reg_fence(acc[mt][i]);
-            if (lane == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
-
-            // ---- epilogue: thread holds rows r0 and r0 + 8 of each sub-tile, columns 8j + 2(lane%4) + {0,1} ----
-            const int n_t = w % g.n_tiles, m_t = w / g.n_tiles;
-            const int n0 = n_t * BN;
-            const int m0 = m_t * BMT;
-            const int c0 = 2 * (lane & 3);
-            const float neg_slope = p.act == 3 ? 0.1f : 0.f;     // ReLU and LeakyReLU(0.1) share one instruction sequence
-#pragma unroll
-            for (int mt = 0; mt < MTX; ++mt) {
-                if (mt >= g.MT) break;
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int r = cw * 64 + wq * 16 + (lane >> 2) + 8 * h;      // row inside the sub-tile
-                    int row = m0 + mt * BM + r;
-                    bool ok = row < p.M;
-                    if (p.s2) {
-                        const int pi = m_t * g.MT + mt;
-                        const int b = fast_div(pi, g.fd_per_img);
-                        const int rem = pi - b * per_img;
-                        const int ty = fast_div(rem, g.fd_tw), tx = rem - ty * p.s2_tw;
-                        const int j = fast_div(r, g.fd_bw), i = r - j * p.s2_bw;
-                        const int yo = ty * p.s2_bh + j, xo = tx * p.s2_bw + i;
-                        ok = (pi < g.n_patches) && (r < p.s2_bw * p.s2_bh) && (yo < p.s2_Ho) && (xo < p.s2_Wo);
-                        row = (b * (p.s2_Ho + 2) + yo + 1) * (p.s2_Wo + 2) + xo + 1;
-                    } else if (p.mask_H > 0 && ok) {
-                        const int Wp = p.mask_W + 2;
-                        const int pp = row - fast_div(row, g.fd_img) * g.fd_img.d;
-                        const int yy = fast_div(pp, g.fd_wp);
-                        const int xx = pp - yy * Wp;
-                        ok = (yy >= 1) && (yy <= p.mask_H) && (xx >= 1) && (xx <= p.mask_W);
-                    }
-                    if (!ok) continue;
-                    if (p.transposed) {
-                        // swap-AB FC: rows are output features, columns are batch entries
-                        const float row_bias = p.bias != nullptr ? __ldg(p.bias + row) : 0.f;
-#pragma unroll
-                        for (int j = 0; j < BN / 8; ++j) {
-#pragma unroll
-                            for (int e = 0; e < 2; ++e) {
-                                const int col = n0 + 8 * j + c0 + e;
-                                if (col < p.N) {
-                                    const float x = v3_act<HS>(acc[mt][4 * j + 2 * h + e] + row_bias, p.act);
-                                    if (p.out_f32) reinterpret_cast<float*>(p.out)[(size_t)col * (size_t)p.out_ld + row] = x;
-                                    else reinterpret_cast<__half*>(p.out)[(size_t)col * (size_t)p.out_ld + row] = __float2half_rn(x);
-                                }
-                            }
-                        }
-                        continue;
-                    }
-                    if constexpr (UP2) {
-                        // 2x2 stride-2 transposed conv (no residual): column n = (2 dy + dx) * Cout + c of input pixel (yy, xx) goes to
-                        // output pixel (2 yy - 1 + dy, 2 xx - 1 + dx) of the (2H+2) x (2W+2) grid.  Cout % 8 == 0, so an 8-column
-                        // group lies in one (dy, dx).
-                        const int bi = fast_div(row, g.fd_img);
-                        const int pp = row - bi * g.fd_img.d;
-                        const int yy = fast_div(pp, g.fd_wp), xx = pp - yy * (p.mask_W + 2);
-                        const int Wo2 = 2 * p.mask_W + 2, co = p.N >> 2;
-                        const int up_row = (bi * (2 * p.mask_H + 2) + 2 * yy - 1) * Wo2 + 2 * xx - 1;
-#pragma unroll
-                        for (int j = 0; j < BN / 8; ++j) {
-                            const int n = n0 + 8 * j + c0;
-                            if (n0 + 8 * j >= p.N) break;
-                            float x0 = acc[mt][4 * j + 2 * h], x1 = acc[mt][4 * j + 2 * h + 1];
-                            if (p.bias != nullptr) { x0 += __ldg(p.bias + n); x1 += __ldg(p.bias + n + 1); }
-                            x0 = v3_act<HS>(x0, p.act); x1 = v3_act<HS>(x1, p.act);
-                            const int q = (n >= co) + (n >= 2 * co) + (n >= 3 * co);
-                            const size_t o = (size_t)(up_row + (q >> 1) * Wo2 + (q & 1)) * (size_t)p.out_ld + (n - q * co);
-                            if (p.out_f32) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + o) = make_float2(x0, x1);
-                            else *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.out) + o) = __floats2half2_rn(x0, x1);
-                        }
-                        continue;
-                    }
-                    const __half* rp = p.res != nullptr ? p.res + (size_t)row * res_ld : nullptr;
-#pragma unroll
-                    for (int j = 0; j < BN / 8; ++j) {
-                        const int n = n0 + 8 * j + c0;
-                        if (n0 + 8 * j >= p.N) break;                  // N % 8 == 0: an 8-column group is all in or all out
-                        float x0 = acc[mt][4 * j + 2 * h], x1 = acc[mt][4 * j + 2 * h + 1];
-                        if (p.bias != nullptr) { x0 += __ldg(p.bias + n); x1 += __ldg(p.bias + n + 1); }
-                        float2 rv = make_float2(0.f, 0.f);
-                        if (rp != nullptr) rv = __half22float2(*reinterpret_cast<const __half2*>(rp + n));
-                        if (p.res_ld < 0) { x0 += rv.x; x1 += rv.y; }
-                        if constexpr (HS) { x0 = hardswish(x0); x1 = hardswish(x1); }
-                        else if (p.act == 1) silu2(x0, x1);
-                        else if (p.act >= 2) { x0 = relu_leaky(x0, neg_slope); x1 = relu_leaky(x1, neg_slope); }
-                        if (p.res_ld > 0) { x0 += p.res_scale * rv.x; x1 += p.res_scale * rv.y; }   // scale 1: the bits of a plain add
-                        if (p.out_f32) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + (size_t)row * (size_t)p.out_ld + n) = make_float2(x0, x1);
-                        else *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.out) + (size_t)row * (size_t)p.out_ld + n) = __floats2half2_rn(x0, x1);
-                    }
-                }
-            }
-        }
+        v3_consumers<BN, UP2, HS, 1>(g, smem_base, full_bar, empty_bar, warp_idx, lane);
     }
 }
 
@@ -380,15 +437,14 @@ int gemm_v3_config(const GemmParams& p_in, GemmV3* g) {
     if (g->MT > 4) return 1;
     // the accumulators of a CTA tile live in registers (MT * BN / 2 per consumer thread): a taller tile than fits runs as the
     // tallest one that does -- results do not depend on the tile shape
-    const int mt_max = V3_ACC_COLS / p.BN < 4 ? V3_ACC_COLS / p.BN : 4;
-    if (g->MT > mt_max) g->MT = mt_max;
-    const int b_bytes = ((p.BN * BK * 2) + 1023) & ~1023;
+    if (g->MT > v3_mt_max(p.BN)) g->MT = v3_mt_max(p.BN);
+    const int b_bytes = v3_b_bytes(p.BN);
     g->b_bytes = b_bytes;
     // 3x3 stride-1: the three dx taps of one (dy, k-block) read the same activation rows shifted by one, so one slab of
     // SLAB_ROWS rows per sub-tile feeds all three -- when two such stages fit (not at MT = 1, BN = 256)
     static const int no_slab_env = env_int("ADAS_B200_NOSLAB", 0);
-    const int slab_stage = g->MT * SLAB_BYTES + 3 * b_bytes;
-    g->slab = p.ntaps == 9 && !p.s2 && !p.no_slab && !no_slab_env && 2 * slab_stage <= V3_DYN_SMEM_MAX - 1024;
+    const int slab_stage = v3_slab_stage_bytes(p.BN, g->MT);
+    g->slab = p.ntaps == 9 && !p.s2 && !p.up2 && !p.no_slab && !no_slab_env && v3_slab_fits(p.BN, g->MT);
     g->a_sub_bytes = g->slab ? SLAB_BYTES : A_STAGE_BYTES;
     g->stage_bytes = g->slab ? slab_stage : g->MT * g->a_sub_bytes + b_bytes;
     int stages = (V3_DYN_SMEM_MAX - 1024) / g->stage_bytes;

@@ -131,6 +131,25 @@ int adas_detect_pair(adas_engine* yolo, adas_engine* ufld, const uint8_t* frames
                      float* scores, int32_t* class_ids, int32_t* cand_index, int32_t* counts,
                      int32_t* n_candidates, int32_t* pts, int32_t* npts, uint8_t* status);
 
+/* adas_detect_pair_rig: adas_detect_pair for a rig of k cameras whose frames may differ in size, in one call: per camera it is
+ * YoloDetector.DetectFrame + UltrafastLaneDetectorV2.DetectFrame (or UltrafastLaneDetector.DetectFrame for a UFLD v1 plan) on that
+ * camera's frames; the reference has no counterpart.  Every camera sends frames_per_camera (F) frames; the two networks run one
+ * batch of k * F frames, each frame letterboxed / resized from its own camera's size, and each frame's boxes and lane points are
+ * in its own camera's pixels.  Outputs as adas_detect_pair's with batch = k * F, camera-major (frame f of camera c at c * F + f).
+ *   cams[c].frames: F x H x W x 3 uint8 BGR, host (staged into one device arena with one copy per camera) or, with
+ *   frames_on_device = 1, the caller's device memory.  Both networks are enqueued on their own streams before either is waited for.
+ * Refused before any device work: k outside [1, ADAS_MAX_RIG_CAMERAS], F < 1, k * F above either engine's max_batch, a null camera
+ * table, frame pointer or output (n_candidates may be NULL), a camera smaller than 1 x 1 or one whose letterbox has no rows or columns, a pair that is not one
+ * detector and one lane engine, engines on different devices.  After a rig call adas_engine_warp_perspective and
+ * adas_ufld_lane_geometry refuse on these engines (they assume frames of one size) until the next adas_yolo_detect /
+ * adas_ufld_detect / adas_detect_pair. */
+#define ADAS_MAX_RIG_CAMERAS 16
+typedef struct adas_rig_camera { const uint8_t* frames; int32_t H, W; } adas_rig_camera;
+int adas_detect_pair_rig(adas_engine* yolo, adas_engine* ufld, const adas_rig_camera* cams, int k, int frames_per_camera,
+                         int frames_on_device, double box_score, double nms_iou, int max_det, float* boxes_xywh, float* scores,
+                         int32_t* class_ids, int32_t* cand_index, int32_t* counts, int32_t* n_candidates, int32_t* pts,
+                         int32_t* npts, uint8_t* status);
+
 /* decode only, from the 4 head tensors concatenated per frame ([batch, total_dim] fp32 host,
  * order loc_row, loc_col, exist_row, exist_col) */
 int adas_ufld_postprocess(int device, const float* heads_host, int batch, int num_grid_row,

@@ -8,7 +8,12 @@ after warm-up.  The two arms cannot be alive together at K = 8 without crowding 
 closed in turn.  K = 1 is one arm (one camera through one pipeline is both).  Prints one JSON line per (K, arm) and the card, its
 power limit and the SM clocks sampled during the timed windows.  Needs a GPU; there is no CPU fallback.
 
+With `--sizes WxH,WxH,...` the cameras differ in frame size (K = the number of sizes): one AdasPipeline(cameras=K,
+frame_sizes=...) against K single-camera pipelines stepped in turn, on device-resident synthetic frames of each camera's size
+(tests/synth.py's frame(seed, h, w)), measured as above.
+
     python tools/multicam_bench.py --cameras 1,2,4,8 --frames 8 --steps 30 --warmup 4 --repeats 3
+    python tools/multicam_bench.py --sizes 1920x1080,1280x800,1280x800,1280x720 --frames 8
 """
 import argparse
 import json
@@ -41,7 +46,8 @@ def card() -> dict:
     return {"nvidia_smi": out, "query": q}
 
 
-def run_arm(plans, K: int, F: int, multi: bool, pool, args, clocks):
+def run_arm(plans, K: int, F: int, multi: bool, pool, args, clocks, sizes=None):
+    """pool: [batches, K, F, H, W, 3] on the device, or with `sizes` a list of K [batches, F, H_c, W_c, 3] device tensors"""
     from adas_b200.pipeline import AdasPipeline
     H, W = bench.FRAME_H, bench.FRAME_W
     kw = dict(device=0, batch=F, box_score=bench.BOX_SCORE, box_nms_iou=bench.NMS_IOU, max_det=bench.MAX_DET)
@@ -49,11 +55,19 @@ def run_arm(plans, K: int, F: int, multi: bool, pool, args, clocks):
     base = used_mib()
     t_build = time.time()
     y, u = plans["yolov8"][0], plans["ufldv2"][0]
-    pipes = [AdasPipeline(y, u, cameras=K, **kw)] if multi else [AdasPipeline(y, u, **kw) for _ in range(K)]
+    pipes = [AdasPipeline(y, u, cameras=K, frame_sizes=sizes, **kw)] if multi else [AdasPipeline(y, u, **kw) for _ in range(K)]
     t_build = time.time() - t_build
-    nb = pool.shape[0]
+    nb = pool[0].shape[0] if sizes is not None else pool.shape[0]
 
     def step(i):
+        if sizes is not None:
+            xs = [p[i % nb] for p in pool]                        # K x [F, H_c, W_c, 3], contiguous
+            if multi:
+                pipes[0].step_pipelined([(x.data_ptr(), tuple(x.shape[:3])) for x in xs], True)
+            else:
+                for x, p in zip(xs, pipes):
+                    p.step_pipelined(x.data_ptr(), True, tuple(x.shape[:3]))
+            return
         x = pool[i % nb]                                          # [K, F, H, W, 3], contiguous
         if multi:
             pipes[0].step_pipelined(x.data_ptr(), True, (K, F, H, W) if K > 1 else (F, H, W))
@@ -93,6 +107,7 @@ def run_arm(plans, K: int, F: int, multi: bool, pool, args, clocks):
     del pipes, trackers
     torch.cuda.synchronize()
     return {"cameras": K, "frames_per_step": F, "arm": "one pipeline" if multi else f"{K} pipelines",
+            "sizes_wh": None if sizes is None else [f"{w}x{h}" for h, w in sizes],
             "frames_per_s": [round(v, 1) for v in fps], "tracker_ms_per_step": [round(v, 3) for v in trk_ms],
             "assoc_round_trip_ms_per_step": [round(v, 3) for v in wait_ms], "assoc_launches_per_step": [round(v, 2) for v in launches],
             "device_mib_after_warmup": round(mem, 0), "build_s": round(t_build, 1),
@@ -106,6 +121,7 @@ def main():
     ap.add_argument("--steps", type=int, default=30)
     ap.add_argument("--warmup", type=int, default=4)
     ap.add_argument("--repeats", type=int, default=3)
+    ap.add_argument("--sizes", default=None, help="WxH,WxH,...: one camera per size, of different frame sizes (replaces --cameras)")
     ap.add_argument("--out", default=None, help="also write the JSON lines to this file")
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -117,7 +133,20 @@ def main():
     lines = [json.dumps({"card": card()})]
     print(lines[0], flush=True)
     try:
-        for K in [int(k) for k in args.cameras.split(",")]:
+        if args.sizes:
+            sys.path.insert(0, os.path.join(ROOT, "tests"))
+            import synth
+            sizes = [(int(h), int(w)) for w, h in (s.lower().split("x") for s in args.sizes.split(","))]
+            K = len(sizes)
+            pool = [torch.from_numpy(np.stack([np.stack([synth.frame(500 + 37 * c + b * F + f, h, w) for f in range(F)]) for b in range(4)])).cuda()
+                    for c, (h, w) in enumerate(sizes)]                                                 # K x [4 batches, F, H_c, W_c, 3]
+            for multi in [True, False]:
+                res = run_arm(plans, K, F, multi, pool, args, clocks, sizes=sizes)
+                lines.append(json.dumps(res))
+                print(lines[-1], flush=True)
+            del pool
+            torch.cuda.empty_cache()
+        for K in ([] if args.sizes else [int(k) for k in args.cameras.split(",")]):
             streams = [bench.synth_stream(500 + c, 4 * F) for c in range(K)]
             host = np.stack([np.stack([s[b * F:(b + 1) * F] for s in streams]) for b in range(4)])     # [4 batches, K, F, H, W, 3]
             pool = torch.from_numpy(host).cuda()

@@ -23,7 +23,7 @@ SYMBOLS = [
     "adas_engine_infer", "adas_engine_infer_dev", "adas_yolo_detect", "adas_yolo_postprocess", "adas_yolo_preprocess",
     "adas_ufld_detect", "adas_ufld_postprocess", "adas_ufld_v1_postprocess", "adas_lane_geometry", "adas_ufld_lane_geometry", "adas_warp_perspective", "adas_engine_warp_perspective", "adas_ufld_preprocess", "adas_iou_cost", "adas_lap", "adas_associate",
     "adas_engine_stream", "adas_engine_num_buffers", "adas_engine_buffer_info", "adas_engine_write_buffer", "adas_engine_read_buffer",
-    "adas_engine_run", "adas_plan_validate", "adas_engine_event_record", "adas_event_elapsed_ms", "adas_engine_time_ops", "adas_engine_num_steps", "adas_engine_time_step", "adas_detect_pair",
+    "adas_engine_run", "adas_plan_validate", "adas_engine_event_record", "adas_event_elapsed_ms", "adas_engine_time_ops", "adas_engine_num_steps", "adas_engine_time_step", "adas_detect_pair", "adas_detect_pair_rig",
     "adas_comm_unique_id", "adas_comm_create", "adas_comm_destroy", "adas_comm_all_gather", "adas_comm_sync", "adas_comm_read", "adas_comm_info",
     "adas_tracker_create", "adas_tracker_destroy", "adas_tracker_reset", "adas_tracker_update", "adas_tracker_update_batch", "adas_tracker_update_multi", "adas_tracker_get", "adas_tracker_count", "adas_tracker_stats",
 ]
@@ -355,6 +355,45 @@ def detect_pair(yolo: "Engine", ufld: "Engine", frames, box_score: float, nms_io
     check(lib().adas_detect_pair(yolo._h, ufld._h, fptr, 1 if on_device else 0, B, H, W, C.c_double(box_score), C.c_double(nms_iou), max_det,
                                  _p(boxes, C.c_float), _p(scores, C.c_float), _p(cls, C.c_int32), _p(idx, C.c_int32), _p(counts, C.c_int32),
                                  _p(ncand, C.c_int32), _p(pts, C.c_int32), _p(npts, C.c_int32), _p(status, C.c_uint8)))
+    return (boxes, scores, cls, idx, counts, ncand), (pts, npts, status, None)
+
+
+class RigCamera(C.Structure):
+    """adas_rig_camera: one camera's F x H x W x 3 uint8 BGR frames"""
+    _fields_ = [("frames", C.c_void_p), ("H", C.c_int32), ("W", C.c_int32)]
+
+
+def detect_pair_rig(yolo: "Engine", ufld: "Engine", cams, box_score: float, nms_iou: float, max_det: int = 1024, on_device: bool = False):
+    """One library call for a rig of cameras of different frame sizes: YOLO detect and UFLD lane detect of every camera's frames.
+    cams: K host arrays [F, H_c, W_c, 3] uint8, or with on_device K (device pointer, (F, H_c, W_c)) pairs; every camera sends the same
+    F.  Returns detect_pair's (yolo tuple, ufld tuple) for K * F frames, camera-major; each frame's boxes and lane points are in its
+    own camera's pixels."""
+    if on_device:
+        shapes = [tuple(int(v) for v in shp) for _, shp in cams]
+        ptrs = [int(p) for p, _ in cams]
+    else:
+        host = [as_c(a, np.uint8) for a in cams]                       # alive until the call returns
+        shapes = [a.shape[:3] for a in host]
+        ptrs = [a.ctypes.data for a in host]
+    K = len(shapes)
+    F = shapes[0][0] if K else 0
+    if any(s[0] != F for s in shapes):
+        raise ValueError(f"every camera must send the same number of frames: {[s[0] for s in shapes]}")
+    table = (RigCamera * max(1, K))(*[RigCamera(p, s[1], s[2]) for p, s in zip(ptrs, shapes)])
+    B = max(1, K * F)
+    boxes = np.empty((B, max_det, 4), np.float32)
+    scores = np.empty((B, max_det), np.float32)
+    cls = np.empty((B, max_det), np.int32)
+    idx = np.empty((B, max_det), np.int32)
+    counts = np.empty((B,), np.int32)
+    ncand = np.empty((B,), np.int32)
+    mp = ufld._ufld_max_pts()
+    pts = np.empty((B, 4, mp, 2), np.int32)
+    npts = np.empty((B, 4), np.int32)
+    status = np.empty((B, 4), np.uint8)
+    check(lib().adas_detect_pair_rig(yolo._h, ufld._h, table, K, F, 1 if on_device else 0, C.c_double(box_score), C.c_double(nms_iou), max_det,
+                                     _p(boxes, C.c_float), _p(scores, C.c_float), _p(cls, C.c_int32), _p(idx, C.c_int32), _p(counts, C.c_int32),
+                                     _p(ncand, C.c_int32), _p(pts, C.c_int32), _p(npts, C.c_int32), _p(status, C.c_uint8)))
     return (boxes, scores, cls, idx, counts, ncand), (pts, npts, status, None)
 
 

@@ -9,7 +9,7 @@
 #include <vector>
 #include <atomic>
 
-struct adas_lane_geom;      // include/adas_b200.h
+#include "../../include/adas_b200.h"   // adas_lane_geom, ADAS_MAX_RIG_CAMERAS
 
 #include <nvtx3/nvToolsExt.h>     // header-only NVTX v3: ranges cost a few ns unless a tool (nsys / ncu) is attached
 
@@ -161,7 +161,45 @@ struct LetterboxGeom {
     int src_h, src_w, in_h, in_w, new_h, new_w, pad_h, pad_w;
 };
 LetterboxGeom letterbox_geom(int src_h, int src_w, int in_h, int in_w);
+// cv2.resize(INTER_LINEAR) coefficient tables of one (source, destination) size pair, on the device; cached per geometry
+struct ResizeTab {
+    int* xofs = nullptr;     // [dw]   left source column
+    int* xofs1 = nullptr;    // [dw]   right source column
+    short* xa = nullptr;     // [dw*2] coefficients
+    int* yofs = nullptr;     // [dh]   upper source row (clipped)
+    int* yofs1 = nullptr;    // [dh]   lower source row (clipped)
+    short* yb = nullptr;     // [dh*2]
+};
+
+// ---- camera rigs: one pre-/post-processing launch for the frames of several cameras of different sizes -------------------------
+// Frames are camera-major: frame b of a launch is frame b % F of camera b / F.  The table travels by value as a kernel parameter
+// (no upload, no synchronisation), so a launch of one camera is the same kernel with n = 1.
+struct RigCamera {
+    const uint8_t* frames;   // [F, H, W, 3] BGR on the device (nullptr for the decodes)
+    int H, W;                // source frame size: the scale of the decoded boxes and lane points
+    LetterboxGeom g;         // YOLO letterbox of an H x W frame
+    ResizeTab yolo, ufld;    // H x W -> g.new_h x g.new_w, and H x W -> the UFLD resize
+};
+struct RigTable {
+    int n, F;                // cameras, frames per camera
+    RigCamera cam[ADAS_MAX_RIG_CAMERAS];
+};
+static_assert(sizeof(RigTable) <= 2560, "the rig table plus the other launch arguments stay well under the 4 KB kernel-parameter limit");
+// one camera of `B` frames, geometry only (the tables and the letterbox are filled by rig_camera where a launch needs them)
+inline RigTable rig_one(const uint8_t* frames, int B, int H, int W) {
+    RigTable t{};
+    t.n = 1; t.F = B;
+    t.cam[0].frames = frames; t.cam[0].H = H; t.cam[0].W = W;
+    return t;
+}
+// fills c: the letterbox and resize tables for a YOLO input of yolo_h x yolo_w (yolo_h = 0: none) and the tables of the UFLD resize
+// to ufld_w x ufld_resize_h (ufld_w = 0: none); refuses a letterbox with no rows or columns
+int rig_camera(const uint8_t* frames, int H, int W, int yolo_h, int yolo_w, int ufld_w, int ufld_resize_h, RigCamera* c);
 // writes fp16 padded NHWC (C=4: R,G,B,0) and/or fp32 NCHW blob
+int launch_yolo_pre_rig(const RigTable& t, int in_h, int in_w, __half* img_padded, int img_ld, float* blob_nchw, cudaStream_t st);
+int launch_ufld_pre_rig(const RigTable& t, int in_h, int in_w, int resize_h, const float* lut /*3*256 dev*/, __half* img_padded, int img_ld,
+                        float* blob_nchw, cudaStream_t st);
+// the one-camera forms
 int launch_yolo_pre(const uint8_t* frames, int B, const LetterboxGeom& g, __half* img_padded, int img_ld,
                     float* blob_nchw, cudaStream_t st);
 int launch_ufld_pre(const uint8_t* frames, int B, int H, int W, int in_h, int in_w, int resize_h,
@@ -193,11 +231,19 @@ struct YoloPostBufs {
     // outputs (device)
     float* out_box; float* out_score; int32_t* out_cls; int32_t* out_idx; int32_t* out_count;
 };
+// frame b's boxes are un-letterboxed with t.cam[b / t.F].g
+int launch_yolo_post_rig(const float* raw, int kind, const RigTable& t, int A, int nc, double box_score, double nms_iou, int max_det,
+                         YoloPostBufs& w, cudaStream_t st);
 int launch_yolo_post(const float* raw, int kind, int B, int A, int nc, const LetterboxGeom& g, double box_score,
                      double nms_iou, int max_det, YoloPostBufs& w, cudaStream_t st);
 
 // ---- UFLD post-processing (ufld_post.cu) -----------------------------------------------------------
 struct UfldDims { int ngr, ncr, ngc, ncc, nl; };
+// frame b's lane points are scaled to t.cam[b / t.F].W x .H pixels
+int launch_ufld_v1_post_rig(const float* head, int ld, const RigTable& t, int G, int R, int in_w, int in_h, int cfg_w, int cfg_h,
+                            const double* row_anchor, int32_t* pts, int32_t* npts, uint8_t* status, double* coords, int max_pts, cudaStream_t st);
+int launch_ufld_post_rig(const float* heads, int ld, const RigTable& t, UfldDims d, const double* row_anchor, const double* col_anchor,
+                         int32_t* pts, int32_t* npts, uint8_t* status, double* coords, int max_pts, cudaStream_t st);
 int launch_ufld_v1_post(const float* head, int ld, int B, int G, int R, int in_w, int in_h, int cfg_w, int cfg_h, int img_w, int img_h,
                         const double* row_anchor, int32_t* pts, int32_t* npts, uint8_t* status, double* coords, int max_pts, cudaStream_t st);
 int launch_ufld_post(const float* heads, int ld, int B, UfldDims d, int img_w, int img_h, const double* row_anchor,

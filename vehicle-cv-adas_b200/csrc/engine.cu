@@ -72,6 +72,7 @@ struct adas_engine {
     float* d_input = nullptr;        // [max_batch, C, H, W] fp32
     uint8_t* d_frames = nullptr;     // [max_batch * frame_bytes]
     const uint8_t* last_dfr = nullptr; int last_fb = 0, last_fh = 0, last_fw = 0;      // frames of the last detect call, on the device
+    bool last_rig = false;          // the last detect call was adas_detect_pair_rig: its frames are not one [B, H, W, 3] block
     uint8_t* d_warp = nullptr; size_t warp_cap = 0; double* d_warpM = nullptr;          // adas_engine_warp_perspective scratch
     size_t frames_cap = 0;
     float* d_raw = nullptr;          // decoded head tensor (YOLO) [max_batch, ...]
@@ -1213,7 +1214,7 @@ int adas_engine_infer(adas_engine* e, const float* input, int batch, float* cons
 int adas_engine_infer_dev(adas_engine* e, const float* input, int batch, float* const* outs) { return infer_common(e, input, batch, outs, true); }
 
 static int stage_frames(adas_engine* e, const uint8_t* frames, int on_device, int batch, int H, int W, const uint8_t** dptr) {
-    e->last_fb = batch; e->last_fh = H; e->last_fw = W;
+    e->last_fb = batch; e->last_fh = H; e->last_fw = W; e->last_rig = false;
     if (on_device) { *dptr = frames; e->last_dfr = frames; return 0; }
     const size_t bytes = (size_t)batch * H * W * 3;
     if (bytes > e->frames_cap) {
@@ -1303,19 +1304,19 @@ int adas_yolo_preprocess(int device, const uint8_t* frames_host, int batch, int 
 }
 
 // lane decode of the head tensor(s) the plan just produced: v2 row / column anchors or the v1 grid expectation
-static int ufld_post_dispatch(adas_engine* e, int batch, int W, int H, bool want_coords) {
+static int ufld_post_dispatch(adas_engine* e, const RigTable& t, bool want_coords) {
     const uint32_t* m = e->hdr.meta;
     const PlanOutput& o = e->outs[0];
     const float* heads = static_cast<const float*>(e->dbufs[o.buffer].ptr) + o.coff;
     const int mp = e->ufld_max_pts;
     if (e->hdr.model_kind == ADAS_MODEL_UFLDV1) {
         const UfldV1Dataset* ds = ufld_v1_dataset(e->hdr);
-        return launch_ufld_v1_post(heads, (int)e->bufs[o.buffer].C, batch, ds->G, ds->R, (int)e->hdr.in_w, (int)e->hdr.in_h, ds->img_w, ds->img_h, W, H,
-                                   e->d_row_anchor, e->d_pts, e->d_npts, e->d_status, want_coords ? e->d_coords : nullptr, mp, e->stream);
+        return launch_ufld_v1_post_rig(heads, (int)e->bufs[o.buffer].C, t, ds->G, ds->R, (int)e->hdr.in_w, (int)e->hdr.in_h, ds->img_w, ds->img_h,
+                                       e->d_row_anchor, e->d_pts, e->d_npts, e->d_status, want_coords ? e->d_coords : nullptr, mp, e->stream);
     }
     UfldDims d{(int)m[0], (int)m[1], (int)m[2], (int)m[3], (int)m[4]};
-    return launch_ufld_post(heads, (int)e->bufs[o.buffer].C, batch, d, W, H, e->d_row_anchor, e->d_col_anchor, e->d_pts, e->d_npts, e->d_status,
-                            want_coords ? e->d_coords : nullptr, mp, e->stream);
+    return launch_ufld_post_rig(heads, (int)e->bufs[o.buffer].C, t, d, e->d_row_anchor, e->d_col_anchor, e->d_pts, e->d_npts, e->d_status,
+                                want_coords ? e->d_coords : nullptr, mp, e->stream);
 }
 
 int adas_ufld_detect(adas_engine* e, const uint8_t* frames, int frames_on_device, int batch, int H, int W, int32_t* pts, int32_t* npts,
@@ -1338,7 +1339,7 @@ int adas_ufld_detect(adas_engine* e, const uint8_t* frames, int frames_on_device
     if (run_plan(e, batch)) return 1;
     tr.mark("plan");
     const int mp = e->ufld_max_pts;
-    if (ufld_post_dispatch(e, batch, W, H, coords_f != nullptr)) return 1;
+    if (ufld_post_dispatch(e, rig_one(dfr, batch, H, W), coords_f != nullptr)) return 1;
     ADAS_CUDA(cudaMemcpyAsync(pts, e->d_pts, (size_t)batch * 4 * mp * 2 * 4, cudaMemcpyDeviceToHost, e->stream));
     ADAS_CUDA(cudaMemcpyAsync(npts, e->d_npts, (size_t)batch * 4 * 4, cudaMemcpyDeviceToHost, e->stream));
     ADAS_CUDA(cudaMemcpyAsync(status, e->d_status, (size_t)batch * 4, cudaMemcpyDeviceToHost, e->stream));
@@ -1352,6 +1353,8 @@ int adas_ufld_detect(adas_engine* e, const uint8_t* frames, int frames_on_device
 
 int adas_engine_warp_perspective(adas_engine* e, int batch, const double* M, int out_h, int out_w, uint8_t* out_host) {
     ADAS_CHECK(e != nullptr && M != nullptr && out_host != nullptr, "adas_engine_warp_perspective: null argument");
+    ADAS_CHECK(!e->last_rig, "adas_engine_warp_perspective: the last detect call on this engine was a camera rig of several frame sizes; "
+               "warp after an adas_yolo_detect, adas_ufld_detect or adas_detect_pair");
     ADAS_CHECK(e->last_dfr != nullptr && batch >= 1 && batch <= e->last_fb, "adas_engine_warp_perspective: batch %d, but the last detect call on this engine processed %d frames",
                batch, e->last_fb);
     ADAS_CUDA(cudaSetDevice(e->device));
@@ -1372,6 +1375,8 @@ int adas_engine_warp_perspective(adas_engine* e, int batch, const double* M, int
 int adas_ufld_lane_geometry(adas_engine* e, int batch, int img_w, int img_h, int adjust_lanes, const double* M, int bird_w, int bird_h, int32_t* area,
                             int cap_area, int32_t* bird, adas_lane_geom* out) {
     ADAS_CHECK(e != nullptr && is_ufld(e->hdr.model_kind), "adas_ufld_lane_geometry needs a UFLD engine");
+    ADAS_CHECK(!e->last_rig, "adas_ufld_lane_geometry: the last lane detect on this engine was a camera rig of several frame sizes; "
+               "compute geometry after an adas_ufld_detect or adas_detect_pair");
     ADAS_CHECK(batch >= 1 && batch <= e->ufld_last_batch, "adas_ufld_lane_geometry: batch %d, but the last lane detect on this engine decoded %d frames", batch, e->ufld_last_batch);
     ADAS_CHECK(area != nullptr && out != nullptr && (M == nullptr || bird != nullptr), "adas_ufld_lane_geometry: null argument");
     ADAS_CUDA(cudaSetDevice(e->device));
@@ -1432,6 +1437,7 @@ int adas_detect_pair(adas_engine* yolo, adas_engine* ufld, const uint8_t* frames
     }
     e->last_dfr = ufld->last_dfr = frames;
     e->last_fb = ufld->last_fb = batch; e->last_fh = ufld->last_fh = H; e->last_fw = ufld->last_fw = W;
+    e->last_rig = ufld->last_rig = false;
     const LetterboxGeom g = letterbox_geom(H, W, (int)e->hdr.in_h, (int)e->hdr.in_w);
     if (launch_yolo_pre(frames, batch, g, static_cast<__half*>(e->dbufs[0].ptr), (int)e->bufs[0].C, nullptr, e->stream)) return 1;
     {
@@ -1450,7 +1456,7 @@ int adas_detect_pair(adas_engine* yolo, adas_engine* ufld, const uint8_t* frames
     {
         adas_engine* u = ufld;
         const int mp = u->ufld_max_pts;
-        if (ufld_post_dispatch(u, batch, W, H, false)) return 1;
+        if (ufld_post_dispatch(u, rig_one(frames, batch, H, W), false)) return 1;
         ADAS_CUDA(cudaMemcpyAsync(pts, u->d_pts, (size_t)batch * 4 * mp * 2 * 4, cudaMemcpyDeviceToHost, u->stream));
         ADAS_CUDA(cudaMemcpyAsync(npts, u->d_npts, (size_t)batch * 4 * 4, cudaMemcpyDeviceToHost, u->stream));
         ADAS_CUDA(cudaMemcpyAsync(status, u->d_status, (size_t)batch * 4, cudaMemcpyDeviceToHost, u->stream));
@@ -1458,6 +1464,104 @@ int adas_detect_pair(adas_engine* yolo, adas_engine* ufld, const uint8_t* frames
     }
     if (copy_yolo_results_finish(e->yp, batch, max_det, counts, n_candidates, e->h_ncand.data(), e->stream)) return 1;
     ADAS_CUDA(cudaStreamSynchronize(ufld->stream));
+    return 0;
+}
+
+int adas_detect_pair_rig(adas_engine* yolo, adas_engine* ufld, const adas_rig_camera* cams, int k, int frames_per_camera, int frames_on_device,
+                         double box_score, double nms_iou, int max_det, float* boxes_xywh, float* scores, int32_t* class_ids, int32_t* cand_index,
+                         int32_t* counts, int32_t* n_candidates, int32_t* pts, int32_t* npts, uint8_t* status) {
+    NvtxRange nv("adas_detect_pair_rig");
+    // every refusal comes before any device work
+    ADAS_CHECK(yolo != nullptr && ufld != nullptr, "adas_detect_pair_rig: null engine");
+    ADAS_CHECK(!is_ufld(yolo->hdr.model_kind) && is_ufld(ufld->hdr.model_kind), "adas_detect_pair_rig needs a YOLO and a UFLD engine");
+    if (check_has_outputs(yolo, "adas_detect_pair_rig") || check_has_outputs(ufld, "adas_detect_pair_rig")) return 1;
+    ADAS_CHECK(yolo->device == ufld->device, "adas_detect_pair_rig: the YOLO engine is on device %d, the UFLD engine on device %d", yolo->device,
+               ufld->device);
+    ADAS_CHECK(k >= 1 && k <= ADAS_MAX_RIG_CAMERAS, "adas_detect_pair_rig: %d cameras, a rig has 1 to %d", k, ADAS_MAX_RIG_CAMERAS);
+    ADAS_CHECK(frames_per_camera >= 1, "adas_detect_pair_rig: %d frames per camera", frames_per_camera);
+    const long long batch_ll = (long long)k * frames_per_camera;
+    ADAS_CHECK(batch_ll <= yolo->max_batch && batch_ll <= ufld->max_batch,
+               "adas_detect_pair_rig: %d cameras x %d frames = %lld frames, but the engines hold %d (YOLO) and %d (UFLD)", k, frames_per_camera,
+               batch_ll, yolo->max_batch, ufld->max_batch);
+    ADAS_CHECK(cams != nullptr, "adas_detect_pair_rig: null camera table");
+    ADAS_CHECK(boxes_xywh && scores && class_ids && cand_index && counts && pts && npts && status, "adas_detect_pair_rig: null output");
+    adas_engine* e = yolo;
+    adas_engine* u = ufld;
+    const int F = frames_per_camera, batch = (int)batch_ll;
+    const int yin_h = (int)e->hdr.in_h, yin_w = (int)e->hdr.in_w;
+    const int uin_h = (int)u->hdr.in_h, uin_w = (int)u->hdr.in_w;
+    const int resize_h = (int)((double)uin_h / u->ufld_crop);     // int(self.input_height / cfg.crop_ratio)
+    size_t total = 0;                                               // bytes of every camera's frames
+    for (int c = 0; c < k; ++c) {
+        const adas_rig_camera& cm = cams[c];
+        ADAS_CHECK(cm.frames != nullptr, "adas_detect_pair_rig: camera %d: null frame pointer", c);
+        ADAS_CHECK(cm.H >= 1 && cm.W >= 1, "adas_detect_pair_rig: camera %d: frames of %d x %d", c, cm.H, cm.W);
+        const LetterboxGeom g = letterbox_geom(cm.H, cm.W, yin_h, yin_w);
+        ADAS_CHECK(g.new_h >= 1 && g.new_w >= 1, "adas_detect_pair_rig: camera %d: a %d x %d frame letterboxes to %d x %d inside %d x %d", c, cm.H,
+                   cm.W, g.new_h, g.new_w, yin_h, yin_w);
+        total += (size_t)F * cm.H * cm.W * 3;
+    }
+
+    ADAS_CUDA(cudaSetDevice(e->device));
+    const int nc = (int)e->hdr.meta[0], A = (int)e->hdr.meta[1];
+    if (e->yp.flags == nullptr || e->yp_max_det != max_det) {
+        if (e->yp.flags) free_yolo_post(&e->yp);
+        if (alloc_yolo_post(&e->yp, e->max_batch, A, max_det)) return 1;
+        e->yp_max_det = max_det;
+    }
+    e->h_ncand.resize(batch);
+    if (!frames_on_device) {
+        // one arena for the frames of every camera, grown on demand and reused; one copy per camera on the object stream, and the
+        // lane stream waits for the last
+        if (total > e->frames_cap) {
+            if (e->d_frames) ADAS_CUDA(cudaFree(e->d_frames));
+            e->d_frames = nullptr;
+            e->frames_cap = 0;
+            ADAS_CUDA(cudaMalloc(&e->d_frames, total));
+            e->frames_cap = total;
+        }
+    }
+    RigTable t{};
+    t.n = k; t.F = F;
+    size_t off = 0;
+    for (int c = 0; c < k; ++c) {
+        const adas_rig_camera& cm = cams[c];
+        const size_t bytes = (size_t)F * cm.H * cm.W * 3;
+        const uint8_t* dfr = cm.frames;
+        if (!frames_on_device) {
+            ADAS_CUDA(cudaMemcpyAsync(e->d_frames + off, cm.frames, bytes, cudaMemcpyHostToDevice, e->stream));
+            dfr = e->d_frames + off;
+            off += bytes;
+        }
+        if (rig_camera(dfr, cm.H, cm.W, yin_h, yin_w, uin_w, resize_h, &t.cam[c])) return 1;
+    }
+    if (!frames_on_device) {
+        if (!e->ev_frames) ADAS_CUDA(cudaEventCreateWithFlags(&e->ev_frames, cudaEventDisableTiming));
+        ADAS_CUDA(cudaEventRecord(e->ev_frames, e->stream));
+        ADAS_CUDA(cudaStreamWaitEvent(u->stream, e->ev_frames, 0));
+    }
+    // the frames are no single [B, H, W, 3] block: the warp and lane-geometry follow-ups refuse until the next one-size detect call
+    e->last_rig = u->last_rig = true;
+    e->last_dfr = u->last_dfr = nullptr;
+    e->last_fb = u->last_fb = 0;
+    // both networks are enqueued on their own streams before either is waited for, as in adas_detect_pair
+    if (launch_yolo_pre_rig(t, yin_h, yin_w, static_cast<__half*>(e->dbufs[0].ptr), (int)e->bufs[0].C, nullptr, e->stream)) return 1;
+    if (launch_ufld_pre_rig(t, uin_h, uin_w, resize_h, u->d_lut, static_cast<__half*>(u->dbufs[0].ptr), (int)u->bufs[0].C, nullptr, u->stream))
+        return 1;
+    if (run_plan(e, batch)) return 1;
+    if (run_plan(u, batch)) return 1;
+    if (head_decode(e, batch)) return 1;
+    if (lite_post(e, batch)) return 1;
+    if (launch_yolo_post_rig(e->d_raw, (int)e->hdr.model_kind, t, A, nc, box_score, nms_iou, max_det, e->yp, e->stream)) return 1;
+    if (copy_yolo_results_enqueue(e->yp, batch, max_det, boxes_xywh, scores, class_ids, cand_index, counts, e->h_ncand.data(), e->stream)) return 1;
+    const int mp = u->ufld_max_pts;
+    if (ufld_post_dispatch(u, t, false)) return 1;
+    ADAS_CUDA(cudaMemcpyAsync(pts, u->d_pts, (size_t)batch * 4 * mp * 2 * 4, cudaMemcpyDeviceToHost, u->stream));
+    ADAS_CUDA(cudaMemcpyAsync(npts, u->d_npts, (size_t)batch * 4 * 4, cudaMemcpyDeviceToHost, u->stream));
+    ADAS_CUDA(cudaMemcpyAsync(status, u->d_status, (size_t)batch * 4, cudaMemcpyDeviceToHost, u->stream));
+    u->ufld_last_batch = batch;
+    if (copy_yolo_results_finish(e->yp, batch, max_det, counts, n_candidates, e->h_ncand.data(), e->stream)) return 1;
+    ADAS_CUDA(cudaStreamSynchronize(u->stream));
     return 0;
 }
 

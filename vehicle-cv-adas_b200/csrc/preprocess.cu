@@ -39,15 +39,6 @@ LetterboxGeom letterbox_geom(int src_h, int src_w, int in_h, int in_w) {
     return g;
 }
 
-struct ResizeTab {
-    int* xofs = nullptr;     // [dw]   left source column
-    int* xofs1 = nullptr;    // [dw]   right source column
-    short* xa = nullptr;     // [dw*2] coefficients
-    int* yofs = nullptr;     // [dh]   upper source row (clipped)
-    int* yofs1 = nullptr;    // [dh]   lower source row (clipped)
-    short* yb = nullptr;     // [dh*2]
-};
-
 static short sat_short_round(float v) {
     long r = lrintf(v);   // round half to even, like cvRound
     if (r > 32767) r = 32767;
@@ -128,25 +119,50 @@ __device__ __forceinline__ void resize_px(const uint8_t* __restrict__ src, int s
     }
 }
 
-// YOLO letterbox + blob. One thread per network-input pixel.
-__global__ void yolo_pre_kernel(const uint8_t* __restrict__ frames, int B, LetterboxGeom g, ResizeTab t,
-                                __half* __restrict__ img, int img_ld, float* __restrict__ blob) {
-    const long long total = (long long)B * g.in_h * g.in_w;
+int rig_camera(const uint8_t* frames, int H, int W, int yolo_h, int yolo_w, int ufld_w, int ufld_resize_h, RigCamera* c) {
+    c->frames = frames; c->H = H; c->W = W;
+    c->g = LetterboxGeom{}; c->yolo = ResizeTab{}; c->ufld = ResizeTab{};
+    if (yolo_h > 0) {
+        c->g = letterbox_geom(H, W, yolo_h, yolo_w);
+        const LetterboxGeom& g = c->g;
+        // a frame more than in_w (or in_h) times taller than wide letterboxes to 0 columns (rows): nothing to resize into
+        ADAS_CHECK(g.new_w >= 1 && g.new_h >= 1, "yolo_pre: a %d x %d frame letterboxes to %d x %d inside %d x %d", g.src_h, g.src_w, g.new_h,
+                   g.new_w, g.in_h, g.in_w);
+        if (get_resize_tab(W, H, g.new_w, g.new_h, &c->yolo)) return 1;
+    }
+    if (ufld_w > 0 && get_resize_tab(W, H, ufld_w, ufld_resize_h, &c->ufld)) return 1;
+    return 0;
+}
+
+// frame b of a rig launch: its camera and its first byte (64-bit: a 3840 x 2160 frame is 24.9 MB, a camera's block F times that)
+__device__ __forceinline__ const RigCamera& rig_frame(const RigTable& t, int b, const uint8_t** src) {
+    const int c = b / t.F;
+    const RigCamera& cam = t.cam[c];
+    *src = cam.frames + (size_t)(b - c * t.F) * cam.H * cam.W * 3;
+    return cam;
+}
+
+// YOLO letterbox + blob, every frame from its own camera's geometry. One thread per network-input pixel.
+__global__ void yolo_pre_kernel(const RigTable t, int in_h, int in_w, __half* __restrict__ img, int img_ld, float* __restrict__ blob) {
+    const long long total = (long long)t.n * t.F * in_h * in_w;
     const float inv255 = (float)(1.0 / 255.0);   // blobFromImage multiplies in float32
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-        const int x = (int)(i % g.in_w);
-        long long r = i / g.in_w;
-        const int y = (int)(r % g.in_h);
-        const int b = (int)(r / g.in_h);
+        const int x = (int)(i % in_w);
+        long long r = i / in_w;
+        const int y = (int)(r % in_h);
+        const int b = (int)(r / in_h);
+        const uint8_t* src;
+        const RigCamera& cam = rig_frame(t, b, &src);
+        const LetterboxGeom& g = cam.g;
         int bgr[3] = {114, 114, 114};
         const int ry = y - g.pad_h, rx = x - g.pad_w;
         if (ry >= 0 && ry < g.new_h && rx >= 0 && rx < g.new_w)
-            resize_px(frames + (size_t)b * g.src_h * g.src_w * 3, g.src_w, t, ry, rx, bgr);
+            resize_px(src, cam.W, cam.yolo, ry, rx, bgr);
         const float rf = __fmul_rn((float)bgr[2], inv255);
         const float gf = __fmul_rn((float)bgr[1], inv255);
         const float bf = __fmul_rn((float)bgr[0], inv255);
         if (img != nullptr) {
-            const size_t row = ((size_t)b * (g.in_h + 2) + (y + 1)) * (g.in_w + 2) + (x + 1);
+            const size_t row = ((size_t)b * (in_h + 2) + (y + 1)) * (in_w + 2) + (x + 1);
             __half2 lo = __floats2half2_rn(rf, gf);
             __half2 hi = __floats2half2_rn(bf, 0.f);
             uint2 v;
@@ -155,41 +171,52 @@ __global__ void yolo_pre_kernel(const uint8_t* __restrict__ frames, int B, Lette
             *reinterpret_cast<uint2*>(img + row * img_ld) = v;
         }
         if (blob != nullptr) {
-            const size_t plane = (size_t)g.in_h * g.in_w;
-            float* o = blob + (size_t)b * 3 * plane + (size_t)y * g.in_w + x;
+            const size_t plane = (size_t)in_h * in_w;
+            float* o = blob + (size_t)b * 3 * plane + (size_t)y * in_w + x;
             o[0] = rf; o[plane] = gf; o[2 * plane] = bf;
         }
     }
 }
 
-int launch_yolo_pre(const uint8_t* frames, int B, const LetterboxGeom& g, __half* img_padded, int img_ld,
-                    float* blob_nchw, cudaStream_t st) {
-    // a frame more than in_w (or in_h) times taller than wide letterboxes to 0 columns (rows): nothing to resize into
-    ADAS_CHECK(g.new_w >= 1 && g.new_h >= 1, "yolo_pre: a %d x %d frame letterboxes to %d x %d inside %d x %d", g.src_h, g.src_w, g.new_h,
-               g.new_w, g.in_h, g.in_w);
-    ResizeTab t;
-    if (get_resize_tab(g.src_w, g.src_h, g.new_w, g.new_h, &t)) return 1;
-    const long long total = (long long)B * g.in_h * g.in_w;
+static int rig_check(const RigTable& t, const char* fn) {
+    ADAS_CHECK(t.n >= 1 && t.n <= ADAS_MAX_RIG_CAMERAS && t.F >= 1, "%s: %d cameras of %d frames", fn, t.n, t.F);
+    return 0;
+}
+
+int launch_yolo_pre_rig(const RigTable& t, int in_h, int in_w, __half* img_padded, int img_ld, float* blob_nchw, cudaStream_t st) {
+    if (rig_check(t, "yolo_pre")) return 1;
+    for (int c = 0; c < t.n; ++c)
+        ADAS_CHECK(t.cam[c].yolo.xofs != nullptr && t.cam[c].g.in_h == in_h && t.cam[c].g.in_w == in_w,
+                   "yolo_pre: camera %d has no letterbox for a %d x %d input", c, in_h, in_w);
+    const long long total = (long long)t.n * t.F * in_h * in_w;
     int blocks = (int)((total + 255) / 256);
     if (blocks > 132 * 16) blocks = 132 * 16;
-    yolo_pre_kernel<<<blocks, 256, 0, st>>>(frames, B, g, t, img_padded, img_ld, blob_nchw);
+    yolo_pre_kernel<<<blocks, 256, 0, st>>>(t, in_h, in_w, img_padded, img_ld, blob_nchw);
     count_launch();
     ADAS_CUDA(cudaGetLastError());
     return 0;
 }
 
+int launch_yolo_pre(const uint8_t* frames, int B, const LetterboxGeom& g, __half* img_padded, int img_ld,
+                    float* blob_nchw, cudaStream_t st) {
+    RigTable t = rig_one(frames, B, g.src_h, g.src_w);
+    if (rig_camera(frames, g.src_h, g.src_w, g.in_h, g.in_w, 0, 0, &t.cam[0])) return 1;
+    return launch_yolo_pre_rig(t, g.in_h, g.in_w, img_padded, img_ld, blob_nchw, st);
+}
+
 // UFLD: resize to (in_w, resize_h), keep the bottom in_h rows, per-channel LUT (float64 math done on host).
-__global__ void ufld_pre_kernel(const uint8_t* __restrict__ frames, int B, int H, int W, int in_h, int in_w, int row0,
-                                ResizeTab t, const float* __restrict__ lut, __half* __restrict__ img, int img_ld,
-                                float* __restrict__ blob) {
-    const long long total = (long long)B * in_h * in_w;
+__global__ void ufld_pre_kernel(const RigTable t, int in_h, int in_w, int row0, const float* __restrict__ lut, __half* __restrict__ img,
+                                int img_ld, float* __restrict__ blob) {
+    const long long total = (long long)t.n * t.F * in_h * in_w;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const int x = (int)(i % in_w);
         long long r = i / in_w;
         const int y = (int)(r % in_h);
         const int b = (int)(r / in_h);
+        const uint8_t* src;
+        const RigCamera& cam = rig_frame(t, b, &src);
         int bgr[3];
-        resize_px(frames + (size_t)b * H * W * 3, W, t, y + row0, x, bgr);
+        resize_px(src, cam.W, cam.ufld, y + row0, x, bgr);
         const float rf = lut[bgr[2]];
         const float gf = lut[256 + bgr[1]];
         const float bf = lut[512 + bgr[0]];
@@ -210,19 +237,25 @@ __global__ void ufld_pre_kernel(const uint8_t* __restrict__ frames, int B, int H
     }
 }
 
-int launch_ufld_pre(const uint8_t* frames, int B, int H, int W, int in_h, int in_w, int resize_h, const float* lut,
-                    __half* img_padded, int img_ld, float* blob_nchw, cudaStream_t st) {
-    ResizeTab t;
-    if (get_resize_tab(W, H, in_w, resize_h, &t)) return 1;
+int launch_ufld_pre_rig(const RigTable& t, int in_h, int in_w, int resize_h, const float* lut, __half* img_padded, int img_ld,
+                        float* blob_nchw, cudaStream_t st) {
+    if (rig_check(t, "ufld_pre")) return 1;
+    for (int c = 0; c < t.n; ++c) ADAS_CHECK(t.cam[c].ufld.xofs != nullptr, "ufld_pre: camera %d has no resize tables", c);
     ADAS_CHECK(resize_h >= in_h, "ufld_pre: resized height %d smaller than network height %d", resize_h, in_h);
-    const long long total = (long long)B * in_h * in_w;
+    const long long total = (long long)t.n * t.F * in_h * in_w;
     int blocks = (int)((total + 255) / 256);
     if (blocks > 132 * 16) blocks = 132 * 16;
-    ufld_pre_kernel<<<blocks, 256, 0, st>>>(frames, B, H, W, in_h, in_w, resize_h - in_h, t, lut, img_padded, img_ld,
-                                            blob_nchw);
+    ufld_pre_kernel<<<blocks, 256, 0, st>>>(t, in_h, in_w, resize_h - in_h, lut, img_padded, img_ld, blob_nchw);
     count_launch();
     ADAS_CUDA(cudaGetLastError());
     return 0;
+}
+
+int launch_ufld_pre(const uint8_t* frames, int B, int H, int W, int in_h, int in_w, int resize_h, const float* lut,
+                    __half* img_padded, int img_ld, float* blob_nchw, cudaStream_t st) {
+    RigTable t = rig_one(frames, B, H, W);
+    if (rig_camera(frames, H, W, 0, 0, in_w, resize_h, &t.cam[0])) return 1;
+    return launch_ufld_pre_rig(t, in_h, in_w, resize_h, lut, img_padded, img_ld, blob_nchw, st);
 }
 
 }  // namespace adas

@@ -18,13 +18,14 @@ static constexpr int UFLD_THREADS = 384;
 static constexpr int UFLD_MAX_ANCH = 128;
 
 __global__ void __launch_bounds__(UFLD_THREADS)
-ufld_post_kernel(const float* __restrict__ heads, int ld, UfldDims d, int img_w, int img_h,
+ufld_post_kernel(const float* __restrict__ heads, int ld, UfldDims d, const RigTable t,
                  const double* __restrict__ row_anchor, const double* __restrict__ col_anchor, int32_t* __restrict__ pts,
                  int32_t* __restrict__ npts, uint8_t* __restrict__ status, double* __restrict__ coords, int max_pts) {
     __shared__ int s_valid[2][4][UFLD_MAX_ANCH];      // [row/col][lane][anchor]
     __shared__ double s_coord[2][4][UFLD_MAX_ANCH];   // expectation coordinate (float64, pre-truncation)
     const int b = blockIdx.x;
     const int tid = threadIdx.x;
+    const int img_w = t.cam[b / t.F].W, img_h = t.cam[b / t.F].H;     // this frame's camera
     const float* loc_row = heads + (size_t)b * ld;
     const float* loc_col = loc_row + (size_t)d.ngr * d.ncr * d.nl;
     const float* ex_row = loc_col + (size_t)d.ngc * d.ncc * d.nl;
@@ -95,18 +96,23 @@ ufld_post_kernel(const float* __restrict__ heads, int ld, UfldDims d, int img_w,
     }
 }
 
-int launch_ufld_post(const float* heads, int ld, int B, UfldDims d, int img_w, int img_h, const double* row_anchor,
-                     const double* col_anchor, int32_t* pts, int32_t* npts, uint8_t* status, double* coords, int max_pts,
-                     cudaStream_t st) {
+int launch_ufld_post_rig(const float* heads, int ld, const RigTable& t, UfldDims d, const double* row_anchor, const double* col_anchor,
+                         int32_t* pts, int32_t* npts, uint8_t* status, double* coords, int max_pts, cudaStream_t st) {
+    ADAS_CHECK(t.n >= 1 && t.n <= ADAS_MAX_RIG_CAMERAS && t.F >= 1, "ufld_post: %d cameras of %d frames", t.n, t.F);
     ADAS_CHECK(d.nl == 4, "ufld_post: num_lanes must be 4 (got %d)", d.nl);
     ADAS_CHECK(d.ncr <= UFLD_MAX_ANCH && d.ncc <= UFLD_MAX_ANCH, "ufld_post: too many anchors");
     // the expectation divides by num_grid - 1: a 1-cell grid has no coordinate (the reference's int() of the infinity raises)
     ADAS_CHECK(d.ngr >= 2 && d.ngc >= 2, "ufld_post: grids of %d x %d cells, need at least 2 each", d.ngr, d.ngc);
-    ufld_post_kernel<<<B, UFLD_THREADS, 0, st>>>(heads, ld, d, img_w, img_h, row_anchor, col_anchor, pts, npts, status, coords,
-                                                max_pts);
+    ufld_post_kernel<<<t.n * t.F, UFLD_THREADS, 0, st>>>(heads, ld, d, t, row_anchor, col_anchor, pts, npts, status, coords, max_pts);
     count_launch();
     ADAS_CUDA(cudaGetLastError());
     return 0;
+}
+
+int launch_ufld_post(const float* heads, int ld, int B, UfldDims d, int img_w, int img_h, const double* row_anchor,
+                     const double* col_anchor, int32_t* pts, int32_t* npts, uint8_t* status, double* coords, int max_pts,
+                     cudaStream_t st) {
+    return launch_ufld_post_rig(heads, ld, rig_one(nullptr, B, img_h, img_w), d, row_anchor, col_anchor, pts, npts, status, coords, max_pts, st);
 }
 
 // ------------------------------------------------------------------------------------------------------------------------------
@@ -120,11 +126,12 @@ int launch_ufld_post(const float* heads, int ld, int B, UfldDims d, int img_w, i
 //       [int(x * w_ratio), int(y * h_ratio)]                                                                               :112-131
 // One CTA per frame, one thread per (reversed row p, lane l); head layout [griding_num + 1][rows][4].
 __global__ void __launch_bounds__(UFLD_THREADS)
-ufld_v1_post_kernel(const float* __restrict__ head, int ld, int G, int R, int in_w, int in_h, int cfg_w, int cfg_h, int img_w, int img_h,
+ufld_v1_post_kernel(const float* __restrict__ head, int ld, int G, int R, int in_w, int in_h, int cfg_w, int cfg_h, const RigTable t,
                     const double* __restrict__ row_anchor, int32_t* __restrict__ pts, int32_t* __restrict__ npts, uint8_t* __restrict__ status,
                     double* __restrict__ coords, int max_pts) {
     __shared__ double s_loc[4][UFLD_MAX_ANCH];
     const int b = blockIdx.x, tid = threadIdx.x;
+    const int img_w = t.cam[b / t.F].W, img_h = t.cam[b / t.F].H;     // this frame's camera
     const float* out = head + (size_t)b * ld;
     const int stride = R * 4;
     for (int t = tid; t < R * 4; t += UFLD_THREADS) {
@@ -171,13 +178,20 @@ ufld_v1_post_kernel(const float* __restrict__ head, int ld, int G, int R, int in
     }
 }
 
-int launch_ufld_v1_post(const float* head, int ld, int B, int G, int R, int in_w, int in_h, int cfg_w, int cfg_h, int img_w, int img_h,
-                        const double* row_anchor, int32_t* pts, int32_t* npts, uint8_t* status, double* coords, int max_pts, cudaStream_t st) {
+int launch_ufld_v1_post_rig(const float* head, int ld, const RigTable& t, int G, int R, int in_w, int in_h, int cfg_w, int cfg_h,
+                            const double* row_anchor, int32_t* pts, int32_t* npts, uint8_t* status, double* coords, int max_pts, cudaStream_t st) {
+    ADAS_CHECK(t.n >= 1 && t.n <= ADAS_MAX_RIG_CAMERAS && t.F >= 1, "ufld_v1_post: %d cameras of %d frames", t.n, t.F);
     ADAS_CHECK(G >= 3 && R >= 1 && R <= UFLD_MAX_ANCH && max_pts >= R, "ufld_v1_post: bad head %d x %d", G, R);
-    ufld_v1_post_kernel<<<B, UFLD_THREADS, 0, st>>>(head, ld, G, R, in_w, in_h, cfg_w, cfg_h, img_w, img_h, row_anchor, pts, npts, status, coords, max_pts);
+    ufld_v1_post_kernel<<<t.n * t.F, UFLD_THREADS, 0, st>>>(head, ld, G, R, in_w, in_h, cfg_w, cfg_h, t, row_anchor, pts, npts, status, coords, max_pts);
     count_launch();
     ADAS_CUDA(cudaGetLastError());
     return 0;
+}
+
+int launch_ufld_v1_post(const float* head, int ld, int B, int G, int R, int in_w, int in_h, int cfg_w, int cfg_h, int img_w, int img_h,
+                        const double* row_anchor, int32_t* pts, int32_t* npts, uint8_t* status, double* coords, int max_pts, cudaStream_t st) {
+    return launch_ufld_v1_post_rig(head, ld, rig_one(nullptr, B, img_h, img_w), G, R, in_w, in_h, cfg_w, cfg_h, row_anchor, pts, npts, status, coords,
+                                   max_pts, st);
 }
 
 }  // namespace adas

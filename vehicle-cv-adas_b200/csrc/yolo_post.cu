@@ -259,7 +259,7 @@ struct NmsSmem {   // dynamic smem carve-up, cap entries each
 };
 
 __global__ void __launch_bounds__(NMS_THREADS)
-yolo_compact_nms_kernel(const float* __restrict__ raw, int kind, int A, int nc, LetterboxGeom g, double nms_iou,
+yolo_compact_nms_kernel(const float* __restrict__ raw, int kind, int A, int nc, const RigTable t, double nms_iou,
                         int max_det, int cap, int scap, double* __restrict__ work, const int32_t* __restrict__ flags, const int32_t* __restrict__ cls,
                         const float* __restrict__ conf, int32_t* __restrict__ n_cand, float* __restrict__ cand_box,
                         float* __restrict__ cand_conf, int32_t* __restrict__ cand_cls, float* __restrict__ out_box,
@@ -301,7 +301,8 @@ yolo_compact_nms_kernel(const float* __restrict__ raw, int kind, int A, int nc, 
     const int total = s_total;
     const int N = min(total, cap);
 
-    // float32 letterbox undo: (x - pad) * ratio, ratio = float32(old/new)  (utils.py:65-68,82-83)
+    // float32 letterbox undo with the geometry of this frame's camera: (x - pad) * ratio, ratio = float32(old/new)  (utils.py:65-68,82-83)
+    const LetterboxGeom& g = t.cam[b / t.F].g;
     const float ratioh = (float)((double)g.src_h / (double)g.new_h);
     const float ratiow = (float)((double)g.src_w / (double)g.new_w);
     const float padw = (float)g.pad_w, padh = (float)g.pad_h;
@@ -409,8 +410,10 @@ yolo_compact_nms_kernel(const float* __restrict__ raw, int kind, int A, int nc, 
     if (lane == 0) out_count[b] = outn;
 }
 
-int launch_yolo_post(const float* raw, int kind, int B, int A, int nc, const LetterboxGeom& g, double box_score,
-                     double nms_iou, int max_det, YoloPostBufs& w, cudaStream_t st) {
+int launch_yolo_post_rig(const float* raw, int kind, const RigTable& t, int A, int nc, double box_score, double nms_iou, int max_det,
+                         YoloPostBufs& w, cudaStream_t st) {
+    ADAS_CHECK(t.n >= 1 && t.n <= ADAS_MAX_RIG_CAMERAS && t.F >= 1, "yolo_post: %d cameras of %d frames", t.n, t.F);
+    const int B = t.n * t.F;
     const long long total = (long long)B * A;
     int blocks = (int)((total + 127) / 128);
     yolo_select_kernel<<<blocks, 128, 0, st>>>(raw, kind, B, A, nc, box_score, w.flags, w.cls, w.conf);
@@ -429,12 +432,19 @@ int launch_yolo_post(const float* raw, int kind, int B, int A, int nc, const Let
             attr_set[dev] = true;
         }
     }
-    yolo_compact_nms_kernel<<<B, NMS_THREADS, smem, st>>>(raw, kind, A, nc, g, nms_iou, max_det, w.cap, scap, w.nms_work, w.flags, w.cls, w.conf,
+    yolo_compact_nms_kernel<<<B, NMS_THREADS, smem, st>>>(raw, kind, A, nc, t, nms_iou, max_det, w.cap, scap, w.nms_work, w.flags, w.cls, w.conf,
                                                           w.n_cand, w.cand_box, w.cand_conf, w.cand_cls, w.out_box,
                                                           w.out_score, w.out_cls, w.out_idx, w.out_count);
     count_launch();
     ADAS_CUDA(cudaGetLastError());
     return 0;
+}
+
+int launch_yolo_post(const float* raw, int kind, int B, int A, int nc, const LetterboxGeom& g, double box_score,
+                     double nms_iou, int max_det, YoloPostBufs& w, cudaStream_t st) {
+    RigTable t = rig_one(nullptr, B, g.src_h, g.src_w);
+    t.cam[0].g = g;
+    return launch_yolo_post_rig(raw, kind, t, A, nc, box_score, nms_iou, max_det, w, st);
 }
 
 }  // namespace adas

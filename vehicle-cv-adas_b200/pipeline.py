@@ -14,6 +14,10 @@ A rig of several cameras runs through ONE pipeline (`cameras=K`): the engines ho
 `adas_detect_pair` call for the frames of all cameras, and the K trackers (one per camera) advance in one library call with one
 association launch per frame for all of them (`adas_tracker_update_multi`).  Results equal K single-camera pipelines whose
 trackers are updated frame by frame in camera order.
+
+Cameras of different frame sizes (`frame_sizes=[(H, W), ...]`, one per camera) run through the same single call
+(`adas_detect_pair_rig`): every frame is letterboxed / resized from its own camera's size into the one network batch, and each
+camera's boxes and lane points come back in that camera's pixels.
 """
 from __future__ import annotations
 
@@ -38,17 +42,38 @@ class StepResult:
         self.tracks: Optional[List[list]] = None
 
 
+def letterbox_hw(src_h: int, src_w: int, in_h: int, in_w: int):
+    """(rows, columns) an src_h x src_w frame is resized to inside an in_h x in_w network input (Scaler.process_image's letterbox,
+    the arithmetic of the device's letterbox_geom)"""
+    if src_h == src_w:
+        return in_h, in_w
+    hw_scale = src_h / src_w
+    if hw_scale > 1.0:
+        return in_h, int(in_w / hw_scale)
+    return int(in_h * hw_scale) + 1, in_w
+
+
+MAX_RIG_CAMERAS = 16          # ADAS_MAX_RIG_CAMERAS
+
+
 class AdasPipeline:
     def __init__(self, yolo_plan: str, ufld_plan: str, device: int = 0, batch: int = 8, box_score: float = 0.4, box_nms_iou: float = 0.45,
                  max_det: int = 1024, class_names: Optional[List[str]] = None, depth: int = 3, sets: int = 2, track_thresh: float = 0.5,
-                 cameras: int = 1):
+                 cameras: int = 1, frame_sizes=None):
         """`cameras` = K streams of one frame size through one pipeline: with K > 1, step / step_pipelined take [K, F, H, W, 3] frames
         (F <= batch; a host array, a sequence of K [F, H, W, 3] host arrays, or a device pointer with shape (K, F, H, W)) and
-        return one StepResult per camera."""
+        return one StepResult per camera.
+
+        `frame_sizes` = K (H, W) pairs: the cameras may differ in frame size.  step / step_pipelined then take a list of K host arrays
+        [F, H_c, W_c, 3] uint8 (on_device=False) or of K (device pointer, (F, H_c, W_c)) pairs (on_device=True), each camera at its
+        declared size and all with the same F <= batch, and return one StepResult per camera in that camera's pixels."""
         if cameras < 1:
             raise ValueError(f"cameras must be at least 1, got {cameras}")
+        if frame_sizes is not None:
+            frame_sizes = AdasPipeline._check_frame_sizes(cameras, frame_sizes)
         self.batch, self.box_score, self.box_nms_iou, self.max_det = batch, box_score, box_nms_iou, max_det
         self.cameras = cameras
+        self.frame_sizes = frame_sizes
         nb = cameras * batch
         # `sets` independent (object engine, lane engine) pairs: consecutive batches alternate between them so the next batch's
         # kernels are already queued on the device (own streams, own activation buffers) while the previous batch drains --
@@ -64,6 +89,18 @@ class AdasPipeline:
             for e in (y, u):
                 e.run(nb)
                 e.run(nb)
+        if frame_sizes is not None:
+            try:
+                AdasPipeline._check_frame_sizes(cameras, frame_sizes, tuple(self.yolo.input_shape[2:4]))
+                # one rig call per engine pair: the resize tables of every camera and the staging arena exist before the first step
+                zeros = [np.zeros((batch, h, w, 3), np.uint8) for h, w in frame_sizes]
+                for y, u, _ in self.sets:
+                    _capi.detect_pair_rig(y, u, zeros, box_score, box_nms_iou, max_det)
+            except Exception:
+                for y, u, _ in self.sets:
+                    y.close()
+                    u.close()
+                raise
         self._next_set = 0
         self.trackers = [BYTETracker(track_thresh=track_thresh, names=class_names or [], device=device) for _ in range(cameras)]
         for t in self.trackers:
@@ -85,6 +122,8 @@ class AdasPipeline:
     def _detect_both(self, frames, on_device: bool, shape, k: int = 0):
         y, u, lock = self.sets[k]
         with lock:                        # one batch at a time per engine pair
+            if self.frame_sizes is not None:
+                return _capi.detect_pair_rig(y, u, frames, self.box_score, self.box_nms_iou, self.max_det, on_device)
             return _capi.detect_pair(y, u, frames, self.box_score, self.box_nms_iou, self.max_det, on_device, shape)
 
     def _detect(self, frames, on_device: bool, shape):
@@ -113,8 +152,62 @@ class AdasPipeline:
         self.track_seconds = getattr(self, "track_seconds", 0.0) + (time.perf_counter() - t0)
         self.track_batches = getattr(self, "track_batches", 0) + 1
 
+    @staticmethod
+    def _check_frame_sizes(cameras: int, frame_sizes, in_hw=None):
+        """the declared (H, W) of every camera as a list of int pairs; refuses (ValueError) a count other than `cameras`, more than
+        MAX_RIG_CAMERAS cameras, a size below 1 x 1, and -- given the YOLO input size in_hw -- a size whose letterbox is empty"""
+        try:
+            sizes = [(int(h), int(w)) for h, w in frame_sizes]
+        except (TypeError, ValueError):
+            raise ValueError(f"frame_sizes must be {cameras} (H, W) pairs, got {frame_sizes!r}") from None
+        if len(sizes) != cameras:
+            raise ValueError(f"{len(sizes)} frame sizes for {cameras} cameras")
+        if cameras > MAX_RIG_CAMERAS:
+            raise ValueError(f"{cameras} cameras of declared sizes; a rig has at most {MAX_RIG_CAMERAS}")
+        for c, (h, w) in enumerate(sizes):
+            if h < 1 or w < 1:
+                raise ValueError(f"camera {c}: frame size {h} x {w}")
+            if in_hw is not None and min(letterbox_hw(h, w, *in_hw)) < 1:
+                raise ValueError(f"camera {c}: a {h} x {w} frame letterboxes to {letterbox_hw(h, w, *in_hw)} inside {tuple(in_hw)}: nothing to detect in")
+        return sizes
+
+    def _rig_frames(self, frames, on_device: bool, shape):
+        """the frames of one step of a pipeline with declared frame sizes, as adas_detect_pair_rig takes them: K host arrays
+        [F, H_c, W_c, 3] uint8 or K (device pointer, (F, H_c, W_c)) pairs, each camera at its declared size, one F in 1..batch"""
+        K = self.cameras
+        try:
+            cams = list(frames)
+        except TypeError:
+            raise ValueError(f"frames of {K} cameras of declared sizes must be a list of {K} entries, got {type(frames).__name__}") from None
+        if len(cams) != K:
+            raise ValueError(f"frames of {len(cams)} cameras for a pipeline of {K}")
+        out, F = [], None
+        for c, (a, (h, w)) in enumerate(zip(cams, self.frame_sizes)):
+            if on_device:
+                if not (isinstance(a, (tuple, list)) and len(a) == 2 and isinstance(a[1], (tuple, list)) and len(a[1]) == 3):
+                    raise ValueError(f"camera {c}: device frames are (pointer, (frames, H, W)), got {a!r}")
+                f, fh, fw = (int(v) for v in a[1])
+                out.append((int(a[0]), (f, fh, fw)))
+            else:
+                if not (isinstance(a, np.ndarray) and a.dtype == np.uint8 and a.ndim == 4 and a.shape[3] == 3):
+                    what = f"{a.dtype} {a.shape}" if isinstance(a, np.ndarray) else type(a).__name__
+                    raise ValueError(f"camera {c}: frames must be a uint8 [frames, H, W, 3] array, got {what}")
+                f, fh, fw = a.shape[:3]
+                out.append(a)
+            if (fh, fw) != (h, w):
+                raise ValueError(f"camera {c} sends {fh} x {fw} frames; its declared size is {h} x {w}")
+            if F is None:
+                F = f
+            elif f != F:
+                raise ValueError(f"every camera must send the same number of frames: camera {c} sends {f}, camera 0 {F}")
+        if not 1 <= F <= self.batch:
+            raise ValueError(f"{F} frames per camera; this pipeline takes 1 to {self.batch}")
+        return out, on_device, None
+
     def _frames(self, frames, on_device: bool, shape):
         """the frames of one step as adas_detect_pair takes them: with K > 1 cameras, camera-major [K * F, H, W, 3]"""
+        if getattr(self, "frame_sizes", None) is not None:
+            return AdasPipeline._rig_frames(self, frames, on_device, shape)
         K = self.cameras
         if K == 1:
             return frames, on_device, shape
@@ -164,7 +257,7 @@ class AdasPipeline:
 
     def _result(self, yu):
         y, u = yu
-        if self.cameras == 1:
+        if self.cameras == 1 and self.frame_sizes is None:
             r = StepResult(y, u)
             self._track(r)
             return r
